@@ -204,7 +204,7 @@ def workload_config(args, world):
                         "GROUP BY o_orderdate: count(*), sum(l_extendedprice)",
             "sf_per_gpu": args.sf, "sf_total": args.sf * world, "datanodes": world,
             "parallelism": f"{world} datanode(s), one per GPU, SHARD placement on the order key",
-            "l2": "inputs (>= 11 GB per GPU at SF100) are far larger than the 126 MB L2; no flush needed between steps",
+            "l2": "inputs (>= 11 GB per GPU at SF100) are far larger than the 50 MB L2; no flush needed between steps",
             "memory": "gx_pool_reserve(0): free HBM minus 8 GB mapped into the stream-ordered pool at start-up"}
 
 
@@ -232,6 +232,20 @@ def same_result(got, want, int_aggs=(), rtol=1e-9):
 
 def cat_results(parts):
     return tuple(np.concatenate([p[i] for p in parts]) for i in range(3))
+
+
+def dump_outputs(path, result, suffix=""):
+    """Writes what one configs[2] step returned (keys, aggs, nulls of Result.fetch) as float64 .npy files, rows sorted by
+    group key because the device emits groups in hash-table order.  count(*) is bit-cast int64 in aggs; it is converted
+    to its value.  Two builds run with the same arguments see the same generated tables and can be compared file by file."""
+    keys, aggs, nulls = result
+    order = np.lexsort([keys[:, c] for c in reversed(range(keys.shape[1]))]) if keys.shape[1] else np.arange(len(keys))
+    keys, aggs, nulls = keys[order], aggs[order], nulls[order]
+    aggs = aggs.copy()
+    aggs[:, 0] = aggs.view(np.int64)[:, 0]                      # configs[2]: aggregate 0 is count(*)
+    os.makedirs(path, exist_ok=True)
+    for name, a in (("keys", keys), ("aggs", aggs), ("nulls", nulls)):
+        np.save(os.path.join(path, f"{name}{suffix}.npy"), a.astype(np.float64))
 
 
 def phase_table(ctx, names, steps):
@@ -352,6 +366,8 @@ def run_ours(args):
     nl_total = allsum(float(nl))
     checks = {"count_star_equals_lineitem_rows": int(count_total) == int(nl_total),
               "groups_this_node": int(len(keys))}
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, last, f"_rank{rank}" if world > 1 else "")
 
     # ---- the other BASELINE configurations, same run, same tables (extras; the headline stays configs[2])
     extras = {}
@@ -359,13 +375,8 @@ def run_ours(args):
             "o": {"orderkey": g.O_ORDERKEY, "custkey": g.O_CUSTKEY, "orderdate": g.O_ORDERDATE, "shippriority": g.O_SHIPPRIORITY},
             "l": {"orderkey": g.L_ORDERKEY, "extendedprice": g.L_EXTENDEDPRICE, "discount": g.L_DISCOUNT, "shipdate": g.L_SHIPDATE}}
     q1plan = P.q1_plan(g.L_QUANTITY, g.L_EXTENDEDPRICE, g.L_DISCOUNT, g.L_TAX, g.L_SHIPDATE, g.L_RETURNFLAG, g.L_LINESTATUS)
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except (OSError, ValueError):
-        pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    peak = 3350.0                       # GB/s of HBM3, the H100 SXM data sheet's figure; the denominator of every frac_*
+    peak_src = "H100 SXM data sheet, 3350 GB/s (not measured)"
 
     def timed_block(fn, steps, warm=2):
         for _ in range(warm):
@@ -466,8 +477,7 @@ def run_ours(args):
                                  "count_star_equals_lineitem_rows": int(ucount) == int(nl_total),
                                  "probe_sectors_gb_s": (nl * 32.0 / (pm / 1e3) / 1e9) if pm else None,
                                  "probe_alg_frac_hbm": (nl * 24.0 / (pm / 1e3) / 1e9 / peak) if pm else None,
-                                 "note": "one 32-byte DRAM sector per probe is the floor for an unpartitioned probe of a table larger than L2 "
-                                         "(B200 delivers ~42 G random gathers/s, profiles/r01_ubench_random_access.txt)",
+                                 "note": "one 32-byte DRAM sector per probe is the floor for an unpartitioned probe of a table larger than L2",
                                  "phases_ms": ph}
         checks["unclustered_count_star_equals_lineitem_rows"] = extras["unclustered"]["count_star_equals_lineitem_rows"]
         lu.free(); ou.free()
@@ -513,29 +523,16 @@ def run_ours(args):
 
     probe_avg_ms = probe_ms / max(probe_n, 1)
     achieved = nl * ALG_BYTES_PER_PROBE_ROW / (probe_avg_ms / 1e3) / 1e9 if probe_n else None
-    traffic = None
-    traffic_src = None
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "probe_agg_traffic.json")))
-        if seg_n or tma_n:
-            tj = tj.get("gx_k_runjoin_seg" if seg_n else "gx_k_runjoin_tma") or {}
-        traffic = tj.get("dram_bytes_per_launch_sf100")
-        if traffic:
-            traffic_src = "profiles/probe_agg_traffic.json (ncu --set full capture of this kernel at SF100, " + str(tj.get("source", "")) + "); not measured in this run"
-    except (OSError, ValueError):
-        pass
     probe_kernel = ("gx_k_runjoin_seg (fused hash probe + hash aggregate over lineitem; join table streamed through a cp.async.bulk/mbarrier ring)"
                     if seg_n else
                     "gx_k_runjoin_tma (fused hash probe + hash aggregate over lineitem; outer rows delivered by cp.async.bulk onto per-warp mbarriers)"
                     if tma_n else "gx_k_runjoin (fused hash probe + hash aggregate over lineitem)")
     roofline = {"kernel": probe_kernel, "bound": "hbm",
                 "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": (achieved / peak) if achieved else None,
-                "traffic": traffic, "traffic_source": traffic_src,
-                "frac_dram": (traffic * (nl / 600_000_105.0) / (probe_avg_ms / 1e3) / 1e9 / peak) if (traffic and probe_n) else None,
                 "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": nl * ALG_BYTES_PER_PROBE_ROW, "avg_launch_ms": probe_avg_ms,
-                "note": "achieved/frac use SURVEY 8d's 24 B per probe row; frac_dram uses the DRAM bytes ncu measured for this kernel "
-                        "(compact 8-byte slots move fewer bytes than 8d charges), scaled to this run's row count",
+                "note": "achieved/frac use SURVEY 8d's 24 B per probe row; the run-folding probe reads the compact join table "
+                        "once per run, not once per row, so frac can exceed 1",
                 "build_kernel_avg_ms": build_ms / max(build_n, 1),
                 "build_alg_GBps": (no * ALG_BYTES_PER_BUILD_ROW / (build_ms / max(build_n, 1) / 1e3) / 1e9) if build_n else None}
 
@@ -773,6 +770,7 @@ def main():
     ap.add_argument("--no-unclustered", action="store_true", help="skip the row-permuted variant")
     ap.add_argument("--pages-gb", type=float, default=10.0, help="GB of heap pages pushed through the page loader (e2e_pages leg; 0 = skip)")
     ap.add_argument("--cpu-sample-orders", type=int, default=1_500_000)
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's result arrays to DIR/<name>.npy")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3

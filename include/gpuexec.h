@@ -1,5 +1,5 @@
 /*
- * gpuexec.h — C ABI of libgpuexec.so, the B200-native (sm_100a) replacement for
+ * gpuexec.h — C ABI of libgpuexec.so, the H100-native (sm_90a) replacement for
  * OpenTenBase's per-DataNode SeqScan -> HashJoin -> HashAggregate pipeline and the
  * cross-datanode redistribute step.
  *
@@ -19,7 +19,7 @@
  *     failure is available from gx_last_error();
  *   - the library owns all device memory; the caller frees handles explicitly
  *     (the provider does so from a ResourceOwner callback);
- *   - there is NO CPU fallback: if no sm_100a-capable device is present
+ *   - there is NO CPU fallback: if no sm_90a-capable device (H100) is present
  *     gx_init() fails and nothing else is callable.
  */
 #ifndef GPUEXEC_H

@@ -1,4 +1,4 @@
-"""opentenbase_b200 — B200-native (sm_100a) executor hot path for OpenTenBase.
+"""opentenbase_b200 — H100-native (sm_90a) executor hot path for OpenTenBase.
 
 The product is ``libgpuexec.so`` (hand-written CUDA behind the C ABI of
 ``include/gpuexec.h``) plus the C CustomScan provider under ``provider/``.
@@ -95,7 +95,7 @@ class GxHostTable(C.Structure):
 
 
 def build(force: bool = False) -> str:
-    """Compile libgpuexec.so for sm_100a with nvcc (cross-compiles without a GPU)."""
+    """Compile libgpuexec.so for sm_90a with nvcc (cross-compiles without a GPU)."""
     subprocess.check_call(["make", "-C", os.path.join(_HERE, "csrc"), "-s"] + (["-B"] if force else []))
     return LIB_PATH
 

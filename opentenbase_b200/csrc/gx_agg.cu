@@ -86,11 +86,10 @@ __device__ __forceinline__ void merge_word(unsigned long long *addr, int kind, u
 }
 
 // --------------------------------------------------------------- sinks
-// CTA-shared directory (+ dense state words).  Measured on B200
-// (profiles/r01_ubench_agg_update_mechanisms.txt): a CTA-shared table with
-// CAS-loop fp64 adds sustains ~230 G rows/s; for a handful of groups
-// lane-private accumulators ([word][group][lane], bank == lane, no atomics)
-// reach ~440 G rows/s.  Both are used here.
+// CTA-shared directory (+ dense state words): a CTA-shared table with
+// CAS-loop fp64 adds, and for a handful of groups lane-private accumulators
+// ([word][group][lane], bank == lane, no atomics) that need no atomics at all.
+// Both are used here.
 struct SmemTable {
     unsigned long long *tag, *k0, *k1, *w;   // dense: w[slot * nwords + i]; lane-private: see lp_base()
     unsigned int *gidx;                      // lane-private: slot -> dense group number
@@ -432,9 +431,8 @@ __global__ void __launch_bounds__(1024, 1) gx_k_agg(const __grid_constant__ gx_a
 // gx_k_agg<SINK_SMEM_LP>, but the plan is walked once per TILE of LPT_K x 32 rows instead of
 // once per row.  A lane holds LPT_K rows; for every aggregate the expression descriptor is
 // decoded once and its terms are evaluated for the lane's LPT_K rows back to back (LPT_K
-// independent loads in flight per term), then added to the rows' accumulators.  ncu on the
-// row-at-a-time interpreter: 1000 warp instructions per 32 rows and 14 warps per SM with
-// nothing to overlap the column loads (profiles/r01_bench_configs_sf100.json).
+// independent loads in flight per term), then added to the rows' accumulators: the
+// row-at-a-time interpreter has nothing to overlap the column loads with.
 // Plan shape (checked by the host): no join, every aggregate is count(*) or a sum/avg over a
 // chain expression of NOT-NULL float8 columns and constants.
 // LPT_K = rows per lane and tile: 8 when the CTA is small enough for the registers (<= 640 threads), else 4
@@ -895,8 +893,7 @@ __global__ void __launch_bounds__(512, 2) gx_k_count_char(const __grid_constant_
 //   [probe a unique-key join table with an int8 key ->] GROUP BY one 4-byte
 //   column (a scanned int4/date column, or the 4-byte join payload), aggregates
 //   drawn from { count(*), sum/avg(one float8 column) }, no quals, no NULLs.
-// The generic kernel above interprets the plan per row (~220-580 instructions
-// per row measured with ncu, profiles/r01_ncu_generic_kernel.txt): this one is
+// The generic kernel above interprets the plan per row: this one is
 // what the same plan compiles to by hand.  Four consecutive rows per thread:
 // 16-byte vector loads, four independent table probes in flight, equal
 // neighbouring keys probed once (TPC-H lineitem is clustered on the order key)
@@ -927,12 +924,14 @@ __device__ __forceinline__ int4 ld_stream_i4(const int *p)
     asm volatile("ld.global.nc.L1::no_allocate.v4.s32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
     return v;
 }
-// two neighbouring slots (one aligned 32-byte sector) with a single 256-bit load
+// two neighbouring slots (one aligned 32-byte sector): sm_90 has no 256-bit load, so two
+// 128-bit loads of the same sector are issued back to back
 struct gx_slot2 { long long k0; unsigned long long p0; long long k1; unsigned long long p1; };
 __device__ __forceinline__ gx_slot2 ld_slot2(const gx_slot *p)
 {
     gx_slot2 s;
-    asm volatile("ld.global.v4.u64 {%0, %1, %2, %3}, [%4];" : "=l"(s.k0), "=l"(s.p0), "=l"(s.k1), "=l"(s.p1) : "l"(p));
+    asm volatile("ld.global.v2.u64 {%0, %1}, [%4];\n\tld.global.v2.u64 {%2, %3}, [%4+16];"
+                 : "=l"(s.k0), "=l"(s.p0), "=l"(s.k1), "=l"(s.p1) : "l"(p));
     return s;
 }
 __device__ __forceinline__ gx_slot ld_slot(const gx_slot *p)
@@ -988,8 +987,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_fast(const __grid_constant__ gx_
             long long k[4] = { ka.x, ka.y, kb.x, kb.y };
             gx_slot2 sl[4];
             // A run of equal keys that started in the previous lane is not probed again:
-            // ncu showed such cross-lane repeats re-fetching their sector from DRAM
-            // (profiles/r01_ncu_fast_probe_and_bucket_build_sf100.csv).
+            // such cross-lane repeats would fetch their sector again.
             const unsigned int wmask = __activemask();
             const int lane = threadIdx.x & 31;
             long long prevk = __shfl_up_sync(wmask, k[3], 1);
@@ -1094,14 +1092,13 @@ __global__ void __launch_bounds__(1024, 1) gx_k_fast(const __grid_constant__ gx_
 // order-key order: runs of 1..7 rows).  A warp takes 128 consecutive rows, four per lane,
 // finds the run heads, and folds every run to ONE (key, count, sum) entry of a per-warp
 // shared-memory list — the entries of a run that spans lanes are merged there.  Then the
-// list is processed densely, one run per lane: slot function, one 256-bit load of the key's
+// list is processed densely, one run per lane: slot function, one 32-byte sector load of the key's
 // home pair, one group-table update.  Against the row-per-lane kernel above this removes
-// the repeated probes, the divergent per-row code and three of four group updates; ncu had
-// shown that kernel issue-bound at 13.8 of 32 threads per instruction
-// (profiles/r01_ncu_probe_pairs_sf100.csv).
+// the repeated probes, the divergent per-row code and three of four group updates, which
+// keep that kernel issue-bound with few active threads per instruction.
 struct gx_runlist { long long key[128]; double sum[128]; unsigned int cnt[128]; };
 
-// one key against the join table: the home group of slots arrives with a single 256-bit load
+// one key against the join table: the home group of slots arrives as one 32-byte sector (ld_slot2)
 // Branch-free inside the group: a table that is only ever filled (never deleted from) has no
 // match behind an empty slot, so "any slot matches" / "any slot empty" decide the step, and the
 // function has ONE exit (several exits made the compiler clone the group update per exit).
@@ -1234,8 +1231,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin(const __grid_constant__ 
 // ---------------------------------------------------------------------------
 // gx_k_runjoin_seg: the same join + aggregate, with the join table STREAMED instead of gathered.
 //
-// What ncu said about gx_k_runjoin (profiles/r01_ncu_final_sf100_raw.csv, r02_runjoin_variants.txt): 54 % issue
-// utilisation, 64 % of the DRAM peak, the warps parked on the dependent 256-bit slot load of their runs.  But with an
+// gx_k_runjoin's warps wait on the dependent slot load of their runs.  But with an
 // order-preserving slot function and an outer side in key order those loads are not random at all: the CTA's 31 tiles
 // of one iteration are 3968 consecutive rows, their keys lie in [first key, last key] of that chunk, and every home
 // slot of such a key lies in ONE contiguous piece of the table — about 14 KB at TPC-H's densities.  So a producer warp
@@ -1676,10 +1672,9 @@ __global__ void __launch_bounds__(512, 2) gx_k_runjoin2(const __grid_constant__ 
 // ---------------------------------------------------------------------------
 // gx_k_runjoin_tma: gx_k_runjoin with the outer rows delivered by the copy engine.
 //
-// The per-instruction stall samples of gx_k_runjoin (profiles/r01_ncu_final_sf100.ncu-rep, source page) put 14 % of all
-// samples on ONE register move right behind the "prefetch" loads of the next tile: ptxas lands half of the 128-bit
-// loads in temporaries and copies them into the loop-carried registers at once, so the warp waits out the DRAM latency
-// of its rows BEFORE it starts the probe, whose dependent slot load then costs a second one (27 % of the samples).
+// In gx_k_runjoin ptxas lands half of the 128-bit "prefetch" loads of the next tile in temporaries and copies them into
+// the loop-carried registers at once, so the warp waits out the DRAM latency of its rows BEFORE it starts the probe,
+// whose dependent slot load then costs a second one.
 // Here the rows never pass through registers on their way in: lane 0 of every warp asks the copy engine for the warp's
 // next tile (two 1 KB cp.async.bulk transfers, keys and values, completion counted on the warp's own mbarrier) as soon
 // as the lanes have read the current one out of shared memory — before the fold, a whole tile ahead — and nobody waits
@@ -1759,10 +1754,12 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin_tma(const __grid_constan
                 v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y;
             }
         }
+        // ---- the stage is free again: the next tile travels while this one is folded and probed.  The lanes' reads above are
+        // generic-proxy accesses and the copy engine's writes async-proxy ones: without the proxy fence a read still queued behind
+        // the other warps' shared-memory atomics (an outer side out of key order flushes a group per row) can return the next
+        // tile's key.
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncwarp();
-        // ---- the stage is free again: the next tile travels while this one is folded and probed.  No proxy fence between the
-        // lanes' reads above and the engine's writes: the reads have completed (their registers are consumed right below) a
-        // DRAM round trip before the first byte of the next tile can arrive, and the fence costs a MEMBAR.ALL.CTA per tile.
         kp += step; vp += step; left -= stride;
         if (left > 0) request(left >= 32 ? 1024u : (unsigned int) left << 5);
         int NR;
@@ -2591,10 +2588,10 @@ static int launch_runjoin_t(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_args
     GX_CUDA(ctx, cudaGetLastError());
     return GX_OK;
 }
-// Measured at SF100 on one B200 (profiles/r02_runjoin_variants.txt): gx_k_runjoin 2.787 ms, gx_k_runjoin_tma 2.660 ms, with the
-// branch-free fold 2.617 ms, with full probe rounds only 2.514 ms (parity suite, the whole GPU suite, smoke and the bench checks
-// green under it) -> 3 is the default; GX_RUNJOIN_TMA=0 restores gx_k_runjoin
-#define GX_RUNJOIN_TMA_DEFAULT 3          /* 0 off, 1 gx_k_runjoin_tma, 2 + branch-free fold, 3 + probe rounds of 32 lanes only */
+// Probe kernel at SF100 on one H100 80GB HBM3 (700 W), bench.py, two runs each: gx_k_runjoin 4.256 / 4.258 ms,
+// gx_k_runjoin_tma 3.937 / 3.934 ms, with the branch-free fold 4.043 / 4.039 ms, + full probe rounds only 3.971 / 3.965 ms
+// -> 1 is the default; GX_RUNJOIN_TMA=0 restores gx_k_runjoin
+#define GX_RUNJOIN_TMA_DEFAULT 1         /* 0 off, 1 gx_k_runjoin_tma, 2 + branch-free fold, 3 + probe rounds of 32 lanes only */
 // gx_k_runjoin_seg: 31 consumer warps + 1 producer warp, the rest of the CTA's shared memory is the two-deep ring of
 // join-table pieces.  0 slots = the ring does not fit next to this group table (the caller keeps gx_k_runjoin).
 // Ring depth 3 when three buffers of the size a chunk is expected to need fit (table slots per outer row x 3968 rows, + 15 %
@@ -2725,9 +2722,8 @@ static int launch_fast(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_args &FA,
             return launch_runjoin3_t<false, true, false>(ctx, A, FA, smem, name);
         }
     }
-    // gx_k_runjoin2: two CTAs of 512 threads per SM with 16-byte group slots (64 KB + 40 KB of run lists).  MEASURED SLOWER
-    // than one CTA of 1024 threads with 24-byte slots (3.29 vs 2.76 ms at SF100, profiles/r02_runjoin_variants.txt), like the
-    // other attempts to trade CTA size for occupancy on this kernel; kept behind GX_RUNJOIN_V2=1 for the record.
+    // gx_k_runjoin2: two CTAs of 512 threads per SM with 16-byte group slots (64 KB + 40 KB of run lists) instead of
+    // one CTA of 1024 threads with 24-byte slots; opt-in behind GX_RUNJOIN_V2=1.
     {
         const char *v2 = getenv("GX_RUNJOIN_V2");
         if (use_run && v2 && v2[0] == '1' && A.s_slots <= 4096) {
@@ -2917,7 +2913,7 @@ extern "C" int gx_hash_agg(gx_ctx *ctx, const gx_table *outer, const gx_hash *h,
     // plan down the general path below.
     {
         gx_runagg_args RA; memset(&RA, 0, sizeof(RA));
-        { const char *pf = getenv("GX_RUNAGG_PF"); RA.pf = pf ? atoi(pf) : 1; }     // Q3 chain at SF100: 5.68 ms without, 5.52 with the rows, 5.59 with rows + table lines
+        { const char *pf = getenv("GX_RUNAGG_PF"); RA.pf = pf ? atoi(pf) : 1; }     // bit 0: rows two tiles ahead into L2, bit 1: the tile's join-table lines
         const char *e = getenv("GX_NO_RUNAGG");
         bool ok = !(e && e[0] == '1') && plan->strategy == 0 && A.P.has_join && h->unique && A.P.key_type == GX_INT8 && A.P.okey.nulls == nullptr &&
                   outer->nrows > 0 && plan->n_group_cols >= 1;
@@ -2952,8 +2948,7 @@ extern "C" int gx_hash_agg(gx_ctx *ctx, const gx_table *outer, const gx_hash *h,
             static bool attr = false;
             const bool small = RA.nv <= 2 && RA.nc <= 2;           // two CTAs of 384 threads per SM (85 registers each)
             const char *dn = getenv("GX_RUNAGG_DENSE");
-            // 2 x 384 threads: 5.03 ms for the Q3 chain's lineitem side at SF100; 2 x 512 (28 bytes of spills): 4.49 ms
-            const int dense = (small && RA.nv <= 1) ? (dn ? atoi(dn) != 0 : 1) : 0;      // 2 x 640 (48 registers): 4.80 ms, profiles/r02_occupancy_variants.txt
+            const int dense = (small && RA.nv <= 1) ? (dn ? atoi(dn) != 0 : 1) : 0;
             const int threads = (small && !dense) ? 384 : 512, nwarps = threads / 32;
             const size_t smem = (size_t) nwarps * ((size_t) RA_LIST * (1 + RA.nv) + RA_LIST / 2) * 8;
             if (!attr) {
@@ -3063,7 +3058,7 @@ extern "C" int gx_hash_agg(gx_ctx *ctx, const gx_table *outer, const gx_hash *h,
             rc = cudaGetLastError() == cudaSuccess ? GX_OK : GX_ERR_CUDA;
         } else if (use_few) {
             const char *fv = getenv("GX_FG_VARIANT");
-            const bool v768 = !(fv && fv[0] == '0');                 // <4, 768> unless GX_FG_VARIANT=0 asks for <8, 512> (profiles/r02_fewgroups_variants.txt)
+            const bool v768 = !(fv && fv[0] == '0');                 // <4, 768> unless GX_FG_VARIANT=0 asks for <8, 512>
             const int fg_threads = v768 ? 768 : 512, fg_k = v768 ? 4 : 8, fg_warps = fg_threads / 32;
             const size_t fg_smem = (size_t) fg_warps * (1 + FG.nv) * (FG_G + 1) * 32 * 8;
             bool bytekey = plan->n_group_cols <= 2;

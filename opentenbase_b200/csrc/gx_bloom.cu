@@ -7,7 +7,7 @@
 // position (REHASH[i] * hash) >> 27; sized by MinLogSpace(ndv, 0.05) and abandoned above 2^20 buckets
 // (bloomfilter.c:20-35,68).  The hash is the join's own ExecHashGetHashValue for one key column with the
 // default "new hash": CRC32C of the value widened to int64 (hashint4new/hashint8new, hashfunc.c:112-175).
-// A filter is at most 32 MB, i.e. L2-resident on B200: a Find costs one L2 sector, not a DRAM one.
+// A filter is at most 32 MB, i.e. L2-resident on H100 (50 MB of L2): a Find costs one L2 sector, not a DRAM one.
 #include <math.h>
 #include "gx_internal.cuh"
 

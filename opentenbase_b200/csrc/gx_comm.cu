@@ -257,7 +257,7 @@ struct gx_route1_args {
     gx_dcol in[GX_MAX_COLS]; void *out[GX_MAX_COLS]; uint8_t *out_nulls[GX_MAX_COLS];
     long long cap; unsigned long long *cursor;   // [nnodes] rows claimed per destination; [GX_MAX_NODES] overflow flag
 };
-__global__ void __launch_bounds__(RP_THREADS, 4) gx_k_route_onepass(gx_route1_args a)     // 4 CTAs/SM (64 registers): profiles/r02_occupancy_variants.txt
+__global__ void __launch_bounds__(RP_THREADS, 4) gx_k_route_onepass(gx_route1_args a)     // 4 CTAs/SM (64 registers)
 {
     __shared__ unsigned int cur[GX_MAX_NODES];
     __shared__ long long tbase[GX_MAX_NODES];

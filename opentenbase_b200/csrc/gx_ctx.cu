@@ -29,8 +29,8 @@ extern "C" int gx_init(int device, gx_ctx **out)
     if (device < 0 || device >= ndev) { gx_set_global_err("gx_init: device %d out of range [0,%d)", device, ndev); return GX_ERR_ARG; }
     cudaDeviceProp prop;
     if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) { gx_set_global_err("gx_init: %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
-    if (prop.major < 10) {
-        gx_set_global_err("gx_init: device %d is sm_%d%d; libgpuexec is built for sm_100a only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {   // an sm_90a cubin loads on compute capability 9.0 and nothing else
+        gx_set_global_err("gx_init: device %d is sm_%d%d; libgpuexec is built for sm_90a only", device, prop.major, prop.minor);
         return GX_ERR_NODEVICE;
     }
     if ((e = cudaSetDevice(device)) != cudaSuccess) { gx_set_global_err("gx_init: cudaSetDevice: %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
@@ -41,11 +41,10 @@ extern "C" int gx_init(int device, gx_ctx **out)
     ctx->cc_major = prop.major; ctx->cc_minor = prop.minor;
     ctx->hbm_bytes = prop.totalGlobalMem;
     ctx->smem_optin = prop.sharedMemPerBlockOptin;
-    // L2 fetch granularity: a random 32-byte sector miss otherwise drags in 64 bytes
-    // (profiles/r01_ncu_fast_probe_and_bucket_build_sf100.csv: 2 sectors per join-table miss)
+    // L2 fetch granularity: a random 32-byte sector miss may otherwise drag in 64 bytes
     {
         const char *g = getenv("GX_L2_FETCH");
-        size_t gran = g ? (size_t) atoi(g) : 0;      // measured: 32 is no faster than the default 64 (DRAM is the limit); opt-in only
+        size_t gran = g ? (size_t) atoi(g) : 0;      // opt-in only
         if (gran == 32 || gran == 64 || gran == 128) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, gran);
         cudaGetLastError();
     }
@@ -77,8 +76,7 @@ extern "C" void gx_comm_destroy(gx_ctx *ctx);
 // Map `bytes` of HBM into the context's stream-ordered pool up front (one allocation, freed at once; 0 = everything that
 // is free minus 8 GB of headroom for NCCL and the host runtime).  Without it the pool grows on demand, and a query whose
 // temporaries do not fit the blocks already mapped waits for the driver to create and map physical memory in the middle
-// of its critical path: measured 27.8 ms instead of 1.5 ms for one hash build of the Q3 chain, 100-500 ms with two
-// ranks waiting for each other (profiles/r02_pool_reserve.txt).
+// of its critical path, and with several ranks every rank waits for the slowest.
 extern "C" int gx_pool_reserve(gx_ctx *ctx, size_t bytes)
 {
     if (!ctx) return GX_ERR_ARG;
@@ -196,7 +194,7 @@ __global__ void gx_k_l2flush(uint4 *buf, size_t n16, unsigned int v)
     for (; i < n16; i += stride) buf[i] = make_uint4(v, v + 1, v + 2, v + 3);
 }
 
-// Writes a buffer twice the size of L2 (126 MB on B200) so the next timed
+// Writes a buffer several times the size of L2 (50 MB on H100) so the next timed
 // iteration starts from cold caches.
 extern "C" int gx_l2_flush(gx_ctx *ctx)
 {

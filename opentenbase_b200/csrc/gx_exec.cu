@@ -5,15 +5,15 @@
 // inner table is queued first, so the join-table build (compute stream) runs
 // while the outer columns are still arriving.  The probe+aggregate kernel needs
 // the whole outer table and starts when its last chunk has landed: at SF100 the
-// step is 11.4 GB over PCIe against ~4 ms of kernels, so e2e is a PCIe figure
+// step is 11.4 GB over PCIe against a few ms of kernels, so e2e is a PCIe figure
 // and bench.py reports it next to a same-run copy ceiling (gx_h2d_probe).
 #include "gx_internal.cuh"
 #include <unistd.h>
 #include <sys/syscall.h>
 
 // Pinned staging memory is placed on the NUMA node the GPU hangs off.  On a two-socket host a
-// pinned buffer that happens to be allocated on the other socket is copied at a third of the
-// PCIe rate (measured through gx_exec_host on B200 hosts: 15-18 GB/s instead of 48 GB/s), and
+// pinned buffer that happens to be allocated on the other socket is copied at a fraction of the
+// PCIe rate, and
 // which socket a backend's first touch lands on is a coin toss.  The node comes from sysfs
 // (/sys/bus/pci/devices/<bus id>/numa_node); the allocation runs under a temporary
 // MPOL_BIND policy (raw syscall, no libnuma), retried unbound if the node cannot hold it.  Anything that fails leaves the default policy.

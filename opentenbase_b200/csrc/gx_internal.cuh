@@ -1,5 +1,5 @@
 // gx_internal.cuh — internal structures and device helpers of libgpuexec.so.
-// sm_100a only.  No CPU fallback anywhere: every entry point needs a live ctx.
+// sm_90a (H100) only.  No CPU fallback anywhere: every entry point needs a live ctx.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -367,7 +367,7 @@ __device__ __forceinline__ double gx_eval_expr(const gx_dexpr &e, long long r, b
 // join-table probe -------------------------------------------------------
 __device__ __forceinline__ unsigned long long gx_key_hash(long long key) { return gx_mix64((unsigned long long) key); }
 // Slot function.  A probe that misses L2 costs a whole 128-byte line of DRAM traffic
-// (profiles/r01_ncu_*: ~4 sectors per distinct key), i.e. eight 16-byte slots, so it pays
+// (four 32-byte sectors), i.e. eight 16-byte slots, so it pays
 // to keep keys that are probed together in the same line.
 //   mode 0: slot = fmix64(key) & mask                      (any keys)
 //   mode 1: slot = floor((key - kmin) * scale / 2^64)       order-preserving interpolation:
@@ -384,7 +384,7 @@ struct gx_slotfn { int mode; unsigned int win; long long kmin; unsigned long lon
 __device__ __forceinline__ unsigned long long gx_slot_index(long long key, const gx_slotfn &f)
 {
     // Home slots are aligned to amask + 1 slots (2 x 16 B or 4 x 8 B = one 32-byte sector), which a
-    // prober can fetch with a single 256-bit load; linear probing is unchanged.
+    // prober fetches as one 32-byte sector; linear probing is unchanged.
     if (f.mode == 0) return gx_mix64((unsigned long long) key) & f.mask & ~(unsigned long long) f.amask;
     if (f.mode == 2) {
         // key range below 2^32: the same interpolation in 32-bit arithmetic (one wide multiply)

@@ -86,8 +86,8 @@ __global__ void gx_k_fill_slots(gx_slot *slots, long long n)
 
 
 // ---------------------------------------------------------------------------
-// Bucketed build.  Random CAS into a table much larger than L2 tops out at
-// ~16-21 G inserts/s on B200 (profiles/r01_ubench_random_access.txt): every
+// Bucketed build.  Random CAS into a table much larger than L2 is bound by
+// DRAM latency: every
 // insert is a DRAM read-modify-write of a sector that was just cleared.  So the
 // table is cut into sub-tables of GX_SUB slots (32 KB); linear probing wraps
 // INSIDE a sub-table (all probe kernels use gx_next_slot()).  Build rows are
@@ -151,8 +151,8 @@ __global__ void __launch_bounds__(256) gx_k_bbuild_scatter(gx_bbuild_args a)
 }
 // ---------------------------------------------------------------------------
 // Two-level write-combined bucketing (replaces the one-pass scatter above for
-// big tables).  Measured: the one-pass scatter spends ~2.1 ms in per-row L2
-// atomics and ~2.1 ms in 16-byte scattered stores at SF100.  Here a CTA takes a
+// big tables), which spends its time in per-row L2 atomics and 16-byte
+// scattered stores.  Here a CTA takes a
 // tile of 4096 rows, ranks them by bucket digit in shared memory (native 32-bit
 // shared atomics), stages them bucket by bucket and copies each bucket's run out
 // as one contiguous piece: one global atomic per (tile, bucket) instead of one
@@ -540,7 +540,7 @@ __global__ void __launch_bounds__(256) gx_k_sorted_bounds_i8(const long long *__
 // PK selects the row loader: 0 generic (any key type, NULLs, build-side quals, packed payload),
 // 1 = int8 key without NULLs or quals + one 4-byte payload column, 2 = the same without payload
 template <int PK, bool C, bool VERIFY>
-__global__ void __launch_bounds__(FILL_THREADS, C ? 5 : 4) gx_k_sorted_fill(gx_bbuild_args a)      // 5 CTAs/SM: profiles/r02_occupancy_variants.txt
+__global__ void __launch_bounds__(FILL_THREADS, C ? 5 : 4) gx_k_sorted_fill(gx_bbuild_args a)      // 5 CTAs/SM
 {
     extern __shared__ __align__(16) unsigned char fill_smem_raw[];
     gx_fill_smem_t<C> &sm = *(gx_fill_smem_t<C> *) fill_smem_raw;
@@ -618,8 +618,7 @@ __global__ void __launch_bounds__(FILL_THREADS, C ? 5 : 4) gx_k_sorted_fill(gx_b
 //    start[0] = 0 and start[nsub] = nrows are fixed and the ranges [start[s], start[s+1]) tile
 //    [0, nrows), so if no CTA raises the flag every adjacent pair of rows has been compared and
 //    every row sits in the right sub-table — whatever the search returned.  A raised flag sends
-//    the host down the bucketing path.  (Doing the search inside the fill kernel, one sub-table
-//    ahead, was measured slower: 1.91 ms against 0.41 + 1.07 ms.)
+//    the host down the bucketing path.
 __device__ __forceinline__ long long sorted_lower_bound(const long long *__restrict__ keys, long long nrows, const gx_slotfn &sf,
                                                         long long s, long long nsub, double rows_per_sub, int lane, long long seed = -1)
 {
@@ -1203,11 +1202,13 @@ __global__ void __launch_bounds__(256) gx_k_hash_probe(gx_probe_args a)
 template <bool COMPACT> __global__ void gx_k_hash_probe_unique(gx_probe_args a);
 __device__ __forceinline__ void ld_pair(const gx_slot *p, long long &k0, unsigned long long &p0, long long &k1, unsigned long long &p1)
 {
-    asm volatile("ld.global.v4.u64 {%0, %1, %2, %3}, [%4];" : "=l"(k0), "=l"(p0), "=l"(k1), "=l"(p1) : "l"(p));
+    // one 32-byte sector as two 128-bit loads (sm_90 has no 256-bit load)
+    asm volatile("ld.global.v2.u64 {%0, %1}, [%4];\n\tld.global.v2.u64 {%2, %3}, [%4+16];"
+                 : "=l"(k0), "=l"(p0), "=l"(k1), "=l"(p1) : "l"(p));
 }
 template <bool COMPACT>
-// no min-blocks on purpose: any value (even 1 or 4, which leave the occupancy as it is) changes ptxas' schedule and costs
-// 20-35 % here (profiles/r02_occupancy_variants.txt)
+// no min-blocks on purpose: any value (even 1 or 4, which leave the occupancy as it is) changes ptxas' schedule
+// of the independent loads this kernel keeps in flight
 __global__ void __launch_bounds__(256) gx_k_hash_probe_unique(gx_probe_args a)
 {
     const int lane = threadIdx.x & 31;

@@ -493,7 +493,7 @@ extern "C" int gx_scan_filter(gx_ctx *ctx, const gx_table *in, int n_preds, cons
     if (in->nrows > 0) {
         for (int c = 0; c < n_out_cols; c++) { a.out[c] = t->cols[c]; a.out_nulls[c] = t->nulls[c]; }
         const char *k16 = getenv("GX_FILTER_K16");
-        const bool big = !(k16 && k16[0] == '0');                 // 4096-row tiles unless GX_FILTER_K16=0 (2.24 vs 2.39 ms for the Q3 scans at SF100)
+        const bool big = !(k16 && k16[0] == '0');                 // 4096-row tiles unless GX_FILTER_K16=0
         const long long tile_rows = (long long) FT_THREADS * (big ? 16 : 8);
         const long long ntiles = (in->nrows + tile_rows - 1) / tile_rows;
         unsigned long long *d_state = nullptr;

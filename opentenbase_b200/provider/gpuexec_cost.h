@@ -17,7 +17,7 @@
  * start-up cost, as in cost_agg's AGG_HASHED case.
  *
  * Rates are GUCs of the provider (gpuexec.cost_unit_us, gpuexec.host_page_us, gpuexec.pcie_gb_s, gpuexec.hbm_gb_s,
- * gpuexec.startup_us) with the values measured by bench.py on a B200 host as defaults.
+ * gpuexec.startup_us) with defaults taken from bench.py on an H100 host.
  */
 #ifndef GPUEXEC_COST_H
 #define GPUEXEC_COST_H
@@ -42,9 +42,9 @@ gpuexec_default_cost_params(gpuexec_cost_params *p)
 	p->seq_page_cost = 1.0;
 	p->cpu_tuple_cost = 0.01;
 	p->cost_unit_us = 10.0;			/* 8 KB at ~0.8 GB/s: a sequential read that is not entirely cached */
-	p->host_page_us = 0.6;			/* bench.py e2e_pages: one host thread feeds the ring at 13-15 GB/s */
-	p->pcie_gb_s = 50.0;			/* bench.py e2e: 54 GB/s measured, 55 GB/s ceiling */
-	p->hbm_gb_s = 4000.0;			/* the fused kernels run at 3.4-5.7 TB/s of algorithmic bytes */
+	p->host_page_us = 1.5;			/* bench.py e2e_pages on two H100 hosts: one host thread feeds the ring at 5.6-6.9 GB/s */
+	p->pcie_gb_s = 50.0;			/* bench.py e2e on two H100 hosts: 48.9-54.0 GB/s, same-run copy ceiling 50.5-55.3 GB/s */
+	p->hbm_gb_s = 3000.0;			/* what the fused kernels sustain over the staged columns (H100: 3.35 TB/s HBM3) */
 	p->startup_us = 1500.0;			/* context already created; plan compile + ~20 launches + result fetch */
 }
 

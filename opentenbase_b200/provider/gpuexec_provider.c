@@ -2,7 +2,7 @@
  * gpuexec_provider.c — OpenTenBase CustomScan provider for libgpuexec.so.
  *
  * The host side of the drop-in boundary (SURVEY.md §8b), in the reference's own
- * language (C) against the reference's own headers.  It plugs the B200 path in
+ * language (C) against the reference's own headers.  It plugs the H100 path in
  * where the planner would otherwise put
  *
  *      HashAggregate <- [Hash Join <- Seq Scan, Hash <- Seq Scan]
@@ -86,12 +86,12 @@ void		_PG_init(void);
 static bool gpuexec_enabled = true;
 static int	gpuexec_device = 0;
 static int	gpuexec_pool_reserve_mb = 0;	/* HBM mapped into the library's pool when the backend's context is created */
-static int	gpuexec_hbm_limit_mb = 150 * 1024;	/* decline plans whose staged columns + join table would not fit */
-/* the cost model's rates (gpuexec_cost.h); defaults = what bench.py measured on a B200 host */
+static int	gpuexec_hbm_limit_mb = 64 * 1024;	/* decline plans whose staged columns + join table would not fit (80 GB H100) */
+/* the cost model's rates (gpuexec_cost.h) */
 static double gpuexec_cost_unit_us = 10.0;
-static double gpuexec_host_page_us = 0.6;
+static double gpuexec_host_page_us = 1.5;
 static double gpuexec_pcie_gb_s = 50.0;
-static double gpuexec_hbm_gb_s = 4000.0;
+static double gpuexec_hbm_gb_s = 3000.0;
 static double gpuexec_startup_us = 1500.0;
 static create_upper_paths_hook_type prev_upper_paths_hook = NULL;
 
@@ -1468,15 +1468,15 @@ _PG_init(void)
 	DefineCustomIntVariable("gpuexec.pool_reserve_mb", "HBM (MB) mapped into the GPU memory pool when a backend first uses the GPU (0 = grow on demand).", NULL,
 							&gpuexec_pool_reserve_mb, 0, 0, 1024 * 1024, PGC_BACKEND, 0, NULL, NULL, NULL);
 	DefineCustomIntVariable("gpuexec.hbm_limit_mb", "Decline plans whose staged columns and join table are estimated above this many MB of HBM.", NULL,
-							&gpuexec_hbm_limit_mb, 150 * 1024, 64, 1024 * 1024, PGC_USERSET, 0, NULL, NULL, NULL);
+							&gpuexec_hbm_limit_mb, 64 * 1024, 64, 1024 * 1024, PGC_USERSET, 0, NULL, NULL, NULL);
 	DefineCustomRealVariable("gpuexec.cost_unit_us", "Microseconds one unit of planner cost (a sequential page fetch) stands for.", NULL,
 							 &gpuexec_cost_unit_us, 10.0, 0.01, 1e6, PGC_USERSET, 0, NULL, NULL, NULL);
 	DefineCustomRealVariable("gpuexec.host_page_us", "Host microseconds per heap page on the loader's path (visibility pass + copy into the pinned ring).", NULL,
-							 &gpuexec_host_page_us, 0.6, 0.0, 1e6, PGC_USERSET, 0, NULL, NULL, NULL);
+							 &gpuexec_host_page_us, 1.5, 0.0, 1e6, PGC_USERSET, 0, NULL, NULL, NULL);
 	DefineCustomRealVariable("gpuexec.pcie_gb_s", "Host-to-device copy rate of pinned memory in GB/s.", NULL,
 							 &gpuexec_pcie_gb_s, 50.0, 0.1, 1e4, PGC_USERSET, 0, NULL, NULL, NULL);
 	DefineCustomRealVariable("gpuexec.hbm_gb_s", "What the kernels sustain over the staged columns in GB/s.", NULL,
-							 &gpuexec_hbm_gb_s, 4000.0, 1.0, 1e5, PGC_USERSET, 0, NULL, NULL, NULL);
+							 &gpuexec_hbm_gb_s, 3000.0, 1.0, 1e5, PGC_USERSET, 0, NULL, NULL, NULL);
 	DefineCustomRealVariable("gpuexec.startup_us", "Fixed price of one GPU sub-plan in microseconds (plan compile, launches, result fetch).", NULL,
 							 &gpuexec_startup_us, 1500.0, 0.0, 1e9, PGC_USERSET, 0, NULL, NULL, NULL);
 	RegisterCustomScanMethods(&gpuexec_scan_methods);

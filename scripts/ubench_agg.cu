@@ -1,7 +1,7 @@
 // ubench_agg.cu — development microbenchmark (not part of the product):
-// which update mechanism should the shared-memory hash aggregate use on B200?
+// which update mechanism should the shared-memory hash aggregate use on H100?
 // Input: gid[int32] + val[double] (12 B/row like config 2), N rows, G groups.
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o ubench_agg ubench_agg.cu
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o ubench_agg ubench_agg.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cstdint>
@@ -148,7 +148,8 @@ template <class F> static float time_it(F f, int reps = 5)
 int main(int argc, char **argv)
 {
     long long n = argc > 1 ? atoll(argv[1]) : 60000000LL;
-    int sms = 148;
+    int sms = 0;
+    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
     int *gid; double *val, *sum; unsigned long long *cnt;
     CK(cudaMalloc(&gid, n * 4)); CK(cudaMalloc(&val, n * 8));
     CK(cudaMalloc(&sum, 64 * 65536 * 8)); CK(cudaMalloc(&cnt, 64 * 65536 * 8));

@@ -46,20 +46,22 @@ template <class F> static float time_it(F f, int reps = 3)
 int main()
 {
     const long long n = 200000000LL;
+    int sms = 0;
+    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
     unsigned long long *sink; CK(cudaMalloc(&sink, 8));
     for (long long mb : { 64LL, 256LL, 1024LL, 4096LL, 16384LL }) {
         size_t bytes = (size_t) mb << 20; uint64_t slots = bytes / 16;
         ulonglong2 *tab; CK(cudaMalloc(&tab, bytes)); CK(cudaMemset(tab, 0, bytes));
         auto rep = [&](const char *nm, float ms) { printf("table %6lld MB  %-28s %8.3f ms  %7.2f G acc/s  %7.1f GB/s @32B\n", mb, nm, ms, n / ms / 1e6, n * 32.0 / ms / 1e6); fflush(stdout); };
-        rep("gather U=1 run=1 2048thr/SM", time_it([&] { k_gather<1><<<148 * 8, 256>>>(tab, slots - 1, n, sink, 1); }));
-        rep("gather U=4 run=1", time_it([&] { k_gather<4><<<148 * 8, 256>>>(tab, slots - 1, n, sink, 1); }));
-        rep("gather U=8 run=1", time_it([&] { k_gather<8><<<148 * 8, 256>>>(tab, slots - 1, n, sink, 1); }));
-        rep("gather U=4 run=4", time_it([&] { k_gather<4><<<148 * 8, 256>>>(tab, slots - 1, n, sink, 4); }));
-        rep("store 16B", time_it([&] { k_store<<<148 * 8, 256>>>(tab, slots - 1, n); }));
+        rep("gather U=1 run=1 2048thr/SM", time_it([&] { k_gather<1><<<sms * 8, 256>>>(tab, slots - 1, n, sink, 1); }));
+        rep("gather U=4 run=1", time_it([&] { k_gather<4><<<sms * 8, 256>>>(tab, slots - 1, n, sink, 1); }));
+        rep("gather U=8 run=1", time_it([&] { k_gather<8><<<sms * 8, 256>>>(tab, slots - 1, n, sink, 1); }));
+        rep("gather U=4 run=4", time_it([&] { k_gather<4><<<sms * 8, 256>>>(tab, slots - 1, n, sink, 4); }));
+        rep("store 16B", time_it([&] { k_store<<<sms * 8, 256>>>(tab, slots - 1, n); }));
         CK(cudaMemset(tab, 0, bytes));
-        rep("cas only", time_it([&] { k_cas<<<148 * 8, 256>>>((unsigned long long *) tab, slots - 1, n, 0); }, 1));
+        rep("cas only", time_it([&] { k_cas<<<sms * 8, 256>>>((unsigned long long *) tab, slots - 1, n, 0); }, 1));
         CK(cudaMemset(tab, 0, bytes));
-        rep("cas + payload store", time_it([&] { k_cas<<<148 * 8, 256>>>((unsigned long long *) tab, slots - 1, n, 1); }, 1));
+        rep("cas + payload store", time_it([&] { k_cas<<<sms * 8, 256>>>((unsigned long long *) tab, slots - 1, n, 1); }, 1));
         cudaFree(tab);
     }
     return 0;

@@ -203,8 +203,8 @@ def test_costs_follow_the_cost_model():
     r = plan(LINEITEM, "scan 1", "group 1.6", "target var 1.6", "target agg sum_f8 v1.3", "dist none", "groups 2526")
     pages, tuples = 110000.0, 6000000.0
     staged = tuples * (4 + 8) * 1.25
-    feed = max(0.6 * pages, pages * 8192 / 50e3)
-    want = pages + (feed + 3 * staged / 4000e3 + 1500.0) / 10.0
+    feed = max(1.5 * pages, pages * 8192 / 50e3)
+    want = pages + (feed + 3 * staged / 3000e3 + 1500.0) / 10.0
     assert r["startup"] == pytest.approx(want, rel=1e-6)
     assert r["total"] == pytest.approx(want + 0.01 * 2526, rel=1e-6) and r["rows"] == 2526
 
