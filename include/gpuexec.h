@@ -42,8 +42,9 @@ enum {
     GX_ERR_NOMEM     = 3,   /* HBM or pinned host memory exhausted          */
     GX_ERR_NCCL      = 4,   /* NCCL failure / libnccl missing               */
     GX_ERR_STATE     = 5,   /* call sequence error                          */
-    GX_ERR_OVERFLOW  = 6,   /* float8 overflow: reference raises ERROR
-                               (CHECKFLOATVAL, utils/adt/float.c:970-981)   */
+    GX_ERR_OVERFLOW  = 6,   /* float8 overflow from finite inputs: reference
+                               raises ERROR (CHECKFLOATVAL, float.c:970-981);
+                               an infinite input may give an infinite result */
     GX_ERR_NODEVICE  = 7    /* no usable GPU: the path is unavailable       */
 };
 
@@ -69,8 +70,8 @@ enum {
     GX_AGG_SUM_I4     = 5, /* int4_sum -> int8   (utils/adt/numeric.c:6154)  */
     GX_AGG_MIN_F8     = 6, /* float8smaller                                  */
     GX_AGG_MAX_F8     = 7, /* float8larger                                   */
-    GX_AGG_SUM_I8     = 8  /* sum(int8) kept as int8 (overflow -> error);
-                              the reference returns numeric: see DESIGN.md   */
+    GX_AGG_SUM_I8     = 8  /* sum(int8): declined with GX_ERR_ARG, the reference
+                              returns numeric (see DESIGN.md §3.2)            */
 };
 
 /* expression opcodes: tiny postfix VM over float8 (the provider pattern-matches

@@ -23,10 +23,16 @@
 //   3  global table only (atomics in L2)
 #include "gx_internal.cuh"
 #include <type_traits>
+#include <cmath>
+#include <unordered_map>
+#include <vector>
 
 int gx_fill_dpreds(gx_ctx *ctx, const gx_table *t, int n_preds, const gx_pred *preds, gx_dpred *out);
 
 enum { WK_ADD_I64 = 0, WK_ADD_F64 = 1, WK_MIN_F64 = 2, WK_MAX_F64 = 3 };
+// initial value of every float8 sum (state words and register accumulators): -0.0 is the exact additive identity,
+// so a group whose inputs are all -0.0 sums to -0.0 as float8pl does when the first input becomes the state
+#define GX_NEG_ZERO_BITS 0x8000000000000000ULL
 
 struct gx_agg_dev {
     gx_dplan P;
@@ -220,10 +226,9 @@ __device__ __forceinline__ void pack_group_key(const gx_dplan &P, long long r, u
         if (g.side == 0) {
             if (gx_is_null(g.col, r)) { nullmask |= 1u << c; continue; }
             v = (unsigned long long) gx_load_int(g.col, r);
-            if (g.type == GX_FLOAT8) {                       // -0 = +0, all NaNs equal (float8eq)
-                double d = __longlong_as_double((long long) v);
-                if (d == 0.0) v = 0; else if (isnan(d)) v = 0x7FF8000000000000ULL;
-            }
+            // -0 = +0 (float8eq).  NaNs keep their bits: hashfloat8 hashes a NaN by its bit pattern, so the
+            // reference's hash aggregate keeps NaN and a NaN of another payload or sign in separate groups.
+            if (g.type == GX_FLOAT8 && __longlong_as_double((long long) v) == 0.0) v = 0;
         } else {
             v = payload >> g.payload_idx;                     // payload_idx holds the bit offset
         }
@@ -656,12 +661,12 @@ __global__ void __launch_bounds__(FG_THREADS, 1) gx_k_fewgroups(const __grid_con
     __shared__ int s_over;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nv = F.nv, nw = 1 + nv;
     if (threadIdx.x < FG_G) { s_state[threadIdx.x] = 0u; s_keys[threadIdx.x] = 0ULL; }
-    if (threadIdx.x < FG_G * (1 + FG_NV)) ((unsigned long long *) s_acc)[threadIdx.x] = 0ULL;
+    if (threadIdx.x < FG_G * (1 + FG_NV)) ((unsigned long long *) s_acc)[threadIdx.x] = threadIdx.x % (1 + FG_NV) ? GX_NEG_ZERO_BITS : 0ULL;
     if (threadIdx.x == 0) s_over = 0;
     // group slot FG_G is a trash can: rows that fail the quals are added there, so the tile body has no per-row branches
     constexpr int GS = FG_G + 1;
     unsigned long long *const acc = fg_smem + (size_t) warp * nw * GS * 32 + lane;     // + (word * GS + group) * 32
-    for (int i = 0; i < nw * GS; i++) acc[i * 32] = 0ULL;
+    for (int i = 0; i < nw * GS; i++) acc[i * 32] = i < GS ? 0ULL : GX_NEG_ZERO_BITS;     // row counts 0, sums -0
     __syncthreads();
     const gx_dplan &P = A.P;
     // keys the CTA has handed out so far; an unused entry holds a value no packed key can take (BYTEKEY keys are
@@ -980,7 +985,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_fast(const __grid_constant__ gx_
     for (long long q = (long long) blockIdx.x * blockDim.x + threadIdx.x; q < nvec; q += stride) {
         const long long r = A.row0 + (q << 2);
         int g[4]; bool hit[4]; double v[4];
-        unsigned int rcnt = 0; double rsum = 0.0;                     // partial handed over by the lane above
+        unsigned int rcnt = 0; double rsum = -0.0;                     // partial handed over by the lane above
         if (HAS_SUM) { double2 a = ld_stream_d2(F.vcol + r), b = ld_stream_d2(F.vcol + r + 2); v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y; }
         if (JOIN) {
             longlong2 ka = ld_stream_ll2(F.okey + r), kb = ld_stream_ll2(F.okey + r + 2);
@@ -1040,7 +1045,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_fast(const __grid_constant__ gx_
                 }
             }
             // partial of a handed-over leading run
-            unsigned int gcnt = 0; double gsum = 0.0;
+            unsigned int gcnt = 0; double gsum = -0.0;
             if (give) {
 #pragma unroll
                 bool in = true;
@@ -1049,20 +1054,20 @@ __global__ void __launch_bounds__(1024, 1) gx_k_fast(const __grid_constant__ gx_
             }
             rcnt = __shfl_down_sync(wmask, gcnt, 1);
             if (HAS_SUM) rsum = __shfl_down_sync(wmask, gsum, 1);
-            if (lane == 31 || !((wmask >> (lane + 1)) & 1u)) { rcnt = 0; rsum = 0.0; }
+            if (lane == 31 || !((wmask >> (lane + 1)) & 1u)) { rcnt = 0; rsum = -0.0; }
         } else {
             int4 gg = ld_stream_i4(F.gcol + r);
             g[0] = gg.x; g[1] = gg.y; g[2] = gg.z; g[3] = gg.w;
             hit[0] = hit[1] = hit[2] = hit[3] = true;
         }
         // combine equal neighbours in registers, then one shared-memory update per run
-        int cur = 0; unsigned int cnt = 0; double sum = 0.0; bool open = false;
+        int cur = 0; unsigned int cnt = 0; double sum = -0.0; bool open = false;
 #pragma unroll
         for (int i = 0; i < 4; i++) {
             if (!hit[i]) continue;
             if (open && g[i] == cur) { cnt++; if (HAS_SUM) sum = __dadd_rn(sum, v[i]); continue; }
             if (open) fast_flush<HAS_CNT, HAS_SUM>(T, A, cur, cnt, sum, F.sum_word);
-            open = true; cur = g[i]; cnt = 1; sum = HAS_SUM ? v[i] : 0.0;
+            open = true; cur = g[i]; cnt = 1; sum = HAS_SUM ? v[i] : -0.0;
         }
         if (open) { cnt += rcnt; if (HAS_SUM) sum = __dadd_rn(sum, rsum); fast_flush<HAS_CNT, HAS_SUM>(T, A, cur, cnt, sum, F.sum_word); }
     }
@@ -1080,7 +1085,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_fast(const __grid_constant__ gx_
                     h = c.key == key; gk = (int) (unsigned int) c.payload;
                 }
             } else gk = F.gcol[r];
-            if (h) fast_flush<HAS_CNT, HAS_SUM>(T, A, gk, 1u, HAS_SUM ? F.vcol[r] : 0.0, F.sum_word);
+            if (h) fast_flush<HAS_CNT, HAS_SUM>(T, A, gk, 1u, HAS_SUM ? F.vcol[r] : -0.0, F.sum_word);
         }
     }
     __syncthreads();
@@ -1181,14 +1186,14 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin(const __grid_constant__ 
         const int base = inc - nh, R = __shfl_sync(0xffffffffu, inc, 31);
         // ---- fold: runs that start in this lane are stored, the rows that continue the previous
         // lane's run are added to that run afterwards
-        unsigned int c0 = 0; double s0 = 0.0;
+        unsigned int c0 = 0; double s0 = -0.0;
         if (act) {
-            int rid = base - 1; unsigned int c = 0; double sacc = 0.0;
+            int rid = base - 1; unsigned int c = 0; double sacc = -0.0;
 #pragma unroll
             for (int i = 0; i < 4; i++) {
                 if (hd[i]) {
                     if (rid >= base) { Q.cnt[rid] = c; if (HAS_SUM) Q.sum[rid] = sacc; } else { c0 = c; s0 = sacc; }
-                    rid++; Q.key[rid] = k[i]; c = 0; sacc = 0.0;
+                    rid++; Q.key[rid] = k[i]; c = 0; sacc = -0.0;
                 }
                 c++; if (HAS_SUM) sacc = __dadd_rn(sacc, v[i]);
             }
@@ -1209,7 +1214,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin(const __grid_constant__ 
         for (int j = lane; j < R; j += 32) {
             const long long key = Q.key[j];
             const unsigned int rc = Q.cnt[j];
-            const double rs = HAS_SUM ? Q.sum[j] : 0.0;
+            const double rs = HAS_SUM ? Q.sum[j] : -0.0;
             int g = 0;
             const bool hit = runjoin_probe<COMPACT>(A, key, g);
             if (hit) fast_flush<HAS_CNT, HAS_SUM>(T, A, g, rc, rs, F.sum_word);
@@ -1221,7 +1226,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin(const __grid_constant__ 
         long long r = A.row0 + (nvec << 2) + (long long) blockIdx.x * blockDim.x + threadIdx.x;
         if (r < A.row1) {
             int gk = 0;
-            if (runjoin_probe<COMPACT>(A, F.okey[r], gk)) fast_flush<HAS_CNT, HAS_SUM>(T, A, gk, 1u, HAS_SUM ? F.vcol[r] : 0.0, F.sum_word);
+            if (runjoin_probe<COMPACT>(A, F.okey[r], gk)) fast_flush<HAS_CNT, HAS_SUM>(T, A, gk, 1u, HAS_SUM ? F.vcol[r] : -0.0, F.sum_word);
         }
     }
     __syncthreads();
@@ -1403,14 +1408,14 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin_seg(const __grid_constan
 #pragma unroll
             for (int o = 1; o < 32; o <<= 1) { int t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
             const int base = inc - nh, R = __shfl_sync(0xffffffffu, inc, 31);
-            unsigned int c0 = 0; double s0 = 0.0;
+            unsigned int c0 = 0; double s0 = -0.0;
             if (act) {
-                int rid = base - 1; unsigned int c = 0; double sacc = 0.0;
+                int rid = base - 1; unsigned int c = 0; double sacc = -0.0;
 #pragma unroll
                 for (int i = 0; i < 4; i++) {
                     if (hd[i]) {
                         if (rid >= base) { Q.cnt[rid] = c; if (HAS_SUM) Q.sum[rid] = sacc; } else { c0 = c; s0 = sacc; }
-                        rid++; Q.key[rid] = k[i]; c = 0; sacc = 0.0;
+                        rid++; Q.key[rid] = k[i]; c = 0; sacc = -0.0;
                     }
                     c++; if (HAS_SUM) sacc = __dadd_rn(sacc, v[i]);
                 }
@@ -1436,7 +1441,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin_seg(const __grid_constan
             for (int jj = lane; jj < R; jj += 32) {
                 const long long key = Q.key[jj];
                 const unsigned int rc = Q.cnt[jj];
-                const double rs = HAS_SUM ? Q.sum[jj] : 0.0;
+                const double rs = HAS_SUM ? Q.sum[jj] : -0.0;
                 int g = 0;
                 const bool hit = runjoin_probe_seg(A, key, g, sg, lo, len);
                 if (hit) fast_flush<HAS_CNT, HAS_SUM>(T, A, g, rc, rs, F.sum_word);
@@ -1450,7 +1455,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin_seg(const __grid_constan
             long long r = A.row0 + (nvec << 2) + (long long) blockIdx.x * blockDim.x + threadIdx.x;
             if (r < A.row1) {
                 int gk = 0;
-                if (runjoin_probe<true>(A, F.okey[r], gk)) fast_flush<HAS_CNT, HAS_SUM>(T, A, gk, 1u, HAS_SUM ? F.vcol[r] : 0.0, F.sum_word);
+                if (runjoin_probe<true>(A, F.okey[r], gk)) fast_flush<HAS_CNT, HAS_SUM>(T, A, gk, 1u, HAS_SUM ? F.vcol[r] : -0.0, F.sum_word);
             }
         }
     }
@@ -1498,14 +1503,14 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin3(const __grid_constant__
         const int base = nl + inc - nh, R = __shfl_sync(0xffffffffu, inc, 31);      // this tile's runs go behind the waiting ones
         // ---- fold: runs that start in this lane are stored, the rows that continue the previous
         // lane's run are added to that run afterwards
-        unsigned int c0 = 0; double s0 = 0.0;
+        unsigned int c0 = 0; double s0 = -0.0;
         if (act) {
-            int rid = base - 1; unsigned int c = 0; double sacc = 0.0;
+            int rid = base - 1; unsigned int c = 0; double sacc = -0.0;
 #pragma unroll
             for (int i = 0; i < 4; i++) {
                 if (hd[i]) {
                     if (rid >= base) { Q.cnt[rid] = c; if (HAS_SUM) Q.sum[rid] = sacc; } else { c0 = c; s0 = sacc; }
-                    rid++; Q.key[rid] = k[i]; c = 0; sacc = 0.0;
+                    rid++; Q.key[rid] = k[i]; c = 0; sacc = -0.0;
                 }
                 c++; if (HAS_SUM) sacc = __dadd_rn(sacc, v[i]);
             }
@@ -1528,7 +1533,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin3(const __grid_constant__
         for (int j = lane; j < full; j += 32) {
             const long long key = Q.key[j];
             const unsigned int rc = Q.cnt[j];
-            const double rs = HAS_SUM ? Q.sum[j] : 0.0;
+            const double rs = HAS_SUM ? Q.sum[j] : -0.0;
             int g = 0;
             const bool hit = runjoin_probe<COMPACT>(A, key, g);
             if (hit) fast_flush<HAS_CNT, HAS_SUM>(T, A, g, rc, rs, F.sum_word);
@@ -1536,7 +1541,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin3(const __grid_constant__
         __syncwarp();
         nl = total - full;
         if (full > 0 && lane < nl) {                                // the remainder moves to the front (sources lie at index >= 32)
-            const long long kk = Q.key[full + lane]; const unsigned int cq = Q.cnt[full + lane]; const double sq = HAS_SUM ? Q.sum[full + lane] : 0.0;
+            const long long kk = Q.key[full + lane]; const unsigned int cq = Q.cnt[full + lane]; const double sq = HAS_SUM ? Q.sum[full + lane] : -0.0;
             Q.key[lane] = kk; Q.cnt[lane] = cq; if (HAS_SUM) Q.sum[lane] = sq;
         }
         __syncwarp();
@@ -1544,7 +1549,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin3(const __grid_constant__
     for (int j = lane; j < nl; j += 32) {                           // what was still waiting when the rows ran out
         int g = 0;
         const bool hit = runjoin_probe<COMPACT>(A, Q.key[j], g);
-        if (hit) fast_flush<HAS_CNT, HAS_SUM>(T, A, g, Q.cnt[j], HAS_SUM ? Q.sum[j] : 0.0, F.sum_word);
+        if (hit) fast_flush<HAS_CNT, HAS_SUM>(T, A, g, Q.cnt[j], HAS_SUM ? Q.sum[j] : -0.0, F.sum_word);
     }
     __syncwarp();
     // the (< 4) rows after the last full vector: one thread each
@@ -1552,7 +1557,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin3(const __grid_constant__
         long long r = A.row0 + (nvec << 2) + (long long) blockIdx.x * blockDim.x + threadIdx.x;
         if (r < A.row1) {
             int gk = 0;
-            if (runjoin_probe<COMPACT>(A, F.okey[r], gk)) fast_flush<HAS_CNT, HAS_SUM>(T, A, gk, 1u, HAS_SUM ? F.vcol[r] : 0.0, F.sum_word);
+            if (runjoin_probe<COMPACT>(A, F.okey[r], gk)) fast_flush<HAS_CNT, HAS_SUM>(T, A, gk, 1u, HAS_SUM ? F.vcol[r] : -0.0, F.sum_word);
         }
     }
     __syncthreads();
@@ -1589,7 +1594,7 @@ __global__ void __launch_bounds__(512, 2) gx_k_runjoin2(const __grid_constant__ 
     unsigned long long *const tab = smem; double *const tsum = (double *) (smem + S);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     gx_runlist &Q = ((gx_runlist *) (smem + (size_t) S * 2))[warp];
-    for (int i = threadIdx.x; i < S; i += blockDim.x) { tab[i] = 0ULL; tsum[i] = 0.0; }
+    for (int i = threadIdx.x; i < S; i += blockDim.x) { tab[i] = 0ULL; tsum[i] = -0.0; }
     __syncthreads();
     const long long nvec = (A.row1 - A.row0) >> 2;              // groups of four rows
     const long long stride = (long long) gridDim.x * blockDim.x;
@@ -1615,14 +1620,14 @@ __global__ void __launch_bounds__(512, 2) gx_k_runjoin2(const __grid_constant__ 
         const int base = inc - nh, R = __shfl_sync(0xffffffffu, inc, 31);
         // ---- fold: runs that start in this lane are stored, the rows that continue the previous
         // lane's run are added to that run afterwards
-        unsigned int c0 = 0; double s0 = 0.0;
+        unsigned int c0 = 0; double s0 = -0.0;
         if (act) {
-            int rid = base - 1; unsigned int c = 0; double sacc = 0.0;
+            int rid = base - 1; unsigned int c = 0; double sacc = -0.0;
 #pragma unroll
             for (int i = 0; i < 4; i++) {
                 if (hd[i]) {
                     if (rid >= base) { Q.cnt[rid] = c; if (HAS_SUM) Q.sum[rid] = sacc; } else { c0 = c; s0 = sacc; }
-                    rid++; Q.key[rid] = k[i]; c = 0; sacc = 0.0;
+                    rid++; Q.key[rid] = k[i]; c = 0; sacc = -0.0;
                 }
                 c++; if (HAS_SUM) sacc = __dadd_rn(sacc, v[i]);
             }
@@ -1643,7 +1648,7 @@ __global__ void __launch_bounds__(512, 2) gx_k_runjoin2(const __grid_constant__ 
         for (int j = lane; j < R; j += 32) {
             const long long key = Q.key[j];
             const unsigned int rc = Q.cnt[j];
-            const double rs = HAS_SUM ? Q.sum[j] : 0.0;
+            const double rs = HAS_SUM ? Q.sum[j] : -0.0;
             int g = 0;
             const bool hit = runjoin_probe<COMPACT>(A, key, g);
             if (hit) packed_flush<HAS_SUM>(tab, tsum, S, A, g, rc, rs);
@@ -1655,7 +1660,7 @@ __global__ void __launch_bounds__(512, 2) gx_k_runjoin2(const __grid_constant__ 
         long long r = A.row0 + (nvec << 2) + (long long) blockIdx.x * blockDim.x + threadIdx.x;
         if (r < A.row1) {
             int gk = 0;
-            if (runjoin_probe<COMPACT>(A, F.okey[r], gk)) packed_flush<HAS_SUM>(tab, tsum, S, A, gk, 1u, HAS_SUM ? F.vcol[r] : 0.0);
+            if (runjoin_probe<COMPACT>(A, F.okey[r], gk)) packed_flush<HAS_SUM>(tab, tsum, S, A, gk, 1u, HAS_SUM ? F.vcol[r] : -0.0);
         }
     }
     __syncthreads();
@@ -1693,7 +1698,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin_tma(const __grid_constan
     gx_runlist &Q = ((gx_runlist *) (smem_tma + (size_t) S * 2))[warp];
     gx_rowstage &R = ((gx_rowstage *) (smem_tma + (size_t) S * 2 + 32 * (sizeof(gx_runlist) / 8)))[warp];
     unsigned long long *const bar = smem_tma + (size_t) S * 2 + 32 * (sizeof(gx_runlist) / 8) + 32 * (sizeof(gx_rowstage) / 8) + warp;
-    for (int i = threadIdx.x; i < S; i += blockDim.x) { tab[i] = 0ULL; tsum[i] = 0.0; }
+    for (int i = threadIdx.x; i < S; i += blockDim.x) { tab[i] = 0ULL; tsum[i] = -0.0; }
     if (lane == 0) {
         gx_mbar_init(bar, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -1731,7 +1736,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin_tma(const __grid_constan
     auto probe_one = [&](int j) {
         const long long key = Q.key[j];
         const unsigned int rc = Q.cnt[j];
-        const double rs = HAS_SUM ? Q.sum[j] : 0.0;
+        const double rs = HAS_SUM ? Q.sum[j] : -0.0;
         int g = 0;
         const bool hit = runjoin_probe<COMPACT>(A, key, g);
         if (hit) packed_flush<HAS_SUM>(tab, tsum, S, A, g, rc, rs);
@@ -1783,7 +1788,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin_tma(const __grid_constan
             const int base = inc - nh + (CARRY ? nc : 0);
             const int r0 = base + (int) h0 - 1, r1 = r0 + (int) h1, r2 = r1 + (int) h2, r3 = r2 + (int) h3;   // run of row i; base - 1 = the previous lane's last run
             const unsigned int c1 = h1 ? 1u : 2u, c2 = h2 ? 1u : c1 + 1u, c3 = h3 ? 1u : c2 + 1u;                // rows of row i's run up to row i, inside this lane
-            double s0 = 0.0, s1 = 0.0, s2 = 0.0, s3 = 0.0;
+            double s0 = -0.0, s1 = -0.0, s2 = -0.0, s3 = -0.0;
             if (HAS_SUM) { s0 = v[0]; s1 = h1 ? v[1] : __dadd_rn(s0, v[1]); s2 = h2 ? v[2] : __dadd_rn(s1, v[2]); s3 = h3 ? v[3] : __dadd_rn(s2, v[3]); }
             const bool q0 = h0, q1 = q0 || h1, q2 = q1 || h2, q3 = q2 || h3;                                     // row i's run started in this lane
             if (h0) Q.key[r0] = k[0];
@@ -1796,7 +1801,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin_tma(const __grid_constan
             if (h3 && q2) { Q.cnt[r2] = c2; if (HAS_SUM) Q.sum[r2] = s2; }
             if (q3) { Q.cnt[r3] = c3; if (HAS_SUM) Q.sum[r3] = s3; }
             // the rows before this lane's first head continue the previous lane's run: added once that run's own lane has stored it
-            unsigned int cc = 0; double sc = 0.0;
+            unsigned int cc = 0; double sc = -0.0;
             if (act && !h0) {
                 cc = h1 ? 1u : h2 ? c1 : h3 ? c2 : c3;
                 if (HAS_SUM) sc = h1 ? s0 : h2 ? s1 : h3 ? s2 : s3;
@@ -1817,14 +1822,14 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin_tma(const __grid_constan
             NR = __shfl_sync(0xffffffffu, inc, 31);
             // ---- fold: runs that start in this lane are stored, the rows that continue the previous
             // lane's run are added to that run afterwards
-            unsigned int c0 = 0; double s0 = 0.0;
+            unsigned int c0 = 0; double s0 = -0.0;
             if (act) {
-                int rid = base - 1; unsigned int c = 0; double sacc = 0.0;
+                int rid = base - 1; unsigned int c = 0; double sacc = -0.0;
 #pragma unroll
                 for (int i = 0; i < 4; i++) {
                     if (hd[i]) {
                         if (rid >= base) { Q.cnt[rid] = c; if (HAS_SUM) Q.sum[rid] = sacc; } else { c0 = c; s0 = sacc; }
-                        rid++; Q.key[rid] = k[i]; c = 0; sacc = 0.0;
+                        rid++; Q.key[rid] = k[i]; c = 0; sacc = -0.0;
                     }
                     c++; if (HAS_SUM) sacc = __dadd_rn(sacc, v[i]);
                 }
@@ -1851,7 +1856,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin_tma(const __grid_constan
         long long r = A.row0 + (nvec << 2) + (long long) blockIdx.x * blockDim.x + threadIdx.x;
         if (r < A.row1) {
             int gk = 0;
-            if (runjoin_probe<COMPACT>(A, F.okey[r], gk)) packed_flush<HAS_SUM>(tab, tsum, S, A, gk, 1u, HAS_SUM ? F.vcol[r] : 0.0);
+            if (runjoin_probe<COMPACT>(A, F.okey[r], gk)) packed_flush<HAS_SUM>(tab, tsum, S, A, gk, 1u, HAS_SUM ? F.vcol[r] : -0.0);
         }
     }
     __syncthreads();
@@ -2015,7 +2020,7 @@ __global__ void __launch_bounds__(DENSE ? 512 : (NV <= 2 ? 384 : 512), (DENSE ||
     if (lane == 0) {
         Qkey[0] = carry_key; Qcnt[0] = RA_BND;
 #pragma unroll
-        for (int q = 0; q < NV; q++) if (q < nv) Qsum[(size_t) q * RA_LIST] = 0.0;
+        for (int q = 0; q < NV; q++) if (q < nv) Qsum[(size_t) q * RA_LIST] = -0.0;
     }
     __syncwarp();
 
@@ -2034,7 +2039,7 @@ __global__ void __launch_bounds__(DENSE ? 512 : (NV <= 2 ? 384 : 512), (DENSE ||
 #pragma unroll
             for (int c = 0; c < NC; c++) {
                 if (c < R.nc) { const double2 a = ld_stream_d2(R.col[c] + r0), b = ld_stream_d2(R.col[c] + r0 + 2); x[c][0] = a.x; x[c][1] = a.y; x[c][2] = b.x; x[c][3] = b.y; }
-                else { x[c][0] = x[c][1] = x[c][2] = x[c][3] = 0.0; }
+                else { x[c][0] = x[c][1] = x[c][2] = x[c][3] = -0.0; }
             }
             ok[0] = ok[1] = ok[2] = ok[3] = true;
             for (int p = 0; p < P.npreds; p++) pred_vec4(P.preds[p], r0, ok);
@@ -2045,7 +2050,7 @@ __global__ void __launch_bounds__(DENSE ? 512 : (NV <= 2 ? 384 : 512), (DENSE ||
                 const long long r = r0 + i < c1 ? r0 + i : last;
                 k[i] = __ldg(okey + r); ok[i] = r0 + i < c1;
 #pragma unroll
-                for (int c = 0; c < NC; c++) x[c][i] = c < R.nc ? __ldg(R.col[c] + r) : 0.0;
+                for (int c = 0; c < NC; c++) x[c][i] = c < R.nc ? __ldg(R.col[c] + r) : -0.0;
                 for (int p = 0; p < P.npreds; p++) if (ok[i]) ok[i] = gx_eval_pred(P.preds[p], r);
             }
         }
@@ -2055,7 +2060,7 @@ __global__ void __launch_bounds__(DENSE ? 512 : (NV <= 2 ? 384 : 512), (DENSE ||
 #pragma unroll
         for (int q = 0; q < NV; q++) {
 #pragma unroll
-            for (int i = 0; i < 4; i++) v[q][i] = 0.0;
+            for (int i = 0; i < 4; i++) v[q][i] = -0.0;
             if (q < nv) {
                 const gx_dexpr &e = P.aggs[R.vagg[q]].expr;
                 slot_term<4, NC>(e.t[0], R.tslot[q][0], x, v[q]);
@@ -2083,11 +2088,11 @@ __global__ void __launch_bounds__(DENSE ? 512 : (NV <= 2 ? 384 : 512), (DENSE ||
         // ---- fold: runs that start in this lane are written, the rows continuing an earlier run are added to it afterwards
         unsigned int cc = 0; double cs[NV];                    // the continuing part
 #pragma unroll
-        for (int q = 0; q < NV; q++) cs[q] = 0.0;
+        for (int q = 0; q < NV; q++) cs[q] = -0.0;
         {
             int e = ebase; unsigned int c = 0; double sacc[NV];
 #pragma unroll
-            for (int q = 0; q < NV; q++) sacc[q] = 0.0;
+            for (int q = 0; q < NV; q++) sacc[q] = -0.0;
 #pragma unroll
             for (int i = 0; i < 4; i++) {
                 if (hd[i]) {
@@ -2099,7 +2104,7 @@ __global__ void __launch_bounds__(DENSE ? 512 : (NV <= 2 ? 384 : 512), (DENSE ||
                         for (int q = 0; q < NV; q++) cs[q] = sacc[q]; }
                     e++; Qkey[e] = k[i]; c = 0;
 #pragma unroll
-                    for (int q = 0; q < NV; q++) sacc[q] = 0.0;
+                    for (int q = 0; q < NV; q++) sacc[q] = -0.0;
                 }
                 if (ok[i]) { c++;
 #pragma unroll
@@ -2130,7 +2135,7 @@ __global__ void __launch_bounds__(DENSE ? 512 : (NV <= 2 ? 384 : 512), (DENSE ||
                     const long long kk = Qkey[full + i]; const unsigned int cq = Qcnt[full + i];
                     double sq[NV];
 #pragma unroll
-                    for (int q = 0; q < NV; q++) sq[q] = q < nv ? Qsum[(size_t) q * RA_LIST + full + i] : 0.0;
+                    for (int q = 0; q < NV; q++) sq[q] = q < nv ? Qsum[(size_t) q * RA_LIST + full + i] : -0.0;
                     __syncwarp(__activemask());
                     Qkey[i] = kk; Qcnt[i] = cq;
 #pragma unroll
@@ -2439,13 +2444,15 @@ static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
         if (nw + 2 > GX_MAX_WORDS) { GX_SET_ERR(ctx, "agg plan: too many state words"); return GX_ERR_ARG; }
         switch (src.fn) {
             case GX_AGG_COUNT_STAR: g.kind = GXU_NONE; cp->agg_word[a] = 0; cp->need_w0 = 1; break;
-            case GX_AGG_COUNT: case GX_AGG_SUM_I4: case GX_AGG_SUM_I8: {
+            case GX_AGG_SUM_I8:
+                // the int64 accumulators wrap, and the reference's sum(int8) is numeric (never overflows)
+                GX_SET_ERR(ctx, "agg %d: sum(int8) is not supported", a); return GX_ERR_ARG;
+            case GX_AGG_COUNT: case GX_AGG_SUM_I4: {
                 GX_CHECK_ARG(ctx, src.arg.nops == 1 && src.arg.ops[0].op == GX_OP_COL, "agg %d: argument must be a plain column", a);
                 int col = src.arg.ops[0].col;
                 GX_CHECK_ARG(ctx, col >= 0 && col < outer->ncols, "agg %d: column out of range", a);
                 int t = outer->types[col];
                 if (src.fn == GX_AGG_SUM_I4) GX_CHECK_ARG(ctx, t == GX_INT4, "agg %d: sum(int4) needs an int4 column", a);
-                if (src.fn == GX_AGG_SUM_I8) GX_CHECK_ARG(ctx, t == GX_INT8, "agg %d: sum(int8) needs an int8 column", a);
                 g.is_int = 1; g.icol = dcol_of(outer, col); nullable = outer->nulls[col] != nullptr;
                 if (src.fn == GX_AGG_COUNT) {
                     if (nullable) { g.kind = GXU_CNT; g.word = new_word(WK_ADD_I64, 0); cp->agg_word[a] = g.word; }
@@ -2484,7 +2491,7 @@ static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
                 } else if (src.fn == GX_AGG_MAX_F8) { // identity of float8larger: -inf
                     double ninf = -__builtin_inf(); long long bits; memcpy(&bits, &ninf, 8);
                     g.kind = GXU_MAX_F64; g.word = new_word(WK_MAX_F64, bits);
-                } else { g.kind = GXU_ADD_F64; g.word = new_word(WK_ADD_F64, 0); }
+                } else { g.kind = GXU_ADD_F64; g.word = new_word(WK_ADD_F64, (long long) GX_NEG_ZERO_BITS); }   // -0: x + -0 == x for every x, -0 included
                 cp->agg_word[a] = g.word;
                 g.cnt_word = nullable ? new_word(WK_ADD_I64, 0) : 0; cp->agg_cnt_word[a] = g.cnt_word;
                 if (!nullable && src.fn == GX_AGG_AVG_F8) cp->need_w0 = 1;    // N of float8_avg
@@ -2526,6 +2533,8 @@ static int launch_agg(gx_ctx *ctx, const gx_agg_dev &A, size_t smem, const char 
     while ((nrows + maxb - 1) / maxb >= (1LL << 32)) maxb *= 2;
     unsigned grid = (unsigned) (nb < maxb ? (nb > 0 ? nb : 1) : maxb);
     gx_launch_scope ls(ctx, name);
+    // second profile name: which sink answered (gx_profile_get)
+    gx_launch_scope which(ctx, SINK == SINK_SMEM_LP ? "agg_smem_lp" : SINK == SINK_SMEM ? "agg_smem" : SINK == SINK_GLOBAL ? "agg_global" : "agg_records", 0);
     gx_k_agg<SINK><<<grid, threads, smem, ctx->stream>>>(A);
     GX_CUDA(ctx, cudaGetLastError());
     return GX_OK;
@@ -2543,6 +2552,7 @@ static int launch_lptile_k(gx_ctx *ctx, const gx_agg_dev &A, size_t smem, const 
     long long nb = (nrows + per_block - 1) / per_block, maxb = (long long) ctx->sm_count;
     unsigned grid = (unsigned) (nb < maxb ? (nb > 0 ? nb : 1) : maxb);
     gx_launch_scope ls(ctx, name);
+    gx_launch_scope which(ctx, K == 8 ? "agg_lptile8" : "agg_lptile4", 0);
     gx_k_agg_lptile<K><<<grid, threads, smem, ctx->stream>>>(A);
     GX_CUDA(ctx, cudaGetLastError());
     return GX_OK;
@@ -2567,6 +2577,7 @@ static int launch_fast_t(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_args &F
     while ((A.row1 - A.row0 + maxb - 1) / maxb >= (1LL << 32)) maxb *= 2;
     unsigned grid = (unsigned) (nb < maxb ? (nb > 0 ? nb : 1) : maxb);
     gx_launch_scope ls(ctx, name);
+    gx_launch_scope which(ctx, JOIN ? "probe_agg_fast" : "agg_fast", 0);
     gx_k_fast<JOIN, HAS_CNT, HAS_SUM><<<grid, 1024, smem, ctx->stream>>>(A, FA);
     GX_CUDA(ctx, cudaGetLastError());
     return GX_OK;
@@ -2584,6 +2595,7 @@ static int launch_runjoin_t(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_args
     while ((A.row1 - A.row0 + maxb - 1) / maxb >= (1LL << 32)) maxb *= 2;
     unsigned grid = (unsigned) (nb < maxb ? (nb > 0 ? nb : 1) : maxb);
     gx_launch_scope ls(ctx, name);
+    gx_launch_scope which(ctx, "probe_agg_run", 0);
     gx_k_runjoin<HAS_CNT, HAS_SUM, COMPACT><<<grid, 1024, smem, ctx->stream>>>(A, FA);
     GX_CUDA(ctx, cudaGetLastError());
     return GX_OK;
@@ -2643,6 +2655,7 @@ static int launch_runjoin3_t(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_arg
     while ((A.row1 - A.row0 + maxb - 1) / maxb >= (1LL << 32)) maxb *= 2;
     unsigned grid = (unsigned) (nb < maxb ? (nb > 0 ? nb : 1) : maxb);
     gx_launch_scope ls(ctx, name);
+    gx_launch_scope which(ctx, "probe_agg_run3", 0);
     gx_k_runjoin3<HAS_CNT, HAS_SUM, COMPACT><<<grid, 1024, table_bytes + 32 * sizeof(gx_runlist3), ctx->stream>>>(A, FA);
     GX_CUDA(ctx, cudaGetLastError());
     return GX_OK;
@@ -2685,6 +2698,7 @@ static int launch_runjoin2_t(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_arg
     while ((A.row1 - A.row0 + maxb - 1) / maxb >= (1LL << 31)) maxb *= 2;      // 31-bit row counters per CTA
     unsigned grid = (unsigned) (nb < maxb ? (nb > 0 ? nb : 1) : maxb);
     gx_launch_scope ls(ctx, name);
+    gx_launch_scope which(ctx, "probe_agg_run2", 0);
     gx_k_runjoin2<HAS_SUM, COMPACT><<<grid, 512, smem, ctx->stream>>>(A, FA);
     GX_CUDA(ctx, cudaGetLastError());
     return GX_OK;
@@ -2817,9 +2831,8 @@ static void remember_layout(gx_result *r, const compiled_plan *cp)
 static int run_radix(gx_ctx *ctx, compiled_plan *cp, const gx_agg_plan *plan, long long nrows_in, gx_result **out);
 int gx_result_layout_words(gx_result *r, int *wkind, long long *winit);
 
-extern "C" int gx_hash_agg(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, gx_result **out)
+static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, gx_result **out)
 {
-    if (!ctx || !outer || !plan || !out) return GX_ERR_ARG;
     compiled_plan cp;
     int rc = compile_plan(ctx, outer, h, plan, &cp); if (rc) return rc;
     gx_agg_dev &A = cp.A;
@@ -2984,6 +2997,7 @@ extern "C" int gx_hash_agg(gx_ctx *ctx, const gx_table *outer, const gx_hash *h,
             RA.out = d_out; RA.out_cap = out_cap; RA.cursor = ctx->d_scratch + 12;
             {
                 gx_launch_scope ls(ctx, "runagg");
+                gx_launch_scope which(ctx, dense ? "runagg_dense" : (small && RA.nv <= 1) ? "runagg_small1" : small ? "runagg_small2" : "runagg_wide", 0);
                 if (dense) gx_k_runagg<1, 2, 1><<<grid, threads, smem, ctx->stream>>>(A, RA);
                 else if (small && RA.nv <= 1) gx_k_runagg<1, 2><<<grid, threads, smem, ctx->stream>>>(A, RA);
                 else if (small) gx_k_runagg<2, 2><<<grid, threads, smem, ctx->stream>>>(A, RA);
@@ -3054,6 +3068,7 @@ extern "C" int gx_hash_agg(gx_ctx *ctx, const gx_table *outer, const gx_hash *h,
         if (use_fast) rc = launch_fast(ctx, A, FA, A.P.has_join != 0, cp.need_w0 != 0, FA.vcol != nullptr, dense_bytes(S), kname, use_run);
         else if (use_few && countchar_ok) {
             gx_launch_scope ls(ctx, kname);
+            gx_launch_scope which(ctx, "agg_count_char", 0);
             gx_k_count_char<<<ctx->sm_count * 2, 512, 0, ctx->stream>>>(A, (const signed char *) A.P.gcols[0].col.data);
             rc = cudaGetLastError() == cudaSuccess ? GX_OK : GX_ERR_CUDA;
         } else if (use_few) {
@@ -3075,6 +3090,7 @@ extern "C" int gx_hash_agg(gx_ctx *ctx, const gx_table *outer, const gx_hash *h,
             long long nb = (outer->nrows + (long long) fg_warps * 32 * fg_k - 1) / ((long long) fg_warps * 32 * fg_k);
             const unsigned fg_grid = (unsigned) (nb < ctx->sm_count ? nb : ctx->sm_count);
             gx_launch_scope ls(ctx, kname);
+            gx_launch_scope which(ctx, "agg_fewgroups", 0);
             if (v768) { if (bytekey) gx_k_fewgroups<true, 4, 768><<<fg_grid, 768, fg_smem, ctx->stream>>>(A, FG); else gx_k_fewgroups<false, 4, 768><<<fg_grid, 768, fg_smem, ctx->stream>>>(A, FG); }
             else { if (bytekey) gx_k_fewgroups<true, 8, 512><<<fg_grid, 512, fg_smem, ctx->stream>>>(A, FG); else gx_k_fewgroups<false, 8, 512><<<fg_grid, 512, fg_smem, ctx->stream>>>(A, FG); }
             rc = cudaGetLastError() == cudaSuccess ? GX_OK : GX_ERR_CUDA;
@@ -3104,6 +3120,190 @@ extern "C" int gx_hash_agg(gx_ctx *ctx, const gx_table *outer, const gx_hash *h,
     }
     GX_SET_ERR(ctx, "hash_agg: group table kept overflowing");
     return GX_ERR_STATE;
+}
+
+// ---- float8 overflow, decided while the input is still there ---------------------------------------------------
+// float8pl / float8mi / float8mul / float8_accum (CHECKFLOATVAL, float.c:40-60) raise "value out of range: overflow"
+// when a result is infinite and no input was: an infinite INPUT may give an infinite result.  The kernels do not check
+// per operation, so a finite overflow ends as an infinite state word.  After the aggregate, one small kernel scans the
+// float8 state words of the result; only when one is infinite, a second aggregate over the same input, quals, join and
+// groups sums 0 * c1 * c2 * ... over the columns of each argument: NaN exactly where a group had a non-finite input
+// (and strict in the same columns as the argument).  An infinite state with finite inputs is GX_ERR_OVERFLOW.
+// Not seen (DESIGN.md §7): an overflow whose infinity does not survive to the state (min(x*x) with other rows finite,
+// x*x - x*x ending as NaN), and any overflow in an argument with a non-finite constant (every row has an infinite
+// or NaN input there).
+struct gx_infscan_args { const unsigned long long *recs; long long n; int RW, nchk, need_w0, _pad; int word[GX_MAX_AGGS], cw[GX_MAX_AGGS]; int *flag; };
+__global__ void gx_k_inf_scan(const gx_infscan_args S)
+{
+    const long long stride = (long long) gridDim.x * blockDim.x;
+    for (long long gI = (long long) blockIdx.x * blockDim.x + threadIdx.x; gI < S.n; gI += stride) {
+        const unsigned long long *w = S.recs + (size_t) gI * S.RW + 3;
+        for (int a = 0; a < S.nchk; a++) {
+            const long long cnt = S.cw[a] ? (long long) w[S.cw[a]] : (S.need_w0 ? (long long) w[0] : 1);
+            if (cnt != 0 && isinf(__longlong_as_double((long long) w[S.word[a]]))) *S.flag = 1;
+        }
+    }
+}
+
+struct gx_group_key {
+    unsigned long long m, k0, k1;
+    bool operator==(const gx_group_key &o) const { return m == o.m && k0 == o.k0 && k1 == o.k1; }
+};
+struct gx_group_key_hash { size_t operator()(const gx_group_key &k) const { return (size_t) (k.k0 * 0x9E3779B97F4A7C15ULL ^ k.k1 * 0xC2B2AE3D27D4EB4FULL ^ k.m); } };
+
+// the float8 state words of r's aggregates that can overflow (chk[i] = aggregate number); sums_only: SUM/AVG
+static void f8_checked_words(const gx_result *r, bool sums_only, gx_infscan_args *S, int *chk)
+{
+    memset(S, 0, sizeof(*S));
+    for (int a = 0; a < r->plan.n_aggs; a++) {
+        const int fn = r->plan.aggs[a].fn;
+        const bool sum = fn == GX_AGG_SUM_F8 || fn == GX_AGG_AVG_F8;
+        if (!sum && (sums_only || (fn != GX_AGG_MIN_F8 && fn != GX_AGG_MAX_F8))) continue;
+        chk[S->nchk] = a; S->word[S->nchk] = r->agg_word[a]; S->cw[S->nchk] = r->agg_cnt_word[a]; S->nchk++;
+    }
+    S->RW = r->rec_words; S->need_w0 = r->need_w0;
+}
+// does any group of recs[0, n) hold a non-empty infinite checked word?
+static int any_inf_word(gx_ctx *ctx, gx_infscan_args S, const unsigned long long *recs, long long n, bool *any)
+{
+    *any = false;
+    if (S.nchk == 0 || n == 0) return GX_OK;
+    S.recs = recs; S.n = n; S.flag = (int *) (ctx->d_scratch + 24);
+    GX_CUDA(ctx, cudaMemsetAsync(S.flag, 0, sizeof(int), ctx->stream));
+    {
+        gx_launch_scope ls(ctx, "agg_inf_scan");
+        const long long nb = (n + 255) / 256, maxb = (long long) ctx->sm_count * 4;
+        gx_k_inf_scan<<<(unsigned) (nb < maxb ? nb : maxb), 256, 0, ctx->stream>>>(S);
+    }
+    GX_CUDA(ctx, cudaGetLastError());
+    GX_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + 24, S.flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    GX_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    *any = *(int *) (ctx->h_scratch + 24) != 0;
+    return GX_OK;
+}
+static long long rec_count(const gx_infscan_args &S, const unsigned long long *w, int i)
+{
+    return S.cw[i] ? (long long) w[S.cw[i]] : (S.need_w0 ? (long long) w[0] : 1);
+}
+
+static int check_f8_overflow(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, gx_result *r)
+{
+    gx_infscan_args S; int chk[GX_MAX_AGGS];
+    f8_checked_words(r, false, &S, chk);
+    // an argument with a non-finite constant has an infinite (or NaN) input in every row: never an overflow
+    int keep = 0;
+    for (int i = 0; i < S.nchk; i++) {
+        const gx_expr &src = plan->aggs[chk[i]].arg;
+        bool finite = true;
+        for (int j = 0; j < src.nops; j++) if (src.ops[j].op == GX_OP_CONST && !std::isfinite(src.ops[j].k)) finite = false;
+        if (finite) { chk[keep] = chk[i]; S.word[keep] = S.word[i]; S.cw[keep] = S.cw[i]; keep++; }
+    }
+    S.nchk = keep;
+    bool any;
+    int rc = any_inf_word(ctx, S, (const unsigned long long *) r->d_recs, r->ngroups, &any);
+    if (rc != GX_OK || !any) return rc;
+
+    // the verification aggregate: one sum(0 * c1 * c2 * ...) per checked argument
+    gx_agg_plan vp = *plan;
+    vp.n_aggs = S.nchk;
+    for (int i = 0; i < S.nchk; i++) {
+        const gx_expr &src = plan->aggs[chk[i]].arg;
+        gx_agg &va = vp.aggs[i]; memset(&va, 0, sizeof(va));
+        va.fn = GX_AGG_SUM_F8;
+        gx_expr &e = va.arg;
+        e.ops[e.nops].op = GX_OP_CONST; e.ops[e.nops].k = 0.0; e.nops++;
+        for (int j = 0; j < src.nops; j++) {
+            if (src.ops[j].op != GX_OP_COL) continue;
+            GX_CHECK_ARG(ctx, e.nops + 2 <= GX_MAX_EXPR_OPS, "agg %d: too many columns to check for overflow", chk[i]);
+            e.ops[e.nops].op = GX_OP_COL; e.ops[e.nops].col = src.ops[j].col; e.nops++;
+            e.ops[e.nops].op = GX_OP_MUL; e.nops++;
+        }
+    }
+    gx_result *v = nullptr;
+    rc = hash_agg_run(ctx, outer, h, &vp, &v);
+    if (rc != GX_OK) return rc;
+    const int ng = plan->n_group_cols;
+    const unsigned long long mmask = (1ULL << ng) - 1;
+    std::vector<unsigned long long> hr((size_t) r->ngroups * r->rec_words), hv((size_t) v->ngroups * v->rec_words + 1);
+    cudaError_t e = cudaMemcpyAsync(hr.data(), r->d_recs, hr.size() * 8, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess && v->ngroups) e = cudaMemcpyAsync(hv.data(), v->d_recs, (size_t) v->ngroups * v->rec_words * 8, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) { gx_result_free(v); GX_SET_ERR(ctx, "hash_agg: %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
+    std::unordered_map<gx_group_key, long long, gx_group_key_hash> at;
+    at.reserve((size_t) v->ngroups);
+    for (long long gI = 0; gI < v->ngroups; gI++) {
+        const unsigned long long *rec = hv.data() + (size_t) gI * v->rec_words;
+        at[{ rec[0] & mmask, rec[1], rec[2] }] = gI;
+    }
+    rc = GX_OK;
+    for (long long gI = 0; gI < r->ngroups && rc == GX_OK; gI++) {
+        const unsigned long long *rec = hr.data() + (size_t) gI * r->rec_words, *w = rec + 3;
+        for (int i = 0; i < S.nchk && rc == GX_OK; i++) {
+            double x; memcpy(&x, &w[S.word[i]], 8);
+            if (rec_count(S, w, i) == 0 || !std::isinf(x)) continue;
+            auto it = at.find({ rec[0] & mmask, rec[1], rec[2] });
+            if (it == at.end()) { GX_SET_ERR(ctx, "hash_agg: overflow check lost a group"); rc = GX_ERR_STATE; break; }
+            double nonfinite; memcpy(&nonfinite, &hv[(size_t) it->second * v->rec_words + 3 + v->agg_word[i]], 8);
+            if (!std::isnan(nonfinite)) { GX_SET_ERR(ctx, "value out of range: overflow"); rc = GX_ERR_OVERFLOW; }
+        }
+    }
+    gx_result_free(v);
+    return rc;
+}
+
+// The same rule for the Finalize step across datanodes (float8pl / float8_combine, float.c:2725): every datanode's
+// gx_hash_agg already rejected its own finite overflows, so an infinite partial sum comes from an infinite input.
+// A merged SUM/AVG word that is infinite while none of the partial records merged into it was is an overflow of
+// the combine itself.  spans: the partial records (device), merged: the merged groups (device).
+static int check_combine_overflow(gx_ctx *ctx, const gx_result *r, const std::vector<std::pair<const unsigned long long *, long long>> &spans,
+                                  const unsigned long long *merged, long long nmerged)
+{
+    gx_infscan_args S; int chk[GX_MAX_AGGS];
+    f8_checked_words(r, true, &S, chk);
+    bool any;
+    int rc = any_inf_word(ctx, S, merged, nmerged, &any);
+    if (rc != GX_OK || !any) return rc;
+    const int RW = r->rec_words;
+    const unsigned long long mmask = (1ULL << r->plan.n_group_cols) - 1;
+    long long nin = 0;
+    for (auto &sp : spans) nin += sp.second;
+    std::vector<unsigned long long> hm((size_t) nmerged * RW), hin((size_t) nin * RW + 1);
+    cudaError_t e = cudaMemcpyAsync(hm.data(), merged, hm.size() * 8, cudaMemcpyDeviceToHost, ctx->stream);
+    long long off = 0;
+    for (auto &sp : spans) {
+        if (e == cudaSuccess && sp.second) e = cudaMemcpyAsync(hin.data() + (size_t) off * RW, sp.first, (size_t) sp.second * RW * 8, cudaMemcpyDeviceToHost, ctx->stream);
+        off += sp.second;
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) { GX_SET_ERR(ctx, "combine: %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
+    // per group: which checked words were infinite in some partial record
+    std::unordered_map<gx_group_key, unsigned int, gx_group_key_hash> inf_in;
+    for (long long k = 0; k < nin; k++) {
+        const unsigned long long *rec = hin.data() + (size_t) k * RW, *w = rec + 3;
+        unsigned int bits = 0;
+        for (int i = 0; i < S.nchk; i++) { double x; memcpy(&x, &w[S.word[i]], 8); if (std::isinf(x)) bits |= 1u << i; }
+        if (bits) inf_in[{ rec[0] & mmask, rec[1], rec[2] }] |= bits;
+    }
+    for (long long gI = 0; gI < nmerged; gI++) {
+        const unsigned long long *rec = hm.data() + (size_t) gI * RW, *w = rec + 3;
+        for (int i = 0; i < S.nchk; i++) {
+            double x; memcpy(&x, &w[S.word[i]], 8);
+            if (rec_count(S, w, i) == 0 || !std::isinf(x)) continue;
+            auto it = inf_in.find({ rec[0] & mmask, rec[1], rec[2] });
+            if (it == inf_in.end() || !((it->second >> i) & 1u)) { GX_SET_ERR(ctx, "value out of range: overflow"); return GX_ERR_OVERFLOW; }
+        }
+    }
+    return GX_OK;
+}
+
+extern "C" int gx_hash_agg(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, gx_result **out)
+{
+    if (!ctx || !outer || !plan || !out) return GX_ERR_ARG;
+    int rc = hash_agg_run(ctx, outer, h, plan, out);
+    if (rc != GX_OK) return rc;
+    rc = check_f8_overflow(ctx, outer, h, plan, *out);
+    if (rc != GX_OK) { gx_result_free(*out); *out = nullptr; }
+    return rc;
 }
 
 // single-block exclusive scan (same as gx_table.cu's, kept local to this TU)
@@ -3203,7 +3403,10 @@ int gx_combine_records(gx_ctx *ctx, gx_result *r, unsigned long long *d_recs, lo
     A.P.nwords = r->nwords; A.P.nkw = 2;
     int rc = gx_result_layout_words(r, A.wkind, A.winit); if (rc) { GX_SET_ERR(ctx, "combine: unknown result"); return rc; }
     A.counters = ctx->d_scratch + 8;
-    return gx_aggregate_records(ctx, A, d_recs, nrec, d_out, ngroups_out);
+    rc = gx_aggregate_records(ctx, A, d_recs, nrec, d_out, ngroups_out);
+    if (rc == GX_OK) rc = check_combine_overflow(ctx, r, { { d_recs, nrec } }, *d_out, *ngroups_out);
+    if (rc != GX_OK && *d_out) { gx_tmp_free(ctx, *d_out); *d_out = nullptr; *ngroups_out = 0; }
+    return rc;
 }
 
 // small-result Finalize: pack this rank's partial records into a fixed-capacity segment
@@ -3248,6 +3451,17 @@ int gx_combine_gathered(gx_ctx *ctx, gx_result *r, const unsigned long long *d_g
     if (rc != GX_OK) { gx_tmp_free(ctx, d_groups); return rc; }
     *anybig = c[3] != 0;
     if (*anybig) { gx_tmp_free(ctx, d_groups); *d_out = nullptr; *ngroups_out = 0; return GX_OK; }
+    // segment s: [n, big, n records]; its record count sits in the header
+    std::vector<std::pair<const unsigned long long *, long long>> spans;
+    for (int s = 0; s < nseg; s++) {
+        const unsigned long long *seg = d_gather + (size_t) s * (2 + cap * RW);
+        long long n = 0;
+        GX_CUDA(ctx, cudaMemcpyAsync(&n, seg, sizeof(n), cudaMemcpyDeviceToHost, ctx->stream));
+        GX_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        spans.push_back({ seg + 2, n });
+    }
+    rc = check_combine_overflow(ctx, r, spans, d_groups, c[0]);
+    if (rc != GX_OK) { gx_tmp_free(ctx, d_groups); return rc; }
     *d_out = d_groups; *ngroups_out = c[0];
     return GX_OK;
 }
@@ -3320,7 +3534,7 @@ struct gx_final_args {
     const unsigned long long *recs; long long ngroups; int RW, ng, na, need_w0;
     int gword[GX_MAX_GROUP_COLS], gshift[GX_MAX_GROUP_COLS], gtype[GX_MAX_GROUP_COLS];
     int fn[GX_MAX_AGGS], word[GX_MAX_AGGS], cw[GX_MAX_AGGS];
-    long long *key_out; double *agg_out; unsigned char *null_out; int *overflow;
+    long long *key_out; double *agg_out; unsigned char *null_out;
 };
 __global__ void gx_k_finalize(const gx_final_args F)
 {
@@ -3348,13 +3562,12 @@ __global__ void gx_k_finalize(const gx_final_args F)
                 case GX_AGG_COUNT_STAR: ires = (long long) w[0]; is_int = true; break;
                 case GX_AGG_COUNT: ires = (long long) w[word]; is_int = true; break;
                 case GX_AGG_SUM_I4: case GX_AGG_SUM_I8: ires = (long long) w[word]; is_int = true; isnull = cnt == 0; break;
-                case GX_AGG_AVG_F8: { const double sx = __longlong_as_double((long long) w[word]); if (cnt == 0) isnull = true; else res = sx / (double) cnt; break; }
+                case GX_AGG_AVG_F8: { const double sx = __longlong_as_double((long long) w[word]) + 0.0; if (cnt == 0) isnull = true; else res = sx / (double) cnt; break; }
                 default: res = __longlong_as_double((long long) w[word]); isnull = cnt == 0; break;
             }
             if (isnull) { res = 0.0; ires = 0; }
             F.agg_out[gI * F.na + a] = is_int ? __longlong_as_double(ires) : res;
             if (F.null_out) F.null_out[gI * (F.ng + F.na) + F.ng + a] = isnull;
-            if (!is_int && !isnull && (fn == GX_AGG_SUM_F8 || fn == GX_AGG_AVG_F8) && isinf(res)) *F.overflow = 1;
         }
     }
 }
@@ -3370,10 +3583,8 @@ static int fetch_on_device(gx_result *r, const result_layout &L, int64_t *key_ou
     for (int a = 0; a < na; a++) { F.fn[a] = r->plan.aggs[a].fn; F.word[a] = r->agg_word[a]; F.cw[a] = r->agg_cnt_word[a]; }
     char *d = nullptr;
     const size_t kb = n * (ng > 0 ? ng : 1) * 8, ab = n * (na > 0 ? na : 1) * 8, nb = (n * (ng + na) + 15) & ~(size_t) 15;
-    GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d, kb + ab + nb + 16));
+    GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d, kb + ab + nb));
     F.key_out = (long long *) d; F.agg_out = (double *) (d + kb); F.null_out = null_out ? (unsigned char *) (d + kb + ab) : nullptr;
-    F.overflow = (int *) (d + kb + ab + nb);
-    GX_CUDA(ctx, cudaMemsetAsync(F.overflow, 0, sizeof(int), ctx->stream));
     {
         gx_launch_scope ls(ctx, "finalize");
         gx_k_finalize<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(F);
@@ -3382,11 +3593,9 @@ static int fetch_on_device(gx_result *r, const result_layout &L, int64_t *key_ou
     if (e == cudaSuccess && ng) e = cudaMemcpyAsync(key_out, F.key_out, n * ng * 8, cudaMemcpyDeviceToHost, ctx->stream);
     if (e == cudaSuccess && na) e = cudaMemcpyAsync(agg_out, F.agg_out, n * na * 8, cudaMemcpyDeviceToHost, ctx->stream);
     if (e == cudaSuccess && null_out) e = cudaMemcpyAsync(null_out, F.null_out, n * (ng + na), cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->h_scratch + 16, F.overflow, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
     gx_tmp_free(ctx, d);
     if (e != cudaSuccess) { GX_SET_ERR(ctx, "result_fetch: %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
-    if (*(int *) (ctx->h_scratch + 16)) { GX_SET_ERR(ctx, "value out of range: overflow"); return GX_ERR_OVERFLOW; }
     return GX_OK;
 }
 
@@ -3439,16 +3648,12 @@ extern "C" int gx_result_fetch(gx_result *r, int64_t max_groups, int64_t *key_ou
                 case GX_AGG_COUNT_STAR: ires = (long long) w[0]; is_int = true; break;
                 case GX_AGG_COUNT: ires = (long long) w[word]; is_int = true; break;
                 case GX_AGG_SUM_I4: case GX_AGG_SUM_I8: ires = (long long) w[word]; is_int = true; isnull = cnt == 0; break;
-                case GX_AGG_AVG_F8: { double sx; memcpy(&sx, &w[word], 8); if (cnt == 0) isnull = 1; else res = sx / (double) cnt; break; }
+                case GX_AGG_AVG_F8: { double sx; memcpy(&sx, &w[word], 8); sx += 0.0; if (cnt == 0) isnull = 1; else res = sx / (double) cnt; break; }
                 default: { memcpy(&res, &w[word], 8); isnull = cnt == 0; break; }
             }
             if (isnull) { res = 0.0; ires = 0; }
             if (is_int) memcpy(&agg_out[g * na + a], &ires, 8); else agg_out[g * na + a] = res;
             if (null_out) null_out[g * (ng + na) + ng + a] = isnull;
-            // float8pl's CHECKFLOATVAL: a finite-input sum that reached infinity is an ERROR in the reference
-            if (!is_int && !isnull && (fn == GX_AGG_SUM_F8 || fn == GX_AGG_AVG_F8) && __builtin_isinf(res)) {
-                free(h); GX_SET_ERR(ctx, "value out of range: overflow"); return GX_ERR_OVERFLOW;
-            }
         }
     }
     free(h);
@@ -3507,11 +3712,8 @@ extern "C" int gx_result_fetch_states(gx_result *r, int64_t max_groups, int64_t 
                 case GX_AGG_COUNT_STAR: n = rows; break;
                 case GX_AGG_COUNT: n = (long long) w[word]; break;
                 case GX_AGG_SUM_I4: case GX_AGG_SUM_I8: memcpy(&v, &w[word], 8); isnull = cnt == 0; break;
-                case GX_AGG_AVG_F8: memcpy(&v, &w[word], 8); break;              // {N, Sx}: never NULL (initial state '{0,0,0}')
+                case GX_AGG_AVG_F8: memcpy(&v, &w[word], 8); v += 0.0; break;    // {N, Sx}: never NULL; Sx starts at +0 ('{0,0,0}')
                 default: memcpy(&v, &w[word], 8); isnull = cnt == 0; break;      // sum / min / max: strict, NULL until the first input
-            }
-            if ((fn == GX_AGG_SUM_F8 || fn == GX_AGG_AVG_F8) && !isnull && __builtin_isinf(v)) {
-                free(h); GX_SET_ERR(ctx, "value out of range: overflow"); return GX_ERR_OVERFLOW;
             }
             val_out[gI * na + a] = isnull ? 0.0 : v; cnt_out[gI * na + a] = n;
             if (null_out) null_out[gI * (ng + na) + ng + a] = isnull;

@@ -40,3 +40,16 @@ def test_q3_two_datanodes_with_redistribute(env, orders, want):
     assert "OK q3 parity vs oracle" in r.stdout, r.stdout[-2000:]
     for w in want:
         assert w in r.stdout, r.stdout[-2000:]
+
+
+@pytest.mark.gpu
+@pytest.mark.skipif(_ngpus() < 2, reason="needs two GPUs")
+@pytest.mark.parametrize("env", [{}, {"GX_NO_GATHER_COMBINE": "1"}], ids=["gathered", "records"])
+def test_combine_float8_overflow_rule(env):
+    """two finite partial sums overflowing in combine are GX_ERR_OVERFLOW; an infinite partial is not"""
+    s = socket.socket(); s.bind(("127.0.0.1", 0)); port = s.getsockname()[1]; s.close()
+    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
+           "--master-port", str(port), os.path.join(ROOT, "scripts", "combine_fp_multi.py")]
+    r = subprocess.run(cmd, capture_output=True, text=True, timeout=600, cwd=ROOT, env=dict(os.environ, **env))
+    assert r.returncode == 0, (r.stdout + r.stderr)[-3000:]
+    assert "OK combine overflow rule" in r.stdout, r.stdout[-2000:]
