@@ -278,7 +278,14 @@ int  gx_scan_filter(gx_ctx *ctx, const gx_table *in, int n_preds,
  * key_col must be INT4/INT8/DATE.  Up to two payload columns totalling <= 8
  * bytes are stored in the slot; n_payload == 0 stores the build row number.
  * NULL keys are dropped (hashStrict, nodeHash.c:2071-2079).  unique = 1 is the
- * planner's inner_unique (nodeHashjoin.c:859-861). */
+ * planner's inner_unique (nodeHashjoin.c:859-861).
+ * Skew limit: linear probing wraps inside 2048-slot sub-tables, and every sub-table
+ * keeps at least one free slot so that a probe for a missing key ends.  A build side
+ * whose rows cannot be spread that way — one key repeated about 700 to 2047 times
+ * or more (the exact count depends on the load factor and on the keys sharing its
+ * sub-table), or many distinct keys that collide under the hash — is declined with
+ * GX_ERR_ARG, the message giving how many rows hashed into one sub-table.  The table
+ * is freed and the context stays usable. */
 int  gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col,
                    int n_preds, const gx_pred *preds,
                    int n_payload, const int32_t *payload_cols, int unique,

@@ -1069,7 +1069,12 @@ __global__ void __launch_bounds__(1024, 1) gx_k_fast(const __grid_constant__ gx_
             if (open) fast_flush<HAS_CNT, HAS_SUM>(T, A, cur, cnt, sum, F.sum_word);
             open = true; cur = g[i]; cnt = 1; sum = HAS_SUM ? v[i] : -0.0;
         }
-        if (open) { cnt += rcnt; if (HAS_SUM) sum = __dadd_rn(sum, rsum); fast_flush<HAS_CNT, HAS_SUM>(T, A, cur, cnt, sum, F.sum_word); }
+        // the partial handed down belongs to row 3's key: it joins row 3's run, or is dropped when that key has no
+        // partner (the open run is then an earlier key's)
+        if (open) {
+            if (hit[3]) { cnt += rcnt; if (HAS_SUM) sum = __dadd_rn(sum, rsum); }
+            fast_flush<HAS_CNT, HAS_SUM>(T, A, cur, cnt, sum, F.sum_word);
+        }
     }
     // the (< 4) rows after the last full vector: one thread each
     {

@@ -131,14 +131,14 @@ void gx_set_global_err(const char *fmt, ...);
 
 #define GX_CHECK_ARG(ctx, cond, ...) do { if (!(cond)) { GX_SET_ERR(ctx, __VA_ARGS__); return GX_ERR_ARG; } } while (0)
 
-// launch accounting + optional per-kernel CUDA-event timing
+// launch accounting + optional per-kernel CUDA-event timing (name nullptr: nothing is recorded)
 struct gx_launch_scope {
     gx_ctx *ctx; const char *name;
     int slot;
     gx_launch_scope(gx_ctx *c, const char *n, int nlaunch = 1) : ctx(c), name(n), slot(-1) {
         ctx->launches += nlaunch;
         // events are only recorded here (asynchronously); gx_profile_get() resolves them
-        if (ctx->profile && ctx->prof_used < GX_PROF_POOL) {
+        if (name && ctx->profile && ctx->prof_used < GX_PROF_POOL) {
             slot = ctx->prof_used++;
             ctx->prof_pool[slot].name = name;
             cudaEventRecord(ctx->prof_pool[slot].a, ctx->stream);

@@ -24,6 +24,9 @@ struct gx_build_args {
     unsigned long long *special; int special_cap;
     gx_slotfn sf;                 // gx_slot_index
     long long *counters;          // [0] entries inserted, [1] special count
+    // direct build only: rows claimed per sub-table, how many one sub-table may hold, and the largest
+    // claim count seen past that limit (0 = none)
+    unsigned int *sub_claims; unsigned int sub_limit; unsigned int *sub_over;
 };
 
 __device__ __forceinline__ unsigned long long pack_payload(const gx_build_args &a, long long r)
@@ -60,12 +63,18 @@ __global__ void __launch_bounds__(256) gx_k_hash_build(gx_build_args a)
             continue;
         }
         unsigned long long s = gx_slot_index(key, a.sf);
-        for (;;) {
+        // a sub-table must keep a free slot, or probe walks that miss in it never end: rows past the limit
+        // are not inserted and fail the build.  So the CAS walk below always meets an empty slot.
+        const unsigned int claim = atomicAdd(&a.sub_claims[s >> GX_SUB_LOG2], 1u);
+        if (claim >= a.sub_limit) { atomicMax(a.sub_over, claim + 1); continue; }
+        bool placed = false;
+        for (int step = 0; step < GX_SUB; step++) {
             long long old = (long long) atomicCAS((unsigned long long *) &a.slots[s].key,
                                                   (unsigned long long) GX_EMPTY_KEY, (unsigned long long) key);
-            if (old == GX_EMPTY_KEY) { a.slots[s].payload = payload; break; }
+            if (old == GX_EMPTY_KEY) { a.slots[s].payload = payload; placed = true; break; }
             s = gx_next_slot(s, a.mask);
         }
+        if (!placed) { atomicMax(a.sub_over, claim + 1); continue; }
         inserted++;
     }
     // one atomic per warp
@@ -143,7 +152,7 @@ __global__ void __launch_bounds__(256) gx_k_bbuild_scatter(gx_bbuild_args a)
 #pragma unroll
         for (int u = 0; u < BSCAT; u++) {
             if (!ok[u]) continue;
-            if (pos[u] >= GX_SUB) { *a.overflow = 1; continue; }
+            if (pos[u] >= GX_SUB - 1) { *a.overflow = 1; continue; }      // a sub-table keeps one slot free
             longlong2 v; v.x = key[u]; v.y = (long long) payload[u];
             ((longlong2 *) a.pairs)[sub[u] * GX_SUB + pos[u]] = v;
         }
@@ -287,7 +296,7 @@ __global__ void __launch_bounds__(BP_THREADS, 2) gx_k_bpart2(gx_bpart_args a)
         for (unsigned int j = threadIdx.x; j < total; j += blockDim.x) {
             unsigned int d = m.bid[j];
             unsigned int pos = m.gbase[d] + (j - m.base[d]);
-            if (pos >= GX_SUB) { *a.overflow = 1; continue; }
+            if (pos >= GX_SUB - 1) { *a.overflow = 1; continue; }       // a sub-table keeps one slot free
             ((longlong2 *) a.pairs)[(((long long) b1 << a.bits_lo) | d) * GX_SUB + pos] = m.stage[j];
         }
         __syncthreads();
@@ -461,7 +470,7 @@ __global__ void __launch_bounds__(FILL_THREADS, 4) gx_k_bbuild_fill(gx_bbuild_ar
     unsigned int steps = 0, placed = 0;
     for (long long sub = blockIdx.x; sub < a.nsub; sub += gridDim.x) {
         unsigned int n = a.cursor[sub];
-        if (n > GX_SUB) n = 0;                         // overflowed: the host rebuilds directly
+        if (n >= GX_SUB) n = 0;                        // overflowed: the host rebuilds directly
         const longlong2 *src = (const longlong2 *) a.pairs + sub * GX_SUB;
         gx_subtable_build<false>(sm, n, a.b.sf,
                           [&](unsigned int i, long long &k, unsigned long long &p) { longlong2 v = src[i]; k = v.x; p = (unsigned long long) v.y; return true; },
@@ -560,7 +569,7 @@ __global__ void __launch_bounds__(FILL_THREADS, C ? 5 : 4) gx_k_sorted_fill(gx_b
         const long long nsubn = sub + gridDim.x;
         if (nsubn < a.nsub) { nlo = a.start[nsubn]; nhi = a.start[nsubn + 1]; }
         unsigned int n = (unsigned int) (hi - lo);
-        if (hi - lo > GX_SUB) { n = 0; if (threadIdx.x == 0) *a.overflow = 1; }
+        if (hi - lo >= GX_SUB) { n = 0; if (threadIdx.x == 0) *a.overflow = 1; }     // a sub-table keeps one slot free
         if (VERIFY && hi < lo) { n = 0; bad = 1; }
         if (PK != 0 && nhi - nlo <= GX_SUB) {
             const long long l = nlo + (long long) threadIdx.x * 16;          // 16 keys = one 128-byte line
@@ -908,6 +917,8 @@ extern "C" int gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col, in
                     }
                     { gx_launch_scope ls(ctx, "build_bounds"); gx_k_sorted_bounds_search<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>((const long long *) a.key.data, inner->nrows, a.sf, ba.nsub, h->nslots, d_start); }
                     gx_launch_scope ls(ctx, "build");
+                    gx_launch_scope path(ctx, "build_sorted_search", 0);           // second profile names: which build path ran
+                    gx_launch_scope form(ctx, compact ? "build_compact" : nullptr, 0);
                     if (compact && pk == 1) gx_k_sorted_fill<1, true, true><<<ctx->sm_count * 10, FILL_THREADS, FILL_SMEM_BYTES_C, ctx->stream>>>(ba);
                     else if (compact && pk == 2) gx_k_sorted_fill<2, true, true><<<ctx->sm_count * 10, FILL_THREADS, FILL_SMEM_BYTES_C, ctx->stream>>>(ba);
                     else if (compact) gx_k_sorted_fill<0, true, true><<<ctx->sm_count * 10, FILL_THREADS, FILL_SMEM_BYTES_C, ctx->stream>>>(ba);
@@ -924,6 +935,8 @@ extern "C" int gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col, in
                     }
                     {
                         gx_launch_scope ls(ctx, "build", 2);
+                        gx_launch_scope path(ctx, "build_sorted_pass", 0);
+                        gx_launch_scope form(ctx, compact ? "build_compact" : nullptr, 0);
                         gx_k_sorted_special<<<1, 256, 0, ctx->stream>>>(a, d_start, d_flag);
                         const unsigned int fgrid = ctx->sm_count * 8;
                         if (compact && pk == 1) gx_k_sorted_fill<1, true, false><<<ctx->sm_count * 10, FILL_THREADS, FILL_SMEM_BYTES_C, ctx->stream>>>(ba);
@@ -990,13 +1003,18 @@ extern "C" int gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col, in
                     attr = true;
                 }
                 gx_launch_scope ls(ctx, "build_scatter", 2);
+                gx_launch_scope which(ctx, "build_bucket2", 0);
                 gx_k_bpart1<<<ctx->sm_count * 2, BP_THREADS, bp_smem_bytes(1 << pa.bits_hi), ctx->stream>>>(pa);
                 gx_k_bpart2<<<ctx->sm_count * 2, BP_THREADS, bp_smem_bytes(1 << pa.bits_lo), ctx->stream>>>(pa);
             }
             gx_tmp_free(ctx, pa.l1); gx_tmp_free(ctx, pa.cur1);
             if (e != cudaSuccess) two_level = false;            // no room for the level-1 buffer: one-pass scatter
         }
-        if (!two_level) { gx_launch_scope ls(ctx, "build_scatter"); gx_k_bbuild_scatter<<<grid, 256, 0, ctx->stream>>>(ba); }
+        if (!two_level) {
+            gx_launch_scope ls(ctx, "build_scatter");
+            gx_launch_scope which(ctx, "build_bucket1", 0);
+            gx_k_bbuild_scatter<<<grid, 256, 0, ctx->stream>>>(ba);
+        }
         {
             static bool attr = false;
             if (!attr) { cudaFuncSetAttribute(gx_k_bbuild_fill, cudaFuncAttributeMaxDynamicSharedMemorySize, FILL_SMEM_BYTES); attr = true; }
@@ -1020,10 +1038,32 @@ extern "C" int gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col, in
     if (inner->nrows > 0 && !bucketed) {
         GX_CUDA(ctx, cudaMemsetAsync(ctx->d_scratch, 0, 2 * sizeof(long long), ctx->stream));
         { gx_launch_scope ls(ctx, "build_clear"); gx_k_fill_slots<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(h->slots, h->nslots); }
-        gx_launch_scope ls(ctx, "build");
-        long long nb = (inner->nrows + 255) / 256;
-        long long maxb = (long long) ctx->sm_count * 8;
-        gx_k_hash_build<<<(unsigned) (nb < maxb ? nb : maxb), 256, 0, ctx->stream>>>(a);
+        // probe walks wrap inside a sub-table (or the whole table when it is smaller): each keeps a free slot
+        const long long wrap = h->nslots < GX_SUB ? h->nslots : GX_SUB, nsub = h->nslots / wrap;
+        unsigned int *claims = nullptr;
+        GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &claims, (size_t) (nsub + 1) * sizeof(unsigned int)));
+        GX_CUDA(ctx, cudaMemsetAsync(claims, 0, (size_t) (nsub + 1) * sizeof(unsigned int), ctx->stream));
+        a.sub_claims = claims; a.sub_limit = (unsigned int) (wrap - 1); a.sub_over = claims + nsub;
+        unsigned int h_sub_over = 0;
+        cudaError_t e;
+        {
+            gx_launch_scope ls(ctx, "build");
+            gx_launch_scope which(ctx, "build_direct", 0);
+            long long nb = (inner->nrows + 255) / 256;
+            long long maxb = (long long) ctx->sm_count * 8;
+            gx_k_hash_build<<<(unsigned) (nb < maxb ? nb : maxb), 256, 0, ctx->stream>>>(a);
+            e = cudaGetLastError();
+        }
+        if (e == cudaSuccess) e = cudaMemcpyAsync(&h_sub_over, a.sub_over, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+        gx_tmp_free(ctx, claims);
+        if (e != cudaSuccess) { GX_SET_ERR(ctx, "hash_build: %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
+        if (h_sub_over) {
+            GX_SET_ERR(ctx, "hash_build: %u build rows hash into one %lld-slot sub-table of the join table, which holds at most %lld "
+                       "(a build key repeated that often, or keys that collide under the table's hash)",
+                       h_sub_over, wrap, wrap - 1);
+            return GX_ERR_ARG;
+        }
     } else if (inner->nrows == 0) {
         gx_launch_scope ls(ctx, "build_clear"); gx_k_fill_slots<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(h->slots, h->nslots);
     }
