@@ -1252,45 +1252,11 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin(const __grid_constant__ 
 // Nothing depends on the layout for correctness: a probe whose slot group is not inside the staged window (keys out
 // of order, a chain that walks past the window, a chunk denser than the ring buffer) reads global memory as before,
 // and a chunk whose key range is far wider than the buffer is not staged at all.
-// Every wait is bounded (GX_SEG_SPIN_LIMIT polls): a protocol error raises flag 16 and the host redoes the query with
+// Every wait is bounded (GX_MBAR_SPIN_LIMIT polls, gx_mbar_wait): a protocol error raises flag 16 and the host redoes the query with
 // gx_k_runjoin instead of hanging the device.
 #define GX_SEG_CW          31                     /* consumer warps; warp 31 is the producer */
-#define GX_SEG_SPIN_LIMIT  (1u << 22)
 #define GX_SEG_MAXBUF      4
 struct gx_seg_ctl { unsigned long long full[GX_SEG_MAXBUF], empty[GX_SEG_MAXBUF], lo[GX_SEG_MAXBUF]; unsigned int len[GX_SEG_MAXBUF]; };
-
-__device__ __forceinline__ unsigned int gx_smem_u32(const void *p) { return (unsigned int) __cvta_generic_to_shared(p); }
-__device__ __forceinline__ void gx_mbar_init(void *bar, unsigned int count)
-{
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(gx_smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void gx_mbar_arrive(void *bar)
-{
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(gx_smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void gx_mbar_arrive_expect_tx(void *bar, unsigned int bytes)
-{
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(gx_smem_u32(bar)), "r"(bytes) : "memory");
-}
-// false when the phase did not complete within the poll budget (try_wait itself sleeps in hardware between polls)
-__device__ __forceinline__ bool gx_mbar_wait(void *bar, unsigned int parity)
-{
-    const unsigned int a = gx_smem_u32(bar);
-#pragma unroll 1
-    for (unsigned int n = 0; n < GX_SEG_SPIN_LIMIT; n++) {
-        unsigned int ok;
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(ok) : "r"(a), "r"(parity) : "memory");
-        if (ok) return true;
-    }
-    return false;
-}
-// one bulk-async copy global -> shared (16-byte aligned addresses, size a multiple of 16); completion is counted on `bar`
-__device__ __forceinline__ void gx_bulk_g2s(void *dst, const void *src, unsigned int bytes, void *bar)
-{
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 :: "r"(gx_smem_u32(dst)), "l"(src), "r"(bytes), "r"(gx_smem_u32(bar)) : "memory");
-}
 
 // one key against the compact join table, the slot groups inside [lo, lo + len) taken from the staged copy `sg`
 __device__ __forceinline__ bool runjoin_probe_seg(const gx_agg_dev &A, long long key, int &g,

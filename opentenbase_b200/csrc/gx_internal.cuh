@@ -413,6 +413,42 @@ __device__ __forceinline__ unsigned long long gx_next_slot(unsigned long long s,
     return (s & ~w) | ((s + 1) & w);
 }
 
+// mbarrier and bulk-async copy (TMA) helpers.  Every wait is bounded: a caller whose wait gives up raises a flag and
+// the host redoes the work with a kernel that does not stage through the copy engine, instead of hanging the device.
+#define GX_MBAR_SPIN_LIMIT (1u << 22)
+__device__ __forceinline__ unsigned int gx_smem_u32(const void *p) { return (unsigned int) __cvta_generic_to_shared(p); }
+__device__ __forceinline__ void gx_mbar_init(void *bar, unsigned int count)
+{
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(gx_smem_u32(bar)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void gx_mbar_arrive(void *bar)
+{
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(gx_smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void gx_mbar_arrive_expect_tx(void *bar, unsigned int bytes)
+{
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(gx_smem_u32(bar)), "r"(bytes) : "memory");
+}
+// false when the phase did not complete within the poll budget (try_wait itself sleeps in hardware between polls)
+__device__ __forceinline__ bool gx_mbar_wait(void *bar, unsigned int parity)
+{
+    const unsigned int a = gx_smem_u32(bar);
+#pragma unroll 1
+    for (unsigned int n = 0; n < GX_MBAR_SPIN_LIMIT; n++) {
+        unsigned int ok;
+        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+                     : "=r"(ok) : "r"(a), "r"(parity) : "memory");
+        if (ok) return true;
+    }
+    return false;
+}
+// one bulk-async copy global -> shared (16-byte aligned addresses, size a multiple of 16); completion is counted on `bar`
+__device__ __forceinline__ void gx_bulk_g2s(void *dst, const void *src, unsigned int bytes, void *bar)
+{
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 :: "r"(gx_smem_u32(dst)), "l"(src), "r"(bytes), "r"(gx_smem_u32(bar)) : "memory");
+}
+
 // Copy K selected rows of one column (row r[j] -> position dst[j]): the K loads are independent and issued together,
 // the type is decoded once per column instead of once per row (projection / compaction / scatter kernels).
 template <int K>

@@ -314,6 +314,11 @@ __global__ void __launch_bounds__(BP_THREADS, 2) gx_k_bpart2(gx_bpart_args a)
 // the sub-table wrap to its start; they are rare and go through a CAS loop afterwards.
 // Any prober that walks from slot(key) to the right (gx_next_slot) finds every key before
 // it meets an empty slot, exactly as with CAS insertion.
+// The caller's LOAD hands over row i: from the bucket pairs (gx_k_bbuild_fill), straight from the
+// columns (gx_k_sorted_fill), or from the shared-memory stage the copy engine filled while the
+// previous sub-table was built (gx_k_sorted_fill_staged, which puts its two stages behind this struct).
+// The finished sub-table leaves with plain 16-byte stores; the trailing barrier frees the table, the
+// histogram and the caller's rows for the next sub-table.
 #define FILL_THREADS 256
 #define FILL_ROWS (GX_SUB / FILL_THREADS)          // rows (and slots) per thread
 template <bool C> struct gx_fill_smem_t {
@@ -546,9 +551,9 @@ __global__ void __launch_bounds__(256) gx_k_sorted_bounds_i8(const long long *__
     if (__any_sync(0xffffffffu, bad) && lane == 0) *unsorted = 1;
 }
 
-// PK selects the row loader: 0 generic (any key type, NULLs, build-side quals, packed payload),
-// 1 = int8 key without NULLs or quals + one 4-byte payload column, 2 = the same without payload
-template <int PK, bool C, bool VERIFY>
+// The generic row loader (any key type, NULLs, build-side quals, packed payload); in the VERIFY form an int8 key
+// without NULLs.  The shapes of a plain key + one 4-byte column (or none) go to gx_k_sorted_fill_staged below.
+template <bool C, bool VERIFY>
 __global__ void __launch_bounds__(FILL_THREADS, C ? 5 : 4) gx_k_sorted_fill(gx_bbuild_args a)      // 5 CTAs/SM
 {
     extern __shared__ __align__(16) unsigned char fill_smem_raw[];
@@ -559,31 +564,23 @@ __global__ void __launch_bounds__(FILL_THREADS, C ? 5 : 4) gx_k_sorted_fill(gx_b
     unsigned int steps = 0, placed = 0;
     int bad = 0;
     const long long *keys = (const long long *) a.b.key.data;
-    const unsigned int *pay4 = (const unsigned int *) a.b.payload[0].data;
     long long lo = 0, hi = 0;
     if (blockIdx.x < a.nsub) { lo = a.start[blockIdx.x]; hi = a.start[blockIdx.x + 1]; }
     for (long long sub = blockIdx.x; sub < a.nsub; sub += gridDim.x) {
-        // the next sub-table's row range: fetch its bounds now and pull its rows towards L2
-        // while this one is being built
         long long nlo = 0, nhi = 0;
         const long long nsubn = sub + gridDim.x;
         if (nsubn < a.nsub) { nlo = a.start[nsubn]; nhi = a.start[nsubn + 1]; }
         unsigned int n = (unsigned int) (hi - lo);
         if (hi - lo >= GX_SUB) { n = 0; if (threadIdx.x == 0) *a.overflow = 1; }     // a sub-table keeps one slot free
         if (VERIFY && hi < lo) { n = 0; bad = 1; }
-        if (PK != 0 && nhi - nlo <= GX_SUB) {
-            const long long l = nlo + (long long) threadIdx.x * 16;          // 16 keys = one 128-byte line
-            if (l < nhi) asm volatile("prefetch.global.L2 [%0];" :: "l"(keys + l));
-            if (PK == 1) { const long long l4 = nlo + (long long) threadIdx.x * 32; if (l4 < nhi) asm volatile("prefetch.global.L2 [%0];" :: "l"(pay4 + l4)); }
-        }
-        if (PK == 0 && !VERIFY)
+        if (!VERIFY)
             gx_subtable_build<C>(sm, n, a.b.sf,
                               [&](unsigned int i, long long &k, unsigned long long &p) {
                                   long long r = lo + i;
                                   if (!build_row_ok(a.b, r)) return false;
                                   k = gx_load_int(a.b.key, r); p = pack_payload(a.b, r); return true; },
                               (char *) out + (size_t) sub * GX_SUB * slot_bytes, steps, placed);
-        else if (PK == 0)                                      // int8 key without NULLs; quals and any payload
+        else                                                   // int8 key without NULLs; quals and any payload
             gx_subtable_build<C>(sm, n, a.b.sf,
                               [&](unsigned int i, long long &k, unsigned long long &p) {
                                   const long long r = lo + i;
@@ -593,25 +590,93 @@ __global__ void __launch_bounds__(FILL_THREADS, C ? 5 : 4) gx_k_sorted_fill(gx_b
                                   if (!build_row_ok(a.b, r)) return false;
                                   p = pack_payload(a.b, r); return true; },
                               (char *) out + (size_t) sub * GX_SUB * slot_bytes, steps, placed, sub, &bad);
-        else if (!VERIFY)
-            gx_subtable_build<C>(sm, n, a.b.sf,
-                              [&](unsigned int i, long long &k, unsigned long long &p) {
-                                  k = __ldg(keys + lo + i);
-                                  p = PK == 1 ? (unsigned long long) __ldg(pay4 + lo + i) : (unsigned long long) (lo + i);
-                                  return true; },
-                              (char *) out + (size_t) sub * GX_SUB * slot_bytes, steps, placed);
-        else
-            gx_subtable_build<C>(sm, n, a.b.sf,
-                              [&](unsigned int i, long long &k, unsigned long long &p) {
-                                  const long long r = lo + i;
-                                  k = __ldg(keys + r);
-                                  const long long kp = r > 0 ? __ldg(keys + r - 1) : k;    // the neighbour's load: an L1 hit
-                                  if (kp > k || k == GX_EMPTY_KEY) bad = 1;
-                                  p = PK == 1 ? (unsigned long long) __ldg(pay4 + r) : (unsigned long long) r;
-                                  return true; },
-                              (char *) out + (size_t) sub * GX_SUB * slot_bytes, steps, placed, sub, &bad);
         lo = nlo; hi = nhi;
     }
+    if (VERIFY && bad) *a.unsorted = 1;
+    fill_report(a.b, steps, placed);
+}
+
+// ---------------------------------------------------------------------------
+// The key-ordered fill for the loader shapes of a table kept in primary-key order (TPC-H orders):
+// PK 1 = an int8 key without NULLs or quals + one 4-byte payload column, PK 2 = the same key, payload = row number.
+// Persistent: CTA b owns the contiguous block of sub-tables [nsub b / grid, nsub (b + 1) / grid), so its input is one
+// contiguous row range and its output one contiguous piece of the table.  The rows of a sub-table never pass through
+// a global load in the row loop: thread 0 copies them into a two-deep stage ring with cp.async.bulk (completion counted
+// on the stage's mbarrier) two sub-tables ahead, so the copy of sub-table s + 1 travels while s is histogrammed,
+// scanned and placed.  A stage holds a 16-byte aligned superset of the key range including the row before it (the
+// order check's predecessor) and of the payload range; the rounding reads at most 15 bytes past a column's last row,
+// inside the last row's 16-byte block.  The finished sub-table leaves with plain 16-byte stores, which the CTA does
+// not wait for.  Checks, flags and chain counters are those of gx_k_sorted_fill; a wait that gives up raises bit 2 of
+// *overflow and the host rebuilds with gx_k_sorted_fill.
+#define FSTAGE_KEYS (GX_SUB + 4)                   // rows [lo - 1, hi) rounded out to even rows: at most 2047 + 3
+#define FSTAGE_PAYS (GX_SUB + 8)                   // rows [lo, hi) rounded out to multiples of 4: at most 2047 + 6
+template <int PK> struct __align__(16) gx_fill_stage {
+    long long key[FSTAGE_KEYS];
+    unsigned int pay[PK == 1 ? FSTAGE_PAYS : 4];
+    unsigned long long bar;
+    long long lo, hi;                              // the staged sub-table's row range, written by thread 0 before its arrive
+};
+template <int PK, bool C> constexpr int staged_smem_bytes() { return (int) (sizeof(gx_fill_smem_t<C>) + 2 * sizeof(gx_fill_stage<PK>)); }
+
+template <int PK, bool C, bool VERIFY>
+__global__ void __launch_bounds__(FILL_THREADS, C ? 3 : 2) gx_k_sorted_fill_staged(gx_bbuild_args a)      // what shared memory allows
+{
+    extern __shared__ __align__(16) unsigned char fill_smem_raw[];
+    gx_fill_smem_t<C> &sm = *(gx_fill_smem_t<C> *) fill_smem_raw;
+    gx_fill_stage<PK> *const stage = (gx_fill_stage<PK> *) (fill_smem_raw + sizeof(gx_fill_smem_t<C>));
+    void *const out = C ? (void *) a.cslots : (void *) a.b.slots;
+    const size_t slot_bytes = C ? sizeof(gx_cslot) : sizeof(gx_slot);
+    if (!VERIFY && *a.unsorted) return;
+    const long long s0 = a.nsub * blockIdx.x / gridDim.x, s1 = a.nsub * (blockIdx.x + 1) / gridDim.x;
+    const long long *keys = (const long long *) a.b.key.data;
+    const unsigned int *pay4 = (const unsigned int *) a.b.payload[0].data;
+    // thread 0: stage the rows of sub-table s.  An empty or overflowing range stages nothing and completes the phase at once.
+    auto issue = [&](long long s, gx_fill_stage<PK> &st) {
+        const long long lo = a.start[s], hi = a.start[s + 1];
+        st.lo = lo; st.hi = hi;
+        if (hi <= lo || hi - lo >= GX_SUB) { gx_mbar_arrive(&st.bar); return; }
+        const long long k0 = (lo > 0 ? lo - 1 : 0) & ~1LL, k1 = (hi + 1) & ~1LL;
+        const long long p0 = lo & ~3LL, p1 = (hi + 3) & ~3LL;
+        const unsigned int kb = (unsigned int) (k1 - k0) * 8u, pb = PK == 1 ? (unsigned int) (p1 - p0) * 4u : 0u;
+        // the CTA's generic-proxy reads of the stage's previous rows are ordered before the copy engine's writes
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        gx_mbar_arrive_expect_tx(&st.bar, kb + pb);
+        gx_bulk_g2s(st.key, keys + k0, kb, &st.bar);
+        if (PK == 1) gx_bulk_g2s(st.pay, pay4 + p0, pb, &st.bar);
+    };
+    if (threadIdx.x == 0) {
+        gx_mbar_init(&stage[0].bar, 1); gx_mbar_init(&stage[1].bar, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        if (s0 < s1) issue(s0, stage[0]);
+        if (s0 + 1 < s1) issue(s0 + 1, stage[1]);
+    }
+    __syncthreads();
+    unsigned int steps = 0, placed = 0;
+    int bad = 0;
+    bool stuck = false;
+    for (long long s = s0; s < s1; s++) {
+        gx_fill_stage<PK> &st = stage[(s - s0) & 1];
+        if (__syncthreads_or(!gx_mbar_wait(&st.bar, (unsigned int) ((s - s0) >> 1) & 1u))) { stuck = true; break; }
+        const long long lo = st.lo, hi = st.hi;
+        unsigned int n = (unsigned int) (hi - lo);
+        if (hi - lo >= GX_SUB) { n = 0; if (threadIdx.x == 0) atomicOr(a.overflow, 1); }       // a sub-table keeps one slot free
+        if (hi < lo) { n = 0; bad = 1; }
+        const long long *sk = st.key + (lo - ((lo > 0 ? lo - 1 : 0) & ~1LL));                 // row lo; sk[-1] is row lo - 1
+        const unsigned int *sp = st.pay + (lo & 3);
+        gx_subtable_build<C>(sm, n, a.b.sf,
+                          [&](unsigned int i, long long &k, unsigned long long &p) {
+                              k = sk[i];
+                              if (VERIFY) {
+                                  const long long kp = lo + i > 0 ? sk[(int) i - 1] : k;
+                                  if (kp > k || k == GX_EMPTY_KEY) bad = 1;
+                              }
+                              p = PK == 1 ? (unsigned long long) sp[i] : (unsigned long long) (lo + i);
+                              return true; },
+                          (char *) out + (size_t) s * GX_SUB * slot_bytes, steps, placed, VERIFY ? s : -1, &bad);
+        // gx_subtable_build ends with a barrier: nobody reads this stage any more
+        if (threadIdx.x == 0 && s + 2 < s1) issue(s + 2, st);
+    }
+    if (stuck && threadIdx.x == 0) atomicOr(a.overflow, 2);
     if (VERIFY && bad) *a.unsorted = 1;
     fill_report(a.b, steps, placed);
 }
@@ -756,6 +821,30 @@ static void gx_set_interpolation(gx_hash *h, long long kmin, double range_d)
     h->scale = sc >= 18446744073709551615.0L ? ~0ULL : (unsigned long long) sc;
 }
 
+// The fill of the key-ordered build.  pk 1 / 2: gx_k_sorted_fill_staged, one resident grid; pk 0 (and the rebuild after
+// a staged wait gave up): gx_k_sorted_fill.  The second profile name tells which one ran.
+template <int PK, bool C, bool VERIFY> static void sorted_fill_staged(gx_ctx *ctx, const gx_bbuild_args &ba)
+{
+    static int per_sm = 0;
+    if (!per_sm) {
+        cudaFuncSetAttribute(gx_k_sorted_fill_staged<PK, C, VERIFY>, cudaFuncAttributeMaxDynamicSharedMemorySize, staged_smem_bytes<PK, C>());
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gx_k_sorted_fill_staged<PK, C, VERIFY>, FILL_THREADS,
+                                                          staged_smem_bytes<PK, C>()) != cudaSuccess || per_sm < 1) per_sm = 1;
+    }
+    gx_launch_scope which(ctx, "build_fill_staged", 0);
+    gx_k_sorted_fill_staged<PK, C, VERIFY><<<per_sm * ctx->sm_count, FILL_THREADS, staged_smem_bytes<PK, C>(), ctx->stream>>>(ba);
+}
+template <bool C, bool VERIFY> static void sorted_fill(gx_ctx *ctx, const gx_bbuild_args &ba, int pk)
+{
+    if (pk == 1) { sorted_fill_staged<1, C, VERIFY>(ctx, ba); return; }
+    if (pk == 2) { sorted_fill_staged<2, C, VERIFY>(ctx, ba); return; }
+    const int bytes = C ? FILL_SMEM_BYTES_C : FILL_SMEM_BYTES;
+    static bool attr = false;
+    if (!attr) { cudaFuncSetAttribute(gx_k_sorted_fill<C, VERIFY>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes); attr = true; }
+    gx_launch_scope which(ctx, "build_fill_rows", 0);
+    gx_k_sorted_fill<C, VERIFY><<<ctx->sm_count * (C ? 10 : 8), FILL_THREADS, bytes, ctx->stream>>>(ba);
+}
+
 extern "C" int gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col, int n_preds, const gx_pred *preds,
                              int n_payload, const int32_t *payload_cols, int unique, gx_hash **out)
 {
@@ -895,36 +984,19 @@ extern "C" int gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col, in
                 if (compact && gx_tmp_alloc(ctx, (void **) &h->cslots, (size_t) h->nslots * sizeof(gx_cslot)) != cudaSuccess) { h->cslots = nullptr; compact = false; }
                 h->amask = compact ? 3u : 1u; h->cspan = compact ? (unsigned long long) (kmax - kmin) + 1ULL : 0ULL;
                 a.sf.amask = h->amask; ba.b = a; ba.cslots = h->cslots;
-                static bool sattr = false;
-                if (!sattr) {
-                    cudaFuncSetAttribute(gx_k_sorted_fill<0, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, FILL_SMEM_BYTES);
-                    cudaFuncSetAttribute(gx_k_sorted_fill<1, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, FILL_SMEM_BYTES);
-                    cudaFuncSetAttribute(gx_k_sorted_fill<2, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, FILL_SMEM_BYTES);
-                    cudaFuncSetAttribute(gx_k_sorted_fill<1, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, FILL_SMEM_BYTES_C);
-                    cudaFuncSetAttribute(gx_k_sorted_fill<2, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, FILL_SMEM_BYTES_C);
-                    sattr = true;
-                }
+                // the staged fill copies 16-byte aligned blocks of the key and payload columns
+                if (pk != 0 && (((uintptr_t) a.key.data & 15) != 0 || (pk == 1 && ((uintptr_t) a.payload[0].data & 15) != 0))) pk = 0;
+                auto fill = [&](int use_pk) {
+                    if (searched) { if (compact) sorted_fill<true, true>(ctx, ba, use_pk); else sorted_fill<false, true>(ctx, ba, use_pk); }
+                    else if (compact) sorted_fill<true, false>(ctx, ba, use_pk);
+                    else sorted_fill<false, false>(ctx, ba, use_pk);
+                };
                 if (searched) {
-                    static bool fattr = false;
-                    if (!fattr) {
-                        cudaFuncSetAttribute(gx_k_sorted_fill<0, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FILL_SMEM_BYTES);
-                        cudaFuncSetAttribute(gx_k_sorted_fill<0, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FILL_SMEM_BYTES_C);
-                        cudaFuncSetAttribute(gx_k_sorted_fill<1, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FILL_SMEM_BYTES);
-                        cudaFuncSetAttribute(gx_k_sorted_fill<2, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FILL_SMEM_BYTES);
-                        cudaFuncSetAttribute(gx_k_sorted_fill<1, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FILL_SMEM_BYTES_C);
-                        cudaFuncSetAttribute(gx_k_sorted_fill<2, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FILL_SMEM_BYTES_C);
-                        fattr = true;
-                    }
                     { gx_launch_scope ls(ctx, "build_bounds"); gx_k_sorted_bounds_search<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>((const long long *) a.key.data, inner->nrows, a.sf, ba.nsub, h->nslots, d_start); }
                     gx_launch_scope ls(ctx, "build");
                     gx_launch_scope path(ctx, "build_sorted_search", 0);           // second profile names: which build path ran
                     gx_launch_scope form(ctx, compact ? "build_compact" : nullptr, 0);
-                    if (compact && pk == 1) gx_k_sorted_fill<1, true, true><<<ctx->sm_count * 10, FILL_THREADS, FILL_SMEM_BYTES_C, ctx->stream>>>(ba);
-                    else if (compact && pk == 2) gx_k_sorted_fill<2, true, true><<<ctx->sm_count * 10, FILL_THREADS, FILL_SMEM_BYTES_C, ctx->stream>>>(ba);
-                    else if (compact) gx_k_sorted_fill<0, true, true><<<ctx->sm_count * 10, FILL_THREADS, FILL_SMEM_BYTES_C, ctx->stream>>>(ba);
-                    else if (pk == 1) gx_k_sorted_fill<1, false, true><<<ctx->sm_count * 8, FILL_THREADS, FILL_SMEM_BYTES, ctx->stream>>>(ba);
-                    else if (pk == 2) gx_k_sorted_fill<2, false, true><<<ctx->sm_count * 8, FILL_THREADS, FILL_SMEM_BYTES, ctx->stream>>>(ba);
-                    else gx_k_sorted_fill<0, false, true><<<ctx->sm_count * 8, FILL_THREADS, FILL_SMEM_BYTES, ctx->stream>>>(ba);
+                    fill(pk);
                 } else {
                     {
                         gx_launch_scope ls(ctx, "build_bounds");
@@ -938,17 +1010,27 @@ extern "C" int gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col, in
                         gx_launch_scope path(ctx, "build_sorted_pass", 0);
                         gx_launch_scope form(ctx, compact ? "build_compact" : nullptr, 0);
                         gx_k_sorted_special<<<1, 256, 0, ctx->stream>>>(a, d_start, d_flag);
-                        const unsigned int fgrid = ctx->sm_count * 8;
-                        if (compact && pk == 1) gx_k_sorted_fill<1, true, false><<<ctx->sm_count * 10, FILL_THREADS, FILL_SMEM_BYTES_C, ctx->stream>>>(ba);
-                        else if (compact) gx_k_sorted_fill<2, true, false><<<ctx->sm_count * 10, FILL_THREADS, FILL_SMEM_BYTES_C, ctx->stream>>>(ba);
-                        else if (pk == 1) gx_k_sorted_fill<1, false, false><<<fgrid, FILL_THREADS, FILL_SMEM_BYTES, ctx->stream>>>(ba);
-                        else if (pk == 2) gx_k_sorted_fill<2, false, false><<<fgrid, FILL_THREADS, FILL_SMEM_BYTES, ctx->stream>>>(ba);
-                        else gx_k_sorted_fill<0, false, false><<<fgrid, FILL_THREADS, FILL_SMEM_BYTES, ctx->stream>>>(ba);
+                        fill(pk);
                     }
                 }
                 cudaError_t e2 = cudaGetLastError();
                 if (e2 == cudaSuccess) e2 = cudaMemcpyAsync(ctx->h_scratch, ctx->d_scratch, 8 * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream);
                 if (e2 == cudaSuccess) e2 = cudaStreamSynchronize(ctx->stream);
+                if (e2 == cudaSuccess && pk != 0 && ((int) ctx->h_scratch[7] & 2)) {
+                    // a bounded wait of the staged fill gave up: the same build with the generic row loader
+                    fprintf(stderr, "gpuexec: a bounded mbarrier wait of gx_k_sorted_fill_staged gave up; rebuilding with gx_k_sorted_fill\n");
+                    cudaMemsetAsync(ctx->d_scratch + 3, 0, sizeof(long long), ctx->stream);
+                    cudaMemsetAsync(ctx->d_scratch + 5, 0, 3 * sizeof(long long), ctx->stream);      // [5] steps, [6] unsorted, [7] overflow
+                    {
+                        gx_launch_scope ls(ctx, "build");
+                        gx_launch_scope path(ctx, searched ? "build_sorted_search" : "build_sorted_pass", 0);
+                        gx_launch_scope form(ctx, compact ? "build_compact" : nullptr, 0);
+                        fill(0);
+                    }
+                    e2 = cudaGetLastError();
+                    if (e2 == cudaSuccess) e2 = cudaMemcpyAsync(ctx->h_scratch, ctx->d_scratch, 8 * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream);
+                    if (e2 == cudaSuccess) e2 = cudaStreamSynchronize(ctx->stream);
+                }
                 gx_tmp_free(ctx, d_start);
                 if (e2 != cudaSuccess) { GX_SET_ERR(ctx, "hash_build: %s", cudaGetErrorString(e2)); return GX_ERR_CUDA; }
                 if ((int) ctx->h_scratch[6] == 0) {
