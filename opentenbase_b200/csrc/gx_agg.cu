@@ -41,6 +41,7 @@ struct gx_agg_dev {
     // join table
     const gx_slot *slots; unsigned long long mask;
     const gx_cslot *cslots; unsigned long long cspan;      // compact form of the table (gx_k_runjoin reads it directly)
+    const unsigned int *narrow;                            // narrow form (gx_nslot_*), same cspan
     const unsigned long long *special; int special_count; int _pad0; gx_slotfn sf;
     long long row0, row1;
     // shared-memory table
@@ -1112,11 +1113,18 @@ struct gx_runlist { long long key[128]; double sum[128]; unsigned int cnt[128]; 
 // Branch-free inside the group: a table that is only ever filled (never deleted from) has no
 // match behind an empty slot, so "any slot matches" / "any slot empty" decide the step, and the
 // function has ONE exit (several exits made the compiler clone the group update per exit).
-template <bool COMPACT>
+template <int FMT>
 __device__ __forceinline__ bool runjoin_probe(const gx_agg_dev &A, long long key, int &g)
 {
     bool found = false;
-    if (COMPACT) {
+    if (FMT == GX_SLOTS_NARROW) {
+        const unsigned long long dd = (unsigned long long) key - (unsigned long long) A.sf.kmin;
+        if (dd < A.cspan) {                                    // else outside the build side's key span (also the reserved key)
+            const unsigned int tag = gx_nslot_tag(key, A.sf);
+            unsigned long long p = gx_slot_index(key, A.sf);
+            while (!gx_nslot_group(gx_nslot_ld(A.narrow + p), tag, A.sf, found, g)) p = gx_next_quad(p, A.mask);   // four 4-byte slots
+        }
+    } else if (FMT == GX_SLOTS_COMPACT) {
         const unsigned long long dd = (unsigned long long) key - (unsigned long long) A.sf.kmin;
         if (dd < A.cspan) {                                    // else outside the build side's key span (also the reserved key)
             const unsigned int d = GX_CSLOT_D(key, A.sf.kmin);
@@ -1146,7 +1154,7 @@ __device__ __forceinline__ bool runjoin_probe(const gx_agg_dev &A, long long key
     return found;
 }
 
-template <bool HAS_CNT, bool HAS_SUM, bool COMPACT>
+template <bool HAS_CNT, bool HAS_SUM, int FMT>
 __global__ void __launch_bounds__(1024, 1) gx_k_runjoin(const __grid_constant__ gx_agg_dev A, const gx_fast_args F)
 {
     extern __shared__ unsigned long long smem[];
@@ -1173,10 +1181,11 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin(const __grid_constant__ 
     // the loop is warp-uniform: lanes past the end carry no rows
     while (__any_sync(0xffffffffu, act)) {
         // ---- the join-table lines this tile's runs will read: requested now, they arrive while the runs are folded
-        if (COMPACT && F.pf && act) {
+        if (FMT != GX_SLOTS_WIDE && F.pf && act) {
             const unsigned long long dd = (unsigned long long) k[0] - (unsigned long long) A.sf.kmin;
             if (dd < A.cspan) {
-                const gx_cslot *pa = A.cslots + gx_slot_index(k[0], A.sf);
+                const unsigned long long s = gx_slot_index(k[0], A.sf);
+                const void *pa = FMT == GX_SLOTS_NARROW ? (const void *) (A.narrow + s) : (const void *) (A.cslots + s);
                 if (F.pf == 2) asm volatile("prefetch.global.L1 [%0];" :: "l"(pa)); else asm volatile("prefetch.global.L2 [%0];" :: "l"(pa));
             }
         }
@@ -1221,7 +1230,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin(const __grid_constant__ 
             const unsigned int rc = Q.cnt[j];
             const double rs = HAS_SUM ? Q.sum[j] : -0.0;
             int g = 0;
-            const bool hit = runjoin_probe<COMPACT>(A, key, g);
+            const bool hit = runjoin_probe<FMT>(A, key, g);
             if (hit) fast_flush<HAS_CNT, HAS_SUM>(T, A, g, rc, rs, F.sum_word);
         }
         __syncwarp();
@@ -1231,7 +1240,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin(const __grid_constant__ 
         long long r = A.row0 + (nvec << 2) + (long long) blockIdx.x * blockDim.x + threadIdx.x;
         if (r < A.row1) {
             int gk = 0;
-            if (runjoin_probe<COMPACT>(A, F.okey[r], gk)) fast_flush<HAS_CNT, HAS_SUM>(T, A, gk, 1u, HAS_SUM ? F.vcol[r] : -0.0, F.sum_word);
+            if (runjoin_probe<FMT>(A, F.okey[r], gk)) fast_flush<HAS_CNT, HAS_SUM>(T, A, gk, 1u, HAS_SUM ? F.vcol[r] : -0.0, F.sum_word);
         }
     }
     __syncthreads();
@@ -1258,13 +1267,24 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin(const __grid_constant__ 
 #define GX_SEG_MAXBUF      4
 struct gx_seg_ctl { unsigned long long full[GX_SEG_MAXBUF], empty[GX_SEG_MAXBUF], lo[GX_SEG_MAXBUF]; unsigned int len[GX_SEG_MAXBUF]; };
 
-// one key against the compact join table, the slot groups inside [lo, lo + len) taken from the staged copy `sg`
+// one key against the compact (FMT) join table, the slot groups inside [lo, lo + len) taken from the staged copy `sg`
+template <int FMT>
 __device__ __forceinline__ bool runjoin_probe_seg(const gx_agg_dev &A, long long key, int &g,
                                                   const unsigned long long *sg, unsigned long long lo, unsigned int len)
 {
     bool found = false;
     const unsigned long long dd = (unsigned long long) key - (unsigned long long) A.sf.kmin;
-    if (dd < A.cspan) {
+    if (FMT == GX_SLOTS_NARROW && dd < A.cspan) {
+        const unsigned int tag = gx_nslot_tag(key, A.sf);
+        unsigned long long p = gx_slot_index(key, A.sf);
+        for (;;) {
+            const unsigned long long off = p - lo;                 // p < lo wraps to a huge value
+            // lo, len and p are multiples of 4: the group is inside or outside as a whole
+            const uint4 q = off < (unsigned long long) len ? *(const uint4 *) ((const unsigned int *) sg + off) : gx_nslot_ld(A.narrow + p);
+            if (gx_nslot_group(q, tag, A.sf, found, g)) break;
+            p = gx_next_quad(p, A.mask);
+        }
+    } else if (FMT == GX_SLOTS_COMPACT && dd < A.cspan) {
         const unsigned int d = GX_CSLOT_D(key, A.sf.kmin);
         unsigned long long p = gx_slot_index(key, A.sf);
         for (;;) {
@@ -1288,7 +1308,7 @@ __device__ __forceinline__ bool runjoin_probe_seg(const gx_agg_dev &A, long long
     return found;
 }
 
-template <bool HAS_CNT, bool HAS_SUM>
+template <bool HAS_CNT, bool HAS_SUM, int FMT>
 __global__ void __launch_bounds__(1024, 1) gx_k_runjoin_seg(const __grid_constant__ gx_agg_dev A, const gx_fast_args F, const unsigned int seg_slots, const int nbuf)
 {
     extern __shared__ __align__(128) unsigned long long smem_seg[];
@@ -1348,8 +1368,10 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin_seg(const __grid_constan
                 if (!stuck) {
                     ctl->lo[b] = lo; ctl->len[b] = len;
                     if (len) {
-                        gx_mbar_arrive_expect_tx(&ctl->full[b], len * 8u);
-                        gx_bulk_g2s(seg0 + (size_t) b * seg_slots, A.cslots + lo, len * 8u, &ctl->full[b]);
+                        const unsigned int bytes = len * (FMT == GX_SLOTS_NARROW ? 4u : 8u);
+                        gx_mbar_arrive_expect_tx(&ctl->full[b], bytes);
+                        gx_bulk_g2s(seg0 + (size_t) b * seg_slots, FMT == GX_SLOTS_NARROW ? (const void *) (A.narrow + lo) : (const void *) (A.cslots + lo),
+                                    bytes, &ctl->full[b]);
                     } else gx_mbar_arrive(&ctl->full[b]);
                 }
             }
@@ -1414,7 +1436,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin_seg(const __grid_constan
                 const unsigned int rc = Q.cnt[jj];
                 const double rs = HAS_SUM ? Q.sum[jj] : -0.0;
                 int g = 0;
-                const bool hit = runjoin_probe_seg(A, key, g, sg, lo, len);
+                const bool hit = runjoin_probe_seg<FMT>(A, key, g, sg, lo, len);
                 if (hit) fast_flush<HAS_CNT, HAS_SUM>(T, A, g, rc, rs, F.sum_word);
             }
             __syncwarp();
@@ -1426,7 +1448,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin_seg(const __grid_constan
             long long r = A.row0 + (nvec << 2) + (long long) blockIdx.x * blockDim.x + threadIdx.x;
             if (r < A.row1) {
                 int gk = 0;
-                if (runjoin_probe<true>(A, F.okey[r], gk)) fast_flush<HAS_CNT, HAS_SUM>(T, A, gk, 1u, HAS_SUM ? F.vcol[r] : -0.0, F.sum_word);
+                if (runjoin_probe<FMT>(A, F.okey[r], gk)) fast_flush<HAS_CNT, HAS_SUM>(T, A, gk, 1u, HAS_SUM ? F.vcol[r] : -0.0, F.sum_word);
             }
         }
     }
@@ -1436,7 +1458,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin_seg(const __grid_constan
 }
 
 struct gx_runlist3 { long long key[160]; double sum[160]; unsigned int cnt[160]; };   // 31 waiting + 128 new runs
-template <bool HAS_CNT, bool HAS_SUM, bool COMPACT>
+template <bool HAS_CNT, bool HAS_SUM, int FMT>
 __global__ void __launch_bounds__(1024, 1) gx_k_runjoin3(const __grid_constant__ gx_agg_dev A, const gx_fast_args F)
 {
     extern __shared__ unsigned long long smem[];
@@ -1506,7 +1528,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin3(const __grid_constant__
             const unsigned int rc = Q.cnt[j];
             const double rs = HAS_SUM ? Q.sum[j] : -0.0;
             int g = 0;
-            const bool hit = runjoin_probe<COMPACT>(A, key, g);
+            const bool hit = runjoin_probe<FMT>(A, key, g);
             if (hit) fast_flush<HAS_CNT, HAS_SUM>(T, A, g, rc, rs, F.sum_word);
         }
         __syncwarp();
@@ -1519,7 +1541,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin3(const __grid_constant__
     }
     for (int j = lane; j < nl; j += 32) {                           // what was still waiting when the rows ran out
         int g = 0;
-        const bool hit = runjoin_probe<COMPACT>(A, Q.key[j], g);
+        const bool hit = runjoin_probe<FMT>(A, Q.key[j], g);
         if (hit) fast_flush<HAS_CNT, HAS_SUM>(T, A, g, Q.cnt[j], HAS_SUM ? Q.sum[j] : -0.0, F.sum_word);
     }
     __syncwarp();
@@ -1528,7 +1550,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin3(const __grid_constant__
         long long r = A.row0 + (nvec << 2) + (long long) blockIdx.x * blockDim.x + threadIdx.x;
         if (r < A.row1) {
             int gk = 0;
-            if (runjoin_probe<COMPACT>(A, F.okey[r], gk)) fast_flush<HAS_CNT, HAS_SUM>(T, A, gk, 1u, HAS_SUM ? F.vcol[r] : -0.0, F.sum_word);
+            if (runjoin_probe<FMT>(A, F.okey[r], gk)) fast_flush<HAS_CNT, HAS_SUM>(T, A, gk, 1u, HAS_SUM ? F.vcol[r] : -0.0, F.sum_word);
         }
     }
     __syncthreads();
@@ -1555,7 +1577,7 @@ __device__ __forceinline__ void packed_flush(unsigned long long *tab, double *ts
     if (HAS_SUM) atomicAdd(&tsum[s], sum);
 }
 
-template <bool HAS_SUM, bool COMPACT>
+template <bool HAS_SUM, int FMT>
 __global__ void __launch_bounds__(512, 2) gx_k_runjoin2(const __grid_constant__ gx_agg_dev A, const gx_fast_args F)
 {
     extern __shared__ unsigned long long smem[];
@@ -1621,7 +1643,7 @@ __global__ void __launch_bounds__(512, 2) gx_k_runjoin2(const __grid_constant__ 
             const unsigned int rc = Q.cnt[j];
             const double rs = HAS_SUM ? Q.sum[j] : -0.0;
             int g = 0;
-            const bool hit = runjoin_probe<COMPACT>(A, key, g);
+            const bool hit = runjoin_probe<FMT>(A, key, g);
             if (hit) packed_flush<HAS_SUM>(tab, tsum, S, A, g, rc, rs);
         }
         __syncwarp();
@@ -1631,7 +1653,7 @@ __global__ void __launch_bounds__(512, 2) gx_k_runjoin2(const __grid_constant__ 
         long long r = A.row0 + (nvec << 2) + (long long) blockIdx.x * blockDim.x + threadIdx.x;
         if (r < A.row1) {
             int gk = 0;
-            if (runjoin_probe<COMPACT>(A, F.okey[r], gk)) packed_flush<HAS_SUM>(tab, tsum, S, A, gk, 1u, HAS_SUM ? F.vcol[r] : -0.0);
+            if (runjoin_probe<FMT>(A, F.okey[r], gk)) packed_flush<HAS_SUM>(tab, tsum, S, A, gk, 1u, HAS_SUM ? F.vcol[r] : -0.0);
         }
     }
     __syncthreads();
@@ -1659,7 +1681,7 @@ __global__ void __launch_bounds__(512, 2) gx_k_runjoin2(const __grid_constant__ 
 // Bounded waits as in gx_k_runjoin_seg: flag 16 sends the plan back to gx_k_runjoin.
 struct gx_rowstage { long long key[128]; double val[128]; };
 
-template <bool HAS_SUM, bool COMPACT, bool FOLD2, bool CARRY>
+template <bool HAS_SUM, int FMT, bool FOLD2, bool CARRY>
 __global__ void __launch_bounds__(1024, 1) gx_k_runjoin_tma(const __grid_constant__ gx_agg_dev A, const gx_fast_args F)
 {
     extern __shared__ __align__(128) unsigned long long smem_tma[];
@@ -1709,7 +1731,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin_tma(const __grid_constan
         const unsigned int rc = Q.cnt[j];
         const double rs = HAS_SUM ? Q.sum[j] : -0.0;
         int g = 0;
-        const bool hit = runjoin_probe<COMPACT>(A, key, g);
+        const bool hit = runjoin_probe<FMT>(A, key, g);
         if (hit) packed_flush<HAS_SUM>(tab, tsum, S, A, g, rc, rs);
     };
     // CARRY (GX_RUNJOIN_TMA=3): probe rounds only ever run with 32 lanes.  A tile holds ~33 runs, so half the tiles pay a second
@@ -1827,7 +1849,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin_tma(const __grid_constan
         long long r = A.row0 + (nvec << 2) + (long long) blockIdx.x * blockDim.x + threadIdx.x;
         if (r < A.row1) {
             int gk = 0;
-            if (runjoin_probe<COMPACT>(A, F.okey[r], gk)) packed_flush<HAS_SUM>(tab, tsum, S, A, gk, 1u, HAS_SUM ? F.vcol[r] : -0.0);
+            if (runjoin_probe<FMT>(A, F.okey[r], gk)) packed_flush<HAS_SUM>(tab, tsum, S, A, gk, 1u, HAS_SUM ? F.vcol[r] : -0.0);
         }
     }
     __syncthreads();
@@ -2373,9 +2395,9 @@ static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
         P.n_payload = h->n_payload;
         for (int i = 0; i < h->n_payload; i++) P.payload_types[i] = h->payload_types[i];
         cp->A.slots = h->slots; cp->A.mask = (unsigned long long) h->nslots - 1;
-        cp->A.cslots = h->cslots; cp->A.cspan = h->cspan;
+        cp->A.cslots = h->cslots; cp->A.narrow = h->narrow; cp->A.cspan = h->cspan;
         cp->A.special = h->special_payload; cp->A.special_count = h->special_count;
-        cp->A.sf.mode = h->mode; cp->A.sf.win = h->win; cp->A.sf.shift = h->shift; cp->A.sf.amask = h->amask; cp->A.sf.kmin = h->kmin; cp->A.sf.scale = h->scale; cp->A.sf.mask = (unsigned long long) h->nslots - 1;
+        cp->A.sf = gx_hash_slotfn(h);
     }
     // group columns: pack by byte width into k0 then k1
     int used[2] = { 0, 0 };
@@ -2553,12 +2575,12 @@ static int launch_fast_t(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_args &F
     GX_CUDA(ctx, cudaGetLastError());
     return GX_OK;
 }
-template <bool HAS_CNT, bool HAS_SUM, bool COMPACT>
+template <bool HAS_CNT, bool HAS_SUM, int FMT>
 static int launch_runjoin_t(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_args &FA, size_t smem, const char *name)
 {
     static bool attr_set = false;
     if (!attr_set) {
-        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runjoin<HAS_CNT, HAS_SUM, COMPACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
+        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runjoin<HAS_CNT, HAS_SUM, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
         attr_set = true;
     }
     long long nvec = (A.row1 - A.row0 + 3) / 4;
@@ -2567,7 +2589,7 @@ static int launch_runjoin_t(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_args
     unsigned grid = (unsigned) (nb < maxb ? (nb > 0 ? nb : 1) : maxb);
     gx_launch_scope ls(ctx, name);
     gx_launch_scope which(ctx, "probe_agg_run", 0);
-    gx_k_runjoin<HAS_CNT, HAS_SUM, COMPACT><<<grid, 1024, smem, ctx->stream>>>(A, FA);
+    gx_k_runjoin<HAS_CNT, HAS_SUM, FMT><<<grid, 1024, smem, ctx->stream>>>(A, FA);
     GX_CUDA(ctx, cudaGetLastError());
     return GX_OK;
 }
@@ -2594,12 +2616,12 @@ static unsigned int runjoin_seg_slots(const gx_ctx *ctx, size_t table_bytes, con
     if (slots > 4096) slots = 4096;                              // 32 KB per buffer
     return (unsigned int) (slots & ~(size_t) 31);
 }
-template <bool HAS_CNT, bool HAS_SUM>
+template <bool HAS_CNT, bool HAS_SUM, int FMT>
 static int launch_runjoin_seg_t(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_args &FA, size_t table_bytes, unsigned int seg_slots, int nbuf, const char *name)
 {
     static bool attr_set = false;
     if (!attr_set) {
-        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runjoin_seg<HAS_CNT, HAS_SUM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
+        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runjoin_seg<HAS_CNT, HAS_SUM, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
         attr_set = true;
     }
     const size_t smem = table_bytes + GX_SEG_CW * sizeof(gx_runlist) + (size_t) nbuf * seg_slots * 8 + sizeof(gx_seg_ctl);
@@ -2609,16 +2631,16 @@ static int launch_runjoin_seg_t(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_
     unsigned grid = (unsigned) (nb < maxb ? (nb > 0 ? nb : 1) : maxb);
     gx_launch_scope ls(ctx, name);
     gx_launch_scope which(ctx, "probe_agg_seg", 0);              // same kernel under a second profile name: tells gx_profile_get() which variant ran
-    gx_k_runjoin_seg<HAS_CNT, HAS_SUM><<<grid, 1024, smem, ctx->stream>>>(A, FA, seg_slots, nbuf);
+    gx_k_runjoin_seg<HAS_CNT, HAS_SUM, FMT><<<grid, 1024, smem, ctx->stream>>>(A, FA, seg_slots, nbuf);
     GX_CUDA(ctx, cudaGetLastError());
     return GX_OK;
 }
-template <bool HAS_CNT, bool HAS_SUM, bool COMPACT>
+template <bool HAS_CNT, bool HAS_SUM, int FMT>
 static int launch_runjoin3_t(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_args &FA, size_t table_bytes, const char *name)
 {
     static bool attr_set = false;
     if (!attr_set) {
-        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runjoin3<HAS_CNT, HAS_SUM, COMPACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
+        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runjoin3<HAS_CNT, HAS_SUM, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
         attr_set = true;
     }
     long long nvec = (A.row1 - A.row0 + 3) / 4;
@@ -2627,18 +2649,18 @@ static int launch_runjoin3_t(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_arg
     unsigned grid = (unsigned) (nb < maxb ? (nb > 0 ? nb : 1) : maxb);
     gx_launch_scope ls(ctx, name);
     gx_launch_scope which(ctx, "probe_agg_run3", 0);
-    gx_k_runjoin3<HAS_CNT, HAS_SUM, COMPACT><<<grid, 1024, table_bytes + 32 * sizeof(gx_runlist3), ctx->stream>>>(A, FA);
+    gx_k_runjoin3<HAS_CNT, HAS_SUM, FMT><<<grid, 1024, table_bytes + 32 * sizeof(gx_runlist3), ctx->stream>>>(A, FA);
     GX_CUDA(ctx, cudaGetLastError());
     return GX_OK;
 }
-template <bool HAS_SUM, bool COMPACT>
+template <bool HAS_SUM, int FMT>
 static int launch_runjoin_tma_t(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_args &FA, size_t smem, const char *name)
 {
     static bool attr_set = false;
     if (!attr_set) {
-        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runjoin_tma<HAS_SUM, COMPACT, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
-        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runjoin_tma<HAS_SUM, COMPACT, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
-        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runjoin_tma<HAS_SUM, COMPACT, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
+        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runjoin_tma<HAS_SUM, FMT, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
+        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runjoin_tma<HAS_SUM, FMT, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
+        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runjoin_tma<HAS_SUM, FMT, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
         attr_set = true;
     }
     const char *fv = getenv("GX_RUNJOIN_TMA");
@@ -2649,19 +2671,21 @@ static int launch_runjoin_tma_t(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_
     unsigned grid = (unsigned) (nb < maxb ? (nb > 0 ? nb : 1) : maxb);
     gx_launch_scope ls(ctx, name);
     gx_launch_scope which(ctx, "probe_agg_tma", 0);              // second profile name: which variant ran
-    if (variant == 3) gx_k_runjoin_tma<HAS_SUM, COMPACT, true, true><<<grid, 1024, smem, ctx->stream>>>(A, FA);
-    else if (variant == 2) gx_k_runjoin_tma<HAS_SUM, COMPACT, true, false><<<grid, 1024, smem, ctx->stream>>>(A, FA);
-    else gx_k_runjoin_tma<HAS_SUM, COMPACT, false, false><<<grid, 1024, smem, ctx->stream>>>(A, FA);
+    if (variant == 3) gx_k_runjoin_tma<HAS_SUM, FMT, true, true><<<grid, 1024, smem, ctx->stream>>>(A, FA);
+    else if (variant == 2) gx_k_runjoin_tma<HAS_SUM, FMT, true, false><<<grid, 1024, smem, ctx->stream>>>(A, FA);
+    else gx_k_runjoin_tma<HAS_SUM, FMT, false, false><<<grid, 1024, smem, ctx->stream>>>(A, FA);
     GX_CUDA(ctx, cudaGetLastError());
     return GX_OK;
 }
-template <bool HAS_SUM, bool COMPACT>
+template <bool HAS_SUM, int FMT>
 static int launch_runjoin2_t(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_args &FA, const char *name)
 {
     static bool attr_set = false;
     const size_t smem = (size_t) A.s_slots * 16 + 16 * sizeof(gx_runlist);
     if (!attr_set) {
-        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runjoin2<HAS_SUM, COMPACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem > 100 * 1024 ? (int) smem : 100 * 1024));
+        // once per instantiation, so for the largest group table launch_fast hands it (4096 slots), not the first caller's
+        const int smem_max = (int) (4096 * 16 + 16 * sizeof(gx_runlist));
+        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runjoin2<HAS_SUM, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
         attr_set = true;
     }
     long long nvec = (A.row1 - A.row0 + 3) / 4;
@@ -2670,7 +2694,7 @@ static int launch_runjoin2_t(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_arg
     unsigned grid = (unsigned) (nb < maxb ? (nb > 0 ? nb : 1) : maxb);
     gx_launch_scope ls(ctx, name);
     gx_launch_scope which(ctx, "probe_agg_run2", 0);
-    gx_k_runjoin2<HAS_SUM, COMPACT><<<grid, 512, smem, ctx->stream>>>(A, FA);
+    gx_k_runjoin2<HAS_SUM, FMT><<<grid, 512, smem, ctx->stream>>>(A, FA);
     GX_CUDA(ctx, cudaGetLastError());
     return GX_OK;
 }
@@ -2691,30 +2715,35 @@ static bool gx_runjoin_tma_enabled()
     const char *e = getenv("GX_RUNJOIN_TMA");
     return e && e[0] ? e[0] != '0' : GX_RUNJOIN_TMA_DEFAULT != 0;
 }
+// calls fn with the slot format of the plan's join table as a compile-time constant (std::integral_constant)
+template <class FN> static int with_slot_format(const gx_agg_dev &A, FN fn)
+{
+    if (A.narrow) return fn(std::integral_constant<int, GX_SLOTS_NARROW>());
+    if (A.cslots) return fn(std::integral_constant<int, GX_SLOTS_COMPACT>());
+    return fn(std::integral_constant<int, GX_SLOTS_WIDE>());
+}
 static int launch_fast(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_args &FA, bool join, bool cnt, bool sum, size_t smem, const char *name, bool use_run)
 {
     // gx_k_runjoin3: finished runs wait for a full round of 32 (GX_RUNJOIN_CARRY=1; A/B against gx_k_runjoin)
     {
         const char *cv = getenv("GX_RUNJOIN_CARRY");
-        if (use_run && cv && cv[0] == '1' && smem + 32 * sizeof(gx_runlist3) <= ctx->smem_optin - 1024) {
-            if (A.cslots) {
-                if (cnt && sum) return launch_runjoin3_t<true, true, true>(ctx, A, FA, smem, name);
-                if (cnt) return launch_runjoin3_t<true, false, true>(ctx, A, FA, smem, name);
-                return launch_runjoin3_t<false, true, true>(ctx, A, FA, smem, name);
-            }
-            if (cnt && sum) return launch_runjoin3_t<true, true, false>(ctx, A, FA, smem, name);
-            if (cnt) return launch_runjoin3_t<true, false, false>(ctx, A, FA, smem, name);
-            return launch_runjoin3_t<false, true, false>(ctx, A, FA, smem, name);
-        }
+        if (use_run && cv && cv[0] == '1' && smem + 32 * sizeof(gx_runlist3) <= ctx->smem_optin - 1024)
+            return with_slot_format(A, [&](auto f) {
+                constexpr int F = decltype(f)::value;
+                if (cnt && sum) return launch_runjoin3_t<true, true, F>(ctx, A, FA, smem, name);
+                if (cnt) return launch_runjoin3_t<true, false, F>(ctx, A, FA, smem, name);
+                return launch_runjoin3_t<false, true, F>(ctx, A, FA, smem, name);
+            });
     }
     // gx_k_runjoin2: two CTAs of 512 threads per SM with 16-byte group slots (64 KB + 40 KB of run lists) instead of
     // one CTA of 1024 threads with 24-byte slots; opt-in behind GX_RUNJOIN_V2=1.
     {
         const char *v2 = getenv("GX_RUNJOIN_V2");
-        if (use_run && v2 && v2[0] == '1' && A.s_slots <= 4096) {
-            if (A.cslots) return sum ? launch_runjoin2_t<true, true>(ctx, A, FA, name) : launch_runjoin2_t<false, true>(ctx, A, FA, name);
-            return sum ? launch_runjoin2_t<true, false>(ctx, A, FA, name) : launch_runjoin2_t<false, false>(ctx, A, FA, name);
-        }
+        if (use_run && v2 && v2[0] == '1' && A.s_slots <= 4096)
+            return with_slot_format(A, [&](auto f) {
+                constexpr int F = decltype(f)::value;
+                return sum ? launch_runjoin2_t<true, F>(ctx, A, FA, name) : launch_runjoin2_t<false, F>(ctx, A, FA, name);
+            });
     }
     // the run-folding join kernel keeps a per-warp run list next to the group table
     const size_t run_bytes = 32 * sizeof(gx_runlist);
@@ -2722,31 +2751,32 @@ static int launch_fast(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_args &FA,
     if (use_run && gx_runjoin_tma_enabled() && A.s_slots <= 4096 && (A.row0 & 1) == 0 &&
         ((uintptr_t) FA.okey & 15) == 0 && ((uintptr_t) FA.vcol & 15) == 0) {
         const size_t tma_smem = (size_t) A.s_slots * 16 + 32 * sizeof(gx_runlist) + 32 * sizeof(gx_rowstage) + 32 * 8;
-        if (tma_smem + 1024 <= ctx->smem_optin) {
-            if (A.cslots) return sum ? launch_runjoin_tma_t<true, true>(ctx, A, FA, tma_smem, name) : launch_runjoin_tma_t<false, true>(ctx, A, FA, tma_smem, name);
-            return sum ? launch_runjoin_tma_t<true, false>(ctx, A, FA, tma_smem, name) : launch_runjoin_tma_t<false, false>(ctx, A, FA, tma_smem, name);
-        }
+        if (tma_smem + 1024 <= ctx->smem_optin)
+            return with_slot_format(A, [&](auto f) {
+                constexpr int F = decltype(f)::value;
+                return sum ? launch_runjoin_tma_t<true, F>(ctx, A, FA, tma_smem, name) : launch_runjoin_tma_t<false, F>(ctx, A, FA, tma_smem, name);
+            });
     }
     // compact table + order-preserving slots: the streamed-table variant (gx_k_runjoin_seg)
-    if (use_run && A.cslots && A.sf.mode != 0 && gx_runjoin_seg_enabled()) {
+    if (use_run && (A.cslots || A.narrow) && A.sf.mode != 0 && gx_runjoin_seg_enabled()) {
         int nbuf = 2;
         const unsigned int seg_slots = runjoin_seg_slots(ctx, smem, A, &nbuf);
-        if (seg_slots >= 512) {
-            if (cnt && sum) return launch_runjoin_seg_t<true, true>(ctx, A, FA, smem, seg_slots, nbuf, name);
-            if (cnt) return launch_runjoin_seg_t<true, false>(ctx, A, FA, smem, seg_slots, nbuf, name);
-            return launch_runjoin_seg_t<false, true>(ctx, A, FA, smem, seg_slots, nbuf, name);
-        }
+        auto seg = [&](auto f) {
+            constexpr int F = decltype(f)::value;
+            if (cnt && sum) return launch_runjoin_seg_t<true, true, F>(ctx, A, FA, smem, seg_slots, nbuf, name);
+            if (cnt) return launch_runjoin_seg_t<true, false, F>(ctx, A, FA, smem, seg_slots, nbuf, name);
+            return launch_runjoin_seg_t<false, true, F>(ctx, A, FA, smem, seg_slots, nbuf, name);
+        };
+        if (seg_slots >= 512)
+            return A.narrow ? seg(std::integral_constant<int, GX_SLOTS_NARROW>()) : seg(std::integral_constant<int, GX_SLOTS_COMPACT>());
     }
-    if (use_run) {
-        if (A.cslots) {
-            if (cnt && sum) return launch_runjoin_t<true, true, true>(ctx, A, FA, smem + run_bytes, name);
-            if (cnt) return launch_runjoin_t<true, false, true>(ctx, A, FA, smem + run_bytes, name);
-            return launch_runjoin_t<false, true, true>(ctx, A, FA, smem + run_bytes, name);
-        }
-        if (cnt && sum) return launch_runjoin_t<true, true, false>(ctx, A, FA, smem + run_bytes, name);
-        if (cnt) return launch_runjoin_t<true, false, false>(ctx, A, FA, smem + run_bytes, name);
-        return launch_runjoin_t<false, true, false>(ctx, A, FA, smem + run_bytes, name);
-    }
+    if (use_run)
+        return with_slot_format(A, [&](auto f) {
+            constexpr int F = decltype(f)::value;
+            if (cnt && sum) return launch_runjoin_t<true, true, F>(ctx, A, FA, smem + run_bytes, name);
+            if (cnt) return launch_runjoin_t<true, false, F>(ctx, A, FA, smem + run_bytes, name);
+            return launch_runjoin_t<false, true, F>(ctx, A, FA, smem + run_bytes, name);
+        });
     if (join) {
         if (cnt && sum) return launch_fast_t<true, true, true>(ctx, A, FA, smem, name);
         if (cnt) return launch_fast_t<true, true, false>(ctx, A, FA, smem, name);
@@ -3033,8 +3063,8 @@ static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
         const bool use_few = strategy == 1 && gmax && fewgroups_ok && est <= 2 * FG_G;
         { const char *dbg = getenv("GX_DEBUG_AGG");
           if (dbg && dbg[0] == '1')
-              fprintf(stderr, "gpuexec: hash_agg attempt %d strategy %d S %lld gmax %d fast_ok %d use_fast %d use_run %d cslots %d slot mode %d seg %d tma %d rows %lld\n",
-                      attempt, strategy, S, gmax, (int) fast_ok, (int) use_fast, (int) use_run, A.cslots != nullptr, A.sf.mode,
+              fprintf(stderr, "gpuexec: hash_agg attempt %d strategy %d S %lld gmax %d fast_ok %d use_fast %d use_run %d cslots %d narrow %d slot mode %d seg %d tma %d rows %lld\n",
+                      attempt, strategy, S, gmax, (int) fast_ok, (int) use_fast, (int) use_run, A.cslots != nullptr, A.narrow != nullptr, A.sf.mode,
                       (int) gx_runjoin_seg_enabled(), (int) gx_runjoin_tma_enabled(), (long long) outer->nrows); }
         if (use_fast) rc = launch_fast(ctx, A, FA, A.P.has_join != 0, cp.need_w0 != 0, FA.vcol != nullptr, dense_bytes(S), kname, use_run);
         else if (use_few && countchar_ok) {

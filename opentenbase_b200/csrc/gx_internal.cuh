@@ -74,6 +74,32 @@ struct gx_slot { long long key; unsigned long long payload; };   // 16 B
 // 31-bit compare).
 #define GX_CSLOT_D(key, kmin) ((unsigned int) (((((unsigned long long) (key)) - ((unsigned long long) (kmin))) << 1) | 1ULL))
 struct gx_cslot { unsigned int d; unsigned int payload; };
+// Narrow slot (4 B): one uint32 w = tag | (payload - pbase) << tbits with tag = ((key - kmin) mod 2^(tbits-1)) << 1 | 1,
+// so an occupied slot is never 0, which marks an empty one.  It serves the key-ordered build of an int8 key with one
+// 4-byte payload column whose values span at most 2^pbits, pbits = 32 - tbits (o_orderdate: 2406 days).  tbits is the
+// smallest width with 2^(tbits-1) >= 4 (keys_per_slot GX_SUB + 64) (gx_nslot_tbits):
+//  * probes never leave their home sub-table, and the keys that home in one sub-table lie within keys_per_slot GX_SUB
+//    (+ under 64 of interpolation rounding) of each other, so two different keys that can meet there differ by less
+//    than the tag modulus 2^(tbits-1) and never share a tag;
+//  * reconstruction (gx_k_expand_slots): an entry in slot i homes in the same sub-table, so its key offset lies within
+//    one sub-table's key span of i keys_per_slot, at most a quarter of the modulus; the offset congruent to the tag
+//    nearest that estimate is the key's (gx_tag_key).
+// Placement (slot function, amask = 3) is that of gx_cslot, so the home group of four slots is 16 B.  As for gx_cslot,
+// probe keys outside [kmin, kmax] are rejected before the tag compare.  The helpers below are the only code that knows
+// the encoding.
+enum { GX_SLOTS_WIDE = 0, GX_SLOTS_COMPACT = 1, GX_SLOTS_NARROW = 2 };      // gx_slot, gx_cslot, narrow uint32
+static inline unsigned int gx_nslot_tbits(double keys_per_slot)
+{
+    const double need = 4.0 * (keys_per_slot * GX_SUB + 64.0);
+    unsigned int t = 2;
+    while (t < 32 && (double) (1ULL << (t - 1)) < need) t++;
+    return t;
+}
+
+// the slot function of a join table (gx_slot_index); tbits / pbase: the narrow slot format's parameters (gx_nslot_*),
+// 0 for the other forms
+struct gx_slotfn { int mode; unsigned int win; long long kmin; unsigned long long scale; unsigned long long mask; unsigned int shift; unsigned int amask;
+                   unsigned int tbits; int pbase; };
 
 struct gx_hash {
     gx_ctx *ctx;
@@ -91,6 +117,7 @@ struct gx_hash {
     // compact form (gx_cslot): produced by the key-ordered build when key range and payload allow;
     // the 16-byte form is materialised from it on demand for consumers that only read that one
     gx_cslot *cslots; unsigned long long cspan;   // cspan = kmax - kmin + 1
+    unsigned int *narrow; unsigned int tbits; int pbase;   // narrow form (GX_SLOTS_NARROW) instead of cslots, same cspan
     double keys_per_slot;           // key range / slot range of the interpolation (compact -> wide reconstruction)
     unsigned int amask;             // home slots are aligned to amask + 1 (2 for 16 B slots, 4 for compact ones)
     // rows whose key equals GX_EMPTY_KEY cannot live in the table: side list
@@ -98,6 +125,14 @@ struct gx_hash {
 };
 
 int gx_hash_wide(gx_ctx *ctx, gx_hash *h);
+// the slot function (and slot format parameters) a table was built with
+static inline gx_slotfn gx_hash_slotfn(const gx_hash *h)
+{
+    gx_slotfn f;
+    f.mode = h->mode; f.win = h->win; f.kmin = h->kmin; f.scale = h->scale; f.mask = (unsigned long long) h->nslots - 1;
+    f.shift = h->shift; f.amask = h->amask; f.tbits = h->tbits; f.pbase = h->pbase;
+    return f;
+}
 cudaError_t gx_stage_mark(gx_ctx *ctx, const void *host);   // gx_exec.cu: record "copy of this staging slot enqueued"   // materialise the 16-byte slot array of a compact table
 
 // A group-state record: [k0][k1][w0..w(nwords-1)], 8-byte words.
@@ -380,7 +415,6 @@ __device__ __forceinline__ unsigned long long gx_key_hash(long long key) { retur
 // with a multiplicative hash, which breaks up the pile-ups that locally bunched keys
 // (TPC-H order keys: 8 used of every 32) cause under pure interpolation while keeping
 // every key inside the same few cache lines and the same sub-table.
-struct gx_slotfn { int mode; unsigned int win; long long kmin; unsigned long long scale; unsigned long long mask; unsigned int shift; unsigned int amask; };
 __device__ __forceinline__ unsigned long long gx_slot_index(long long key, const gx_slotfn &f)
 {
     // Home slots are aligned to amask + 1 slots (2 x 16 B or 4 x 8 B = one 32-byte sector), which a
@@ -411,6 +445,49 @@ __device__ __forceinline__ unsigned long long gx_next_slot(unsigned long long s,
 {
     const unsigned long long w = mask < (GX_SUB - 1) ? mask : (unsigned long long) (GX_SUB - 1);
     return (s & ~w) | ((s + 1) & w);
+}
+
+// narrow slots (see gx_nslot_tbits) --------------------------------------
+__device__ __forceinline__ unsigned int gx_nslot_tag(long long key, const gx_slotfn &f)
+{
+    return GX_CSLOT_D(key, f.kmin) & ((1u << f.tbits) - 1u);
+}
+// does a payload fit the slot's 32 - tbits bits above pbase?
+__device__ __forceinline__ bool gx_nslot_fits(long long payload, const gx_slotfn &f)
+{
+    return (unsigned long long) (payload - (long long) f.pbase) < (1ULL << (32 - f.tbits));
+}
+__device__ __forceinline__ unsigned int gx_nslot_make(long long key, long long payload, const gx_slotfn &f)
+{
+    return gx_nslot_tag(key, f) | ((unsigned int) (payload - (long long) f.pbase) << f.tbits);
+}
+__device__ __forceinline__ int gx_nslot_payload(unsigned int w, const gx_slotfn &f) { return f.pbase + (int) (w >> f.tbits); }
+// a home group of four narrow slots: one 16-byte load
+__device__ __forceinline__ uint4 gx_nslot_ld(const unsigned int *p)
+{
+    uint4 v;
+    asm volatile("ld.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
+    return v;
+}
+// one group of a probe walk: true when the walk ends here (a slot holds the tag, or a slot is empty - a table that is only
+// ever filled has no match behind an empty slot); found and payload tell which
+__device__ __forceinline__ bool gx_nslot_group(const uint4 &q, unsigned int tag, const gx_slotfn &f, bool &found, int &payload)
+{
+    const unsigned int tm = (1u << f.tbits) - 1u;
+    const bool h0 = (q.x & tm) == tag, h1 = (q.y & tm) == tag, h2 = (q.z & tm) == tag, h3 = (q.w & tm) == tag;
+    found = h0 | h1 | h2 | h3;
+    payload = gx_nslot_payload(h0 ? q.x : h1 ? q.y : h2 ? q.z : q.w, f);
+    return found | (q.x == 0u) | (q.y == 0u) | (q.z == 0u) | (q.w == 0u);
+}
+// the key of a compact or narrow entry in slot i from its tag bits v = (key - kmin) mod 2^mbits: the offset congruent to v
+// nearest the interpolation's estimate i keys_per_slot
+__device__ __forceinline__ long long gx_tag_key(long long i, unsigned long long v, int mbits, long long kmin, double keys_per_slot)
+{
+    const long long M = 1LL << mbits, est = (long long) ((double) i * keys_per_slot);
+    long long off = (est & ~(M - 1)) | (long long) v;
+    if (off - est > M / 2) off -= M;
+    else if (est - off > M / 2) off += M;
+    return kmin + off;
 }
 
 // mbarrier and bulk-async copy (TMA) helpers.  Every wait is bounded: a caller whose wait gives up raises a flag and

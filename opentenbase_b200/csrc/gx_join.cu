@@ -111,7 +111,8 @@ struct gx_bbuild_args {
     gx_slot *pairs;             // nsub fixed-capacity buckets of GX_SUB pairs (a fuller bucket cannot be built anyway)
     int *overflow;
     long long *start; int *unsorted;   // key-ordered build: first row of every sub-table
-    gx_cslot *cslots;                  // compact output (gx_k_sorted_fill<.., true>)
+    gx_cslot *cslots;                  // compact output (gx_k_sorted_fill<GX_SLOTS_COMPACT, ..>)
+    unsigned int *narrow;              // narrow output (gx_k_sorted_fill<GX_SLOTS_NARROW, ..>)
 };
 
 __device__ __forceinline__ bool build_row_ok(const gx_build_args &a, long long r)
@@ -321,21 +322,27 @@ __global__ void __launch_bounds__(BP_THREADS, 2) gx_k_bpart2(gx_bpart_args a)
 // histogram and the caller's rows for the next sub-table.
 #define FILL_THREADS 256
 #define FILL_ROWS (GX_SUB / FILL_THREADS)          // rows (and slots) per thread
-template <bool C> struct gx_fill_smem_t {
-    typename std::conditional<C, gx_cslot, gx_slot>::type tab[GX_SUB];
+template <int F> struct gx_slot_of { typedef gx_slot type; };
+template <> struct gx_slot_of<GX_SLOTS_COMPACT> { typedef gx_cslot type; };
+template <> struct gx_slot_of<GX_SLOTS_NARROW> { typedef unsigned int type; };
+template <int F> struct gx_fill_smem_t {
+    typename gx_slot_of<F>::type tab[GX_SUB];
     unsigned int cnt[GX_SUB];                      // histogram, then e[s]
     int wsum[FILL_THREADS / 32], wmin[FILL_THREADS / 32];
 };
-typedef gx_fill_smem_t<false> gx_fill_smem;
+typedef gx_fill_smem_t<GX_SLOTS_WIDE> gx_fill_smem;
 #define FILL_SMEM_BYTES ((int) sizeof(gx_fill_smem))
-#define FILL_SMEM_BYTES_C ((int) sizeof(gx_fill_smem_t<true>))
 #define FILL_INF (1 << 29)
 
-// C = compact 8-byte slots {key - kmin + 1, payload}; dst then points at gx_cslot
-template <bool C, class LOAD>
-__device__ __forceinline__ void gx_subtable_build(gx_fill_smem_t<C> &sm, unsigned int n, const gx_slotfn &sf, LOAD load, void *dst,
-                                                  unsigned int &steps, unsigned int &placed, long long want_sub = -1, int *misplaced = nullptr)
+// F = the slot format GX_SLOTS_*; dst points at that slot type.  A narrow row whose payload does not fit the slot's
+// payload bits raises pay_miss (and is placed with a truncated payload: the host rebuilds in the 8-byte form).
+template <int F, class LOAD>
+__device__ __forceinline__ void gx_subtable_build(gx_fill_smem_t<F> &sm, unsigned int n, const gx_slotfn &sf, LOAD load, void *dst,
+                                                  unsigned int &steps, unsigned int &placed, int &pay_miss,
+                                                  long long want_sub = -1, int *misplaced = nullptr)
 {
+    constexpr bool C = F != GX_SLOTS_WIDE;                     // 32-bit key words (compact and narrow)
+    constexpr int SB = (int) sizeof(typename gx_slot_of<F>::type);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     // ---- clear: histogram and table
     {
@@ -345,7 +352,7 @@ __device__ __forceinline__ void gx_subtable_build(gx_fill_smem_t<C> &sm, unsigne
         if (C) {
             uint4 *t4 = (uint4 *) sm.tab;
 #pragma unroll
-            for (int u = 0; u < FILL_ROWS / 2; u++) t4[tid + u * FILL_THREADS] = z;
+            for (int u = 0; u < FILL_ROWS * SB / 16; u++) t4[tid + u * FILL_THREADS] = z;
         } else {
             longlong2 e; e.x = GX_EMPTY_KEY; e.y = 0;
             longlong2 *t2 = (longlong2 *) sm.tab;
@@ -369,7 +376,11 @@ __device__ __forceinline__ void gx_subtable_build(gx_fill_smem_t<C> &sm, unsigne
             if (want_sub >= 0 && (long long) (fs >> GX_SUB_LOG2) != want_sub) *misplaced = 1;   // caller's row range was wrong
             unsigned int sl = (unsigned int) (fs & (GX_SUB - 1));
             sr[u] = sl | (atomicAdd(&sm.cnt[sl], 1u) << GX_SUB_LOG2);
-            if (C) { key[u] = GX_CSLOT_D(k64, sf.kmin); pay[u] = (unsigned int) p64; }
+            if (F == GX_SLOTS_NARROW) {
+                const long long pv = (long long) (int) (unsigned int) p64;       // the 4-byte payload column is signed
+                if (!gx_nslot_fits(pv, sf)) pay_miss = 1;
+                key[u] = gx_nslot_make(k64, pv, sf); pay[u] = 0;
+            } else if (C) { key[u] = GX_CSLOT_D(k64, sf.kmin); pay[u] = (unsigned int) p64; }
             else { key[u] = k64; pay[u] = p64; }
         }
     }
@@ -415,7 +426,8 @@ __device__ __forceinline__ void gx_subtable_build(gx_fill_smem_t<C> &sm, unsigne
         unsigned int sl = sr[u] & (GX_SUB - 1), pos = sl + sm.cnt[sl] + (sr[u] >> GX_SUB_LOG2);
         steps += pos - sl; placed++;
         if (pos < GX_SUB) {
-            if (C) { uint2 v; v.x = (unsigned int) key[u]; v.y = (unsigned int) pay[u]; ((uint2 *) sm.tab)[pos] = v; }
+            if (F == GX_SLOTS_NARROW) ((unsigned int *) sm.tab)[pos] = (unsigned int) key[u];
+            else if (C) { uint2 v; v.x = (unsigned int) key[u]; v.y = (unsigned int) pay[u]; ((uint2 *) sm.tab)[pos] = v; }
             else { longlong2 v; v.x = key[u]; v.y = (long long) pay[u]; ((longlong2 *) sm.tab)[pos] = v; }
             sr[u] = 0xffffffffu;
         } else wrapped = 1;
@@ -427,7 +439,8 @@ __device__ __forceinline__ void gx_subtable_build(gx_fill_smem_t<C> &sm, unsigne
             unsigned int sl = 0;                      // everything from its slot to the end is full: continue from the start
             for (;;) {
                 bool won;
-                if (C) {
+                if (F == GX_SLOTS_NARROW) won = atomicCAS((unsigned int *) sm.tab + sl, 0u, (unsigned int) key[u]) == 0u;
+                else if (C) {
                     gx_cslot *t = (gx_cslot *) sm.tab;
                     won = atomicCAS(&t[sl].d, 0u, (unsigned int) key[u]) == 0u;
                     if (won) t[sl].payload = (unsigned int) pay[u];
@@ -447,7 +460,7 @@ __device__ __forceinline__ void gx_subtable_build(gx_fill_smem_t<C> &sm, unsigne
         const uint4 *t4 = (const uint4 *) sm.tab;
         uint4 *d4 = (uint4 *) dst;
 #pragma unroll
-        for (int u = 0; u < FILL_ROWS / 2; u++) d4[tid + u * FILL_THREADS] = t4[tid + u * FILL_THREADS];
+        for (int u = 0; u < FILL_ROWS * SB / 16; u++) d4[tid + u * FILL_THREADS] = t4[tid + u * FILL_THREADS];
     } else {
         const longlong2 *t2 = (const longlong2 *) sm.tab;
         longlong2 *d2 = (longlong2 *) dst;
@@ -473,13 +486,14 @@ __global__ void __launch_bounds__(FILL_THREADS, 4) gx_k_bbuild_fill(gx_bbuild_ar
     extern __shared__ __align__(16) unsigned char fill_smem_raw[];
     gx_fill_smem &sm = *(gx_fill_smem *) fill_smem_raw;
     unsigned int steps = 0, placed = 0;
+    int pay_miss = 0;                                  // narrow form only
     for (long long sub = blockIdx.x; sub < a.nsub; sub += gridDim.x) {
         unsigned int n = a.cursor[sub];
         if (n >= GX_SUB) n = 0;                        // overflowed: the host rebuilds directly
         const longlong2 *src = (const longlong2 *) a.pairs + sub * GX_SUB;
-        gx_subtable_build<false>(sm, n, a.b.sf,
+        gx_subtable_build<GX_SLOTS_WIDE>(sm, n, a.b.sf,
                           [&](unsigned int i, long long &k, unsigned long long &p) { longlong2 v = src[i]; k = v.x; p = (unsigned long long) v.y; return true; },
-                          a.b.slots + sub * GX_SUB, steps, placed);
+                          a.b.slots + sub * GX_SUB, steps, placed, pay_miss);
     }
     fill_report(a.b, steps, 0);                        // entries are counted from the cursors (gx_k_bbuild_total)
 }
@@ -553,16 +567,21 @@ __global__ void __launch_bounds__(256) gx_k_sorted_bounds_i8(const long long *__
 
 // The generic row loader (any key type, NULLs, build-side quals, packed payload); in the VERIFY form an int8 key
 // without NULLs.  The shapes of a plain key + one 4-byte column (or none) go to gx_k_sorted_fill_staged below.
-template <bool C, bool VERIFY>
-__global__ void __launch_bounds__(FILL_THREADS, C ? 5 : 4) gx_k_sorted_fill(gx_bbuild_args a)      // 5 CTAs/SM
+// Output of the key-ordered fills in slot format F
+template <int F> __device__ __forceinline__ char *fill_out(const gx_bbuild_args &a)
+{
+    return F == GX_SLOTS_NARROW ? (char *) a.narrow : F == GX_SLOTS_COMPACT ? (char *) a.cslots : (char *) a.b.slots;
+}
+template <int F, bool VERIFY>
+__global__ void __launch_bounds__(FILL_THREADS, F != GX_SLOTS_WIDE ? 5 : 4) gx_k_sorted_fill(gx_bbuild_args a)      // 5 CTAs/SM
 {
     extern __shared__ __align__(16) unsigned char fill_smem_raw[];
-    gx_fill_smem_t<C> &sm = *(gx_fill_smem_t<C> *) fill_smem_raw;
-    void *const out = C ? (void *) a.cslots : (void *) a.b.slots;
-    const size_t slot_bytes = C ? sizeof(gx_cslot) : sizeof(gx_slot);
+    gx_fill_smem_t<F> &sm = *(gx_fill_smem_t<F> *) fill_smem_raw;
+    char *const out = fill_out<F>(a);
+    const size_t slot_bytes = sizeof(typename gx_slot_of<F>::type);
     if (!VERIFY && *a.unsorted) return;
     unsigned int steps = 0, placed = 0;
-    int bad = 0;
+    int bad = 0, pay_miss = 0;
     const long long *keys = (const long long *) a.b.key.data;
     long long lo = 0, hi = 0;
     if (blockIdx.x < a.nsub) { lo = a.start[blockIdx.x]; hi = a.start[blockIdx.x + 1]; }
@@ -571,17 +590,17 @@ __global__ void __launch_bounds__(FILL_THREADS, C ? 5 : 4) gx_k_sorted_fill(gx_b
         const long long nsubn = sub + gridDim.x;
         if (nsubn < a.nsub) { nlo = a.start[nsubn]; nhi = a.start[nsubn + 1]; }
         unsigned int n = (unsigned int) (hi - lo);
-        if (hi - lo >= GX_SUB) { n = 0; if (threadIdx.x == 0) *a.overflow = 1; }     // a sub-table keeps one slot free
+        if (hi - lo >= GX_SUB) { n = 0; if (threadIdx.x == 0) atomicOr(a.overflow, 1); }     // a sub-table keeps one slot free
         if (VERIFY && hi < lo) { n = 0; bad = 1; }
         if (!VERIFY)
-            gx_subtable_build<C>(sm, n, a.b.sf,
+            gx_subtable_build<F>(sm, n, a.b.sf,
                               [&](unsigned int i, long long &k, unsigned long long &p) {
                                   long long r = lo + i;
                                   if (!build_row_ok(a.b, r)) return false;
                                   k = gx_load_int(a.b.key, r); p = pack_payload(a.b, r); return true; },
-                              (char *) out + (size_t) sub * GX_SUB * slot_bytes, steps, placed);
+                              out + (size_t) sub * GX_SUB * slot_bytes, steps, placed, pay_miss);
         else                                                   // int8 key without NULLs; quals and any payload
-            gx_subtable_build<C>(sm, n, a.b.sf,
+            gx_subtable_build<F>(sm, n, a.b.sf,
                               [&](unsigned int i, long long &k, unsigned long long &p) {
                                   const long long r = lo + i;
                                   k = __ldg(keys + r);
@@ -589,10 +608,11 @@ __global__ void __launch_bounds__(FILL_THREADS, C ? 5 : 4) gx_k_sorted_fill(gx_b
                                   if (kp > k || k == GX_EMPTY_KEY) bad = 1;          // order is checked on every row, kept or not
                                   if (!build_row_ok(a.b, r)) return false;
                                   p = pack_payload(a.b, r); return true; },
-                              (char *) out + (size_t) sub * GX_SUB * slot_bytes, steps, placed, sub, &bad);
+                              out + (size_t) sub * GX_SUB * slot_bytes, steps, placed, pay_miss, sub, &bad);
         lo = nlo; hi = nhi;
     }
     if (VERIFY && bad) *a.unsorted = 1;
+    if (pay_miss) atomicOr(a.overflow, 4);
     fill_report(a.b, steps, placed);
 }
 
@@ -607,7 +627,7 @@ __global__ void __launch_bounds__(FILL_THREADS, C ? 5 : 4) gx_k_sorted_fill(gx_b
 // order check's predecessor) and of the payload range; the rounding reads at most 15 bytes past a column's last row,
 // inside the last row's 16-byte block.  The finished sub-table leaves with plain 16-byte stores, which the CTA does
 // not wait for.  Checks, flags and chain counters are those of gx_k_sorted_fill; a wait that gives up raises bit 2 of
-// *overflow and the host rebuilds with gx_k_sorted_fill.
+// *overflow and the host rebuilds with gx_k_sorted_fill.  Both raise bit 4 for a payload outside the narrow form's window.
 #define FSTAGE_KEYS (GX_SUB + 4)                   // rows [lo - 1, hi) rounded out to even rows: at most 2047 + 3
 #define FSTAGE_PAYS (GX_SUB + 8)                   // rows [lo, hi) rounded out to multiples of 4: at most 2047 + 6
 template <int PK> struct __align__(16) gx_fill_stage {
@@ -616,16 +636,16 @@ template <int PK> struct __align__(16) gx_fill_stage {
     unsigned long long bar;
     long long lo, hi;                              // the staged sub-table's row range, written by thread 0 before its arrive
 };
-template <int PK, bool C> constexpr int staged_smem_bytes() { return (int) (sizeof(gx_fill_smem_t<C>) + 2 * sizeof(gx_fill_stage<PK>)); }
+template <int PK, int F> constexpr int staged_smem_bytes() { return (int) (sizeof(gx_fill_smem_t<F>) + 2 * sizeof(gx_fill_stage<PK>)); }
 
-template <int PK, bool C, bool VERIFY>
-__global__ void __launch_bounds__(FILL_THREADS, C ? 3 : 2) gx_k_sorted_fill_staged(gx_bbuild_args a)      // what shared memory allows
+template <int PK, int F, bool VERIFY>
+__global__ void __launch_bounds__(FILL_THREADS, F != GX_SLOTS_WIDE ? 3 : 2) gx_k_sorted_fill_staged(gx_bbuild_args a)      // what shared memory allows
 {
     extern __shared__ __align__(16) unsigned char fill_smem_raw[];
-    gx_fill_smem_t<C> &sm = *(gx_fill_smem_t<C> *) fill_smem_raw;
-    gx_fill_stage<PK> *const stage = (gx_fill_stage<PK> *) (fill_smem_raw + sizeof(gx_fill_smem_t<C>));
-    void *const out = C ? (void *) a.cslots : (void *) a.b.slots;
-    const size_t slot_bytes = C ? sizeof(gx_cslot) : sizeof(gx_slot);
+    gx_fill_smem_t<F> &sm = *(gx_fill_smem_t<F> *) fill_smem_raw;
+    gx_fill_stage<PK> *const stage = (gx_fill_stage<PK> *) (fill_smem_raw + sizeof(gx_fill_smem_t<F>));
+    char *const out = fill_out<F>(a);
+    const size_t slot_bytes = sizeof(typename gx_slot_of<F>::type);
     if (!VERIFY && *a.unsorted) return;
     const long long s0 = a.nsub * blockIdx.x / gridDim.x, s1 = a.nsub * (blockIdx.x + 1) / gridDim.x;
     const long long *keys = (const long long *) a.b.key.data;
@@ -652,7 +672,7 @@ __global__ void __launch_bounds__(FILL_THREADS, C ? 3 : 2) gx_k_sorted_fill_stag
     }
     __syncthreads();
     unsigned int steps = 0, placed = 0;
-    int bad = 0;
+    int bad = 0, pay_miss = 0;
     bool stuck = false;
     for (long long s = s0; s < s1; s++) {
         gx_fill_stage<PK> &st = stage[(s - s0) & 1];
@@ -663,7 +683,7 @@ __global__ void __launch_bounds__(FILL_THREADS, C ? 3 : 2) gx_k_sorted_fill_stag
         if (hi < lo) { n = 0; bad = 1; }
         const long long *sk = st.key + (lo - ((lo > 0 ? lo - 1 : 0) & ~1LL));                 // row lo; sk[-1] is row lo - 1
         const unsigned int *sp = st.pay + (lo & 3);
-        gx_subtable_build<C>(sm, n, a.b.sf,
+        gx_subtable_build<F>(sm, n, a.b.sf,
                           [&](unsigned int i, long long &k, unsigned long long &p) {
                               k = sk[i];
                               if (VERIFY) {
@@ -672,12 +692,13 @@ __global__ void __launch_bounds__(FILL_THREADS, C ? 3 : 2) gx_k_sorted_fill_stag
                               }
                               p = PK == 1 ? (unsigned long long) sp[i] : (unsigned long long) (lo + i);
                               return true; },
-                          (char *) out + (size_t) s * GX_SUB * slot_bytes, steps, placed, VERIFY ? s : -1, &bad);
+                          out + (size_t) s * GX_SUB * slot_bytes, steps, placed, pay_miss, VERIFY ? s : -1, &bad);
         // gx_subtable_build ends with a barrier: nobody reads this stage any more
         if (threadIdx.x == 0 && s + 2 < s1) issue(s + 2, st);
     }
     if (stuck && threadIdx.x == 0) atomicOr(a.overflow, 2);
     if (VERIFY && bad) *a.unsorted = 1;
+    if (pay_miss) atomicOr(a.overflow, 4);
     fill_report(a.b, steps, placed);
 }
 // ---------------------------------------------------------------------------
@@ -782,18 +803,27 @@ __global__ void gx_k_bbuild_total(const unsigned int *cursor, long long n, long 
 }
 __global__ void gx_k_scan_i64(long long *v, long long n, long long *total);   // gx_agg.cu
 
-// key-density estimate for the slot function: min / max over a strided sample
-__global__ void gx_k_key_range(gx_dcol key, long long nrows, long long stride, long long *minmax)
+// key-density estimate for the slot function: min / max over a strided sample; the same for the payload column
+// (pay.data non-null: the narrow slot form's payload window) of the sampled rows with a key
+__global__ void gx_k_key_range(gx_dcol key, gx_dcol pay, long long nrows, long long stride, long long *minmax, long long *pminmax)
 {
     long long i = ((long long) blockIdx.x * blockDim.x + threadIdx.x) * stride;
-    long long lo = 0x7fffffffffffffffLL, hi = -0x7fffffffffffffffLL - 1;
-    if (i < nrows && !gx_is_null(key, i)) { lo = hi = gx_load_int(key, i); }
+    long long lo = 0x7fffffffffffffffLL, hi = -0x7fffffffffffffffLL - 1, plo = lo, phi = hi;
+    if (i < nrows && !gx_is_null(key, i)) {
+        lo = hi = gx_load_int(key, i);
+        if (pay.data) plo = phi = gx_load_int(pay, i);
+    }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
         long long a = __shfl_down_sync(0xffffffffu, lo, o), b = __shfl_down_sync(0xffffffffu, hi, o);
         lo = a < lo ? a : lo; hi = b > hi ? b : hi;
+        a = __shfl_down_sync(0xffffffffu, plo, o); b = __shfl_down_sync(0xffffffffu, phi, o);
+        plo = a < plo ? a : plo; phi = b > phi ? b : phi;
     }
-    if ((threadIdx.x & 31) == 0) { atomicMin(&minmax[0], lo); atomicMax(&minmax[1], hi); }
+    if ((threadIdx.x & 31) == 0) {
+        atomicMin(&minmax[0], lo); atomicMax(&minmax[1], hi);
+        if (pay.data) { atomicMin(&pminmax[0], plo); atomicMax(&pminmax[1], phi); }
+    }
 }
 
 // Interpolation is tried when the key span is at most this many times the row count: TPC-H order
@@ -823,26 +853,27 @@ static void gx_set_interpolation(gx_hash *h, long long kmin, double range_d)
 
 // The fill of the key-ordered build.  pk 1 / 2: gx_k_sorted_fill_staged, one resident grid; pk 0 (and the rebuild after
 // a staged wait gave up): gx_k_sorted_fill.  The second profile name tells which one ran.
-template <int PK, bool C, bool VERIFY> static void sorted_fill_staged(gx_ctx *ctx, const gx_bbuild_args &ba)
+template <int PK, int F, bool VERIFY> static void sorted_fill_staged(gx_ctx *ctx, const gx_bbuild_args &ba)
 {
     static int per_sm = 0;
     if (!per_sm) {
-        cudaFuncSetAttribute(gx_k_sorted_fill_staged<PK, C, VERIFY>, cudaFuncAttributeMaxDynamicSharedMemorySize, staged_smem_bytes<PK, C>());
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gx_k_sorted_fill_staged<PK, C, VERIFY>, FILL_THREADS,
-                                                          staged_smem_bytes<PK, C>()) != cudaSuccess || per_sm < 1) per_sm = 1;
+        cudaFuncSetAttribute(gx_k_sorted_fill_staged<PK, F, VERIFY>, cudaFuncAttributeMaxDynamicSharedMemorySize, staged_smem_bytes<PK, F>());
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gx_k_sorted_fill_staged<PK, F, VERIFY>, FILL_THREADS,
+                                                          staged_smem_bytes<PK, F>()) != cudaSuccess || per_sm < 1) per_sm = 1;
     }
     gx_launch_scope which(ctx, "build_fill_staged", 0);
-    gx_k_sorted_fill_staged<PK, C, VERIFY><<<per_sm * ctx->sm_count, FILL_THREADS, staged_smem_bytes<PK, C>(), ctx->stream>>>(ba);
+    gx_k_sorted_fill_staged<PK, F, VERIFY><<<per_sm * ctx->sm_count, FILL_THREADS, staged_smem_bytes<PK, F>(), ctx->stream>>>(ba);
 }
-template <bool C, bool VERIFY> static void sorted_fill(gx_ctx *ctx, const gx_bbuild_args &ba, int pk)
+// F: slot format; the narrow form only serves pk 1 (and pk 0, the generic loader)
+template <int F, bool VERIFY> static void sorted_fill(gx_ctx *ctx, const gx_bbuild_args &ba, int pk)
 {
-    if (pk == 1) { sorted_fill_staged<1, C, VERIFY>(ctx, ba); return; }
-    if (pk == 2) { sorted_fill_staged<2, C, VERIFY>(ctx, ba); return; }
-    const int bytes = C ? FILL_SMEM_BYTES_C : FILL_SMEM_BYTES;
+    if (pk == 1) { sorted_fill_staged<1, F, VERIFY>(ctx, ba); return; }
+    if constexpr (F != GX_SLOTS_NARROW) { if (pk == 2) { sorted_fill_staged<2, F, VERIFY>(ctx, ba); return; } }
+    const int bytes = (int) sizeof(gx_fill_smem_t<F>);
     static bool attr = false;
-    if (!attr) { cudaFuncSetAttribute(gx_k_sorted_fill<C, VERIFY>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes); attr = true; }
+    if (!attr) { cudaFuncSetAttribute(gx_k_sorted_fill<F, VERIFY>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes); attr = true; }
     gx_launch_scope which(ctx, "build_fill_rows", 0);
-    gx_k_sorted_fill<C, VERIFY><<<ctx->sm_count * (C ? 10 : 8), FILL_THREADS, bytes, ctx->stream>>>(ba);
+    gx_k_sorted_fill<F, VERIFY><<<ctx->sm_count * (F != GX_SLOTS_WIDE ? 10 : 8), FILL_THREADS, bytes, ctx->stream>>>(ba);
 }
 
 extern "C" int gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col, int n_preds, const gx_pred *preds,
@@ -884,6 +915,9 @@ extern "C" int gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col, in
     // keys span at most GX_INTERP_MAX_SPREAD x their count
     h->mode = 0; h->kmin = 0; h->scale = 0; h->shift = 0; h->amask = 1u;
     bool have_ends = false, counts_read = false;
+    // one int4/date payload column: its sampled range decides whether the narrow slot form can hold it
+    const bool pay4 = n_payload == 1 && (a.payload[0].type == GX_INT4 || a.payload[0].type == GX_DATE);
+    bool have_prange = false; long long pmin = 0, pmax = 0;
     { const char *w = getenv("GX_SLOT_WIN"); h->win = w ? (unsigned int) atoi(w) : 31u; }
     {
         const char *fm = getenv("GX_SLOT_MODE");
@@ -894,8 +928,12 @@ extern "C" int gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col, in
             long long nthreads = (inner->nrows + stride - 1) / stride;
             long long init[2] = { 0x7fffffffffffffffLL, -0x7fffffffffffffffLL - 1 };
             GX_CUDA(ctx, cudaMemcpyAsync(ctx->d_scratch + 4, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
-            { gx_launch_scope ls(ctx, "build_sample"); gx_k_key_range<<<(unsigned) ((nthreads + 255) / 256), 256, 0, ctx->stream>>>(a.key, inner->nrows, stride, ctx->d_scratch + 4); }
+            GX_CUDA(ctx, cudaMemcpyAsync(ctx->d_scratch + 16, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
+            gx_dcol pay; memset(&pay, 0, sizeof(pay));
+            if (pay4) pay = a.payload[0];
+            { gx_launch_scope ls(ctx, "build_sample"); gx_k_key_range<<<(unsigned) ((nthreads + 255) / 256), 256, 0, ctx->stream>>>(a.key, pay, inner->nrows, stride, ctx->d_scratch + 4, ctx->d_scratch + 16); }
             GX_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + 4, ctx->d_scratch + 4, 2 * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream));
+            GX_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + 16, ctx->d_scratch + 16, 2 * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream));
             // the column's first and last key ride along: the key-ordered build path below needs them
             {
                 const int ksz0 = gx_type_size(kt);
@@ -906,6 +944,7 @@ extern "C" int gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col, in
             }
             GX_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
             long long lo = ctx->h_scratch[4], hi = ctx->h_scratch[5];
+            pmin = ctx->h_scratch[16]; pmax = ctx->h_scratch[17]; have_prange = pay4 && pmin <= pmax;
             if (hi > lo) {
                 double range = (double) hi - (double) lo + 1.0;
                 if (range <= GX_INTERP_MAX_SPREAD * (double) inner->nrows || want == 1) {
@@ -980,22 +1019,43 @@ extern "C" int gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col, in
                 const double keys_per_slot = range_d / (double) (h->nslots - GX_SUB);
                 bool compact = (pk != 0 || searched) && small_payload && h->mode != 0 && keys_per_slot * GX_SUB < 268435456.0 &&
                                !(nocompact && nocompact[0] == '1');
+                // narrow 4-byte slots (pk 1) when the tag the key span needs leaves room for the sampled payload range, which
+                // is centred in the window; a payload the sample missed is caught by the fill (bit 4 of the overflow word)
+                bool narrow = false;
+                if (compact && pk == 1 && have_prange) {
+                    const unsigned int tbits = gx_nslot_tbits(keys_per_slot);
+                    const long long pwin = tbits < 32 ? 1LL << (32 - tbits) : 0;         // payload values a slot holds
+                    if (pmax - pmin < pwin) {
+                        long long pb = pmin - (pwin - 1 - (pmax - pmin)) / 2;
+                        if (pb < (long long) INT32_MIN) pb = INT32_MIN;                     // the window stays inside int4
+                        if (pb > (long long) INT32_MAX - (pwin - 1)) pb = (long long) INT32_MAX - (pwin - 1);
+                        narrow = true; h->tbits = tbits; h->pbase = (int) pb;
+                    }
+                }
                 h->keys_per_slot = keys_per_slot;
-                if (compact && gx_tmp_alloc(ctx, (void **) &h->cslots, (size_t) h->nslots * sizeof(gx_cslot)) != cudaSuccess) { h->cslots = nullptr; compact = false; }
+                if (narrow && gx_tmp_alloc(ctx, (void **) &h->narrow, (size_t) h->nslots * sizeof(unsigned int)) != cudaSuccess) { h->narrow = nullptr; narrow = false; }
+                if (!narrow) { h->tbits = 0; h->pbase = 0; }
+                if (compact && !narrow && gx_tmp_alloc(ctx, (void **) &h->cslots, (size_t) h->nslots * sizeof(gx_cslot)) != cudaSuccess) { h->cslots = nullptr; compact = false; }
                 h->amask = compact ? 3u : 1u; h->cspan = compact ? (unsigned long long) (kmax - kmin) + 1ULL : 0ULL;
-                a.sf.amask = h->amask; ba.b = a; ba.cslots = h->cslots;
+                a.sf.amask = h->amask; a.sf.tbits = h->tbits; a.sf.pbase = h->pbase; ba.b = a; ba.cslots = h->cslots; ba.narrow = h->narrow;
+                auto drop_compact = [&]() {
+                    gx_tmp_free(ctx, h->cslots); gx_tmp_free(ctx, h->narrow); h->cslots = nullptr; h->narrow = nullptr;
+                    h->amask = 1u; h->cspan = 0; h->tbits = 0; h->pbase = 0; a.sf.tbits = 0; a.sf.pbase = 0;
+                };
                 // the staged fill copies 16-byte aligned blocks of the key and payload columns
                 if (pk != 0 && (((uintptr_t) a.key.data & 15) != 0 || (pk == 1 && ((uintptr_t) a.payload[0].data & 15) != 0))) pk = 0;
                 auto fill = [&](int use_pk) {
-                    if (searched) { if (compact) sorted_fill<true, true>(ctx, ba, use_pk); else sorted_fill<false, true>(ctx, ba, use_pk); }
-                    else if (compact) sorted_fill<true, false>(ctx, ba, use_pk);
-                    else sorted_fill<false, false>(ctx, ba, use_pk);
+                    if (narrow) { if (searched) sorted_fill<GX_SLOTS_NARROW, true>(ctx, ba, use_pk); else sorted_fill<GX_SLOTS_NARROW, false>(ctx, ba, use_pk); }
+                    else if (compact) { if (searched) sorted_fill<GX_SLOTS_COMPACT, true>(ctx, ba, use_pk); else sorted_fill<GX_SLOTS_COMPACT, false>(ctx, ba, use_pk); }
+                    else if (searched) sorted_fill<GX_SLOTS_WIDE, true>(ctx, ba, use_pk);
+                    else sorted_fill<GX_SLOTS_WIDE, false>(ctx, ba, use_pk);
                 };
                 if (searched) {
                     { gx_launch_scope ls(ctx, "build_bounds"); gx_k_sorted_bounds_search<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>((const long long *) a.key.data, inner->nrows, a.sf, ba.nsub, h->nslots, d_start); }
                     gx_launch_scope ls(ctx, "build");
                     gx_launch_scope path(ctx, "build_sorted_search", 0);           // second profile names: which build path ran
                     gx_launch_scope form(ctx, compact ? "build_compact" : nullptr, 0);
+                    gx_launch_scope nform(ctx, narrow ? "build_narrow" : nullptr, 0);
                     fill(pk);
                 } else {
                     {
@@ -1009,6 +1069,7 @@ extern "C" int gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col, in
                         gx_launch_scope ls(ctx, "build", 2);
                         gx_launch_scope path(ctx, "build_sorted_pass", 0);
                         gx_launch_scope form(ctx, compact ? "build_compact" : nullptr, 0);
+                        gx_launch_scope nform(ctx, narrow ? "build_narrow" : nullptr, 0);
                         gx_k_sorted_special<<<1, 256, 0, ctx->stream>>>(a, d_start, d_flag);
                         fill(pk);
                     }
@@ -1016,34 +1077,51 @@ extern "C" int gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col, in
                 cudaError_t e2 = cudaGetLastError();
                 if (e2 == cudaSuccess) e2 = cudaMemcpyAsync(ctx->h_scratch, ctx->d_scratch, 8 * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream);
                 if (e2 == cudaSuccess) e2 = cudaStreamSynchronize(ctx->stream);
-                if (e2 == cudaSuccess && pk != 0 && ((int) ctx->h_scratch[7] & 2)) {
-                    // a bounded wait of the staged fill gave up: the same build with the generic row loader
-                    fprintf(stderr, "gpuexec: a bounded mbarrier wait of gx_k_sorted_fill_staged gave up; rebuilding with gx_k_sorted_fill\n");
+                // the fill once more, in the form `compact` / `narrow` now name; `why` is its second profile name
+                auto refill = [&](int use_pk, const char *why) {
                     cudaMemsetAsync(ctx->d_scratch + 3, 0, sizeof(long long), ctx->stream);
                     cudaMemsetAsync(ctx->d_scratch + 5, 0, 3 * sizeof(long long), ctx->stream);      // [5] steps, [6] unsorted, [7] overflow
                     {
                         gx_launch_scope ls(ctx, "build");
                         gx_launch_scope path(ctx, searched ? "build_sorted_search" : "build_sorted_pass", 0);
                         gx_launch_scope form(ctx, compact ? "build_compact" : nullptr, 0);
-                        fill(0);
+                        gx_launch_scope nform(ctx, why, 0);
+                        fill(use_pk);
                     }
                     e2 = cudaGetLastError();
                     if (e2 == cudaSuccess) e2 = cudaMemcpyAsync(ctx->h_scratch, ctx->d_scratch, 8 * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream);
                     if (e2 == cudaSuccess) e2 = cudaStreamSynchronize(ctx->stream);
+                };
+                // a bounded wait of the staged fill gave up: the same build with the generic row loader
+                auto stuck = [&]() { return e2 == cudaSuccess && pk != 0 && ((int) ctx->h_scratch[7] & 2); };
+                const char *stuck_msg = "gpuexec: a bounded mbarrier wait of gx_k_sorted_fill_staged gave up; rebuilding with gx_k_sorted_fill\n";
+                if (stuck()) { fprintf(stderr, "%s", stuck_msg); refill(0, narrow ? "build_narrow" : nullptr); }
+                if (e2 == cudaSuccess && narrow && ((int) ctx->h_scratch[7] & 4) && (int) ctx->h_scratch[6] == 0) {
+                    // a payload outside the narrow window (a value the sample missed): the same build in the 8-byte form
+                    gx_tmp_free(ctx, h->narrow); h->narrow = nullptr; narrow = false;
+                    h->tbits = 0; h->pbase = 0; a.sf.tbits = 0; a.sf.pbase = 0;
+                    if (gx_tmp_alloc(ctx, (void **) &h->cslots, (size_t) h->nslots * sizeof(gx_cslot)) != cudaSuccess) {
+                        h->cslots = nullptr; gx_tmp_free(ctx, d_start);
+                        GX_SET_ERR(ctx, "hash_build: cudaMalloc of %lld compact slots failed", (long long) h->nslots);
+                        return GX_ERR_NOMEM;
+                    }
+                    ba.b = a; ba.cslots = h->cslots; ba.narrow = nullptr;
+                    refill(pk, "build_narrow_refill");
+                    if (stuck()) { fprintf(stderr, "%s", stuck_msg); refill(0, "build_narrow_refill"); }
                 }
                 gx_tmp_free(ctx, d_start);
                 if (e2 != cudaSuccess) { GX_SET_ERR(ctx, "hash_build: %s", cudaGetErrorString(e2)); return GX_ERR_CUDA; }
                 if ((int) ctx->h_scratch[6] == 0) {
                     h->avg_chain = ctx->h_scratch[3] > 0 ? (double) ctx->h_scratch[5] / (double) ctx->h_scratch[3] : 0.0;
-                    if ((int) ctx->h_scratch[7] == 0 && h->avg_chain <= 4.0) {
+                    if (((int) ctx->h_scratch[7] & ~4) == 0 && h->avg_chain <= 4.0) {      // bit 4 was answered by the refill above
                         nscattered = ctx->h_scratch[3]; h->sorted_build = 1; counts_read = true;
                         if (compact) { gx_tmp_free(ctx, h->slots); h->slots = nullptr; }      // the 16-byte form is made on demand (gx_hash_wide)
                         break;
                     }
-                    if (compact) { gx_tmp_free(ctx, h->cslots); h->cslots = nullptr; h->amask = 1u; h->cspan = 0; }
+                    if (compact) drop_compact();
                     h->mode = 0; continue;                                               // clustered keys: rebuild with the mixing hash
                 }
-                if (compact) { gx_tmp_free(ctx, h->cslots); h->cslots = nullptr; h->amask = 1u; h->cspan = 0; }
+                if (compact) drop_compact();
                 // not in key order: back to the sampled slot function and the bucketing passes
                 h->kmin = save_kmin; h->scale = save_scale; h->mode = save_mode; h->shift = save_shift;
                 a.sf.mode = h->mode; a.sf.kmin = h->kmin; a.sf.scale = h->scale; a.sf.shift = h->shift; a.sf.amask = h->amask;
@@ -1166,34 +1244,37 @@ extern "C" int gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col, in
     return GX_OK;
 }
 
-// compact table -> 16-byte slots, for the consumers that only read that form.  The full key is
-// rebuilt from its 31 stored bits and the slot's position: the interpolation maps slot i back to
-// key offset ~ i * keys_per_slot (the entry sits within a chain length and a 32-slot window of its
-// home), and the offset congruent to the stored bits nearest to that estimate is the key's.
-__global__ void gx_k_expand_slots(const gx_cslot *c, gx_slot *w, long long nslots, long long kmin, double keys_per_slot)
+// compact or narrow table -> 16-byte slots, for the consumers that only read that form.  The full key is rebuilt from
+// its stored tag bits and the slot's position (gx_tag_key): the interpolation maps slot i back to key offset
+// ~ i * keys_per_slot, and the entry's home lies in the same sub-table.
+template <int F>
+__global__ void gx_k_expand_slots(const void *c, gx_slot *w, long long nslots, gx_slotfn f, double keys_per_slot)
 {
     long long stride = (long long) gridDim.x * blockDim.x;
     for (long long i = (long long) blockIdx.x * blockDim.x + threadIdx.x; i < nslots; i += stride) {
-        gx_cslot v = c[i];
         longlong2 o;
         o.x = GX_EMPTY_KEY; o.y = 0;
-        if (v.d) {
-            const long long est = (long long) ((double) i * keys_per_slot);
-            long long off = (est & ~0x7FFFFFFFLL) | (long long) (v.d >> 1);
-            if (off - est > 0x40000000LL) off -= 0x80000000LL;
-            else if (est - off > 0x40000000LL) off += 0x80000000LL;
-            o.x = kmin + off; o.y = (long long) (unsigned long long) v.payload;
+        if (F == GX_SLOTS_NARROW) {
+            const unsigned int v = ((const unsigned int *) c)[i];
+            if (v) {
+                o.x = gx_tag_key(i, (v & ((1u << f.tbits) - 1u)) >> 1, (int) f.tbits - 1, f.kmin, keys_per_slot);
+                o.y = (long long) (unsigned long long) (unsigned int) gx_nslot_payload(v, f);
+            }
+        } else {
+            const gx_cslot v = ((const gx_cslot *) c)[i];
+            if (v.d) { o.x = gx_tag_key(i, v.d >> 1, 31, f.kmin, keys_per_slot); o.y = (long long) (unsigned long long) v.payload; }
         }
         ((longlong2 *) w)[i] = o;
     }
 }
 int gx_hash_wide(gx_ctx *ctx, gx_hash *h)
 {
-    if (h->slots || !h->cslots) return GX_OK;
+    if (h->slots || (!h->cslots && !h->narrow)) return GX_OK;
     cudaError_t e = gx_tmp_alloc(ctx, (void **) &h->slots, (size_t) h->nslots * sizeof(gx_slot));
     if (e != cudaSuccess) { h->slots = nullptr; GX_SET_ERR(ctx, "hash table: cudaMalloc of %lld slots failed: %s", (long long) h->nslots, cudaGetErrorString(e)); return GX_ERR_NOMEM; }
     gx_launch_scope ls(ctx, "build_expand");
-    gx_k_expand_slots<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(h->cslots, h->slots, h->nslots, h->kmin, h->keys_per_slot);
+    if (h->narrow) gx_k_expand_slots<GX_SLOTS_NARROW><<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(h->narrow, h->slots, h->nslots, gx_hash_slotfn(h), h->keys_per_slot);
+    else gx_k_expand_slots<GX_SLOTS_COMPACT><<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(h->cslots, h->slots, h->nslots, gx_hash_slotfn(h), h->keys_per_slot);
     GX_CUDA(ctx, cudaGetLastError());
     return GX_OK;
 }
@@ -1212,6 +1293,7 @@ extern "C" void gx_hash_free(gx_hash *h)
     if (!h) return;
     gx_tmp_free(h->ctx, h->slots);
     gx_tmp_free(h->ctx, h->cslots);
+    gx_tmp_free(h->ctx, h->narrow);
     gx_tmp_free(h->ctx, h->special_payload);
     free(h);
 }
@@ -1224,6 +1306,7 @@ struct gx_probe_args {
     long long nrows;
     const gx_slot *slots; unsigned long long mask;
     const gx_cslot *cslots; unsigned long long cspan;       // compact 8-byte form (half the bytes: an L2-resident table more often)
+    const unsigned int *narrow;                            // narrow 4-byte form (gx_nslot_*), same cspan
     const unsigned long long *special; int special_count; int _pad2; gx_slotfn sf;
     gx_dcol out_src[GX_MAX_COLS];
     void *out[GX_MAX_COLS];
@@ -1321,14 +1404,14 @@ __global__ void __launch_bounds__(256) gx_k_hash_probe(gx_probe_args a)
 // flight together, matches are numbered with ballots and the warp claims its output range with ONE atomic per
 // tile; the surviving rows are copied column by column.
 #define PT_K 4
-template <bool COMPACT> __global__ void gx_k_hash_probe_unique(gx_probe_args a);
+template <int F> __global__ void gx_k_hash_probe_unique(gx_probe_args a);
 __device__ __forceinline__ void ld_pair(const gx_slot *p, long long &k0, unsigned long long &p0, long long &k1, unsigned long long &p1)
 {
     // one 32-byte sector as two 128-bit loads (sm_90 has no 256-bit load)
     asm volatile("ld.global.v2.u64 {%0, %1}, [%4];\n\tld.global.v2.u64 {%2, %3}, [%4+16];"
                  : "=l"(k0), "=l"(p0), "=l"(k1), "=l"(p1) : "l"(p));
 }
-template <bool COMPACT>
+template <int F>
 // no min-blocks on purpose: any value (even 1 or 4, which leave the occupancy as it is) changes ptxas' schedule
 // of the independent loads this kernel keeps in flight
 __global__ void __launch_bounds__(256) gx_k_hash_probe_unique(gx_probe_args a)
@@ -1350,7 +1433,28 @@ __global__ void __launch_bounds__(256) gx_k_hash_probe_unique(gx_probe_args a)
 #pragma unroll
         for (int j = 0; j < PT_K; j++) key[j] = ok[j] ? gx_load_int(a.key, r[j]) : 0;
         long long k0[PT_K], k1[PT_K]; unsigned long long p0[PT_K], p1[PT_K];
-        if (COMPACT) {
+        if (F == GX_SLOTS_NARROW) {
+            // four 4-byte slots per 16-byte group, one load each (gx_nslot_group)
+            uint4 q[PT_K]; unsigned int tg[PT_K];
+#pragma unroll
+            for (int j = 0; j < PT_K; j++) {
+                const bool inspan = ok[j] && ((unsigned long long) key[j] - (unsigned long long) a.sf.kmin) < a.cspan;   // outside the build side's key span: no partner
+                s[j] = gx_slot_index(key[j], a.sf);
+                tg[j] = gx_nslot_tag(key[j], a.sf);
+                q[j] = inspan ? gx_nslot_ld(a.narrow + s[j]) : make_uint4(0u, 0u, 0u, 0u);    // an empty group ends the walk unmatched
+            }
+#pragma unroll
+            for (int j = 0; j < PT_K; j++) {
+                hit[j] = false; pay[j] = 0;
+                if (!ok[j]) continue;
+                for (;;) {
+                    bool f; int pv;
+                    if (gx_nslot_group(q[j], tg[j], a.sf, f, pv)) { hit[j] = f; pay[j] = (unsigned long long) (unsigned int) pv; break; }
+                    s[j] = gx_next_quad(s[j], a.mask);
+                    q[j] = gx_nslot_ld(a.narrow + s[j]);
+                }
+            }
+        } else if (F == GX_SLOTS_COMPACT) {
             // four 8-byte slots {d, payload} per 32-byte sector; d = ((key - kmin) << 1) | 1 truncated to 32 bits, 0 = empty
             unsigned int d[PT_K];
 #pragma unroll
@@ -1452,12 +1556,12 @@ extern "C" int gx_hash_probe_ex(gx_ctx *ctx, const gx_table *outer, int key_col,
     a.key.data = outer->cols[key_col]; a.key.nulls = outer->nulls[key_col]; a.key.type = kt;
     a.npreds = n_preds; a.n_out_outer = n_out_outer; a.n_payload = h->n_payload; a.unique = h->unique; a.join_type = join_type;
     const bool first_match_only_c = h->unique || join_type != GX_JOIN_INNER;
-    const bool use_compact = h->cslots != nullptr && first_match_only_c;       // the 8-byte slots are probed as they are
+    const bool use_compact = (h->cslots != nullptr || h->narrow != nullptr) && first_match_only_c;   // 8- and 4-byte slots are probed as they are
     if (!use_compact) { int wrc = gx_hash_wide(ctx, const_cast<gx_hash *>(h)); if (wrc) return wrc; }
     a.nrows = outer->nrows; a.slots = h->slots; a.mask = (unsigned long long) h->nslots - 1;
-    a.cslots = h->cslots; a.cspan = h->cspan;
+    a.cslots = h->cslots; a.narrow = h->narrow; a.cspan = h->cspan;
     a.special = h->special_payload; a.special_count = h->special_count;
-    a.sf.mode = h->mode; a.sf.win = h->win; a.sf.shift = h->shift; a.sf.amask = h->amask; a.sf.kmin = h->kmin; a.sf.scale = h->scale; a.sf.mask = (unsigned long long) h->nslots - 1;
+    a.sf = gx_hash_slotfn(h);
     int rc = gx_fill_dpreds(ctx, outer, n_preds, preds, a.preds); if (rc) return rc;
     int32_t types[GX_MAX_COLS]; bool hn[GX_MAX_COLS];
     for (int c = 0; c < n_out_outer; c++) {
@@ -1493,8 +1597,9 @@ extern "C" int gx_hash_probe_ex(gx_ctx *ctx, const gx_table *outer, int key_col,
         if (first_match_only) {
             long long nt = (outer->nrows + 32 * PT_K * 8 - 1) / (32 * PT_K * 8);
             const unsigned pgrid = (unsigned) (nt < maxb ? (nt > 0 ? nt : 1) : maxb);
-            if (use_compact) gx_k_hash_probe_unique<true><<<pgrid, 256, 0, ctx->stream>>>(a);
-            else gx_k_hash_probe_unique<false><<<pgrid, 256, 0, ctx->stream>>>(a);
+            if (use_compact && h->narrow) gx_k_hash_probe_unique<GX_SLOTS_NARROW><<<pgrid, 256, 0, ctx->stream>>>(a);
+            else if (use_compact) gx_k_hash_probe_unique<GX_SLOTS_COMPACT><<<pgrid, 256, 0, ctx->stream>>>(a);
+            else gx_k_hash_probe_unique<GX_SLOTS_WIDE><<<pgrid, 256, 0, ctx->stream>>>(a);
         } else gx_k_hash_probe<<<grid, 256, 0, ctx->stream>>>(a);
     }
     cudaError_t e = cudaMemcpyAsync(ctx->h_scratch, a.cursor, sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream);

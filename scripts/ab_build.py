@@ -28,7 +28,8 @@ ctx.profile(True)
 reps = 20
 for _ in range(reps):
     ht = ctx.hash_build(ot, 0, [1], unique=True); info = ht.info(); nent = ht.nentries; ht.free()
-names = ("build", "build_bounds", "build_sample", "build_fill_staged", "build_fill_rows", "build_sorted_search", "build_compact")
+names = ("build", "build_bounds", "build_sample", "build_fill_staged", "build_fill_rows", "build_sorted_search", "build_compact",
+         "build_narrow", "build_narrow_refill")
 ph = {k: ctx.profile_get(k) for k in names}
 ctx.profile(False)
 ot.free()
