@@ -132,8 +132,16 @@ typedef struct gx_agg_plan {
                                             shared-memory vs radix strategy  */
     int32_t   strategy;                  /* 0 = auto, 1 = force shared-memory
                                             privatised, 2 = force two-pass radix */
-    int32_t   _pad;
+    int32_t   join_type;                 /* GX_JOIN_INNER (0), GX_JOIN_SEMI or
+                                            GX_JOIN_ANTI; see below            */
 } gx_agg_plan;
+/* join_type of an aggregate over a hash join (ExecHashJoinImpl, nodeHashjoin.c:569-634):
+ *   INNER  every (outer row, build row) pair with equal keys is one input row of the aggregate;
+ *   SEMI   an outer row is consumed once if at least one build row has its key, however many do;
+ *   ANTI   the outer rows without a partner are consumed, NULL keys included (HJ_FILL_OUTER_TUPLE).
+ * The outer quals (preds) apply before the join, as for INNER; a NULL key has no partner.  SEMI and
+ * ANTI carry no inner column: a group column of side 1 is GX_ERR_ARG.  Any other join type (LEFT
+ * included) is GX_ERR_ARG, and the context stays usable. */
 
 /* ---- context ------------------------------------------------------------ */
 /* Lazily creates the CUDA context (never from postmaster's _PG_init: fork after

@@ -73,7 +73,7 @@ class GxAggPlan(C.Structure):
                 ("group_cols", GxColRef * 4),
                 ("aggs", GxAgg * 8),
                 ("est_groups", C.c_int64),
-                ("strategy", C.c_int32), ("_pad", C.c_int32)]
+                ("strategy", C.c_int32), ("join_type", C.c_int32)]
 
 
 class GxHeapDesc(C.Structure):
@@ -202,7 +202,7 @@ def mk_pred(col, op, const, is_float=False) -> GxPred:
     return q
 
 
-def make_plan(preds=(), outer_key_col=-1, group_cols=(), aggs=(), est_groups=0, strategy=0) -> GxAggPlan:
+def make_plan(preds=(), outer_key_col=-1, group_cols=(), aggs=(), est_groups=0, strategy=0, join_type=0) -> GxAggPlan:
     """preds: (col, op, const[, is_float]); group_cols: (side, col);
     aggs: (fn, [(op, col, k), ...])  — postfix argument program."""
     p = GxAggPlan()
@@ -221,6 +221,7 @@ def make_plan(preds=(), outer_key_col=-1, group_cols=(), aggs=(), est_groups=0, 
             p.aggs[i].arg.ops[j].op, p.aggs[i].arg.ops[j].col, p.aggs[i].arg.ops[j].k = op, col, float(k)
     p.est_groups = est_groups
     p.strategy = strategy
+    p.join_type = join_type
     return p
 
 

@@ -349,7 +349,12 @@ __device__ __forceinline__ unsigned long long lp_reduce_word(const SmemTable &T,
     return acc;                                   // valid in lane 0
 }
 
-template <int SINK>
+// XF < 0: no join, or an INNER join walked row by row over the 16-byte table.  XF = GX_SLOTS_*: a SEMI / ANTI join
+// (nodeHashjoin.c:569-634), an existence test per outer row in the format the build wrote: PT_K x 32 rows per warp and
+// tile, their home-group loads in flight together (gx_probe_first, the walk gx_k_hash_probe_unique runs).  SEMI consumes
+// a row once when its key has a partner, however many; ANTI a row that passed the quals and has none, a NULL key
+// included (HJ_FILL_OUTER_TUPLE).  Neither reads an inner column.
+template <int SINK, int XF>
 __global__ void __launch_bounds__(1024, 1) gx_k_agg(const __grid_constant__ gx_agg_dev A)
 {
     extern __shared__ unsigned long long smem[];
@@ -379,33 +384,59 @@ __global__ void __launch_bounds__(1024, 1) gx_k_agg(const __grid_constant__ gx_a
         __syncthreads();
     }
     const gx_dplan &P = A.P;
-    long long stride = (long long) gridDim.x * blockDim.x;
-    // warp-uniform loop: every lane of a warp makes the same number of trips (lanes past the end idle)
     const int lane = threadIdx.x & 31;
-    for (long long r = A.row0 + (long long) blockIdx.x * blockDim.x + threadIdx.x; r - lane < A.row1; r += stride) {
-        bool ok = r < A.row1;
+    if constexpr (XF >= 0) {
+        const bool anti = P.join_type == GX_JOIN_ANTI;
+        const long long tile = 32LL * PT_K, step = (long long) gridDim.x * nwarps * tile;
+        for (long long base = A.row0 + ((long long) blockIdx.x * nwarps + (threadIdx.x >> 5)) * tile; base < A.row1; base += step) {
+            long long r[PT_K], key[PT_K]; bool scanned[PT_K], ok[PT_K], hit[PT_K]; unsigned long long pay[PT_K];
 #pragma unroll
-        for (int p = 0; p < GX_MAX_PREDS; p++) if (p < P.npreds) ok = ok && gx_eval_pred(P.preds[p], ok ? r : A.row0);
-        if (!P.has_join) {
-            // exactly the lanes that consume a row now; the barrier only pays when a row has several
-            // state words to update (with one counter it cost 20 % on the config-1 shape)
-            const unsigned int m = P.nwords >= 3 ? __ballot_sync(0xffffffffu, ok) : 0u;
-            if (ok) consume_row<SINK>(A, T, r, 0ULL, m);
-            continue;
+            for (int j = 0; j < PT_K; j++) { r[j] = base + j * 32 + lane; scanned[j] = r[j] < A.row1; }
+            for (int p = 0; p < P.npreds; p++) pred_tile<PT_K>(P.preds[p], r, scanned);
+#pragma unroll
+            for (int j = 0; j < PT_K; j++) ok[j] = scanned[j] && !gx_is_null(P.okey, r[j]);      // a NULL key never has a partner
+#pragma unroll
+            for (int j = 0; j < PT_K; j++) key[j] = ok[j] ? gx_load_int(P.okey, r[j]) : 0;
+            gx_probe_first<XF, PT_K>(A, ok, key, hit, pay);
+            unsigned int pass = 0;
+#pragma unroll
+            for (int j = 0; j < PT_K; j++) pass |= (unsigned int) (anti ? scanned[j] && !hit[j] : hit[j]) << j;
+            // one inlined copy of the aggregate update per tile, not PT_K: the row of step j is base + 32 j + lane
+#pragma unroll 1
+            for (int j = 0; j < PT_K; j++) {
+                const bool take = (pass >> j) & 1u;
+                const unsigned int m = P.nwords >= 3 ? __ballot_sync(0xffffffffu, take) : 0u;
+                if (take) consume_row<SINK>(A, T, base + j * 32 + lane, 0ULL, m);
+            }
         }
-        if (!ok) continue;
-        if (gx_is_null(P.okey, r)) continue;                  // NULL outer key never joins
-        long long key = gx_load_int(P.okey, r);
-        if (key == GX_EMPTY_KEY) {
-            for (int i = 0; i < A.special_count; i++) { consume_row<SINK>(A, T, r, A.special[i]); if (P.unique) break; }
-            continue;
-        }
-        unsigned long long s = gx_slot_index(key, A.sf);
-        for (;;) {
-            gx_slot sl = A.slots[s];
-            if (sl.key == GX_EMPTY_KEY) break;
-            if (sl.key == key) { consume_row<SINK>(A, T, r, sl.payload); if (P.unique) break; }
-            s = gx_next_slot(s, A.mask);
+    } else {
+        long long stride = (long long) gridDim.x * blockDim.x;
+        // warp-uniform loop: every lane of a warp makes the same number of trips (lanes past the end idle)
+        for (long long r = A.row0 + (long long) blockIdx.x * blockDim.x + threadIdx.x; r - lane < A.row1; r += stride) {
+            bool ok = r < A.row1;
+#pragma unroll
+            for (int p = 0; p < GX_MAX_PREDS; p++) if (p < P.npreds) ok = ok && gx_eval_pred(P.preds[p], ok ? r : A.row0);
+            if (!P.has_join) {
+                // exactly the lanes that consume a row now; the barrier only pays when a row has several
+                // state words to update (with one counter it cost 20 % on the config-1 shape)
+                const unsigned int m = P.nwords >= 3 ? __ballot_sync(0xffffffffu, ok) : 0u;
+                if (ok) consume_row<SINK>(A, T, r, 0ULL, m);
+                continue;
+            }
+            if (!ok) continue;
+            if (gx_is_null(P.okey, r)) continue;                  // NULL outer key never joins
+            long long key = gx_load_int(P.okey, r);
+            if (key == GX_EMPTY_KEY) {
+                for (int i = 0; i < A.special_count; i++) { consume_row<SINK>(A, T, r, A.special[i]); if (P.unique) break; }
+                continue;
+            }
+            unsigned long long s = gx_slot_index(key, A.sf);
+            for (;;) {
+                gx_slot sl = A.slots[s];
+                if (sl.key == GX_EMPTY_KEY) break;
+                if (sl.key == key) { consume_row<SINK>(A, T, r, sl.payload); if (P.unique) break; }
+                s = gx_next_slot(s, A.mask);
+            }
         }
     }
     if (!IS_SMEM) return;
@@ -2377,15 +2408,27 @@ struct compiled_plan {
     int need_w0;
 };
 
+// LEFT is not among them: its inner-side group columns would have to turn NULL on a miss in every sink
+int gx_check_agg_join_type(gx_ctx *ctx, const gx_agg_plan *plan)
+{
+    const int jt = plan->join_type;
+    GX_CHECK_ARG(ctx, jt == GX_JOIN_INNER || jt == GX_JOIN_SEMI || jt == GX_JOIN_ANTI,
+                 "agg plan: join type %d not supported under an aggregate (inner %d, semi %d, anti %d)", jt, GX_JOIN_INNER, GX_JOIN_SEMI, GX_JOIN_ANTI);
+    return GX_OK;
+}
+
 static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, compiled_plan *cp)
 {
     memset(cp, 0, sizeof(*cp));
     gx_dplan &P = cp->A.P;
     GX_CHECK_ARG(ctx, plan->n_aggs >= 0 && plan->n_aggs <= GX_MAX_AGGS, "agg plan: n_aggs %d", plan->n_aggs);
     GX_CHECK_ARG(ctx, plan->n_group_cols >= 0 && plan->n_group_cols <= GX_MAX_GROUP_COLS, "agg plan: n_group_cols %d", plan->n_group_cols);
+    int rc = gx_check_agg_join_type(ctx, plan); if (rc) return rc;
     P.npreds = plan->n_preds;
-    int rc = gx_fill_dpreds(ctx, outer, plan->n_preds, plan->preds, P.preds); if (rc) return rc;
+    rc = gx_fill_dpreds(ctx, outer, plan->n_preds, plan->preds, P.preds); if (rc) return rc;
     P.has_join = plan->outer_key_col >= 0;
+    P.join_type = plan->join_type;
+    GX_CHECK_ARG(ctx, P.has_join || P.join_type == GX_JOIN_INNER, "agg plan: a semi or anti join needs an outer key column");
     if (P.has_join) {
         GX_CHECK_ARG(ctx, h != nullptr, "agg plan: join requested but no hash table given");
         GX_CHECK_ARG(ctx, plan->outer_key_col < outer->ncols, "agg plan: outer key column out of range");
@@ -2411,6 +2454,7 @@ static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
             GX_CHECK_ARG(ctx, col >= 0 && col < outer->ncols, "agg plan: group column %d out of range", col);
             g.col = dcol_of(outer, col); type = outer->types[col];
         } else {
+            GX_CHECK_ARG(ctx, P.join_type == GX_JOIN_INNER, "agg plan: a semi or anti join carries no inner column (group column %d)", c);
             GX_CHECK_ARG(ctx, h != nullptr && h->n_payload > 0, "agg plan: group column refers to a join payload but none is carried");
             int pi = plan->group_cols[c].col;
             GX_CHECK_ARG(ctx, pi >= 0 && pi < h->n_payload, "agg plan: payload index %d out of range", pi);
@@ -2512,13 +2556,20 @@ static size_t smem_bytes_for(int S, int nkw, int nwords) { return (size_t) S * 8
 
 static int ilog2(long long x) { int l = 0; while ((1LL << l) < x) l++; return l; }
 
-template <int SINK>
-static int launch_agg(gx_ctx *ctx, const gx_agg_dev &A, size_t smem, const char *name, int threads = 1024)
+template <class FN> static int with_slot_format(const gx_agg_dev &A, FN fn)
 {
-    static bool attr_set[8] = { false };
-    if (!attr_set[SINK]) {
-        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_agg<SINK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
-        attr_set[SINK] = true;
+    if (A.narrow) return fn(std::integral_constant<int, GX_SLOTS_NARROW>());
+    if (A.cslots) return fn(std::integral_constant<int, GX_SLOTS_COMPACT>());
+    return fn(std::integral_constant<int, GX_SLOTS_WIDE>());
+}
+
+template <int SINK, int XF>
+static int launch_agg_k(gx_ctx *ctx, const gx_agg_dev &A, size_t smem, const char *name, int threads)
+{
+    static bool attr_set = false;
+    if (!attr_set) {
+        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_agg<SINK, XF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
+        attr_set = true;
     }
     long long nrows = A.row1 - A.row0;
     long long nb = (nrows + threads - 1) / threads, maxb = (long long) ctx->sm_count;
@@ -2528,9 +2579,19 @@ static int launch_agg(gx_ctx *ctx, const gx_agg_dev &A, size_t smem, const char 
     gx_launch_scope ls(ctx, name);
     // second profile name: which sink answered (gx_profile_get)
     gx_launch_scope which(ctx, SINK == SINK_SMEM_LP ? "agg_smem_lp" : SINK == SINK_SMEM ? "agg_smem" : SINK == SINK_GLOBAL ? "agg_global" : "agg_records", 0);
-    gx_k_agg<SINK><<<grid, threads, smem, ctx->stream>>>(A);
+    // third profile name of a SEMI / ANTI plan: the slot format its existence probe read
+    gx_launch_scope fmt(ctx, XF == GX_SLOTS_NARROW ? "probe_agg_exist_narrow" : XF == GX_SLOTS_COMPACT ? "probe_agg_exist_compact" :
+                             XF == GX_SLOTS_WIDE ? "probe_agg_exist_wide" : nullptr, 0);
+    gx_k_agg<SINK, XF><<<grid, threads, smem, ctx->stream>>>(A);
     GX_CUDA(ctx, cudaGetLastError());
     return GX_OK;
+}
+// the kernel of the plan's join type: row by row (no join, INNER), or the existence probe in the table's own format
+template <int SINK>
+static int launch_agg(gx_ctx *ctx, const gx_agg_dev &A, size_t smem, const char *name, int threads = 1024)
+{
+    if (A.P.join_type == GX_JOIN_INNER) return launch_agg_k<SINK, -1>(ctx, A, smem, name, threads);
+    return with_slot_format(A, [&](auto f) { return launch_agg_k<SINK, decltype(f)::value>(ctx, A, smem, name, threads); });
 }
 
 template <int K>
@@ -2716,12 +2777,6 @@ static bool gx_runjoin_tma_enabled()
     return e && e[0] ? e[0] != '0' : GX_RUNJOIN_TMA_DEFAULT != 0;
 }
 // calls fn with the slot format of the plan's join table as a compile-time constant (std::integral_constant)
-template <class FN> static int with_slot_format(const gx_agg_dev &A, FN fn)
-{
-    if (A.narrow) return fn(std::integral_constant<int, GX_SLOTS_NARROW>());
-    if (A.cslots) return fn(std::integral_constant<int, GX_SLOTS_COMPACT>());
-    return fn(std::integral_constant<int, GX_SLOTS_WIDE>());
-}
 static int launch_fast(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_args &FA, bool join, bool cnt, bool sum, size_t smem, const char *name, bool use_run)
 {
     // gx_k_runjoin3: finished runs wait for a full round of 32 (GX_RUNJOIN_CARRY=1; A/B against gx_k_runjoin)
@@ -2857,7 +2912,9 @@ static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
     // ---- does the plan have the shape the specialised kernel was written for?
     gx_fast_args FA; memset(&FA, 0, sizeof(FA));
     { const char *pf = getenv("GX_RUNJOIN_PF"); FA.pf = pf ? atoi(pf) : 0; }
-    bool fast_ok = plan->n_preds == 0 && plan->n_group_cols == 1 && tagkey && outer->nrows > 0;
+    // the specialised kernels below join; a SEMI / ANTI plan takes gx_k_agg's existence probe
+    const bool exist = A.P.join_type != GX_JOIN_INNER;
+    bool fast_ok = !exist && plan->n_preds == 0 && plan->n_group_cols == 1 && tagkey && outer->nrows > 0;
     if (fast_ok) {
         const gx_dgroupcol &gc = A.P.gcols[0];
         if (A.P.has_join) {
@@ -2878,9 +2935,9 @@ static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
         }
     }
 
-    // only gx_k_runjoin reads the compact table form; everything else needs the 16-byte slots
+    // only gx_k_runjoin and the existence probe read the compact and narrow table forms; everything else needs the 16-byte slots
     auto need_wide = [&]() -> int {
-        if (!h || A.slots) return GX_OK;
+        if (!h || A.slots || exist) return GX_OK;
         int wrc = gx_hash_wide(ctx, const_cast<gx_hash *>(h));
         A.slots = h->slots;
         return wrc;
@@ -2929,7 +2986,7 @@ static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
         gx_runagg_args RA; memset(&RA, 0, sizeof(RA));
         { const char *pf = getenv("GX_RUNAGG_PF"); RA.pf = pf ? atoi(pf) : 1; }     // bit 0: rows two tiles ahead into L2, bit 1: the tile's join-table lines
         const char *e = getenv("GX_NO_RUNAGG");
-        bool ok = !(e && e[0] == '1') && plan->strategy == 0 && A.P.has_join && h->unique && A.P.key_type == GX_INT8 && A.P.okey.nulls == nullptr &&
+        bool ok = !(e && e[0] == '1') && !exist && plan->strategy == 0 && A.P.has_join && h->unique && A.P.key_type == GX_INT8 && A.P.okey.nulls == nullptr &&
                   outer->nrows > 0 && plan->n_group_cols >= 1;
         bool has_key = false;
         for (int c = 0; c < plan->n_group_cols && ok; c++) {
@@ -3479,7 +3536,7 @@ static int run_radix(gx_ctx *ctx, compiled_plan *cp, const gx_agg_plan *plan, lo
         GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d_recs, (size_t) (cap > 0 ? cap : 1) * RW * 8));
         GX_CUDA(ctx, cudaMemsetAsync(A.counters, 0, 4 * sizeof(long long), ctx->stream));
         A.recs = d_recs; A.rec_cap = cap; A.s_slots = 0;
-        int rc = launch_agg<SINK_RECORD>(ctx, A, 0, A.P.has_join ? "probe_records" : "scan_records");
+        int rc = launch_agg<SINK_RECORD>(ctx, A, 0, A.P.join_type != GX_JOIN_INNER ? "probe_agg" : A.P.has_join ? "probe_records" : "scan_records");
         long long c[4];
         if (rc == GX_OK) rc = read_counters(ctx, c);
         if (rc != GX_OK) { gx_tmp_free(ctx, d_recs); return rc; }

@@ -126,9 +126,10 @@ extern "C" int gx_exec_host(gx_ctx *ctx, const gx_host_table *outer, const gx_ho
                             int inner_unique, const gx_agg_plan *plan, gx_result **out)
 {
     if (!ctx || !outer || !plan || !out) return GX_ERR_ARG;
+    int rc = gx_check_agg_join_type(ctx, plan); if (rc) return rc;      // before any upload
     gx_table *to = nullptr, *ti = nullptr; gx_hash *h = nullptr;
     const bool join = inner && plan->outer_key_col >= 0;
-    int rc = GX_OK, rr = 0;
+    int rr = 0;
     if (join) rc = upload_alloc(ctx, inner, &ti);
     if (rc == GX_OK) rc = upload_alloc(ctx, outer, &to);
     if (rc == GX_OK) {

@@ -197,6 +197,8 @@ static inline void gx_tmp_free(gx_ctx *ctx, void *p) { if (p) cudaFreeAsync(p, c
 int gx_table_alloc_like(gx_ctx *ctx, int ncols, const int32_t *types, const bool *has_nulls,
                         int64_t capacity, gx_table **out);
 int gx_result_alloc(gx_ctx *ctx, const gx_agg_plan *plan, const int32_t *group_types, int64_t cap, gx_result **out);
+// GX_ERR_ARG unless the plan's join type is one gx_hash_agg runs (INNER, SEMI, ANTI)
+int gx_check_agg_join_type(gx_ctx *ctx, const gx_agg_plan *plan);
 
 // device-side plan descriptors -------------------------------------------
 struct gx_dcol { const void *data; const uint8_t *nulls; int type; int _pad; };
@@ -228,7 +230,7 @@ struct gx_dplan {
     gx_dgroupcol gcols[GX_MAX_GROUP_COLS];
     gx_dagg aggs[GX_MAX_AGGS];
     int payload_types[GX_MAX_PAYLOAD];
-    int n_payload; int _pad;
+    int n_payload; int join_type;       // GX_JOIN_INNER / _SEMI / _ANTI
 };
 
 #ifdef __CUDACC__
@@ -479,6 +481,94 @@ __device__ __forceinline__ bool gx_nslot_group(const uint4 &q, unsigned int tag,
     payload = gx_nslot_payload(h0 ? q.x : h1 ? q.y : h2 ? q.z : q.w, f);
     return found | (q.x == 0u) | (q.y == 0u) | (q.z == 0u) | (q.w == 0u);
 }
+// two 16-byte slots (one 32-byte sector) as two 128-bit loads (sm_90 has no 256-bit load)
+__device__ __forceinline__ void gx_ld_pair(const gx_slot *p, long long &k0, unsigned long long &p0, long long &k1, unsigned long long &p1)
+{
+    asm volatile("ld.global.v2.u64 {%0, %1}, [%4];\n\tld.global.v2.u64 {%2, %3}, [%4+16];"
+                 : "=l"(k0), "=l"(p0), "=l"(k1), "=l"(p1) : "l"(p));
+}
+#define PT_K 4                            /* rows per lane of a probe tile (gx_k_hash_probe_unique, gx_k_agg_exist) */
+// First-match walk of K probe keys per lane over a join table in the format the build wrote (F: gx_slot, gx_cslot or
+// narrow), never the 16-byte expansion of a compact or narrow one.  Every row's home group is loaded before any walk
+// starts, so the K loads are in flight together.  ok[j] = false: no probe, hit[j] = false.  hit[j] / pay[j]: the key has a
+// partner / the first partner's payload.  A key INT64_MIN lives in the side list of a 16-byte table (the compact and
+// narrow builds take no such key, and their span test rejects it).  TAB: an argument block carrying the join-table
+// fields (slots, cslots, narrow, cspan, mask, sf, special, special_count).
+template <int F, int K, class TAB>
+__device__ __forceinline__ void gx_probe_first(const TAB &a, const bool (&ok)[K], const long long (&key)[K], bool (&hit)[K], unsigned long long (&pay)[K])
+{
+    unsigned long long s[K];
+    long long k0[K], k1[K]; unsigned long long p0[K], p1[K];
+    if (F == GX_SLOTS_NARROW) {
+        // four 4-byte slots per 16-byte group, one load each (gx_nslot_group)
+        uint4 q[K]; unsigned int tg[K];
+#pragma unroll
+        for (int j = 0; j < K; j++) {
+            const bool inspan = ok[j] && ((unsigned long long) key[j] - (unsigned long long) a.sf.kmin) < a.cspan;   // outside the build side's key span: no partner
+            s[j] = gx_slot_index(key[j], a.sf);
+            tg[j] = gx_nslot_tag(key[j], a.sf);
+            q[j] = inspan ? gx_nslot_ld(a.narrow + s[j]) : make_uint4(0u, 0u, 0u, 0u);    // an empty group ends the walk unmatched
+        }
+#pragma unroll
+        for (int j = 0; j < K; j++) {
+            hit[j] = false; pay[j] = 0;
+            if (!ok[j]) continue;
+            for (;;) {
+                bool f; int pv;
+                if (gx_nslot_group(q[j], tg[j], a.sf, f, pv)) { hit[j] = f; pay[j] = (unsigned long long) (unsigned int) pv; break; }
+                s[j] = gx_next_quad(s[j], a.mask);
+                q[j] = gx_nslot_ld(a.narrow + s[j]);
+            }
+        }
+    } else if (F == GX_SLOTS_COMPACT) {
+        // four 8-byte slots {d, payload} per 32-byte sector; d = ((key - kmin) << 1) | 1 truncated to 32 bits, 0 = empty
+        unsigned int d[K];
+#pragma unroll
+        for (int j = 0; j < K; j++) {
+            const bool inspan = ok[j] && ((unsigned long long) key[j] - (unsigned long long) a.sf.kmin) < a.cspan;   // outside the build side's key span: no partner
+            s[j] = gx_slot_index(key[j], a.sf);
+            d[j] = GX_CSLOT_D(key[j], a.sf.kmin);
+            k0[j] = k1[j] = 0; p0[j] = p1[j] = 0;
+            if (inspan) gx_ld_pair((const gx_slot *) (a.cslots + s[j]), k0[j], p0[j], k1[j], p1[j]);
+            else d[j] = 0xfffffffeu;                               // even: matches no stored d (they are odd), the all-zero group ends the walk
+        }
+#pragma unroll
+        for (int j = 0; j < K; j++) {
+            hit[j] = false; pay[j] = 0;
+            if (!ok[j]) continue;
+            for (;;) {
+                const unsigned int d0 = (unsigned int) k0[j], d1 = (unsigned int) p0[j], d2 = (unsigned int) k1[j], d3 = (unsigned int) p1[j];
+                const unsigned long long m = d0 == d[j] ? (unsigned long long) k0[j] : d1 == d[j] ? p0[j] : d2 == d[j] ? (unsigned long long) k1[j] : p1[j];
+                hit[j] = (d0 == d[j]) | (d1 == d[j]) | (d2 == d[j]) | (d3 == d[j]);
+                pay[j] = m >> 32;
+                if (hit[j] | (d0 == 0u) | (d1 == 0u) | (d2 == 0u) | (d3 == 0u)) break;
+                s[j] = gx_next_quad(s[j], a.mask);
+                gx_ld_pair((const gx_slot *) (a.cslots + s[j]), k0[j], p0[j], k1[j], p1[j]);
+            }
+        }
+    } else {
+#pragma unroll
+        for (int j = 0; j < K; j++) {
+            s[j] = gx_slot_index(key[j], a.sf);            k0[j] = k1[j] = GX_EMPTY_KEY; p0[j] = p1[j] = 0;
+            if (ok[j] && key[j] != GX_EMPTY_KEY) gx_ld_pair(a.slots + s[j], k0[j], p0[j], k1[j], p1[j]);
+        }
+#pragma unroll
+        for (int j = 0; j < K; j++) {
+            hit[j] = false; pay[j] = 0;
+            if (!ok[j]) continue;
+            if (key[j] == GX_EMPTY_KEY) { hit[j] = a.special_count > 0; if (hit[j]) pay[j] = a.special[0]; continue; }
+            for (;;) {
+                if (k0[j] == key[j]) { hit[j] = true; pay[j] = p0[j]; break; }
+                if (k0[j] == GX_EMPTY_KEY) break;
+                if (k1[j] == key[j]) { hit[j] = true; pay[j] = p1[j]; break; }
+                if (k1[j] == GX_EMPTY_KEY) break;
+                s[j] = gx_next_pair(s[j], a.mask);
+                gx_ld_pair(a.slots + s[j], k0[j], p0[j], k1[j], p1[j]);
+            }
+        }
+    }
+}
+
 // the key of a compact or narrow entry in slot i from its tag bits v = (key - kmin) mod 2^mbits: the offset congruent to v
 // nearest the interpolation's estimate i keys_per_slot
 __device__ __forceinline__ long long gx_tag_key(long long i, unsigned long long v, int mbits, long long kmin, double keys_per_slot)

@@ -1403,14 +1403,7 @@ __global__ void __launch_bounds__(256) gx_k_hash_probe(gx_probe_args a)
 // tiles of 4 x 32 rows: the four key loads and then the four home-pair loads (one 32-byte sector each) are in
 // flight together, matches are numbered with ballots and the warp claims its output range with ONE atomic per
 // tile; the surviving rows are copied column by column.
-#define PT_K 4
 template <int F> __global__ void gx_k_hash_probe_unique(gx_probe_args a);
-__device__ __forceinline__ void ld_pair(const gx_slot *p, long long &k0, unsigned long long &p0, long long &k1, unsigned long long &p1)
-{
-    // one 32-byte sector as two 128-bit loads (sm_90 has no 256-bit load)
-    asm volatile("ld.global.v2.u64 {%0, %1}, [%4];\n\tld.global.v2.u64 {%2, %3}, [%4+16];"
-                 : "=l"(k0), "=l"(p0), "=l"(k1), "=l"(p1) : "l"(p));
-}
 template <int F>
 // no min-blocks on purpose: any value (even 1 or 4, which leave the occupancy as it is) changes ptxas' schedule
 // of the independent loads this kernel keeps in flight
@@ -1421,7 +1414,7 @@ __global__ void __launch_bounds__(256) gx_k_hash_probe_unique(gx_probe_args a)
     const long long nwarp = ((long long) gridDim.x * blockDim.x) >> 5, wid = ((long long) blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const long long tile = 32LL * PT_K;
     for (long long base = wid * tile; base < a.nrows; base += nwarp * tile) {
-        long long r[PT_K], key[PT_K]; bool ok[PT_K], hit[PT_K], quals_ok[PT_K]; unsigned long long pay[PT_K], s[PT_K];
+        long long r[PT_K], key[PT_K]; bool ok[PT_K], hit[PT_K], quals_ok[PT_K]; unsigned long long pay[PT_K];
 #pragma unroll
         for (int j = 0; j < PT_K; j++) { r[j] = base + j * 32 + lane; quals_ok[j] = r[j] < a.nrows; }
         for (int p = 0; p < a.npreds; p++) {
@@ -1432,75 +1425,7 @@ __global__ void __launch_bounds__(256) gx_k_hash_probe_unique(gx_probe_args a)
         for (int j = 0; j < PT_K; j++) ok[j] = quals_ok[j] && !gx_is_null(a.key, r[j]);      // a NULL key never matches (hashStrict)
 #pragma unroll
         for (int j = 0; j < PT_K; j++) key[j] = ok[j] ? gx_load_int(a.key, r[j]) : 0;
-        long long k0[PT_K], k1[PT_K]; unsigned long long p0[PT_K], p1[PT_K];
-        if (F == GX_SLOTS_NARROW) {
-            // four 4-byte slots per 16-byte group, one load each (gx_nslot_group)
-            uint4 q[PT_K]; unsigned int tg[PT_K];
-#pragma unroll
-            for (int j = 0; j < PT_K; j++) {
-                const bool inspan = ok[j] && ((unsigned long long) key[j] - (unsigned long long) a.sf.kmin) < a.cspan;   // outside the build side's key span: no partner
-                s[j] = gx_slot_index(key[j], a.sf);
-                tg[j] = gx_nslot_tag(key[j], a.sf);
-                q[j] = inspan ? gx_nslot_ld(a.narrow + s[j]) : make_uint4(0u, 0u, 0u, 0u);    // an empty group ends the walk unmatched
-            }
-#pragma unroll
-            for (int j = 0; j < PT_K; j++) {
-                hit[j] = false; pay[j] = 0;
-                if (!ok[j]) continue;
-                for (;;) {
-                    bool f; int pv;
-                    if (gx_nslot_group(q[j], tg[j], a.sf, f, pv)) { hit[j] = f; pay[j] = (unsigned long long) (unsigned int) pv; break; }
-                    s[j] = gx_next_quad(s[j], a.mask);
-                    q[j] = gx_nslot_ld(a.narrow + s[j]);
-                }
-            }
-        } else if (F == GX_SLOTS_COMPACT) {
-            // four 8-byte slots {d, payload} per 32-byte sector; d = ((key - kmin) << 1) | 1 truncated to 32 bits, 0 = empty
-            unsigned int d[PT_K];
-#pragma unroll
-            for (int j = 0; j < PT_K; j++) {
-                const bool inspan = ok[j] && ((unsigned long long) key[j] - (unsigned long long) a.sf.kmin) < a.cspan;   // outside the build side's key span: no partner
-                s[j] = gx_slot_index(key[j], a.sf);
-                d[j] = GX_CSLOT_D(key[j], a.sf.kmin);
-                k0[j] = k1[j] = 0; p0[j] = p1[j] = 0;
-                if (inspan) ld_pair((const gx_slot *) (a.cslots + s[j]), k0[j], p0[j], k1[j], p1[j]);
-                else d[j] = 0xfffffffeu;                               // even: matches no stored d (they are odd), the all-zero group ends the walk
-            }
-#pragma unroll
-            for (int j = 0; j < PT_K; j++) {
-                hit[j] = false; pay[j] = 0;
-                if (!ok[j]) continue;
-                for (;;) {
-                    const unsigned int d0 = (unsigned int) k0[j], d1 = (unsigned int) p0[j], d2 = (unsigned int) k1[j], d3 = (unsigned int) p1[j];
-                    const unsigned long long m = d0 == d[j] ? (unsigned long long) k0[j] : d1 == d[j] ? p0[j] : d2 == d[j] ? (unsigned long long) k1[j] : p1[j];
-                    hit[j] = (d0 == d[j]) | (d1 == d[j]) | (d2 == d[j]) | (d3 == d[j]);
-                    pay[j] = m >> 32;
-                    if (hit[j] | (d0 == 0u) | (d1 == 0u) | (d2 == 0u) | (d3 == 0u)) break;
-                    s[j] = gx_next_quad(s[j], a.mask);
-                    ld_pair((const gx_slot *) (a.cslots + s[j]), k0[j], p0[j], k1[j], p1[j]);
-                }
-            }
-        } else {
-#pragma unroll
-        for (int j = 0; j < PT_K; j++) {
-            s[j] = gx_slot_index(key[j], a.sf);            k0[j] = k1[j] = GX_EMPTY_KEY; p0[j] = p1[j] = 0;
-            if (ok[j] && key[j] != GX_EMPTY_KEY) ld_pair(a.slots + s[j], k0[j], p0[j], k1[j], p1[j]);
-        }
-#pragma unroll
-        for (int j = 0; j < PT_K; j++) {
-            hit[j] = false; pay[j] = 0;
-            if (!ok[j]) continue;
-            if (key[j] == GX_EMPTY_KEY) { hit[j] = a.special_count > 0; if (hit[j]) pay[j] = a.special[0]; continue; }
-            for (;;) {
-                if (k0[j] == key[j]) { hit[j] = true; pay[j] = p0[j]; break; }
-                if (k0[j] == GX_EMPTY_KEY) break;
-                if (k1[j] == key[j]) { hit[j] = true; pay[j] = p1[j]; break; }
-                if (k1[j] == GX_EMPTY_KEY) break;
-                s[j] = gx_next_pair(s[j], a.mask);
-                ld_pair(a.slots + s[j], k0[j], p0[j], k1[j], p1[j]);
-            }
-        }
-        }
+        gx_probe_first<F, PT_K>(a, ok, key, hit, pay);
         __syncwarp();
         // which rows produce output (nodeHashjoin.c:569-668): INNER/SEMI the matched ones, ANTI the unmatched ones
         // (HJ_FILL_OUTER_TUPLE without a match), LEFT all of them (unmatched with a NULL inner side)

@@ -428,7 +428,8 @@ gpuexec_serialise(const GpuExecState *st)
 				j;
 
 	l = put_int(l, GX_ABI_VERSION);
-	l = put_int(l, st->has_join);
+	/* 0 = no join, else 1 + GX_JOIN_*: an INNER join keeps the word it had before SEMI and ANTI existed */
+	l = put_int(l, st->has_join ? 1 + p->join_type : 0);
 	l = serialise_rel(l, &st->outer);
 	if (st->has_join)
 	{
@@ -490,7 +491,9 @@ gpuexec_deserialise(List *priv, GpuExecState *st)
 	if (get_int(&lc) != GX_ABI_VERSION)
 		ereport(ERROR, (errmsg("gpuexec: coordinator and datanode run different provider versions")));
 	memset(p, 0, sizeof(*p));
-	st->has_join = get_int(&lc);
+	i = get_int(&lc);
+	st->has_join = i != 0;
+	p->join_type = i != 0 ? i - 1 : GX_JOIN_INNER;
 	deserialise_rel(&lc, &st->outer);
 	if (st->has_join)
 	{
@@ -795,6 +798,8 @@ gpuexec_explain(CustomScanState *node, List *ancestors, ExplainState *es)
 	GpuExecState *st = (GpuExecState *) node;
 
 	ExplainPropertyText("GPU Strategy", st->has_join ? "hash build + fused probe/aggregate" : "scan + hash aggregate", es);
+	if (st->has_join)
+		ExplainPropertyText("GPU Join Type", st->plan.join_type == GX_JOIN_SEMI ? "Semi" : st->plan.join_type == GX_JOIN_ANTI ? "Anti" : "Inner", es);
 	ExplainPropertyText("GPU Output", st->partial ? "partial states (Finalize above the redistribute)" : "final values (GROUP BY covers the distribution key)", es);
 	if (es->analyze && st->done_exec)
 	{
@@ -847,6 +852,8 @@ gpuexec_plan_path(PlannerInfo *root, RelOptInfo *rel, CustomPath *best_path,
 /* ---- plan-shape analysis -------------------------------------------------
  * Accepts:   Agg(HASHED/PLAIN) over  SeqScan(R)                       (configs 1, 2, Q1)
  *            Agg over HashJoin[INNER, one int4/int8 equi-key](SeqScan(R), SeqScan(S))   (config 3)
+ *            Agg over HashJoin[SEMI / ANTI, the same key shape]  (EXISTS / NOT EXISTS: TPC-H Q4, Q21, Q22 shapes),
+ *            with GROUP BY columns and aggregate arguments from the outer side only
  * with "Var op Const" quals on the scans, Var group keys, no HAVING / grouping sets /
  * DISTINCT / ORDER BY aggregates / FILTER, and aggregates count(*), count(x),
  * sum/avg/min/max(float8 expr), sum(int4); every target-list entry must be a group Var or a
@@ -1153,7 +1160,16 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 		Var		   *lv,
 				   *rv;
 
-		if (hp->jpath.jointype != JOIN_INNER || list_length(hp->path_hashclauses) != 1 || hp->jpath.joinrestrictinfo == NIL ||
+		/* LEFT, RIGHT, FULL and the JOIN_UNIQUE_* forms stay on the CPU */
+		if (hp->jpath.jointype == JOIN_INNER)
+			plan->join_type = GX_JOIN_INNER;
+		else if (hp->jpath.jointype == JOIN_SEMI)
+			plan->join_type = GX_JOIN_SEMI;
+		else if (hp->jpath.jointype == JOIN_ANTI)
+			plan->join_type = GX_JOIN_ANTI;
+		else
+			return false;
+		if (list_length(hp->path_hashclauses) != 1 || hp->jpath.joinrestrictinfo == NIL ||
 			list_length(hp->jpath.joinrestrictinfo) != 1)
 			return false;
 		/* both inputs must be plain scans of co-located shards: a RemoteSubplan below the join
@@ -1214,7 +1230,7 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 			plan->group_cols[plan->n_group_cols].side = 0;
 			plan->group_cols[plan->n_group_cols].col = c;
 		}
-		else if (out->has_join && v->varno == out->inner.rti && out->n_payload < GX_MAX_PAYLOAD)
+		else if (out->has_join && plan->join_type == GX_JOIN_INNER && v->varno == out->inner.rti && out->n_payload < GX_MAX_PAYLOAD)
 		{
 			c = rel_column(&out->inner, v->varno, v->varattno, v->vartype, v->vartypmod);
 			if (c < 0)

@@ -503,7 +503,9 @@ static int plan_main(const char *path)
 			op->pathtype = T_SeqScan; op->parent = plan_rels[r].rel; op->rows = op->parent->tuples; op->total_cost = op->parent->pages + 0.01 * op->rows;
 			ip->pathtype = remote ? T_RemoteSubplan : T_SeqScan; ip->parent = plan_rels[r2].rel; ip->rows = ip->parent->tuples; ip->total_cost = ip->parent->pages + 0.01 * ip->rows;
 			ri->clause = plan_op(lv->vartype == INT8OID ? F_INT8EQ : lv->vartype == INT4OID ? F_INT4EQ : F_TEXTEQ, swap ? (Node *) rv : (Node *) lv, swap ? (Node *) lv : (Node *) rv);
-			hp->jpath.path.pathtype = T_HashJoin; hp->jpath.jointype = strstr(line, "left") ? JOIN_LEFT : JOIN_INNER; hp->jpath.inner_unique = u != 0;
+			hp->jpath.path.pathtype = T_HashJoin; hp->jpath.inner_unique = u != 0;
+			hp->jpath.jointype = strstr(line, "left") ? JOIN_LEFT : strstr(line, "semi") ? JOIN_SEMI : strstr(line, "anti") ? JOIN_ANTI :
+				strstr(line, "right") ? JOIN_RIGHT : strstr(line, "full") ? JOIN_FULL : JOIN_INNER;
 			hp->jpath.outerjoinpath = op; hp->jpath.innerjoinpath = ip; hp->jpath.joinrestrictinfo = list_make1(ri); hp->path_hashclauses = list_make1(ri);
 			input_rel = makeNode(RelOptInfo); input_rel->reloptkind = RELOPT_JOINREL; input_rel->rows = op->rows;
 			hp->jpath.path.parent = input_rel; hp->jpath.path.rows = op->rows; hp->jpath.path.total_cost = op->total_cost + ip->total_cost + 0.02 * op->rows;
@@ -721,6 +723,7 @@ int main(int argc, char **argv)
 		for (i = 0; i < desc.n_inner_preds; i++)
 			if (desc.inner_preds[i].ival != got.inner_preds[i].ival || memcmp(&desc.inner_preds[i].fval, &got.inner_preds[i].fval, 8) != 0) { fprintf(stderr, "harness: inner qual constant %d changed\n", i); return 3; }
 		if (desc.plan.est_groups != got.plan.est_groups) { fprintf(stderr, "harness: est_groups changed\n"); return 3; }
+		if (desc.plan.join_type != got.plan.join_type) { fprintf(stderr, "harness: join type changed\n"); return 3; }
 		printf("ship ok: %d nodes, %zu bytes\n%s\n", list_length(priv), strlen(wire), wire);
 		return 0;
 	}
