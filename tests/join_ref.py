@@ -15,27 +15,15 @@ import numpy as np
 
 import opentenbase_b200 as g
 import exact_ref as X
+import qual_ref as Q
 
 NULL = np.iinfo(np.int64).min
 
 
 def quals(cols, nulls, preds, n):
-    """rows passing every qual (col, op, const[, is_float]); a NULL fails, float8 compares as float8_cmp (NaN last)"""
-    keep = np.ones(n, bool)
-    for p in preds:
-        col, op, k = p[0], p[1], p[2]
-        v = np.asarray(cols[col])
-        if v.dtype.kind == "f":
-            x, k = v.astype(np.float64), float(k)
-            c = np.where(np.isnan(x), 0 if np.isnan(k) else 1, np.where(np.isnan(k), -1, np.sign(x - k)))
-        else:
-            x, k = v.astype(np.int64), int(k)
-            c = np.where(x > k, 1, np.where(x < k, -1, 0))
-        ok = {g.GX_LT: c < 0, g.GX_LE: c <= 0, g.GX_EQ: c == 0, g.GX_GE: c >= 0, g.GX_GT: c > 0, g.GX_NE: c != 0}[op]
-        if nulls is not None and nulls[col] is not None:
-            ok &= ~np.asarray(nulls[col]).astype(bool)
-        keep &= ok
-    return keep
+    """rows passing every qual (col, op, const[, is_float]) under tests/qual_ref.py's semantics: a NULL fails, float8
+    compares as float8_cmp (NaN last), an int8 numpy column is "char" and compares as uint8"""
+    return Q.quals(cols, nulls, preds, n)
 
 
 def _key(v, nl):
