@@ -352,6 +352,35 @@ int  gx_hash_probe_ex(gx_ctx *ctx, const gx_table *outer, int key_col,
 int  gx_hash_agg(gx_ctx *ctx, const gx_table *outer, const gx_hash *h,
                  const gx_agg_plan *plan, gx_result **out);
 
+/* Aggregate over a chain of unique INNER hash joins in one probe pass, without an intermediate join
+ * (a left-deep HashJoin(HashJoin(outer, d1), d2) ... whose every level has inner_unique, nodeHashjoin.c:859-861).
+ * The outer table probes steps[0].h, then steps[1].h, ...; an outer row reaches the aggregate only when every
+ * step finds its key, and at most once, since every table was built with unique = 1.
+ *   steps[i].key   side 0: outer column key.col; side s (1 <= s <= i): payload column key.col of step s
+ *                  (steps are numbered from 1).  The key column is INT4, INT8 or DATE; a payload key widens
+ *                  as a column key does (INT4/DATE sign-extended, INT8 whole; INT64_MIN is an ordinary key).
+ *                  A payload is never NULL: gx_hash_build declines a nullable payload column.
+ *   plan           outer_key_col = -1, join_type = GX_JOIN_INNER; the preds apply to the outer table;
+ *                  group_cols[c].side = 0 for an outer column or s (1..n_steps) for payload column col of
+ *                  step s; aggregate arguments read outer columns only.
+ * The result is an ordinary gx_result.  n_steps == 1 is gx_hash_agg with outer_key_col = steps[0].key.col.
+ * Steps 2.. are probed in the 16-byte slot form: a table built compact or narrow gets that form materialised and
+ * attached to it (as gx_hash_agg does for the single-join kernels that need it), nslots x 16 bytes of HBM held until
+ * gx_hash_free.
+ * GX_ERR_ARG, the context staying usable: n_steps outside 1..GX_MAX_JOINS, a NULL or non-unique table, a key
+ * of its own or a later step, a key column not INT4/INT8/DATE, a payload index out of range, a group column
+ * side past n_steps, plan->outer_key_col >= 0, or a join type other than GX_JOIN_INNER. */
+#define GX_MAX_JOINS 3
+typedef struct gx_join_step {
+    const gx_hash *h;         /* built with unique = 1                                            */
+    gx_colref      key;       /* side 0: outer column; side s (1 <= s < this step's number):
+                                 payload column key.col of step s                                 */
+    int32_t        join_type; /* GX_JOIN_INNER; anything else is GX_ERR_ARG                        */
+    int32_t        _pad;
+} gx_join_step;
+int  gx_hash_agg_joins(gx_ctx *ctx, const gx_table *outer, int n_steps, const gx_join_step *steps,
+                       const gx_agg_plan *plan, gx_result **out);
+
 /* Combine partial states across datanodes: redistribute groups on the group
  * key, then Finalize HashAggregate (xc_groupby.out:193-205; combine fns
  * int8pl / float8pl / float8_combine).  No-op when no communicator. */

@@ -76,6 +76,13 @@ class GxAggPlan(C.Structure):
                 ("strategy", C.c_int32), ("join_type", C.c_int32)]
 
 
+class GxJoinStep(C.Structure):
+    _fields_ = [("h", C.c_void_p), ("key", GxColRef), ("join_type", C.c_int32), ("_pad", C.c_int32)]
+
+
+GX_MAX_JOINS = 3
+
+
 class GxHeapDesc(C.Structure):
     _fields_ = [("natts", C.c_int32), ("ncols", C.c_int32),
                 ("att_len", C.c_int16 * 64), ("att_align", C.c_int8 * 64),
@@ -166,6 +173,7 @@ def _declare(L):
         "gx_hash_probe": (C.c_int, [vp, vp, C.c_int, C.c_int, C.POINTER(GxPred), vp, C.c_int, C.POINTER(i32), pp]),
         "gx_hash_probe_ex": (C.c_int, [vp, vp, C.c_int, C.c_int, C.POINTER(GxPred), vp, C.c_int, C.c_int, C.POINTER(i32), pp]),
         "gx_hash_agg": (C.c_int, [vp, vp, vp, C.POINTER(GxAggPlan), pp]),
+        "gx_hash_agg_joins": (C.c_int, [vp, vp, C.c_int, C.POINTER(GxJoinStep), C.POINTER(GxAggPlan), pp]),
         "gx_result_combine": (C.c_int, [vp, vp]),
         "gx_result_ngroups": (i64, [vp]),
         "gx_result_fetch": (C.c_int, [vp, i64, vp, vp, vp]),
@@ -566,6 +574,18 @@ class Context:
     def hash_agg(self, outer: Table, plan: GxAggPlan, ht: HashTable | None = None) -> Result:
         h = C.c_void_p()
         self._chk(lib().gx_hash_agg(self.h, outer.h, ht.h if ht else None, C.byref(plan), C.byref(h)))
+        return Result(self, h, plan)
+
+    def hash_agg_joins(self, outer: Table, steps, plan: GxAggPlan) -> Result:
+        """steps: (HashTable, (side, col)[, join_type]) per join of the chain, in probe order"""
+        arr = (GxJoinStep * max(len(steps), 1))()
+        for i, st in enumerate(steps):
+            ht, (side, col) = st[0], st[1]
+            arr[i].h = ht.h if ht is not None else None
+            arr[i].key.side, arr[i].key.col = side, col
+            arr[i].join_type = st[2] if len(st) > 2 else GX_JOIN_INNER
+        h = C.c_void_p()
+        self._chk(lib().gx_hash_agg_joins(self.h, outer.h, len(steps), arr, C.byref(plan), C.byref(h)))
         return Result(self, h, plan)
 
     # ---- communicator / routing

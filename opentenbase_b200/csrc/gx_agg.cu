@@ -34,6 +34,18 @@ enum { WK_ADD_I64 = 0, WK_ADD_F64 = 1, WK_MIN_F64 = 2, WK_MAX_F64 = 3 };
 // so a group whose inputs are all -0.0 sums to -0.0 as float8pl does when the first input becomes the state
 #define GX_NEG_ZERO_BITS 0x8000000000000000ULL
 
+// steps 2.. of a join chain (gx_hash_agg_joins): the table in its 16-byte form (the fields gx_probe_first reads; the
+// compact and narrow pointers stay null), and where the step's key comes from
+struct gx_chain_step {
+    const gx_slot *slots; const gx_cslot *cslots; const unsigned int *narrow;
+    unsigned long long cspan, mask;
+    gx_slotfn sf;
+    const unsigned long long *special; int special_count;
+    int src;                 // 0: outer column kcol; s >= 1: payload word of step s
+    gx_dcol kcol;
+    int kshift, kbytes;      // payload key: bit offset and width in the payload word (4: sign-extended, 8: whole)
+};
+
 struct gx_agg_dev {
     gx_dplan P;
     long long winit[GX_MAX_WORDS];
@@ -56,7 +68,13 @@ struct gx_agg_dev {
     // record sink (radix stage A)
     unsigned long long *recs; long long rec_cap;
     long long *counters;     // [0] ngroups in g_tab, [1] overflow flags, [2] record cursor
+    // join chain: steps in all (0 = not a chain; step 1 is the join table above), steps 2..chain_n
+    int chain_n; int _pad2;
+    gx_chain_step chain[GX_MAX_JOINS - 1];
 };
+// gx_k_agg takes gx_agg_dev by value (__grid_constant__): 2832 bytes with the chain steps, 3112 with gx_k_runagg's second
+// argument, inside the 4 KB of kernel parameters every architecture accepts
+static_assert(sizeof(gx_agg_dev) <= 4096, "gx_agg_dev outgrew the kernel parameter space");
 
 #define TAG_LOCK 1ULL
 
@@ -178,6 +196,8 @@ __device__ __forceinline__ unsigned long long *global_upsert(const gx_agg_dev &A
 }
 
 enum { SINK_SMEM = 1, SINK_RECORD = 2, SINK_GLOBAL = 3, SINK_SMEM_LP = 4 };
+// gx_k_agg's XF of a join chain: GX_XF_CHAIN + the first table's slot format
+enum { GX_XF_CHAIN = 4 };
 
 template <int SINK>
 struct Sink {
@@ -263,11 +283,45 @@ __device__ __forceinline__ void apply_aggs(const gx_dplan &P, bool need_w0, long
     }
 }
 
+// the group columns of a row that passed every step of a join chain: side s >= 1 reads the payload word pw[s - 1]
+__device__ __forceinline__ void pack_chain_key(const gx_dplan &P, long long r, const unsigned long long (&pw)[GX_MAX_JOINS],
+                                               unsigned long long &k0, unsigned long long &k1, unsigned int &nullmask)
+{
+    k0 = 0; k1 = 0; nullmask = 0;
+#pragma unroll
+    for (int c = 0; c < GX_MAX_GROUP_COLS; c++) {
+        if (c >= P.ngroup) break;
+        const gx_dgroupcol &g = P.gcols[c];
+        unsigned long long v;
+        if (g.side == 0) {
+            if (gx_is_null(g.col, r)) { nullmask |= 1u << c; continue; }
+            v = (unsigned long long) gx_load_int(g.col, r);
+            if (g.type == GX_FLOAT8 && __longlong_as_double((long long) v) == 0.0) v = 0;      // -0 = +0, as pack_group_key
+        } else {
+            v = (g.side == 1 ? pw[0] : g.side == 2 ? pw[1] : pw[2]) >> g.payload_idx;     // payload_idx holds the bit offset
+        }
+        if (g.bytes < 8) v &= (1ULL << (8 * g.bytes)) - 1;
+        if (g.word == 0) k0 |= v << g.shift; else k1 |= v << g.shift;
+    }
+}
+
+template <int SINK>
+__device__ __forceinline__ void consume_key(const gx_agg_dev &A, const SmemTable &T, long long r, unsigned long long k0, unsigned long long k1,
+                                            unsigned int nullmask, unsigned int cm);
+
 template <int SINK>
 __device__ __forceinline__ void consume_row(const gx_agg_dev &A, const SmemTable &T, long long r, unsigned long long payload, unsigned int cm = 0)
 {
     unsigned long long k0, k1; unsigned int nullmask;
     pack_group_key(A.P, r, payload, k0, k1, nullmask);
+    consume_key<SINK>(A, T, r, k0, k1, nullmask, cm);
+}
+
+// one row with its packed group key into the sink
+template <int SINK>
+__device__ __forceinline__ void consume_key(const gx_agg_dev &A, const SmemTable &T, long long r, unsigned long long k0, unsigned long long k1,
+                                            unsigned int nullmask, unsigned int cm)
+{
     Sink<SINK> sink; sink.wstride = 1;
     // The table lookups below leave their probe loops at different iterations; without an explicit
     // reconvergence point the lanes then run the whole aggregate section in separate passes
@@ -354,6 +408,9 @@ __device__ __forceinline__ unsigned long long lp_reduce_word(const SmemTable &T,
 // tile, their home-group loads in flight together (gx_probe_first, the walk gx_k_hash_probe_unique runs).  SEMI consumes
 // a row once when its key has a partner, however many; ANTI a row that passed the quals and has none, a NULL key
 // included (HJ_FILL_OUTER_TUPLE).  Neither reads an inner column.
+// XF = GX_XF_CHAIN + GX_SLOTS_*: a chain of unique INNER joins (gx_hash_agg_joins), step 1 probed in the format its build
+// wrote, steps 2.. in their 16-byte form, each with a key from the outer row or from an earlier step's payload; a row that
+// every step matches is consumed once, its group key packed from the outer row and the steps' payload words.
 template <int SINK, int XF>
 __global__ void __launch_bounds__(1024, 1) gx_k_agg(const __grid_constant__ gx_agg_dev A)
 {
@@ -385,7 +442,62 @@ __global__ void __launch_bounds__(1024, 1) gx_k_agg(const __grid_constant__ gx_a
     }
     const gx_dplan &P = A.P;
     const int lane = threadIdx.x & 31;
-    if constexpr (XF >= 0) {
+    if constexpr (XF >= GX_XF_CHAIN) {
+        const long long tile = 32LL * PT_K, step = (long long) gridDim.x * nwarps * tile;
+        for (long long base = A.row0 + ((long long) blockIdx.x * nwarps + (threadIdx.x >> 5)) * tile; base < A.row1; base += step) {
+            long long r[PT_K], key[PT_K]; bool ok[PT_K], hit[PT_K]; unsigned long long pw[GX_MAX_JOINS][PT_K];
+#pragma unroll
+            for (int j = 0; j < PT_K; j++) { r[j] = base + j * 32 + lane; ok[j] = r[j] < A.row1; }
+            for (int p = 0; p < P.npreds; p++) pred_tile<PT_K>(P.preds[p], r, ok);
+#pragma unroll
+            for (int j = 0; j < PT_K; j++) ok[j] = ok[j] && !gx_is_null(P.okey, r[j]);          // a NULL key never joins
+#pragma unroll
+            for (int j = 0; j < PT_K; j++) key[j] = ok[j] ? gx_load_int(P.okey, r[j]) : 0;
+            gx_probe_first<XF - GX_XF_CHAIN, PT_K>(A, ok, key, hit, pw[0]);
+#pragma unroll
+            for (int s = 1; s < GX_MAX_JOINS; s++) {
+#pragma unroll
+                for (int j = 0; j < PT_K; j++) pw[s][j] = 0;
+                if (s >= A.chain_n) continue;
+                const gx_chain_step &cs = A.chain[s - 1];
+#pragma unroll
+                for (int j = 0; j < PT_K; j++) {
+                    // the rows every earlier step matched; a key from the outer row may be NULL, a payload never is
+                    bool live = hit[j]; long long k = 0;
+                    if (cs.src == 0) {
+                        live = live && !gx_is_null(cs.kcol, r[j]);
+                        if (live) k = gx_load_int(cs.kcol, r[j]);
+                    } else {
+                        const unsigned long long w = (cs.src == 1 ? pw[0][j] : pw[1][j]) >> cs.kshift;      // src <= s
+                        k = cs.kbytes == 8 ? (long long) w : (long long) (int) (unsigned int) w;          // int4 / date: sign-extended
+                    }
+                    ok[j] = live; key[j] = k;
+                }
+                gx_probe_first<GX_SLOTS_WIDE, PT_K>(cs, ok, key, hit, pw[s]);
+            }
+            unsigned int pass = 0;
+#pragma unroll
+            for (int j = 0; j < PT_K; j++) pass |= (unsigned int) hit[j] << j;
+            // one inlined copy of the aggregate update per tile: row j's payload words are picked by selects, not an index
+#pragma unroll 1
+            for (int j = 0; j < PT_K; j++) {
+                const bool take = (pass >> j) & 1u;
+                const unsigned int m = P.nwords >= 3 ? __ballot_sync(0xffffffffu, take) : 0u;
+                if (!take) continue;
+                unsigned long long pj[GX_MAX_JOINS];
+#pragma unroll
+                for (int s = 0; s < GX_MAX_JOINS; s++) {
+                    pj[s] = pw[s][0];
+#pragma unroll
+                    for (int i = 1; i < PT_K; i++) if (j == i) pj[s] = pw[s][i];
+                }
+                unsigned long long k0, k1; unsigned int nullmask;
+                const long long row = base + j * 32 + lane;
+                pack_chain_key(P, row, pj, k0, k1, nullmask);
+                consume_key<SINK>(A, T, row, k0, k1, nullmask, m);
+            }
+        }
+    } else if constexpr (XF >= 0) {
         const bool anti = P.join_type == GX_JOIN_ANTI;
         const long long tile = 32LL * PT_K, step = (long long) gridDim.x * nwarps * tile;
         for (long long base = A.row0 + ((long long) blockIdx.x * nwarps + (threadIdx.x >> 5)) * tile; base < A.row1; base += step) {
@@ -2417,7 +2529,11 @@ int gx_check_agg_join_type(gx_ctx *ctx, const gx_agg_plan *plan)
     return GX_OK;
 }
 
-static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, compiled_plan *cp)
+// steps of a join chain that gx_hash_agg_joins has checked (n >= 2); steps[0].h is the plan's own join table
+struct chain_spec { int n; const gx_join_step *steps; };
+
+static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, compiled_plan *cp,
+                        const chain_spec *ch = nullptr)
 {
     memset(cp, 0, sizeof(*cp));
     gx_dplan &P = cp->A.P;
@@ -2442,6 +2558,22 @@ static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
         cp->A.special = h->special_payload; cp->A.special_count = h->special_count;
         cp->A.sf = gx_hash_slotfn(h);
     }
+    if (ch) {
+        cp->A.chain_n = ch->n;
+        for (int s = 1; s < ch->n; s++) {
+            const gx_hash *hs = ch->steps[s].h; const gx_colref &k = ch->steps[s].key;
+            gx_chain_step &cs = cp->A.chain[s - 1];
+            cs.slots = hs->slots; cs.mask = (unsigned long long) hs->nslots - 1; cs.sf = gx_hash_slotfn(hs);
+            cs.special = hs->special_payload; cs.special_count = hs->special_count;
+            cs.src = k.side;
+            if (k.side == 0) cs.kcol = dcol_of(outer, k.col);
+            else {
+                const gx_hash *hk = ch->steps[k.side - 1].h;
+                for (int i = 0; i < k.col; i++) cs.kshift += 8 * gx_type_size(hk->payload_types[i]);
+                cs.kbytes = gx_type_size(hk->payload_types[k.col]);
+            }
+        }
+    }
     // group columns: pack by byte width into k0 then k1
     int used[2] = { 0, 0 };
     P.ngroup = plan->n_group_cols;
@@ -2455,12 +2587,13 @@ static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
             g.col = dcol_of(outer, col); type = outer->types[col];
         } else {
             GX_CHECK_ARG(ctx, P.join_type == GX_JOIN_INNER, "agg plan: a semi or anti join carries no inner column (group column %d)", c);
-            GX_CHECK_ARG(ctx, h != nullptr && h->n_payload > 0, "agg plan: group column refers to a join payload but none is carried");
+            const gx_hash *hg = ch ? ch->steps[g.side - 1].h : h;        // a chain's side s: step s (checked by gx_hash_agg_joins)
+            GX_CHECK_ARG(ctx, hg != nullptr && hg->n_payload > 0, "agg plan: group column refers to a join payload but none is carried");
             int pi = plan->group_cols[c].col;
-            GX_CHECK_ARG(ctx, pi >= 0 && pi < h->n_payload, "agg plan: payload index %d out of range", pi);
+            GX_CHECK_ARG(ctx, pi >= 0 && pi < hg->n_payload, "agg plan: payload index %d out of range", pi);
             int bit = 0;
-            for (int i = 0; i < pi; i++) bit += 8 * gx_type_size(h->payload_types[i]);
-            g.payload_idx = bit; type = h->payload_types[pi];
+            for (int i = 0; i < pi; i++) bit += 8 * gx_type_size(hg->payload_types[i]);
+            g.payload_idx = bit; type = hg->payload_types[pi];
         }
         g.type = type; g.bytes = gx_type_size(type);
         int w = (used[0] + g.bytes <= 8) ? 0 : 1;
@@ -2579,17 +2712,20 @@ static int launch_agg_k(gx_ctx *ctx, const gx_agg_dev &A, size_t smem, const cha
     gx_launch_scope ls(ctx, name);
     // second profile name: which sink answered (gx_profile_get)
     gx_launch_scope which(ctx, SINK == SINK_SMEM_LP ? "agg_smem_lp" : SINK == SINK_SMEM ? "agg_smem" : SINK == SINK_GLOBAL ? "agg_global" : "agg_records", 0);
-    // third profile name of a SEMI / ANTI plan: the slot format its existence probe read
+    // third profile name of a SEMI / ANTI plan or a join chain: the slot format its (first) probe read
     gx_launch_scope fmt(ctx, XF == GX_SLOTS_NARROW ? "probe_agg_exist_narrow" : XF == GX_SLOTS_COMPACT ? "probe_agg_exist_compact" :
-                             XF == GX_SLOTS_WIDE ? "probe_agg_exist_wide" : nullptr, 0);
+                             XF == GX_SLOTS_WIDE ? "probe_agg_exist_wide" : XF == GX_XF_CHAIN + GX_SLOTS_NARROW ? "probe_agg_chain_narrow" :
+                             XF == GX_XF_CHAIN + GX_SLOTS_COMPACT ? "probe_agg_chain_compact" : XF == GX_XF_CHAIN + GX_SLOTS_WIDE ? "probe_agg_chain_wide" : nullptr, 0);
     gx_k_agg<SINK, XF><<<grid, threads, smem, ctx->stream>>>(A);
     GX_CUDA(ctx, cudaGetLastError());
     return GX_OK;
 }
-// the kernel of the plan's join type: row by row (no join, INNER), or the existence probe in the table's own format
+// the kernel of the plan's join type: row by row (no join, INNER), the existence probe or the join chain in the (first)
+// table's own format
 template <int SINK>
 static int launch_agg(gx_ctx *ctx, const gx_agg_dev &A, size_t smem, const char *name, int threads = 1024)
 {
+    if (A.chain_n > 1) return with_slot_format(A, [&](auto f) { return launch_agg_k<SINK, GX_XF_CHAIN + decltype(f)::value>(ctx, A, smem, name, threads); });
     if (A.P.join_type == GX_JOIN_INNER) return launch_agg_k<SINK, -1>(ctx, A, smem, name, threads);
     return with_slot_format(A, [&](auto f) { return launch_agg_k<SINK, decltype(f)::value>(ctx, A, smem, name, threads); });
 }
@@ -2887,10 +3023,11 @@ static void remember_layout(gx_result *r, const compiled_plan *cp)
 static int run_radix(gx_ctx *ctx, compiled_plan *cp, const gx_agg_plan *plan, long long nrows_in, gx_result **out);
 int gx_result_layout_words(gx_result *r, int *wkind, long long *winit);
 
-static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, gx_result **out)
+static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, gx_result **out,
+                        const chain_spec *ch = nullptr)
 {
     compiled_plan cp;
-    int rc = compile_plan(ctx, outer, h, plan, &cp); if (rc) return rc;
+    int rc = compile_plan(ctx, outer, h, plan, &cp, ch); if (rc) return rc;
     gx_agg_dev &A = cp.A;
     const int nwords = A.P.nwords, RW = 3 + nwords;
     long long est = plan->est_groups > 0 ? plan->est_groups : 1024;
@@ -2912,8 +3049,9 @@ static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
     // ---- does the plan have the shape the specialised kernel was written for?
     gx_fast_args FA; memset(&FA, 0, sizeof(FA));
     { const char *pf = getenv("GX_RUNJOIN_PF"); FA.pf = pf ? atoi(pf) : 0; }
-    // the specialised kernels below join; a SEMI / ANTI plan takes gx_k_agg's existence probe
-    const bool exist = A.P.join_type != GX_JOIN_INNER;
+    // the specialised kernels below join one table and know one payload word; a SEMI / ANTI plan takes gx_k_agg's
+    // existence probe, a join chain its chain probe (both read the first table in the format its build wrote)
+    const bool exist = A.P.join_type != GX_JOIN_INNER || A.chain_n > 1;
     bool fast_ok = !exist && plan->n_preds == 0 && plan->n_group_cols == 1 && tagkey && outer->nrows > 0;
     if (fast_ok) {
         const gx_dgroupcol &gc = A.P.gcols[0];
@@ -3113,7 +3251,7 @@ static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
         GX_CUDA(ctx, cudaMemsetAsync(A.counters, 0, 4 * sizeof(long long), ctx->stream));
         A.g_tab = g_tab; A.g_mask = (unsigned long long) g_cap - 1;
         A.s_slots = strategy == 1 ? (int) S : 0; A.s_log2 = ilog2(S); A.s_tagkey = tagkey; A.s_gmax = gmax;
-        const char *kname = h ? "probe_agg" : "agg";
+        const char *kname = A.chain_n > 1 ? "probe_agg_chain" : h ? "probe_agg" : "agg";
         const bool use_fast = strategy == 1 && !gmax && fast_ok;
         const bool use_run = use_fast && A.P.has_join && runjoin_env && dense_bytes(S) + run_bytes <= ctx->smem_optin - 1024;
         if (!use_run) { rc = need_wide(); if (rc) { gx_tmp_free(ctx, g_tab); return rc; } }
@@ -3244,7 +3382,8 @@ static long long rec_count(const gx_infscan_args &S, const unsigned long long *w
     return S.cw[i] ? (long long) w[S.cw[i]] : (S.need_w0 ? (long long) w[0] : 1);
 }
 
-static int check_f8_overflow(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, gx_result *r)
+static int check_f8_overflow(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, gx_result *r,
+                             const chain_spec *ch = nullptr)
 {
     gx_infscan_args S; int chk[GX_MAX_AGGS];
     f8_checked_words(r, false, &S, chk);
@@ -3278,7 +3417,7 @@ static int check_f8_overflow(gx_ctx *ctx, const gx_table *outer, const gx_hash *
         }
     }
     gx_result *v = nullptr;
-    rc = hash_agg_run(ctx, outer, h, &vp, &v);
+    rc = hash_agg_run(ctx, outer, h, &vp, &v, ch);
     if (rc != GX_OK) return rc;
     const int ng = plan->n_group_cols;
     const unsigned long long mmask = (1ULL << ng) - 1;
@@ -3360,6 +3499,49 @@ extern "C" int gx_hash_agg(gx_ctx *ctx, const gx_table *outer, const gx_hash *h,
     int rc = hash_agg_run(ctx, outer, h, plan, out);
     if (rc != GX_OK) return rc;
     rc = check_f8_overflow(ctx, outer, h, plan, *out);
+    if (rc != GX_OK) { gx_result_free(*out); *out = nullptr; }
+    return rc;
+}
+
+// the width of a join key taken from a payload column, or 0 when the column cannot be one
+static int payload_key_type(const gx_hash *h, int col) { return col >= 0 && col < h->n_payload ? h->payload_types[col] : 0; }
+
+extern "C" int gx_hash_agg_joins(gx_ctx *ctx, const gx_table *outer, int n_steps, const gx_join_step *steps,
+                                 const gx_agg_plan *plan, gx_result **out)
+{
+    if (!ctx || !outer || !plan || !out) return GX_ERR_ARG;
+    GX_CHECK_ARG(ctx, n_steps >= 1 && n_steps <= GX_MAX_JOINS && steps != nullptr, "join chain: %d steps (1..%d)", n_steps, GX_MAX_JOINS);
+    GX_CHECK_ARG(ctx, plan->outer_key_col < 0, "join chain: the plan's outer_key_col must be -1 (the steps carry the keys)");
+    GX_CHECK_ARG(ctx, plan->join_type == GX_JOIN_INNER, "join chain: plan join type %d (inner only)", plan->join_type);
+    for (int s = 0; s < n_steps; s++) {
+        const gx_join_step &st = steps[s];
+        GX_CHECK_ARG(ctx, st.join_type == GX_JOIN_INNER, "join chain: step %d has join type %d (inner only)", s + 1, st.join_type);
+        GX_CHECK_ARG(ctx, st.h != nullptr, "join chain: step %d has no join table", s + 1);
+        GX_CHECK_ARG(ctx, st.h->unique, "join chain: the table of step %d was not built unique", s + 1);
+        const int side = st.key.side, col = st.key.col;
+        GX_CHECK_ARG(ctx, side >= 0 && side <= s, "join chain: the key of step %d refers to step %d (outer side 0 or an earlier step)", s + 1, side);
+        int kt;
+        if (side == 0) {
+            GX_CHECK_ARG(ctx, col >= 0 && col < outer->ncols, "join chain: key column %d of step %d out of range", col, s + 1);
+            kt = outer->types[col];
+        } else {
+            kt = payload_key_type(steps[side - 1].h, col);
+            GX_CHECK_ARG(ctx, kt != 0, "join chain: key of step %d: payload index %d of step %d out of range", s + 1, col, side);
+        }
+        GX_CHECK_ARG(ctx, kt == GX_INT4 || kt == GX_INT8 || kt == GX_DATE, "join chain: key of step %d has type %d (int4, int8 or date)", s + 1, kt);
+    }
+    for (int c = 0; c < plan->n_group_cols && c < GX_MAX_GROUP_COLS; c++)
+        GX_CHECK_ARG(ctx, plan->group_cols[c].side >= 0 && plan->group_cols[c].side <= n_steps,
+                     "join chain: group column %d refers to step %d of %d", c, plan->group_cols[c].side, n_steps);
+    gx_agg_plan p = *plan;
+    p.outer_key_col = steps[0].key.col;          // step 1's key is an outer column (side 0, checked above)
+    if (n_steps == 1) return gx_hash_agg(ctx, outer, steps[0].h, &p, out);
+    // steps 2.. are probed in their 16-byte form; step 1 in the format its build wrote
+    for (int s = 1; s < n_steps; s++) { int rc = gx_hash_wide(ctx, const_cast<gx_hash *>(steps[s].h)); if (rc) return rc; }
+    const chain_spec ch = { n_steps, steps };
+    int rc = hash_agg_run(ctx, outer, steps[0].h, &p, out, &ch);
+    if (rc != GX_OK) return rc;
+    rc = check_f8_overflow(ctx, outer, steps[0].h, &p, *out, &ch);
     if (rc != GX_OK) { gx_result_free(*out); *out = nullptr; }
     return rc;
 }
@@ -3536,7 +3718,8 @@ static int run_radix(gx_ctx *ctx, compiled_plan *cp, const gx_agg_plan *plan, lo
         GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d_recs, (size_t) (cap > 0 ? cap : 1) * RW * 8));
         GX_CUDA(ctx, cudaMemsetAsync(A.counters, 0, 4 * sizeof(long long), ctx->stream));
         A.recs = d_recs; A.rec_cap = cap; A.s_slots = 0;
-        int rc = launch_agg<SINK_RECORD>(ctx, A, 0, A.P.join_type != GX_JOIN_INNER ? "probe_agg" : A.P.has_join ? "probe_records" : "scan_records");
+        int rc = launch_agg<SINK_RECORD>(ctx, A, 0, A.chain_n > 1 ? "probe_agg_chain" : A.P.join_type != GX_JOIN_INNER ? "probe_agg" :
+                                                    A.P.has_join ? "probe_records" : "scan_records");
         long long c[4];
         if (rc == GX_OK) rc = read_counters(ctx, c);
         if (rc != GX_OK) { gx_tmp_free(ctx, d_recs); return rc; }

@@ -110,6 +110,25 @@ typedef struct GpuRelInfo
 	int32		types[GX_MAX_COLS];		/* GX_* */
 } GpuRelInfo;
 
+/* steps 2.. of a join chain (gx_hash_agg_joins); step 1 is the single join's inner side below */
+typedef struct GpuJoinStep
+{
+	GpuRelInfo	rel;
+	int			key_col;		/* build key column of rel */
+	int			n_payload;
+	int32		payload_cols[GX_MAX_PAYLOAD];
+	int			n_preds;
+	gx_pred		preds[GX_MAX_PREDS];
+	gx_colref	probe;			/* probe key: side 0 an outer column, side s a payload column of step s */
+	double		tuples;			/* planner only (HBM estimate), not shipped */
+	Relation	r;
+	gx_table   *tab;
+	gx_hash    *hash;
+} GpuJoinStep;
+
+/* the descriptor word after the version for a join chain: 0 is no join, 1 + GX_JOIN_* a single join */
+#define GPUEXEC_DESC_CHAIN 100
+
 typedef struct GpuExecState
 {
 	CustomScanState css;
@@ -141,6 +160,10 @@ typedef struct GpuExecState
 	double		load_ms,
 				exec_ms;
 	bool		done_exec;
+	/* a chain of unique INNER joins: step 1 is inner above, steps 2 .. 1 + n_more here; step 1's probe key is
+	 * plan.outer_key_col until gpuexec_run hands the chain to gx_hash_agg_joins */
+	int			n_more;
+	GpuJoinStep more[GX_MAX_JOINS - 1];
 } GpuExecState;
 
 /* handles that must die with the query even when ereport() longjmps past us */
@@ -166,6 +189,15 @@ gpuexec_release_state(GpuExecState *st)
 	st->result = NULL;
 	st->hash = NULL;
 	st->outer_tab = st->inner_tab = NULL;
+	for (int i = 0; i < st->n_more; i++)
+	{
+		if (st->more[i].hash)
+			gx_hash_free(st->more[i].hash);
+		if (st->more[i].tab)
+			gx_table_free(st->more[i].tab);
+		st->more[i].hash = NULL;
+		st->more[i].tab = NULL;
+	}
 }
 
 static void
@@ -428,8 +460,9 @@ gpuexec_serialise(const GpuExecState *st)
 				j;
 
 	l = put_int(l, GX_ABI_VERSION);
-	/* 0 = no join, else 1 + GX_JOIN_*: an INNER join keeps the word it had before SEMI and ANTI existed */
-	l = put_int(l, st->has_join ? 1 + p->join_type : 0);
+	/* 0 = no join, else 1 + GX_JOIN_*: an INNER join keeps the word it had before SEMI and ANTI existed; a chain has
+	 * its own word, and its steps 2.. follow the single join's block */
+	l = put_int(l, st->n_more > 0 ? GPUEXEC_DESC_CHAIN : st->has_join ? 1 + p->join_type : 0);
 	l = serialise_rel(l, &st->outer);
 	if (st->has_join)
 	{
@@ -446,6 +479,28 @@ gpuexec_serialise(const GpuExecState *st)
 			l = put_int(l, st->inner_preds[i].op);
 			l = put_int64(l, st->inner_preds[i].ival);
 			l = put_double(l, st->inner_preds[i].fval);
+		}
+		if (st->n_more > 0)
+			l = put_int(l, st->n_more);
+		for (j = 0; j < st->n_more; j++)
+		{
+			const GpuJoinStep *m = &st->more[j];
+
+			l = serialise_rel(l, &m->rel);
+			l = put_int(l, m->key_col);
+			l = put_int(l, m->probe.side);
+			l = put_int(l, m->probe.col);
+			l = put_int(l, m->n_payload);
+			for (i = 0; i < m->n_payload; i++)
+				l = put_int(l, m->payload_cols[i]);
+			l = put_int(l, m->n_preds);
+			for (i = 0; i < m->n_preds; i++)
+			{
+				l = put_int(l, m->preds[i].col);
+				l = put_int(l, m->preds[i].op);
+				l = put_int64(l, m->preds[i].ival);
+				l = put_double(l, m->preds[i].fval);
+			}
 		}
 	}
 	l = put_int(l, st->partial);
@@ -493,7 +548,8 @@ gpuexec_deserialise(List *priv, GpuExecState *st)
 	memset(p, 0, sizeof(*p));
 	i = get_int(&lc);
 	st->has_join = i != 0;
-	p->join_type = i != 0 ? i - 1 : GX_JOIN_INNER;
+	p->join_type = i != 0 && i != GPUEXEC_DESC_CHAIN ? i - 1 : GX_JOIN_INNER;
+	st->n_more = i == GPUEXEC_DESC_CHAIN ? -1 : 0;		/* read after the first join's block */
 	deserialise_rel(&lc, &st->outer);
 	if (st->has_join)
 	{
@@ -510,6 +566,32 @@ gpuexec_deserialise(List *priv, GpuExecState *st)
 			st->inner_preds[i].op = get_int(&lc);
 			st->inner_preds[i].ival = get_int64(&lc);
 			st->inner_preds[i].fval = get_double(&lc);
+		}
+		if (st->n_more < 0)
+		{
+			st->n_more = get_int(&lc);
+			if (st->n_more < 1 || st->n_more > GX_MAX_JOINS - 1)
+				ereport(ERROR, (errmsg("gpuexec: join chain of %d steps in the plan descriptor", 1 + st->n_more)));
+		}
+		for (j = 0; j < st->n_more; j++)
+		{
+			GpuJoinStep *m = &st->more[j];
+
+			deserialise_rel(&lc, &m->rel);
+			m->key_col = get_int(&lc);
+			m->probe.side = get_int(&lc);
+			m->probe.col = get_int(&lc);
+			m->n_payload = get_int(&lc);
+			for (i = 0; i < m->n_payload; i++)
+				m->payload_cols[i] = get_int(&lc);
+			m->n_preds = get_int(&lc);
+			for (i = 0; i < m->n_preds; i++)
+			{
+				m->preds[i].col = get_int(&lc);
+				m->preds[i].op = get_int(&lc);
+				m->preds[i].ival = get_int64(&lc);
+				m->preds[i].fval = get_double(&lc);
+			}
 		}
 	}
 	st->partial = get_int(&lc);
@@ -589,6 +671,8 @@ gpuexec_begin(CustomScanState *node, EState *estate, int eflags)
 	st->outer_rel = ExecOpenScanRelation(estate, st->outer.rti, eflags);
 	if (st->has_join)
 		st->inner_rel = ExecOpenScanRelation(estate, st->inner.rti, eflags);
+	for (int i = 0; i < st->n_more; i++)
+		st->more[i].r = ExecOpenScanRelation(estate, st->more[i].rel.rti, eflags);
 	h = (GpuHandles *) malloc(sizeof(GpuHandles));
 	h->owner = CurrentResourceOwner;
 	h->state = st;
@@ -608,6 +692,8 @@ gpuexec_run(GpuExecState *st, EState *estate)
 	INSTR_TIME_SET_CURRENT(t0);
 	if (st->has_join)
 		gpuexec_load_relation(st->inner_rel, estate, &st->inner, &st->inner_tab);
+	for (int i = 0; i < st->n_more; i++)
+		gpuexec_load_relation(st->more[i].r, estate, &st->more[i].rel, &st->more[i].tab);
 	gpuexec_load_relation(st->outer_rel, estate, &st->outer, &st->outer_tab);
 	INSTR_TIME_SET_CURRENT(t1);
 	INSTR_TIME_SUBTRACT(t1, t0);
@@ -618,7 +704,32 @@ gpuexec_run(GpuExecState *st, EState *estate)
 		GX_CHECK(gx_hash_build(backend_ctx, st->inner_tab, st->inner_key_col, st->n_inner_preds, st->inner_preds,
 							   st->n_payload, st->payload_cols, st->inner_unique, &st->hash));
 	CHECK_FOR_INTERRUPTS();
-	GX_CHECK(gx_hash_agg(backend_ctx, st->outer_tab, st->hash, &st->plan, &st->result));
+	if (st->n_more > 0)
+	{
+		/* the chain in build order; every table is in st before the next call, so an ERROR frees them all */
+		gx_join_step steps[GX_MAX_JOINS];
+		gx_agg_plan cp = st->plan;
+
+		memset(steps, 0, sizeof(steps));
+		steps[0].h = st->hash;
+		steps[0].key.side = 0;
+		steps[0].key.col = st->plan.outer_key_col;
+		steps[0].join_type = GX_JOIN_INNER;
+		for (int i = 0; i < st->n_more; i++)
+		{
+			GpuJoinStep *m = &st->more[i];
+
+			GX_CHECK(gx_hash_build(backend_ctx, m->tab, m->key_col, m->n_preds, m->preds, m->n_payload, m->payload_cols, 1, &m->hash));
+			steps[1 + i].h = m->hash;
+			steps[1 + i].key = m->probe;
+			steps[1 + i].join_type = GX_JOIN_INNER;
+			CHECK_FOR_INTERRUPTS();
+		}
+		cp.outer_key_col = -1;
+		GX_CHECK(gx_hash_agg_joins(backend_ctx, st->outer_tab, 1 + st->n_more, steps, &cp, &st->result));
+	}
+	else
+		GX_CHECK(gx_hash_agg(backend_ctx, st->outer_tab, st->hash, &st->plan, &st->result));
 	/* The result holds this datanode's groups only.  Whether they are final is the PLANNER's
 	 * business: the hook offers the pushed-down path only when the GROUP BY covers the
 	 * distribution key, and otherwise asks for partial states, which the reference's own
@@ -781,6 +892,9 @@ gpuexec_end(CustomScanState *node)
 		ExecCloseScanRelation(st->outer_rel);
 	if (st->inner_rel)
 		ExecCloseScanRelation(st->inner_rel);
+	for (int i = 0; i < st->n_more; i++)
+		if (st->more[i].r)
+			ExecCloseScanRelation(st->more[i].r);
 }
 
 static void
@@ -800,6 +914,8 @@ gpuexec_explain(CustomScanState *node, List *ancestors, ExplainState *es)
 	ExplainPropertyText("GPU Strategy", st->has_join ? "hash build + fused probe/aggregate" : "scan + hash aggregate", es);
 	if (st->has_join)
 		ExplainPropertyText("GPU Join Type", st->plan.join_type == GX_JOIN_SEMI ? "Semi" : st->plan.join_type == GX_JOIN_ANTI ? "Anti" : "Inner", es);
+	if (st->n_more > 0)
+		ExplainPropertyInteger("GPU Joins", NULL, 1 + st->n_more, es);
 	ExplainPropertyText("GPU Output", st->partial ? "partial states (Finalize above the redistribute)" : "final values (GROUP BY covers the distribution key)", es);
 	if (es->analyze && st->done_exec)
 	{
@@ -854,6 +970,8 @@ gpuexec_plan_path(PlannerInfo *root, RelOptInfo *rel, CustomPath *best_path,
  *            Agg over HashJoin[INNER, one int4/int8 equi-key](SeqScan(R), SeqScan(S))   (config 3)
  *            Agg over HashJoin[SEMI / ANTI, the same key shape]  (EXISTS / NOT EXISTS: TPC-H Q4, Q21, Q22 shapes),
  *            with GROUP BY columns and aggregate arguments from the outer side only
+ *            Agg over a left-deep chain of 2..GX_MAX_JOINS such INNER joins with unique build sides (star joins:
+ *            TPC-H Q3), GROUP BY columns from any relation, aggregate arguments from the outer one (match_chain)
  * with "Var op Const" quals on the scans, Var group keys, no HAVING / grouping sets /
  * DISTINCT / ORDER BY aggregates / FILTER, and aggregates count(*), count(x),
  * sum/avg/min/max(float8 expr), sum(int4); every target-list entry must be a group Var or a
@@ -1127,6 +1245,164 @@ column_is_not_null(PlannerInfo *root, Index rti, AttrNumber attno)
 	return res;
 }
 
+/* payload slot of column c of a join's build side, appended on first use: a probe key of a later step and a group column
+ * that read the same column share one slot */
+static int
+payload_slot(int32 *cols, int *n, int c)
+{
+	int			i;
+
+	for (i = 0; i < *n; i++)
+		if (cols[i] == c)
+			return i;
+	if (*n >= GX_MAX_PAYLOAD)
+		return -1;
+	cols[*n] = c;
+	return (*n)++;
+}
+
+/* the chain step (1..) whose build side scans rti, or 0 */
+static int
+chain_step_of(const GpuExecState *st, Index rti)
+{
+	int			i;
+
+	if (st->inner.rti == rti)
+		return 1;
+	for (i = 0; i < st->n_more; i++)
+		if (st->more[i].rel.rti == rti)
+			return 2 + i;
+	return 0;
+}
+
+/* One level of a left-deep join chain: INNER with a unique build side, exactly one int4eq / int8eq hash clause that is its
+ * whole joinrestrictinfo, and a plain SeqScan of an unprotected relation as the build side.  *iv = the clause's Var of
+ * the build side, *ov = the other one. */
+static bool
+chain_level(PlannerInfo *root, HashPath *hp, Var **ov, Var **iv)
+{
+	Path	   *ip = hp->jpath.innerjoinpath;
+	RestrictInfo *ri;
+	OpExpr	   *clause;
+	Var		   *a,
+			   *b;
+
+	if (hp->jpath.jointype != JOIN_INNER || !hp->jpath.inner_unique)
+		return false;
+	if (list_length(hp->path_hashclauses) != 1 || list_length(hp->jpath.joinrestrictinfo) != 1)
+		return false;
+	if (ip->pathtype != T_SeqScan)		/* a RemoteSubplan below: the inputs are not co-located */
+		return false;
+	ri = (RestrictInfo *) linitial(hp->path_hashclauses);
+	clause = (OpExpr *) ri->clause;
+	if (!IsA(clause, OpExpr) || list_length(clause->args) != 2 || !IsA(linitial(clause->args), Var) || !IsA(lsecond(clause->args), Var))
+		return false;
+	if (clause->opfuncid != F_INT4EQ && clause->opfuncid != F_INT8EQ)
+		return false;
+	a = (Var *) linitial(clause->args);
+	b = (Var *) lsecond(clause->args);
+	if (b->varno != ip->parent->relid)
+	{
+		Var		   *t = a;
+
+		a = b;
+		b = t;
+	}
+	if (b->varno != ip->parent->relid || a->varno == b->varno || relation_is_protected(root, b->varno))
+		return false;
+	*ov = a;
+	*iv = b;
+	return true;
+}
+
+/* Agg over HashJoin(HashJoin(... SeqScan(F), SeqScan(D1)) ..., SeqScan(Dn)), 2 <= n <= GX_MAX_JOINS (gx_hash_agg_joins):
+ * step s builds Ds; its probe key is a column of F or of an earlier D (carried in that step's payload, which has no
+ * NULL flag: the column must be NOT NULL).  Step 1 is described by the single join's fields, steps 2.. by out->more. */
+static bool
+match_chain(PlannerInfo *root, HashPath *top, GpuExecState *out, double *est_bytes, double *est_pages)
+{
+	HashPath   *lv[GX_MAX_JOINS];
+	Path	   *p = &top->jpath.path;
+	gx_agg_plan *plan = &out->plan;
+	int			n = 0,
+				s;
+
+	while (IsA(p, HashPath))
+	{
+		if (n == GX_MAX_JOINS)
+			return false;
+		lv[n++] = (HashPath *) p;
+		p = ((HashPath *) p)->jpath.outerjoinpath;
+	}
+	if (n < 2 || p->pathtype != T_SeqScan)
+		return false;
+	out->has_join = true;
+	out->inner_unique = true;
+	plan->join_type = GX_JOIN_INNER;
+	out->outer.rti = p->parent->relid;
+	if (relation_is_protected(root, out->outer.rti) ||
+		!match_quals(p->parent->baserestrictinfo, &out->outer, plan->preds, &plan->n_preds))
+		return false;
+	*est_bytes = p->parent->tuples;
+	*est_pages = p->parent->pages;
+	out->n_more = n - 1;
+	for (s = 1; s <= n; s++)
+	{
+		HashPath   *hp = lv[n - s];
+		RelOptInfo *irel = hp->jpath.innerjoinpath->parent;
+		GpuRelInfo *rel = s == 1 ? &out->inner : &out->more[s - 2].rel;
+		Var		   *ov,
+				   *iv;
+		int			kc,
+					c,
+					t,
+					side = 0;
+
+		if (!chain_level(root, hp, &ov, &iv))
+			return false;
+		rel->rti = iv->varno;
+		kc = rel_column(rel, iv->varno, iv->varattno, iv->vartype, iv->vartypmod);
+		if (kc < 0)
+			return false;
+		/* the probe key: a column of F, or the payload of the earlier step that scans ov's relation */
+		if (ov->varno == out->outer.rti)
+			c = rel_column(&out->outer, ov->varno, ov->varattno, ov->vartype, ov->vartypmod);
+		else
+		{
+			t = chain_step_of(out, ov->varno);
+			if (t < 1 || t >= s || !column_is_not_null(root, ov->varno, ov->varattno))
+				return false;
+			c = rel_column(t == 1 ? &out->inner : &out->more[t - 2].rel, ov->varno, ov->varattno, ov->vartype, ov->vartypmod);
+			if (c >= 0)
+				c = t == 1 ? payload_slot(out->payload_cols, &out->n_payload, c)
+					: payload_slot(out->more[t - 2].payload_cols, &out->more[t - 2].n_payload, c);
+			side = t;
+		}
+		if (c < 0)
+			return false;
+		if (s == 1)
+		{
+			plan->outer_key_col = c;		/* side 0: step 1 probes with a column of F */
+			out->inner_key_col = kc;
+			if (!match_quals(irel->baserestrictinfo, &out->inner, out->inner_preds, &out->n_inner_preds))
+				return false;
+		}
+		else
+		{
+			GpuJoinStep *m = &out->more[s - 2];
+
+			m->key_col = kc;
+			m->probe.side = side;
+			m->probe.col = c;
+			m->tuples = irel->tuples;
+			if (!match_quals(irel->baserestrictinfo, &m->rel, m->preds, &m->n_preds))
+				return false;
+		}
+		*est_pages += irel->pages;
+	}
+	return true;
+}
+
 static bool
 gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_rel, GpuExecState *out,
 				   List **agg_refs, double *est_rows, double *est_groups, double *est_bytes, double *est_pages)
@@ -1149,6 +1425,11 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 			return false;
 		*est_bytes = input_rel->tuples;
 		*est_pages = input_rel->pages;
+	}
+	else if (IsA(in, HashPath) && IsA(((HashPath *) in)->jpath.outerjoinpath, HashPath))
+	{
+		if (!match_chain(root, (HashPath *) in, out, est_bytes, est_pages))
+			return false;
 	}
 	else if (IsA(in, HashPath))
 	{
@@ -1218,7 +1499,8 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 		SortGroupClause *sgc = (SortGroupClause *) lfirst(lc);
 		TargetEntry *tle = get_sortgroupclause_tle(sgc, parse->targetList);
 		Var		   *v = (Var *) tle->expr;
-		int			c;
+		int			c,
+					s;
 
 		if (!IsA(v, Var) || plan->n_group_cols >= GX_MAX_GROUP_COLS)
 			return false;
@@ -1228,6 +1510,19 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 			if (c < 0)
 				return false;
 			plan->group_cols[plan->n_group_cols].side = 0;
+			plan->group_cols[plan->n_group_cols].col = c;
+		}
+		else if (out->n_more > 0 && (s = chain_step_of(out, v->varno)) > 0)
+		{
+			/* a build-side column of chain step s, in that step's payload (a slot its probe key may share) */
+			c = rel_column(s == 1 ? &out->inner : &out->more[s - 2].rel, v->varno, v->varattno, v->vartype, v->vartypmod);
+			if (c < 0 || !column_is_not_null(root, v->varno, v->varattno))
+				return false;
+			c = s == 1 ? payload_slot(out->payload_cols, &out->n_payload, c)
+				: payload_slot(out->more[s - 2].payload_cols, &out->more[s - 2].n_payload, c);
+			if (c < 0)
+				return false;
+			plan->group_cols[plan->n_group_cols].side = s;
 			plan->group_cols[plan->n_group_cols].col = c;
 		}
 		else if (out->has_join && plan->join_type == GX_JOIN_INNER && v->varno == out->inner.rti && out->n_payload < GX_MAX_PAYLOAD)
@@ -1257,10 +1552,22 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 			payload_bytes += staged_type_bytes(out->inner.types[out->payload_cols[i]]);
 		if (payload_bytes > 8)
 			return false;
+		for (i = 0; i < out->n_more; i++)
+		{
+			const GpuJoinStep *m = &out->more[i];
+			int			j;
+
+			for (payload_bytes = 0, j = 0; j < m->n_payload; j++)
+				payload_bytes += staged_type_bytes(m->rel.types[m->payload_cols[j]]);
+			if (payload_bytes > 8)
+				return false;
+		}
 		for (i = 0; i < plan->n_group_cols; i++)
 		{
-			int32		t = plan->group_cols[i].side == 0 ? out->outer.types[plan->group_cols[i].col]
-				: out->inner.types[out->payload_cols[plan->group_cols[i].col]];
+			const int	side = plan->group_cols[i].side;
+			int32		t = side == 0 ? out->outer.types[plan->group_cols[i].col]
+				: side == 1 ? out->inner.types[out->payload_cols[plan->group_cols[i].col]]
+				: out->more[side - 2].rel.types[out->more[side - 2].payload_cols[plan->group_cols[i].col]];
 			int			b = staged_type_bytes(t),
 						w = used[0] + b <= 8 ? 0 : 1;
 
@@ -1348,11 +1655,25 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 			bytes += outer_rows * (out->outer.types[i] == GX_INT8 || out->outer.types[i] == GX_FLOAT8 ? 8 : out->outer.types[i] == GX_CHAR ? 1 : 4);
 		if (out->has_join)
 		{
-			double		inner_rows = ((HashPath *) in)->jpath.innerjoinpath->parent->tuples;
+			Path	   *first = in;		/* the join whose build side is step 1: the lowest of a chain */
+			double		inner_rows;
 
+			while (IsA(((HashPath *) first)->jpath.outerjoinpath, HashPath))
+				first = ((HashPath *) first)->jpath.outerjoinpath;
+			inner_rows = ((HashPath *) first)->jpath.innerjoinpath->parent->tuples;
 			for (i = 0; i < out->inner.ncols; i++)
 				bytes += inner_rows * (out->inner.types[i] == GX_INT8 || out->inner.types[i] == GX_FLOAT8 ? 8 : out->inner.types[i] == GX_CHAR ? 1 : 4);
 			bytes += inner_rows * 32;
+		}
+		/* every further step of a chain: its staged columns and its join table, as for the first */
+		for (i = 0; i < out->n_more; i++)
+		{
+			const GpuJoinStep *m = &out->more[i];
+			int			j;
+
+			for (j = 0; j < m->rel.ncols; j++)
+				bytes += m->tuples * staged_type_bytes(m->rel.types[j]);
+			bytes += m->tuples * 32;
 		}
 		*est_bytes = bytes * 1.25;
 	}

@@ -156,6 +156,21 @@ int gx_hash_agg(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_a
 	*out = r;
 	return GX_OK;
 }
+/* the chain's steps in order, then the canned result of gx_hash_agg */
+int gx_hash_agg_joins(gx_ctx *ctx, const gx_table *outer, int n_steps, const gx_join_step *steps, const gx_agg_plan *plan, gx_result **out)
+{
+	int			i;
+
+	if (n_steps < 1 || n_steps > GX_MAX_JOINS || plan->outer_key_col >= 0) { snprintf(last_error, sizeof(last_error), "double: join chain of %d steps, outer key %d", n_steps, plan->outer_key_col); return GX_ERR_ARG; }
+	fprintf(stderr, "double: hash_agg_joins steps %d", n_steps);
+	for (i = 0; i < n_steps; i++)
+	{
+		if (!steps[i].h || !steps[i].h->unique) { snprintf(last_error, sizeof(last_error), "double: step %d has no unique table", i + 1); return GX_ERR_ARG; }
+		fprintf(stderr, " (key %d.%d table key %d)", steps[i].key.side, steps[i].key.col, steps[i].h->key_col);
+	}
+	fprintf(stderr, "\n");
+	return gx_hash_agg(ctx, outer, steps[0].h, plan, out);
+}
 int64_t gx_result_ngroups(const gx_result *r) { return r->ngroups; }
 int gx_result_fetch(gx_result *r, int64_t max_groups, int64_t *key_out, double *agg_out, uint8_t *null_out)
 {

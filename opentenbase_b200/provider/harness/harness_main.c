@@ -66,7 +66,18 @@ create_upper_paths_hook_type create_upper_paths_hook = NULL;
 static char last_msg[1024];
 bool errstart(int elevel, const char *filename, int lineno, const char *funcname, const char *domain)
 { return elevel >= ERROR; }
-void errfinish(int dummy,...) { fprintf(stderr, "harness: ereport(ERROR): %s\n", last_msg); exit(3); }
+static ResourceReleaseCallback release_cb;
+/* the transaction abort an ERROR causes: the resource owner's release callbacks run (they free every library handle of
+ * the query), then the context goes away */
+void errfinish(int dummy,...)
+{
+	fprintf(stderr, "harness: ereport(ERROR): %s\n", last_msg);
+	if (release_cb)
+		release_cb(RESOURCE_RELEASE_AFTER_LOCKS, false, true, NULL);
+	if (backend_ctx)
+		gx_shutdown(backend_ctx);
+	exit(3);
+}
 int errmsg(const char *fmt,...) { va_list ap; va_start(ap, fmt); vsnprintf(last_msg, sizeof(last_msg), fmt, ap); va_end(ap); return 0; }
 int errmsg_internal(const char *fmt,...) { return 0; }
 int errcode(int sqlerrcode) { return 0; }
@@ -231,7 +242,7 @@ typedef struct FakeRel
 	char	   *pages;
 	int			buf_base;		/* index of page 0 in LocalBufferBlockPointers */
 } FakeRel;
-static FakeRel fake_rels[2];
+static FakeRel fake_rels[GX_MAX_JOINS + 1];		/* the outer relation and one per join of a chain */
 static int	n_fake_rels = 0;
 
 Relation ExecOpenScanRelation(EState *estate, Index scanrelid, int eflags)
@@ -352,7 +363,8 @@ static char *out_value_list(List *l);
  * Query / RelOptInfo / Path nodes the hook reads, calls gpuexec_upper_paths_hook and PlanCustomPath, and prints what
  * came out: the path shape and costs, the descriptor as it would travel, and the scan tuple. */
 typedef struct PlanRel { RelOptInfo *rel; RangeTblEntry *rte; int ncols; Oid types[GX_MAX_COLS * 2]; int32 typmods[GX_MAX_COLS * 2]; bool notnull[GX_MAX_COLS * 2]; } PlanRel;
-static PlanRel plan_rels[3];
+#define PLAN_MAX_RELS (GX_MAX_JOINS + 2)			/* a chain one join longer than the provider takes */
+static PlanRel plan_rels[PLAN_MAX_RELS + 1];
 
 /* pg_attribute through the syscache, for column_is_not_null(): the scenario's "rel" line marks NOT NULL columns with a '!' */
 static struct { HeapTupleData tup; HeapTupleHeaderData hdr; char pad[64]; FormData_pg_attribute att; } fake_att_tuple;
@@ -361,7 +373,7 @@ HeapTuple SearchSysCache2(int cacheId, Datum key1, Datum key2)
 	int			r, a = DatumGetInt16(key2);
 
 	if (cacheId != ATTNUM) NOT_REACHED("SearchSysCache2 of another cache");
-	for (r = 1; r <= 2; r++)
+	for (r = 1; r <= PLAN_MAX_RELS; r++)
 		if (plan_rels[r].rte && plan_rels[r].rte->relid == DatumGetObjectId(key1) && a >= 1 && a <= plan_rels[r].ncols)
 		{
 			memset(&fake_att_tuple, 0, sizeof(fake_att_tuple));
@@ -389,7 +401,7 @@ static Var *plan_var(int rti, int att)
 {
 	Var		   *v = makeNode(Var);
 
-	if (rti < 1 || rti > 2 || att < 1 || att > plan_rels[rti].ncols) { fprintf(stderr, "harness: no column %d.%d\n", rti, att); exit(2); }
+	if (rti < 1 || rti > PLAN_MAX_RELS || att < 1 || att > plan_rels[rti].ncols) { fprintf(stderr, "harness: no column %d.%d\n", rti, att); exit(2); }
 	v->varno = rti; v->varattno = att; v->vartype = plan_rels[rti].types[att - 1]; v->vartypmod = plan_rels[rti].typmods[att - 1];
 	v->varnoold = rti; v->varoattno = att;
 	return v;
@@ -454,8 +466,8 @@ static int plan_main(const char *path)
 
 	if (!f) { perror(path); return 2; }
 	root->parse = parse;
-	root->simple_rel_array_size = 3;
-	root->simple_rte_array = (RangeTblEntry **) calloc(3, sizeof(RangeTblEntry *));
+	root->simple_rel_array_size = PLAN_MAX_RELS + 1;
+	root->simple_rte_array = (RangeTblEntry **) calloc(PLAN_MAX_RELS + 1, sizeof(RangeTblEntry *));
 	output_rel->reltarget = makeNode(PathTarget);
 	output_rel->rows = 100;
 	_PG_init();
@@ -468,6 +480,7 @@ static int plan_main(const char *path)
 		if (line[0] == '#' || line[0] == '\n') continue;
 		if (sscanf(line, "rel %d tuples %lf pages %lf cols %n", &r, &t, &pg, &n) == 3)
 		{
+			if (r < 1 || r > PLAN_MAX_RELS) { fprintf(stderr, "harness: rel %d\n", r); return 2; }
 			PlanRel    *pr = &plan_rels[r];
 			char	   *tok;
 
@@ -495,12 +508,14 @@ static int plan_main(const char *path)
 		else if (sscanf(line, "join %d.%d %d.%d unique %d %63s", &r, &a, &r2, &a2, &u, w) >= 5)
 		{
 			HashPath   *hp = makeNode(HashPath);
-			Path	   *op = makeNode(Path), *ip = makeNode(Path);
+			/* a second "join" line joins the previous join's result: the left-deep chain HashJoin(HashJoin(..), S) */
+			bool		chained = input_rel && input_rel->cheapest_total_path && IsA(input_rel->cheapest_total_path, HashPath);
+			Path	   *op = chained ? input_rel->cheapest_total_path : makeNode(Path), *ip = makeNode(Path);
 			RestrictInfo *ri = makeNode(RestrictInfo);
 			Var		   *lv = plan_var(r, a), *rv = plan_var(r2, a2);
 			bool		remote = strstr(line, "remote_inner") != NULL, swap = strstr(line, "swapped") != NULL;
 
-			op->pathtype = T_SeqScan; op->parent = plan_rels[r].rel; op->rows = op->parent->tuples; op->total_cost = op->parent->pages + 0.01 * op->rows;
+			if (!chained) { op->pathtype = T_SeqScan; op->parent = plan_rels[r].rel; op->rows = op->parent->tuples; op->total_cost = op->parent->pages + 0.01 * op->rows; }
 			ip->pathtype = remote ? T_RemoteSubplan : T_SeqScan; ip->parent = plan_rels[r2].rel; ip->rows = ip->parent->tuples; ip->total_cost = ip->parent->pages + 0.01 * ip->rows;
 			ri->clause = plan_op(lv->vartype == INT8OID ? F_INT8EQ : lv->vartype == INT4OID ? F_INT4EQ : F_TEXTEQ, swap ? (Node *) rv : (Node *) lv, swap ? (Node *) lv : (Node *) rv);
 			hp->jpath.path.pathtype = T_HashJoin; hp->jpath.inner_unique = u != 0;
@@ -647,6 +662,7 @@ int main(int argc, char **argv)
 	rd(f, magic, 4);
 	if (memcmp(magic, "GXH1", 4) != 0) { fprintf(stderr, "harness: bad magic\n"); return 2; }
 	nrels = rd32(f);
+	if (nrels < 1 || nrels > GX_MAX_JOINS + 1) { fprintf(stderr, "harness: %d relations\n", nrels); return 2; }
 	for (r = 0; r < nrels; r++)
 	{
 		FakeRel    *fr = &fake_rels[r];
@@ -685,7 +701,11 @@ int main(int argc, char **argv)
 			LocalBufferBlockPointers[fake_rels[r].buf_base + i] = (Block) (fake_rels[r].pages + (size_t) i * BLCKSZ);
 
 	memset(&desc, 0, sizeof(desc));
+	/* 0 no join, 1 one join, n > 1 a chain of n joins whose steps 2.. follow the first join's block */
 	desc.has_join = rd32(f);
+	desc.n_more = desc.has_join > 1 ? desc.has_join - 1 : 0;
+	desc.has_join = desc.has_join != 0;
+	if (desc.n_more > GX_MAX_JOINS - 1) { fprintf(stderr, "harness: %d joins\n", 1 + desc.n_more); return 2; }
 	read_relinfo(f, &desc.outer);
 	if (desc.has_join)
 	{
@@ -696,6 +716,19 @@ int main(int argc, char **argv)
 		desc.inner_unique = rd32(f);
 		desc.n_inner_preds = rd32(f);
 		rd(f, desc.inner_preds, sizeof(gx_pred) * desc.n_inner_preds);
+		for (r = 0; r < desc.n_more; r++)
+		{
+			GpuJoinStep *m = &desc.more[r];
+
+			read_relinfo(f, &m->rel);
+			m->key_col = rd32(f);
+			m->probe.side = rd32(f);
+			m->probe.col = rd32(f);
+			m->n_payload = rd32(f);
+			for (i = 0; i < m->n_payload; i++) m->payload_cols[i] = rd32(f);
+			m->n_preds = rd32(f);
+			rd(f, m->preds, sizeof(gx_pred) * m->n_preds);
+		}
 	}
 	desc.partial = rd32(f);
 	rd(f, &desc.plan, sizeof(gx_agg_plan));
