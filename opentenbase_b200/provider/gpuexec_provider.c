@@ -110,16 +110,19 @@ typedef struct GpuRelInfo
 	int32		types[GX_MAX_COLS];		/* GX_* */
 } GpuRelInfo;
 
-/* steps 2.. of a join chain (gx_hash_agg_joins); step 1 is the single join's inner side below */
+/* one hash join of the plan: step s (1..) of a left-deep chain builds its table over rel and probes it with the rows that
+ * passed steps 1 .. s-1 */
 typedef struct GpuJoinStep
 {
 	GpuRelInfo	rel;
 	int			key_col;		/* build key column of rel */
 	int			n_payload;
 	int32		payload_cols[GX_MAX_PAYLOAD];
+	bool		unique;			/* the build keys are unique (inner_unique) */
 	int			n_preds;
 	gx_pred		preds[GX_MAX_PREDS];
-	gx_colref	probe;			/* probe key: side 0 an outer column, side s a payload column of step s */
+	gx_colref	probe;			/* steps 2..: probe key, side 0 an outer column, side s a payload column of step s;
+								 * step 1 probes with plan.outer_key_col */
 	double		tuples;			/* planner only (HBM estimate), not shipped */
 	Relation	r;
 	gx_table   *tab;
@@ -133,23 +136,14 @@ typedef struct GpuExecState
 {
 	CustomScanState css;
 	/* decoded from custom_private */
-	GpuRelInfo	outer,
-				inner;
-	bool		has_join;
-	int			inner_key_col;
-	int			n_payload;
-	int32		payload_cols[GX_MAX_PAYLOAD];
-	bool		inner_unique;
-	int			n_inner_preds;
-	gx_pred		inner_preds[GX_MAX_PREDS];
+	GpuRelInfo	outer;
+	int			n_joins;		/* 0 no join, 1 a join of plan.join_type, 2.. a chain of unique INNER joins */
+	GpuJoinStep join[GX_MAX_JOINS];
 	bool		partial;		/* emit transition states (AGGSPLIT_INITIAL_SERIAL), not final values */
 	gx_agg_plan plan;
 	/* run time */
-	Relation	outer_rel,
-				inner_rel;
-	gx_table   *outer_tab,
-			   *inner_tab;
-	gx_hash    *hash;
+	Relation	outer_rel;
+	gx_table   *outer_tab;
 	gx_result  *result;
 	int64		ngroups,
 				next;
@@ -160,10 +154,6 @@ typedef struct GpuExecState
 	double		load_ms,
 				exec_ms;
 	bool		done_exec;
-	/* a chain of unique INNER joins: step 1 is inner above, steps 2 .. 1 + n_more here; step 1's probe key is
-	 * plan.outer_key_col until gpuexec_run hands the chain to gx_hash_agg_joins */
-	int			n_more;
-	GpuJoinStep more[GX_MAX_JOINS - 1];
 } GpuExecState;
 
 /* handles that must die with the query even when ereport() longjmps past us */
@@ -180,23 +170,18 @@ gpuexec_release_state(GpuExecState *st)
 {
 	if (st->result)
 		gx_result_free(st->result);
-	if (st->hash)
-		gx_hash_free(st->hash);
 	if (st->outer_tab)
 		gx_table_free(st->outer_tab);
-	if (st->inner_tab)
-		gx_table_free(st->inner_tab);
 	st->result = NULL;
-	st->hash = NULL;
-	st->outer_tab = st->inner_tab = NULL;
-	for (int i = 0; i < st->n_more; i++)
+	st->outer_tab = NULL;
+	for (int i = 0; i < st->n_joins; i++)
 	{
-		if (st->more[i].hash)
-			gx_hash_free(st->more[i].hash);
-		if (st->more[i].tab)
-			gx_table_free(st->more[i].tab);
-		st->more[i].hash = NULL;
-		st->more[i].tab = NULL;
+		if (st->join[i].hash)
+			gx_hash_free(st->join[i].hash);
+		if (st->join[i].tab)
+			gx_table_free(st->join[i].tab);
+		st->join[i].hash = NULL;
+		st->join[i].tab = NULL;
 	}
 }
 
@@ -451,6 +436,76 @@ deserialise_rel(ListCell **lc, GpuRelInfo *r)
 	}
 }
 
+/* n quals of four words each: column, operator, integer and float8 constant (their count travels ahead of them) */
+static List *
+put_preds(List *l, int n, const gx_pred *preds)
+{
+	int			i;
+
+	for (i = 0; i < n; i++)
+	{
+		l = put_int(l, preds[i].col);
+		l = put_int(l, preds[i].op);
+		l = put_int64(l, preds[i].ival);
+		l = put_double(l, preds[i].fval);
+	}
+	return l;
+}
+static void
+get_preds(ListCell **lc, int n, gx_pred *preds)
+{
+	int			i;
+
+	for (i = 0; i < n; i++)
+	{
+		preds[i].col = get_int(lc);
+		preds[i].op = get_int(lc);
+		preds[i].ival = get_int64(lc);
+		preds[i].fval = get_double(lc);
+	}
+}
+
+/* one join step's block: rel, key column, [step 2..: probe side and column,] payload, [step 1: unique,] quals */
+static List *
+serialise_step(List *l, const GpuJoinStep *j, bool first)
+{
+	int			i;
+
+	l = serialise_rel(l, &j->rel);
+	l = put_int(l, j->key_col);
+	if (!first)
+	{
+		l = put_int(l, j->probe.side);
+		l = put_int(l, j->probe.col);
+	}
+	l = put_int(l, j->n_payload);
+	for (i = 0; i < j->n_payload; i++)
+		l = put_int(l, j->payload_cols[i]);
+	if (first)
+		l = put_int(l, j->unique);
+	l = put_int(l, j->n_preds);
+	return put_preds(l, j->n_preds, j->preds);
+}
+static void
+deserialise_step(ListCell **lc, GpuJoinStep *j, bool first)
+{
+	int			i;
+
+	deserialise_rel(lc, &j->rel);
+	j->key_col = get_int(lc);
+	if (!first)
+	{
+		j->probe.side = get_int(lc);
+		j->probe.col = get_int(lc);
+	}
+	j->n_payload = get_int(lc);
+	for (i = 0; i < j->n_payload; i++)
+		j->payload_cols[i] = get_int(lc);
+	j->unique = first ? get_int(lc) != 0 : true;	/* every step of a chain is unique */
+	j->n_preds = get_int(lc);
+	get_preds(lc, j->n_preds, j->preds);
+}
+
 static List *
 gpuexec_serialise(const GpuExecState *st)
 {
@@ -460,59 +515,20 @@ gpuexec_serialise(const GpuExecState *st)
 				j;
 
 	l = put_int(l, GX_ABI_VERSION);
-	/* 0 = no join, else 1 + GX_JOIN_*: an INNER join keeps the word it had before SEMI and ANTI existed; a chain has
-	 * its own word, and its steps 2.. follow the single join's block */
-	l = put_int(l, st->n_more > 0 ? GPUEXEC_DESC_CHAIN : st->has_join ? 1 + p->join_type : 0);
+	/* 0 = no join, 1 + GX_JOIN_* one join (an INNER join keeps the word it had before SEMI and ANTI existed), or the chain
+	 * word; a chain's count of further steps and their blocks follow step 1's block */
+	l = put_int(l, st->n_joins == 0 ? 0 : st->n_joins == 1 ? 1 + p->join_type : GPUEXEC_DESC_CHAIN);
 	l = serialise_rel(l, &st->outer);
-	if (st->has_join)
+	for (j = 0; j < st->n_joins; j++)
 	{
-		l = serialise_rel(l, &st->inner);
-		l = put_int(l, st->inner_key_col);
-		l = put_int(l, st->n_payload);
-		for (i = 0; i < st->n_payload; i++)
-			l = put_int(l, st->payload_cols[i]);
-		l = put_int(l, st->inner_unique);
-		l = put_int(l, st->n_inner_preds);
-		for (i = 0; i < st->n_inner_preds; i++)
-		{
-			l = put_int(l, st->inner_preds[i].col);
-			l = put_int(l, st->inner_preds[i].op);
-			l = put_int64(l, st->inner_preds[i].ival);
-			l = put_double(l, st->inner_preds[i].fval);
-		}
-		if (st->n_more > 0)
-			l = put_int(l, st->n_more);
-		for (j = 0; j < st->n_more; j++)
-		{
-			const GpuJoinStep *m = &st->more[j];
-
-			l = serialise_rel(l, &m->rel);
-			l = put_int(l, m->key_col);
-			l = put_int(l, m->probe.side);
-			l = put_int(l, m->probe.col);
-			l = put_int(l, m->n_payload);
-			for (i = 0; i < m->n_payload; i++)
-				l = put_int(l, m->payload_cols[i]);
-			l = put_int(l, m->n_preds);
-			for (i = 0; i < m->n_preds; i++)
-			{
-				l = put_int(l, m->preds[i].col);
-				l = put_int(l, m->preds[i].op);
-				l = put_int64(l, m->preds[i].ival);
-				l = put_double(l, m->preds[i].fval);
-			}
-		}
+		if (j == 1)
+			l = put_int(l, st->n_joins - 1);
+		l = serialise_step(l, &st->join[j], j == 0);
 	}
 	l = put_int(l, st->partial);
 	l = put_int(l, p->n_preds);
 	l = put_int(l, p->outer_key_col);
-	for (i = 0; i < p->n_preds; i++)
-	{
-		l = put_int(l, p->preds[i].col);
-		l = put_int(l, p->preds[i].op);
-		l = put_int64(l, p->preds[i].ival);
-		l = put_double(l, p->preds[i].fval);
-	}
+	l = put_preds(l, p->n_preds, p->preds);
 	l = put_int(l, p->n_group_cols);
 	for (i = 0; i < p->n_group_cols; i++)
 	{
@@ -547,63 +563,23 @@ gpuexec_deserialise(List *priv, GpuExecState *st)
 		ereport(ERROR, (errmsg("gpuexec: coordinator and datanode run different provider versions")));
 	memset(p, 0, sizeof(*p));
 	i = get_int(&lc);
-	st->has_join = i != 0;
 	p->join_type = i != 0 && i != GPUEXEC_DESC_CHAIN ? i - 1 : GX_JOIN_INNER;
-	st->n_more = i == GPUEXEC_DESC_CHAIN ? -1 : 0;		/* read after the first join's block */
+	st->n_joins = i != 0;
 	deserialise_rel(&lc, &st->outer);
-	if (st->has_join)
+	if (st->n_joins)
+		deserialise_step(&lc, &st->join[0], true);
+	if (i == GPUEXEC_DESC_CHAIN)
 	{
-		deserialise_rel(&lc, &st->inner);
-		st->inner_key_col = get_int(&lc);
-		st->n_payload = get_int(&lc);
-		for (i = 0; i < st->n_payload; i++)
-			st->payload_cols[i] = get_int(&lc);
-		st->inner_unique = get_int(&lc);
-		st->n_inner_preds = get_int(&lc);
-		for (i = 0; i < st->n_inner_preds; i++)
-		{
-			st->inner_preds[i].col = get_int(&lc);
-			st->inner_preds[i].op = get_int(&lc);
-			st->inner_preds[i].ival = get_int64(&lc);
-			st->inner_preds[i].fval = get_double(&lc);
-		}
-		if (st->n_more < 0)
-		{
-			st->n_more = get_int(&lc);
-			if (st->n_more < 1 || st->n_more > GX_MAX_JOINS - 1)
-				ereport(ERROR, (errmsg("gpuexec: join chain of %d steps in the plan descriptor", 1 + st->n_more)));
-		}
-		for (j = 0; j < st->n_more; j++)
-		{
-			GpuJoinStep *m = &st->more[j];
-
-			deserialise_rel(&lc, &m->rel);
-			m->key_col = get_int(&lc);
-			m->probe.side = get_int(&lc);
-			m->probe.col = get_int(&lc);
-			m->n_payload = get_int(&lc);
-			for (i = 0; i < m->n_payload; i++)
-				m->payload_cols[i] = get_int(&lc);
-			m->n_preds = get_int(&lc);
-			for (i = 0; i < m->n_preds; i++)
-			{
-				m->preds[i].col = get_int(&lc);
-				m->preds[i].op = get_int(&lc);
-				m->preds[i].ival = get_int64(&lc);
-				m->preds[i].fval = get_double(&lc);
-			}
-		}
+		st->n_joins = 1 + get_int(&lc);
+		if (st->n_joins < 2 || st->n_joins > GX_MAX_JOINS)
+			ereport(ERROR, (errmsg("gpuexec: join chain of %d steps in the plan descriptor", st->n_joins)));
+		for (j = 1; j < st->n_joins; j++)
+			deserialise_step(&lc, &st->join[j], false);
 	}
 	st->partial = get_int(&lc);
 	p->n_preds = get_int(&lc);
 	p->outer_key_col = get_int(&lc);
-	for (i = 0; i < p->n_preds; i++)
-	{
-		p->preds[i].col = get_int(&lc);
-		p->preds[i].op = get_int(&lc);
-		p->preds[i].ival = get_int64(&lc);
-		p->preds[i].fval = get_double(&lc);
-	}
+	get_preds(&lc, p->n_preds, p->preds);
 	p->n_group_cols = get_int(&lc);
 	for (i = 0; i < p->n_group_cols; i++)
 	{
@@ -669,10 +645,8 @@ gpuexec_begin(CustomScanState *node, EState *estate, int eflags)
 	/* scanrelid == 0: ExecInitCustomScan built the scan slot from custom_scan_tlist
 	 * (nodeCustom.c:81-94); we open the base relations ourselves */
 	st->outer_rel = ExecOpenScanRelation(estate, st->outer.rti, eflags);
-	if (st->has_join)
-		st->inner_rel = ExecOpenScanRelation(estate, st->inner.rti, eflags);
-	for (int i = 0; i < st->n_more; i++)
-		st->more[i].r = ExecOpenScanRelation(estate, st->more[i].rel.rti, eflags);
+	for (int i = 0; i < st->n_joins; i++)
+		st->join[i].r = ExecOpenScanRelation(estate, st->join[i].rel.rti, eflags);
 	h = (GpuHandles *) malloc(sizeof(GpuHandles));
 	h->owner = CurrentResourceOwner;
 	h->state = st;
@@ -690,46 +664,41 @@ gpuexec_run(GpuExecState *st, EState *estate)
 				t1;
 
 	INSTR_TIME_SET_CURRENT(t0);
-	if (st->has_join)
-		gpuexec_load_relation(st->inner_rel, estate, &st->inner, &st->inner_tab);
-	for (int i = 0; i < st->n_more; i++)
-		gpuexec_load_relation(st->more[i].r, estate, &st->more[i].rel, &st->more[i].tab);
+	for (int i = 0; i < st->n_joins; i++)
+		gpuexec_load_relation(st->join[i].r, estate, &st->join[i].rel, &st->join[i].tab);
 	gpuexec_load_relation(st->outer_rel, estate, &st->outer, &st->outer_tab);
 	INSTR_TIME_SET_CURRENT(t1);
 	INSTR_TIME_SUBTRACT(t1, t0);
 	st->load_ms = INSTR_TIME_GET_MILLISEC(t1);
 
 	INSTR_TIME_SET_CURRENT(t0);
-	if (st->has_join)
-		GX_CHECK(gx_hash_build(backend_ctx, st->inner_tab, st->inner_key_col, st->n_inner_preds, st->inner_preds,
-							   st->n_payload, st->payload_cols, st->inner_unique, &st->hash));
-	CHECK_FOR_INTERRUPTS();
-	if (st->n_more > 0)
+	/* the tables in chain order; every one is in st before the next call, so an ERROR frees them all */
+	for (int i = 0; i < st->n_joins; i++)
 	{
-		/* the chain in build order; every table is in st before the next call, so an ERROR frees them all */
+		GpuJoinStep *j = &st->join[i];
+
+		GX_CHECK(gx_hash_build(backend_ctx, j->tab, j->key_col, j->n_preds, j->preds, j->n_payload, j->payload_cols, j->unique, &j->hash));
+		CHECK_FOR_INTERRUPTS();
+	}
+	if (st->n_joins >= 2)
+	{
 		gx_join_step steps[GX_MAX_JOINS];
 		gx_agg_plan cp = st->plan;
 
 		memset(steps, 0, sizeof(steps));
-		steps[0].h = st->hash;
+		for (int i = 0; i < st->n_joins; i++)
+		{
+			steps[i].h = st->join[i].hash;
+			steps[i].key = st->join[i].probe;
+			steps[i].join_type = GX_JOIN_INNER;
+		}
 		steps[0].key.side = 0;
 		steps[0].key.col = st->plan.outer_key_col;
-		steps[0].join_type = GX_JOIN_INNER;
-		for (int i = 0; i < st->n_more; i++)
-		{
-			GpuJoinStep *m = &st->more[i];
-
-			GX_CHECK(gx_hash_build(backend_ctx, m->tab, m->key_col, m->n_preds, m->preds, m->n_payload, m->payload_cols, 1, &m->hash));
-			steps[1 + i].h = m->hash;
-			steps[1 + i].key = m->probe;
-			steps[1 + i].join_type = GX_JOIN_INNER;
-			CHECK_FOR_INTERRUPTS();
-		}
 		cp.outer_key_col = -1;
-		GX_CHECK(gx_hash_agg_joins(backend_ctx, st->outer_tab, 1 + st->n_more, steps, &cp, &st->result));
+		GX_CHECK(gx_hash_agg_joins(backend_ctx, st->outer_tab, st->n_joins, steps, &cp, &st->result));
 	}
 	else
-		GX_CHECK(gx_hash_agg(backend_ctx, st->outer_tab, st->hash, &st->plan, &st->result));
+		GX_CHECK(gx_hash_agg(backend_ctx, st->outer_tab, st->n_joins ? st->join[0].hash : NULL, &st->plan, &st->result));
 	/* The result holds this datanode's groups only.  Whether they are final is the PLANNER's
 	 * business: the hook offers the pushed-down path only when the GROUP BY covers the
 	 * distribution key, and otherwise asks for partial states, which the reference's own
@@ -890,11 +859,9 @@ gpuexec_end(CustomScanState *node)
 	}
 	if (st->outer_rel)
 		ExecCloseScanRelation(st->outer_rel);
-	if (st->inner_rel)
-		ExecCloseScanRelation(st->inner_rel);
-	for (int i = 0; i < st->n_more; i++)
-		if (st->more[i].r)
-			ExecCloseScanRelation(st->more[i].r);
+	for (int i = 0; i < st->n_joins; i++)
+		if (st->join[i].r)
+			ExecCloseScanRelation(st->join[i].r);
 }
 
 static void
@@ -911,11 +878,11 @@ gpuexec_explain(CustomScanState *node, List *ancestors, ExplainState *es)
 {
 	GpuExecState *st = (GpuExecState *) node;
 
-	ExplainPropertyText("GPU Strategy", st->has_join ? "hash build + fused probe/aggregate" : "scan + hash aggregate", es);
-	if (st->has_join)
+	ExplainPropertyText("GPU Strategy", st->n_joins ? "hash build + fused probe/aggregate" : "scan + hash aggregate", es);
+	if (st->n_joins)
 		ExplainPropertyText("GPU Join Type", st->plan.join_type == GX_JOIN_SEMI ? "Semi" : st->plan.join_type == GX_JOIN_ANTI ? "Anti" : "Inner", es);
-	if (st->n_more > 0)
-		ExplainPropertyInteger("GPU Joins", NULL, 1 + st->n_more, es);
+	if (st->n_joins > 1)
+		ExplainPropertyInteger("GPU Joins", NULL, st->n_joins, es);
 	ExplainPropertyText("GPU Output", st->partial ? "partial states (Finalize above the redistribute)" : "final values (GROUP BY covers the distribution key)", es);
 	if (es->analyze && st->done_exec)
 	{
@@ -971,7 +938,7 @@ gpuexec_plan_path(PlannerInfo *root, RelOptInfo *rel, CustomPath *best_path,
  *            Agg over HashJoin[SEMI / ANTI, the same key shape]  (EXISTS / NOT EXISTS: TPC-H Q4, Q21, Q22 shapes),
  *            with GROUP BY columns and aggregate arguments from the outer side only
  *            Agg over a left-deep chain of 2..GX_MAX_JOINS such INNER joins with unique build sides (star joins:
- *            TPC-H Q3), GROUP BY columns from any relation, aggregate arguments from the outer one (match_chain)
+ *            TPC-H Q3), GROUP BY columns from any relation, aggregate arguments from the outer one (match_joins)
  * with "Var op Const" quals on the scans, Var group keys, no HAVING / grouping sets /
  * DISTINCT / ORDER BY aggregates / FILTER, and aggregates count(*), count(x),
  * sum/avg/min/max(float8 expr), sum(int4); every target-list entry must be a group Var or a
@@ -1261,25 +1228,22 @@ payload_slot(int32 *cols, int *n, int c)
 	return (*n)++;
 }
 
-/* the chain step (1..) whose build side scans rti, or 0 */
+/* the join step (1..) whose build side scans rti, or 0 */
 static int
-chain_step_of(const GpuExecState *st, Index rti)
+join_step_of(const GpuExecState *st, Index rti)
 {
 	int			i;
 
-	if (st->inner.rti == rti)
-		return 1;
-	for (i = 0; i < st->n_more; i++)
-		if (st->more[i].rel.rti == rti)
-			return 2 + i;
+	for (i = 0; i < st->n_joins; i++)
+		if (st->join[i].rel.rti == rti)
+			return 1 + i;
 	return 0;
 }
 
-/* One level of a left-deep join chain: INNER with a unique build side, exactly one int4eq / int8eq hash clause that is its
- * whole joinrestrictinfo, and a plain SeqScan of an unprotected relation as the build side.  *iv = the clause's Var of
- * the build side, *ov = the other one. */
+/* One level of a left-deep join: exactly one int4eq / int8eq hash clause that is its whole joinrestrictinfo, and a plain
+ * SeqScan of an unprotected relation as the build side.  *iv = the clause's Var of the build side, *ov = the other one. */
 static bool
-chain_level(PlannerInfo *root, HashPath *hp, Var **ov, Var **iv)
+join_level(PlannerInfo *root, HashPath *hp, Var **ov, Var **iv)
 {
 	Path	   *ip = hp->jpath.innerjoinpath;
 	RestrictInfo *ri;
@@ -1287,8 +1251,6 @@ chain_level(PlannerInfo *root, HashPath *hp, Var **ov, Var **iv)
 	Var		   *a,
 			   *b;
 
-	if (hp->jpath.jointype != JOIN_INNER || !hp->jpath.inner_unique)
-		return false;
 	if (list_length(hp->path_hashclauses) != 1 || list_length(hp->jpath.joinrestrictinfo) != 1)
 		return false;
 	if (ip->pathtype != T_SeqScan)		/* a RemoteSubplan below: the inputs are not co-located */
@@ -1315,11 +1277,13 @@ chain_level(PlannerInfo *root, HashPath *hp, Var **ov, Var **iv)
 	return true;
 }
 
-/* Agg over HashJoin(HashJoin(... SeqScan(F), SeqScan(D1)) ..., SeqScan(Dn)), 2 <= n <= GX_MAX_JOINS (gx_hash_agg_joins):
- * step s builds Ds; its probe key is a column of F or of an earlier D (carried in that step's payload, which has no
- * NULL flag: the column must be NOT NULL).  Step 1 is described by the single join's fields, steps 2.. by out->more. */
+/* Agg over HashJoin(HashJoin(... SeqScan(F), SeqScan(D1)) ..., SeqScan(Dn)), 1 <= n <= GX_MAX_JOINS: step s builds Ds.
+ * One join may be INNER, SEMI or ANTI (EXISTS / NOT EXISTS); a chain (gx_hash_agg_joins) must be INNER with a unique
+ * build side on every level.  LEFT, RIGHT, FULL and the JOIN_UNIQUE_* forms stay on the CPU.  Step 1's probe key is a
+ * column of F; a later step's is a column of F or of an earlier D, carried in that step's payload (which has no NULL
+ * flag: the column must be NOT NULL). */
 static bool
-match_chain(PlannerInfo *root, HashPath *top, GpuExecState *out, double *est_bytes, double *est_pages)
+match_joins(PlannerInfo *root, HashPath *top, GpuExecState *out, double *est_bytes, double *est_pages)
 {
 	HashPath   *lv[GX_MAX_JOINS];
 	Path	   *p = &top->jpath.path;
@@ -1334,70 +1298,64 @@ match_chain(PlannerInfo *root, HashPath *top, GpuExecState *out, double *est_byt
 		lv[n++] = (HashPath *) p;
 		p = ((HashPath *) p)->jpath.outerjoinpath;
 	}
-	if (n < 2 || p->pathtype != T_SeqScan)
+	if (p->pathtype != T_SeqScan)
 		return false;
-	out->has_join = true;
-	out->inner_unique = true;
-	plan->join_type = GX_JOIN_INNER;
 	out->outer.rti = p->parent->relid;
-	if (relation_is_protected(root, out->outer.rti) ||
-		!match_quals(p->parent->baserestrictinfo, &out->outer, plan->preds, &plan->n_preds))
+	if (relation_is_protected(root, out->outer.rti))
 		return false;
+	out->n_joins = n;
 	*est_bytes = p->parent->tuples;
 	*est_pages = p->parent->pages;
-	out->n_more = n - 1;
 	for (s = 1; s <= n; s++)
 	{
 		HashPath   *hp = lv[n - s];
+		JoinType	jt = hp->jpath.jointype;
 		RelOptInfo *irel = hp->jpath.innerjoinpath->parent;
-		GpuRelInfo *rel = s == 1 ? &out->inner : &out->more[s - 2].rel;
+		GpuJoinStep *j = &out->join[s - 1];
 		Var		   *ov,
 				   *iv;
-		int			kc,
-					c,
-					t,
-					side = 0;
+		int			c,
+					t = 0;
 
-		if (!chain_level(root, hp, &ov, &iv))
+		if (n == 1 ? (jt != JOIN_INNER && jt != JOIN_SEMI && jt != JOIN_ANTI) : (jt != JOIN_INNER || !hp->jpath.inner_unique))
 			return false;
-		rel->rti = iv->varno;
-		kc = rel_column(rel, iv->varno, iv->varattno, iv->vartype, iv->vartypmod);
-		if (kc < 0)
+		if (!join_level(root, hp, &ov, &iv))
+			return false;
+		plan->join_type = jt == JOIN_SEMI ? GX_JOIN_SEMI : jt == JOIN_ANTI ? GX_JOIN_ANTI : GX_JOIN_INNER;
+		j->unique = hp->jpath.inner_unique;
+		j->tuples = irel->tuples;
+		j->rel.rti = iv->varno;
+		j->key_col = rel_column(&j->rel, iv->varno, iv->varattno, iv->vartype, iv->vartypmod);
+		if (j->key_col < 0)
 			return false;
 		/* the probe key: a column of F, or the payload of the earlier step that scans ov's relation */
 		if (ov->varno == out->outer.rti)
 			c = rel_column(&out->outer, ov->varno, ov->varattno, ov->vartype, ov->vartypmod);
 		else
 		{
-			t = chain_step_of(out, ov->varno);
+			t = join_step_of(out, ov->varno);
 			if (t < 1 || t >= s || !column_is_not_null(root, ov->varno, ov->varattno))
 				return false;
-			c = rel_column(t == 1 ? &out->inner : &out->more[t - 2].rel, ov->varno, ov->varattno, ov->vartype, ov->vartypmod);
+			c = rel_column(&out->join[t - 1].rel, ov->varno, ov->varattno, ov->vartype, ov->vartypmod);
 			if (c >= 0)
-				c = t == 1 ? payload_slot(out->payload_cols, &out->n_payload, c)
-					: payload_slot(out->more[t - 2].payload_cols, &out->more[t - 2].n_payload, c);
-			side = t;
+				c = payload_slot(out->join[t - 1].payload_cols, &out->join[t - 1].n_payload, c);
 		}
 		if (c < 0)
 			return false;
 		if (s == 1)
 		{
-			plan->outer_key_col = c;		/* side 0: step 1 probes with a column of F */
-			out->inner_key_col = kc;
-			if (!match_quals(irel->baserestrictinfo, &out->inner, out->inner_preds, &out->n_inner_preds))
+			/* the outer quals right after step 1's probe key: F's columns are numbered in the order they are first met */
+			plan->outer_key_col = c;
+			if (!match_quals(p->parent->baserestrictinfo, &out->outer, plan->preds, &plan->n_preds))
 				return false;
 		}
 		else
 		{
-			GpuJoinStep *m = &out->more[s - 2];
-
-			m->key_col = kc;
-			m->probe.side = side;
-			m->probe.col = c;
-			m->tuples = irel->tuples;
-			if (!match_quals(irel->baserestrictinfo, &m->rel, m->preds, &m->n_preds))
-				return false;
+			j->probe.side = t;
+			j->probe.col = c;
 		}
+		if (!match_quals(irel->baserestrictinfo, &j->rel, j->preds, &j->n_preds))
+			return false;
 		*est_pages += irel->pages;
 	}
 	return true;
@@ -1426,74 +1384,15 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 		*est_bytes = input_rel->tuples;
 		*est_pages = input_rel->pages;
 	}
-	else if (IsA(in, HashPath) && IsA(((HashPath *) in)->jpath.outerjoinpath, HashPath))
-	{
-		if (!match_chain(root, (HashPath *) in, out, est_bytes, est_pages))
-			return false;
-	}
 	else if (IsA(in, HashPath))
 	{
-		HashPath   *hp = (HashPath *) in;
-		Path	   *op = hp->jpath.outerjoinpath,
-				   *ip = hp->jpath.innerjoinpath;
-		RestrictInfo *ri;
-		OpExpr	   *clause;
-		Var		   *lv,
-				   *rv;
-
-		/* LEFT, RIGHT, FULL and the JOIN_UNIQUE_* forms stay on the CPU */
-		if (hp->jpath.jointype == JOIN_INNER)
-			plan->join_type = GX_JOIN_INNER;
-		else if (hp->jpath.jointype == JOIN_SEMI)
-			plan->join_type = GX_JOIN_SEMI;
-		else if (hp->jpath.jointype == JOIN_ANTI)
-			plan->join_type = GX_JOIN_ANTI;
-		else
+		if (!match_joins(root, (HashPath *) in, out, est_bytes, est_pages))
 			return false;
-		if (list_length(hp->path_hashclauses) != 1 || hp->jpath.joinrestrictinfo == NIL ||
-			list_length(hp->jpath.joinrestrictinfo) != 1)
-			return false;
-		/* both inputs must be plain scans of co-located shards: a RemoteSubplan below the join
-		 * (pathtype T_RemoteSubplan) means the reference redistributes first — decline */
-		if (op->pathtype != T_SeqScan || ip->pathtype != T_SeqScan)
-			return false;
-		ri = (RestrictInfo *) linitial(hp->path_hashclauses);
-		clause = (OpExpr *) ri->clause;
-		if (!IsA(clause, OpExpr) || list_length(clause->args) != 2 || !IsA(linitial(clause->args), Var) || !IsA(lsecond(clause->args), Var))
-			return false;
-		if (clause->opfuncid != F_INT4EQ && clause->opfuncid != F_INT8EQ)
-			return false;
-		lv = (Var *) linitial(clause->args);
-		rv = (Var *) lsecond(clause->args);
-		if (lv->varno != op->parent->relid)
-		{
-			Var		   *t = lv;
-
-			lv = rv;
-			rv = t;
-		}
-		if (lv->varno != op->parent->relid || rv->varno != ip->parent->relid)
-			return false;
-		out->has_join = true;
-		out->outer.rti = op->parent->relid;
-		out->inner.rti = ip->parent->relid;
-		if (relation_is_protected(root, out->outer.rti) || relation_is_protected(root, out->inner.rti))
-			return false;
-		plan->outer_key_col = rel_column(&out->outer, lv->varno, lv->varattno, lv->vartype, lv->vartypmod);
-		out->inner_key_col = rel_column(&out->inner, rv->varno, rv->varattno, rv->vartype, rv->vartypmod);
-		out->inner_unique = hp->jpath.inner_unique;
-		if (plan->outer_key_col < 0 || out->inner_key_col < 0)
-			return false;
-		if (!match_quals(op->parent->baserestrictinfo, &out->outer, plan->preds, &plan->n_preds) ||
-			!match_quals(ip->parent->baserestrictinfo, &out->inner, out->inner_preds, &out->n_inner_preds))
-			return false;
-		*est_bytes = op->parent->tuples;
-		*est_pages = (double) op->parent->pages + (double) ip->parent->pages;
 	}
 	else
 		return false;
 
-	/* GROUP BY: plain Vars of either side; inner-side keys ride in the join payload */
+	/* GROUP BY: plain Vars of the outer side, or of a build side under INNER joins, riding in that join's payload */
 	foreach(lc, parse->groupClause)
 	{
 		SortGroupClause *sgc = (SortGroupClause *) lfirst(lc);
@@ -1512,29 +1411,19 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 			plan->group_cols[plan->n_group_cols].side = 0;
 			plan->group_cols[plan->n_group_cols].col = c;
 		}
-		else if (out->n_more > 0 && (s = chain_step_of(out, v->varno)) > 0)
+		else if (plan->join_type == GX_JOIN_INNER && (s = join_step_of(out, v->varno)) > 0)
 		{
-			/* a build-side column of chain step s, in that step's payload (a slot its probe key may share) */
-			c = rel_column(s == 1 ? &out->inner : &out->more[s - 2].rel, v->varno, v->varattno, v->vartype, v->vartypmod);
+			/* a build-side column of step s, in that step's payload (a slot its probe key or another GROUP BY entry may share) */
+			GpuJoinStep *j = &out->join[s - 1];
+
+			c = rel_column(&j->rel, v->varno, v->varattno, v->vartype, v->vartypmod);
 			if (c < 0 || !column_is_not_null(root, v->varno, v->varattno))
-				return false;
-			c = s == 1 ? payload_slot(out->payload_cols, &out->n_payload, c)
-				: payload_slot(out->more[s - 2].payload_cols, &out->more[s - 2].n_payload, c);
+				return false;		/* gx_hash_build carries payload columns inside the slot: no room for a NULL flag */
+			c = payload_slot(j->payload_cols, &j->n_payload, c);
 			if (c < 0)
 				return false;
 			plan->group_cols[plan->n_group_cols].side = s;
 			plan->group_cols[plan->n_group_cols].col = c;
-		}
-		else if (out->has_join && plan->join_type == GX_JOIN_INNER && v->varno == out->inner.rti && out->n_payload < GX_MAX_PAYLOAD)
-		{
-			c = rel_column(&out->inner, v->varno, v->varattno, v->vartype, v->vartypmod);
-			if (c < 0)
-				return false;
-			if (!column_is_not_null(root, v->varno, v->varattno))
-				return false;		/* gx_hash_build carries payload columns inside the slot: no room for a NULL flag */
-			out->payload_cols[out->n_payload] = c;
-			plan->group_cols[plan->n_group_cols].side = 1;
-			plan->group_cols[plan->n_group_cols].col = out->n_payload++;
 		}
 		else
 			return false;
@@ -1542,32 +1431,27 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 	}
 
 	/* Limits the library would only report at execution time (GX_ERR_ARG -> ERROR): decline here instead, the CPU plan stays.
-	 * The join payload is one 8-byte word (gx_hash_build, csrc/gx_join.cu); the group key is two 8-byte words filled first-fit
+	 * A join's payload is one 8-byte word (gx_hash_build, csrc/gx_join.cu); the group key is two 8-byte words filled first-fit
 	 * in GROUP BY order (compile_plan, csrc/gx_agg.cu). */
 	{
-		int			payload_bytes = 0,
-					used[2] = {0, 0};
+		int			used[2] = {0, 0};
 
-		for (i = 0; i < out->n_payload; i++)
-			payload_bytes += staged_type_bytes(out->inner.types[out->payload_cols[i]]);
-		if (payload_bytes > 8)
-			return false;
-		for (i = 0; i < out->n_more; i++)
+		for (i = 0; i < out->n_joins; i++)
 		{
-			const GpuJoinStep *m = &out->more[i];
-			int			j;
+			const GpuJoinStep *j = &out->join[i];
+			int			k,
+						payload_bytes = 0;
 
-			for (payload_bytes = 0, j = 0; j < m->n_payload; j++)
-				payload_bytes += staged_type_bytes(m->rel.types[m->payload_cols[j]]);
+			for (k = 0; k < j->n_payload; k++)
+				payload_bytes += staged_type_bytes(j->rel.types[j->payload_cols[k]]);
 			if (payload_bytes > 8)
 				return false;
 		}
 		for (i = 0; i < plan->n_group_cols; i++)
 		{
-			const int	side = plan->group_cols[i].side;
-			int32		t = side == 0 ? out->outer.types[plan->group_cols[i].col]
-				: side == 1 ? out->inner.types[out->payload_cols[plan->group_cols[i].col]]
-				: out->more[side - 2].rel.types[out->more[side - 2].payload_cols[plan->group_cols[i].col]];
+			const gx_colref *gc = &plan->group_cols[i];
+			int32		t = gc->side == 0 ? out->outer.types[gc->col]
+				: out->join[gc->side - 1].rel.types[out->join[gc->side - 1].payload_cols[gc->col]];
 			int			b = staged_type_bytes(t),
 						w = used[0] + b <= 8 ? 0 : 1;
 
@@ -1652,28 +1536,15 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 		double		outer_rows = *est_bytes;
 
 		for (i = 0; i < out->outer.ncols; i++)
-			bytes += outer_rows * (out->outer.types[i] == GX_INT8 || out->outer.types[i] == GX_FLOAT8 ? 8 : out->outer.types[i] == GX_CHAR ? 1 : 4);
-		if (out->has_join)
+			bytes += outer_rows * staged_type_bytes(out->outer.types[i]);
+		for (i = 0; i < out->n_joins; i++)
 		{
-			Path	   *first = in;		/* the join whose build side is step 1: the lowest of a chain */
-			double		inner_rows;
+			const GpuJoinStep *j = &out->join[i];
+			int			k;
 
-			while (IsA(((HashPath *) first)->jpath.outerjoinpath, HashPath))
-				first = ((HashPath *) first)->jpath.outerjoinpath;
-			inner_rows = ((HashPath *) first)->jpath.innerjoinpath->parent->tuples;
-			for (i = 0; i < out->inner.ncols; i++)
-				bytes += inner_rows * (out->inner.types[i] == GX_INT8 || out->inner.types[i] == GX_FLOAT8 ? 8 : out->inner.types[i] == GX_CHAR ? 1 : 4);
-			bytes += inner_rows * 32;
-		}
-		/* every further step of a chain: its staged columns and its join table, as for the first */
-		for (i = 0; i < out->n_more; i++)
-		{
-			const GpuJoinStep *m = &out->more[i];
-			int			j;
-
-			for (j = 0; j < m->rel.ncols; j++)
-				bytes += m->tuples * staged_type_bytes(m->rel.types[j]);
-			bytes += m->tuples * 32;
+			for (k = 0; k < j->rel.ncols; k++)
+				bytes += j->tuples * staged_type_bytes(j->rel.types[k]);
+			bytes += j->tuples * 32;
 		}
 		*est_bytes = bytes * 1.25;
 	}

@@ -356,10 +356,22 @@ out_value_list(List *l)
 	return buf;
 }
 
+/* the first of n quals whose constants did not come back bit for bit, or -1 */
+static int
+changed_pred(const gx_pred *sent, const gx_pred *got, int n)
+{
+	int			i;
+
+	for (i = 0; i < n; i++)
+		if (sent[i].ival != got[i].ival || memcmp(&sent[i].fval, &got[i].fval, 8) != 0)
+			return i;
+	return -1;
+}
+
 static char *out_value_list(List *l);
 /* ------------------------------------------------------------ --plan: a hand-built Query through the planner hook
  * The scenario file (written by tests/test_provider_planner_cpu.py) describes base relations, the input path (SeqScan or
- * HashJoin of two SeqScans), quals, GROUP BY, the target list and the input's distribution; this builds the PlannerInfo /
+ * a left-deep chain of HashJoins over SeqScans), quals, GROUP BY, the target list and the input's distribution; this builds the PlannerInfo /
  * Query / RelOptInfo / Path nodes the hook reads, calls gpuexec_upper_paths_hook and PlanCustomPath, and prints what
  * came out: the path shape and costs, the descriptor as it would travel, and the scan tuple. */
 typedef struct PlanRel { RelOptInfo *rel; RangeTblEntry *rte; int ncols; Oid types[GX_MAX_COLS * 2]; int32 typmods[GX_MAX_COLS * 2]; bool notnull[GX_MAX_COLS * 2]; } PlanRel;
@@ -701,34 +713,22 @@ int main(int argc, char **argv)
 			LocalBufferBlockPointers[fake_rels[r].buf_base + i] = (Block) (fake_rels[r].pages + (size_t) i * BLCKSZ);
 
 	memset(&desc, 0, sizeof(desc));
-	/* 0 no join, 1 one join, n > 1 a chain of n joins whose steps 2.. follow the first join's block */
-	desc.has_join = rd32(f);
-	desc.n_more = desc.has_join > 1 ? desc.has_join - 1 : 0;
-	desc.has_join = desc.has_join != 0;
-	if (desc.n_more > GX_MAX_JOINS - 1) { fprintf(stderr, "harness: %d joins\n", 1 + desc.n_more); return 2; }
+	/* the number of joins (0 none); step 1's block carries its unique flag, the blocks of steps 2.. their probe key */
+	desc.n_joins = rd32(f);
+	if (desc.n_joins < 0 || desc.n_joins > GX_MAX_JOINS) { fprintf(stderr, "harness: %d joins\n", desc.n_joins); return 2; }
 	read_relinfo(f, &desc.outer);
-	if (desc.has_join)
+	for (r = 0; r < desc.n_joins; r++)
 	{
-		read_relinfo(f, &desc.inner);
-		desc.inner_key_col = rd32(f);
-		desc.n_payload = rd32(f);
-		for (i = 0; i < desc.n_payload; i++) desc.payload_cols[i] = rd32(f);
-		desc.inner_unique = rd32(f);
-		desc.n_inner_preds = rd32(f);
-		rd(f, desc.inner_preds, sizeof(gx_pred) * desc.n_inner_preds);
-		for (r = 0; r < desc.n_more; r++)
-		{
-			GpuJoinStep *m = &desc.more[r];
+		GpuJoinStep *j = &desc.join[r];
 
-			read_relinfo(f, &m->rel);
-			m->key_col = rd32(f);
-			m->probe.side = rd32(f);
-			m->probe.col = rd32(f);
-			m->n_payload = rd32(f);
-			for (i = 0; i < m->n_payload; i++) m->payload_cols[i] = rd32(f);
-			m->n_preds = rd32(f);
-			rd(f, m->preds, sizeof(gx_pred) * m->n_preds);
-		}
+		read_relinfo(f, &j->rel);
+		j->key_col = rd32(f);
+		if (r > 0) { j->probe.side = rd32(f); j->probe.col = rd32(f); }
+		j->n_payload = rd32(f);
+		for (i = 0; i < j->n_payload; i++) j->payload_cols[i] = rd32(f);
+		j->unique = r == 0 ? rd32(f) != 0 : true;	/* every step of a chain is unique */
+		j->n_preds = rd32(f);
+		rd(f, j->preds, sizeof(gx_pred) * j->n_preds);
 	}
 	desc.partial = rd32(f);
 	rd(f, &desc.plan, sizeof(gx_agg_plan));
@@ -751,10 +751,9 @@ int main(int argc, char **argv)
 		gpuexec_deserialise(back, &got);
 		again = out_value_list(gpuexec_serialise(&got));
 		if (strcmp(wire, again) != 0) { fprintf(stderr, "harness: descriptor changed in transit\n sent %s\n got  %s\n", wire, again); return 3; }
-		for (i = 0; i < desc.plan.n_preds; i++)
-			if (desc.plan.preds[i].ival != got.plan.preds[i].ival || memcmp(&desc.plan.preds[i].fval, &got.plan.preds[i].fval, 8) != 0) { fprintf(stderr, "harness: qual constant %d changed\n", i); return 3; }
-		for (i = 0; i < desc.n_inner_preds; i++)
-			if (desc.inner_preds[i].ival != got.inner_preds[i].ival || memcmp(&desc.inner_preds[i].fval, &got.inner_preds[i].fval, 8) != 0) { fprintf(stderr, "harness: inner qual constant %d changed\n", i); return 3; }
+		if ((i = changed_pred(desc.plan.preds, got.plan.preds, desc.plan.n_preds)) >= 0) { fprintf(stderr, "harness: qual constant %d changed\n", i); return 3; }
+		for (r = 0; r < desc.n_joins; r++)
+			if ((i = changed_pred(desc.join[r].preds, got.join[r].preds, desc.join[r].n_preds)) >= 0) { fprintf(stderr, "harness: qual constant %d of join step %d changed\n", i, r + 1); return 3; }
 		if (desc.plan.est_groups != got.plan.est_groups) { fprintf(stderr, "harness: est_groups changed\n"); return 3; }
 		if (desc.plan.join_type != got.plan.join_type) { fprintf(stderr, "harness: join type changed\n"); return 3; }
 		printf("ship ok: %d nodes, %zu bytes\n%s\n", list_length(priv), strlen(wire), wire);

@@ -133,7 +133,8 @@ def test_config3_join_groupby(gx, data, strategy):
 
 
 @pytest.mark.parametrize("layout", ["key_order", "shuffled", "key_order_filtered", "clustered", "key_order_no_payload",
-                                    "key_order_wide_span", "shuffled_wide_span", "key_order_no_payload_wide_span"])
+                                    "key_order_wide_span", "shuffled_wide_span", "key_order_no_payload_wide_span",
+                                    "key_order_grouped_twice"])
 def test_big_build_paths_agree_with_oracle(gx, layout, monkeypatch):
     """Build sides large enough for the sub-table builders (>= 64 sub-tables): the
     partition-free path for a build side stored in key order, the two-level bucketing
@@ -165,6 +166,8 @@ def test_big_build_paths_agree_with_oracle(gx, layout, monkeypatch):
     if layout == "key_order_no_payload":              # the join only filters: half the orders are kept out of the build side
         payload, group_cols = [], [(0, g.L_SHIPDATE)]
         o = [c[::2].copy() for c in o]
+    elif layout == "key_order_grouped_twice":         # GROUP BY o_orderdate, o_orderdate: two group columns, one payload slot
+        group_cols = [(1, 0), (1, 0)]
     plan = O.make_plan(outer_key_col=g.L_ORDERKEY, group_cols=group_cols,
                        aggs=[(g.GX_AGG_COUNT_STAR, []), (g.GX_AGG_SUM_F8, [(g.GX_OP_COL, g.L_EXTENDEDPRICE, 0)])],
                        est_groups=2600)
@@ -174,7 +177,7 @@ def test_big_build_paths_agree_with_oracle(gx, layout, monkeypatch):
     ot = gx.table_from(g.SCHEMAS[g.T_ORDERS], o); lt = gx.table_from(g.SCHEMAS[g.T_LINEITEM], l)
     ht = gx.hash_build(ot, g.O_ORDERKEY, payload, unique=uniq, preds=inner_preds)
     info = ht.info()
-    if layout in ("key_order", "key_order_filtered", "key_order_no_payload"):
+    if layout in ("key_order", "key_order_filtered", "key_order_no_payload", "key_order_grouped_twice"):
         assert info["slot_mode"] == 2, info          # partition-free key-ordered build
     elif layout == "shuffled":
         assert info["slot_mode"] == 1, info          # interpolation slots, bucketed build

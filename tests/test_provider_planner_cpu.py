@@ -226,6 +226,17 @@ def test_limits_of_the_library_decline_at_plan_time_instead_of_failing_at_run_ti
     assert plan(wide, "scan 1", "group 1.3", "group 1.4", "group 1.1", "target agg sum_f8 v1.5", "dist none") is not None
 
 
+@pytest.mark.parametrize("att,typ", [(3, g.GX_DATE), (5, g.GX_FLOAT8)], ids=["date", "float8"])
+def test_an_inner_column_grouped_twice_takes_one_payload_slot(att, typ):
+    """GROUP BY o_orderdate, o_orderdate (or o_totalprice twice): both group columns read one payload slot, so a float8
+    column fits the 8-byte payload word; the group key is the column twice"""
+    r = plan(LINEITEM, ORDERS, "join 1.1 2.1 unique 1", f"group 2.{att}", f"group 2.{att}", "target agg count_star", "dist none")
+    assert r is not None
+    d = parse_desc(r["desc"])
+    assert [d["inner"]["cols"][c] for c in d["payload"]] == [(att - 1, typ)]
+    assert d["group_cols"] == [(1, 0), (1, 0)]
+
+
 @pytest.mark.parametrize("name,lines,accepted", [
     ("8 aggregates", [LINEITEM, "scan 1", "group 1.7", "target var 1.7"] + ["target agg sum_f8 v1.2"] * 8 + ["dist none"], True),
     ("9 aggregates", [LINEITEM, "scan 1", "group 1.7", "target var 1.7"] + ["target agg sum_f8 v1.2"] * 9 + ["dist none"], False),
