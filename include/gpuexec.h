@@ -70,9 +70,24 @@ enum {
     GX_AGG_SUM_I4     = 5, /* int4_sum -> int8   (utils/adt/numeric.c:6154)  */
     GX_AGG_MIN_F8     = 6, /* float8smaller                                  */
     GX_AGG_MAX_F8     = 7, /* float8larger                                   */
-    GX_AGG_SUM_I8     = 8  /* sum(int8): declined with GX_ERR_ARG, the reference
+    GX_AGG_SUM_I8     = 8, /* sum(int8): declined with GX_ERR_ARG, the reference
                               returns numeric (see DESIGN.md §3.2)            */
+    GX_AGG_COUNT_DISTINCT = 9 /* count(DISTINCT col): process_ordered_aggregate_single
+                              (executor/nodeAgg.c:888) with int8inc_any; see below */
 };
+/* GX_AGG_COUNT_DISTINCT counts the distinct non-NULL values of one column per group.  Its argument is a single
+ * GX_OP_COL over an outer column of type INT4, INT8, DATE or CHAR, compared as int4eq / int8eq / date_eq do
+ * (INT64_MIN is an ordinary value).  NULL inputs are skipped, so a group whose inputs are all NULL counts 0.
+ * gx_result_fetch returns the count as a bit-cast int64, as for GX_AGG_COUNT.
+ * It runs in two steps: the plan is aggregated with the argument appended as one more group column (one record per
+ * distinct (group, value) pair, the plan's other aggregates as partial states), then the pairs are folded back into
+ * the plan's own groups.  So est_groups of such a plan is read as the estimate of distinct (group, value) pairs, and
+ * the float8 overflow rule of gx_result_combine applies to the fold.
+ * GX_ERR_ARG, the context staying usable: a FLOAT8 argument (float8_cmp's "all NaNs are equal" is not the group
+ * keys' equality), an expression argument, DISTINCT aggregates over two different columns, and a group key that
+ * does not fit 16 bytes with the argument packed after it (first fit, GX_MAX_GROUP_COLS columns at most).  Such a
+ * result has no partial states: gx_result_fetch_states is GX_ERR_ARG, and so is gx_result_combine with more than
+ * one rank (distinct counts do not add across datanodes). */
 
 /* expression opcodes: tiny postfix VM over float8 (the provider pattern-matches
  * Var/Const/+,-,* trees from the reference's expression tree and declines

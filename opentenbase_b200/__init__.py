@@ -23,7 +23,7 @@ GX_OK, GX_ERR_CUDA, GX_ERR_ARG, GX_ERR_NOMEM, GX_ERR_NCCL, GX_ERR_STATE, GX_ERR_
 GX_INT4, GX_INT8, GX_FLOAT8, GX_DATE, GX_CHAR = 1, 2, 3, 4, 5
 GX_LT, GX_LE, GX_EQ, GX_GE, GX_GT, GX_NE = 1, 2, 3, 4, 5, 6
 (GX_AGG_COUNT_STAR, GX_AGG_COUNT, GX_AGG_SUM_F8, GX_AGG_AVG_F8, GX_AGG_SUM_I4,
- GX_AGG_MIN_F8, GX_AGG_MAX_F8, GX_AGG_SUM_I8) = 1, 2, 3, 4, 5, 6, 7, 8
+ GX_AGG_MIN_F8, GX_AGG_MAX_F8, GX_AGG_SUM_I8, GX_AGG_COUNT_DISTINCT) = 1, 2, 3, 4, 5, 6, 7, 8, 9
 GX_OP_COL, GX_OP_CONST, GX_OP_ADD, GX_OP_SUB, GX_OP_MUL = 1, 2, 3, 4, 5
 GX_JOIN_INNER, GX_JOIN_LEFT, GX_JOIN_SEMI, GX_JOIN_ANTI = 0, 1, 4, 5
 T_ORDERS, T_LINEITEM, T_CUSTOMER = 1, 2, 3

@@ -3022,6 +3022,8 @@ static void remember_layout(gx_result *r, const compiled_plan *cp)
 
 static int run_radix(gx_ctx *ctx, compiled_plan *cp, const gx_agg_plan *plan, long long nrows_in, gx_result **out);
 int gx_result_layout_words(gx_result *r, int *wkind, long long *winit);
+int gx_aggregate_records(gx_ctx *ctx, gx_agg_dev A, unsigned long long *d_recs, long long nrec,
+                         unsigned long long **d_out, long long *ngroups_out);
 
 static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, gx_result **out,
                         const chain_spec *ch = nullptr)
@@ -3493,14 +3495,149 @@ static int check_combine_overflow(gx_ctx *ctx, const gx_result *r, const std::ve
     return GX_OK;
 }
 
+static int hash_agg_checked(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, gx_result **out,
+                            const chain_spec *ch)
+{
+    int rc = hash_agg_run(ctx, outer, h, plan, out, ch);
+    if (rc != GX_OK) return rc;
+    rc = check_f8_overflow(ctx, outer, h, plan, *out, ch);
+    if (rc != GX_OK) { gx_result_free(*out); *out = nullptr; }
+    return rc;
+}
+
+// ---- count(DISTINCT col) ----------------------------------------------------------------------------------------
+// The reference sorts each group's inputs and counts the changes (process_ordered_aggregate_single, nodeAgg.c:888).
+// Here stage 1 is the plan itself with col appended as one more group column: every kernel the plan would take
+// aggregates it into one record per distinct (group, col) pair, the other aggregates as partial states.  The fold
+// masks col's bits and NULL bit off each pair's key, adds a word that is 1 where col was not NULL, and merges the
+// records by the plan's own key with the combine semantics of gx_result_combine (gx_aggregate_records).
+
+// the column every count(DISTINCT) of the plan reads (*col = -1: none), or GX_ERR_ARG for a shape that is not taken
+static int distinct_column(gx_ctx *ctx, const gx_table *outer, const gx_agg_plan *plan, int *col)
+{
+    *col = -1;
+    if (plan->n_aggs < 0 || plan->n_aggs > GX_MAX_AGGS) return GX_OK;          // compile_plan reports it
+    for (int a = 0; a < plan->n_aggs; a++) {
+        const gx_agg &g = plan->aggs[a];
+        if (g.fn != GX_AGG_COUNT_DISTINCT) continue;
+        GX_CHECK_ARG(ctx, g.arg.nops == 1 && g.arg.ops[0].op == GX_OP_COL, "agg %d: count(DISTINCT) takes a plain column", a);
+        const int c = g.arg.ops[0].col;
+        GX_CHECK_ARG(ctx, c >= 0 && c < outer->ncols, "agg %d: column out of range", a);
+        const int t = outer->types[c];
+        GX_CHECK_ARG(ctx, t == GX_INT4 || t == GX_INT8 || t == GX_DATE || t == GX_CHAR,
+                     "agg %d: count(DISTINCT) over column type %d (int4, int8, date or char)", a, t);
+        GX_CHECK_ARG(ctx, *col < 0 || *col == c, "agg %d: count(DISTINCT) over columns %d and %d in one plan", a, *col, c);
+        *col = c;
+    }
+    if (*col >= 0)
+        GX_CHECK_ARG(ctx, plan->n_group_cols >= 0 && plan->n_group_cols < GX_MAX_GROUP_COLS,
+                     "agg plan: count(DISTINCT) needs a group column slot for its argument (%d group columns)", plan->n_group_cols);
+    return GX_OK;
+}
+
+// stage-1 record -> fold record: the plan's own key, the stage-1 words, and the DISTINCT word
+struct gx_distinct_args {
+    const unsigned long long *in; unsigned long long *out; long long n;
+    int RW1, arg_bit;                        // arg_bit: the argument's NULL bit (its group column number)
+    unsigned long long keep0, keep1;         // bits of the plan's own group columns in k0 / k1
+};
+__global__ void __launch_bounds__(256) gx_k_distinct_fold(const gx_distinct_args D)
+{
+    const long long stride = (long long) gridDim.x * blockDim.x;
+    for (long long i = (long long) blockIdx.x * blockDim.x + threadIdx.x; i < D.n; i += stride) {
+        const unsigned long long *s = D.in + (size_t) i * D.RW1;
+        unsigned long long *d = D.out + (size_t) i * (D.RW1 + 1);
+        d[0] = s[0] & ((1ULL << D.arg_bit) - 1);
+        d[1] = s[1] & D.keep0; d[2] = s[2] & D.keep1;
+        for (int j = 3; j < D.RW1; j++) d[j] = s[j];
+        d[D.RW1] = ((s[0] >> D.arg_bit) & 1) ? 0ULL : 1ULL;
+    }
+}
+
+static int count_distinct_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, int col,
+                              gx_result **out, const chain_spec *ch)
+{
+    const int ng = plan->n_group_cols;
+    gx_agg_plan p1 = *plan;
+    p1.n_group_cols = ng + 1;
+    p1.group_cols[ng].side = 0; p1.group_cols[ng].col = col;
+    int map[GX_MAX_AGGS], n1 = 0;                      // plan aggregate -> stage-1 aggregate (-1: the DISTINCT word)
+    for (int a = 0; a < plan->n_aggs; a++) {
+        if (plan->aggs[a].fn == GX_AGG_COUNT_DISTINCT) { map[a] = -1; continue; }
+        map[a] = n1; p1.aggs[n1++] = plan->aggs[a];
+    }
+    p1.n_aggs = n1;
+    gx_result *s1 = nullptr;
+    int rc = hash_agg_checked(ctx, outer, h, &p1, &s1, ch);
+    if (rc != GX_OK) return rc;
+    const result_layout L1 = (*g_layouts)[s1];
+    const int RW1 = s1->rec_words, nw = s1->nwords + 1;
+    if (nw > GX_MAX_WORDS) { gx_result_free(s1); GX_SET_ERR(ctx, "agg plan: too many state words"); return GX_ERR_ARG; }
+
+    gx_result *r; gx_result_alloc(ctx, plan, s1->group_types, 0, &r);
+    r->nkw = 1; r->nwords = nw; r->rec_words = RW1 + 1; r->need_w0 = s1->need_w0;
+    gx_distinct_args D; memset(&D, 0, sizeof(D));
+    for (int c = 0; c < ng; c++) {
+        const unsigned long long bits = (L1.gbytes[c] < 8 ? (1ULL << (8 * L1.gbytes[c])) - 1 : ~0ULL) << L1.gshift[c];
+        if (L1.gword[c] == 0) D.keep0 |= bits; else { D.keep1 |= bits; r->nkw = 2; }
+    }
+    for (int a = 0; a < plan->n_aggs; a++) {
+        r->agg_word[a] = map[a] < 0 ? s1->nwords : s1->agg_word[map[a]];
+        r->agg_cnt_word[a] = map[a] < 0 ? 0 : s1->agg_cnt_word[map[a]];
+    }
+    result_layout L = L1;
+    L.wkind[s1->nwords] = WK_ADD_I64; L.winit[s1->nwords] = 0;
+    if (!g_layouts) g_layouts = new std::map<gx_result *, result_layout>();
+    (*g_layouts)[r] = L;
+
+    const long long nrec = s1->ngroups;
+    unsigned long long *d_fold = nullptr, *d_out = nullptr; long long ngroups = 0;
+    {
+        gx_launch_scope ls(ctx, "agg_distinct_fold");
+        if (nrec > 0) {
+            cudaError_t e = gx_tmp_alloc(ctx, (void **) &d_fold, (size_t) nrec * (RW1 + 1) * 8);
+            if (e != cudaSuccess) { rc = GX_ERR_NOMEM; GX_SET_ERR(ctx, "count(DISTINCT) fold: %s", cudaGetErrorString(e)); }
+        }
+        if (rc == GX_OK && nrec > 0) {
+            D.in = (const unsigned long long *) s1->d_recs; D.out = d_fold; D.n = nrec; D.RW1 = RW1; D.arg_bit = ng;
+            const long long nb = (nrec + 255) / 256, maxb = (long long) ctx->sm_count * 8;
+            gx_k_distinct_fold<<<(unsigned) (nb < maxb ? nb : maxb), 256, 0, ctx->stream>>>(D);
+            cudaError_t e = cudaGetLastError();
+            if (e != cudaSuccess) { rc = GX_ERR_CUDA; GX_SET_ERR(ctx, "count(DISTINCT) fold: %s", cudaGetErrorString(e)); }
+        }
+        gx_result_free(s1);
+        if (rc == GX_OK) {
+            gx_agg_dev A; memset(&A, 0, sizeof(A));
+            A.P.nwords = nw; A.P.nkw = 2;
+            for (int i = 0; i < GX_MAX_WORDS; i++) { A.wkind[i] = L.wkind[i]; A.winit[i] = L.winit[i]; }
+            A.counters = ctx->d_scratch + 8;
+            rc = gx_aggregate_records(ctx, A, d_fold, nrec, &d_out, &ngroups);
+        }
+        if (rc == GX_OK) rc = check_combine_overflow(ctx, r, { { d_fold, nrec } }, d_out, ngroups);
+    }
+    gx_tmp_free(ctx, d_fold);
+    if (rc == GX_OK && !d_out) {
+        cudaError_t e = gx_tmp_alloc(ctx, (void **) &d_out, 64);
+        if (e != cudaSuccess) { rc = GX_ERR_NOMEM; GX_SET_ERR(ctx, "count(DISTINCT) fold: %s", cudaGetErrorString(e)); }
+    }
+    if (rc != GX_OK) { gx_tmp_free(ctx, d_out); gx_result_free(r); return rc; }
+    r->d_recs = (long long *) d_out; r->ngroups = ngroups; r->cap = ngroups > 0 ? ngroups : 1;
+    *out = r;
+    return GX_OK;
+}
+
+static int hash_agg_entry(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, gx_result **out,
+                          const chain_spec *ch = nullptr)
+{
+    int col;
+    int rc = distinct_column(ctx, outer, plan, &col); if (rc) return rc;
+    return col < 0 ? hash_agg_checked(ctx, outer, h, plan, out, ch) : count_distinct_run(ctx, outer, h, plan, col, out, ch);
+}
+
 extern "C" int gx_hash_agg(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, gx_result **out)
 {
     if (!ctx || !outer || !plan || !out) return GX_ERR_ARG;
-    int rc = hash_agg_run(ctx, outer, h, plan, out);
-    if (rc != GX_OK) return rc;
-    rc = check_f8_overflow(ctx, outer, h, plan, *out);
-    if (rc != GX_OK) { gx_result_free(*out); *out = nullptr; }
-    return rc;
+    return hash_agg_entry(ctx, outer, h, plan, out);
 }
 
 // the width of a join key taken from a payload column, or 0 when the column cannot be one
@@ -3539,11 +3676,7 @@ extern "C" int gx_hash_agg_joins(gx_ctx *ctx, const gx_table *outer, int n_steps
     // steps 2.. are probed in their 16-byte form; step 1 in the format its build wrote
     for (int s = 1; s < n_steps; s++) { int rc = gx_hash_wide(ctx, const_cast<gx_hash *>(steps[s].h)); if (rc) return rc; }
     const chain_spec ch = { n_steps, steps };
-    int rc = hash_agg_run(ctx, outer, steps[0].h, &p, out, &ch);
-    if (rc != GX_OK) return rc;
-    rc = check_f8_overflow(ctx, outer, steps[0].h, &p, *out, &ch);
-    if (rc != GX_OK) { gx_result_free(*out); *out = nullptr; }
-    return rc;
+    return hash_agg_entry(ctx, outer, steps[0].h, &p, out, &ch);
 }
 
 // single-block exclusive scan (same as gx_table.cu's, kept local to this TU)
@@ -3760,6 +3893,11 @@ extern "C" void gx_result_free(gx_result *r)
 }
 
 // accessors for gx_comm.cu (combine across datanodes)
+bool gx_result_has_distinct(const gx_result *r)
+{
+    for (int a = 0; a < r->plan.n_aggs; a++) if (r->plan.aggs[a].fn == GX_AGG_COUNT_DISTINCT) return true;
+    return false;
+}
 int gx_result_layout_words(gx_result *r, int *wkind, long long *winit)
 {
     if (!g_layouts || !g_layouts->count(r)) return GX_ERR_STATE;
@@ -3813,6 +3951,9 @@ __global__ void gx_k_finalize(const gx_final_args F)
     }
 }
 
+// a count(DISTINCT) word holds the count itself once folded: it finalizes as count(col)
+static int final_fn(int fn) { return fn == GX_AGG_COUNT_DISTINCT ? GX_AGG_COUNT : fn; }
+
 static int fetch_on_device(gx_result *r, const result_layout &L, int64_t *key_out, double *agg_out, uint8_t *null_out)
 {
     gx_ctx *ctx = r->ctx;
@@ -3821,7 +3962,7 @@ static int fetch_on_device(gx_result *r, const result_layout &L, int64_t *key_ou
     gx_final_args F; memset(&F, 0, sizeof(F));
     F.recs = (const unsigned long long *) r->d_recs; F.ngroups = r->ngroups; F.RW = r->rec_words; F.ng = ng; F.na = na; F.need_w0 = r->need_w0;
     for (int c = 0; c < ng; c++) { F.gword[c] = L.gword[c]; F.gshift[c] = L.gshift[c]; F.gtype[c] = r->group_types[c]; }
-    for (int a = 0; a < na; a++) { F.fn[a] = r->plan.aggs[a].fn; F.word[a] = r->agg_word[a]; F.cw[a] = r->agg_cnt_word[a]; }
+    for (int a = 0; a < na; a++) { F.fn[a] = final_fn(r->plan.aggs[a].fn); F.word[a] = r->agg_word[a]; F.cw[a] = r->agg_cnt_word[a]; }
     char *d = nullptr;
     const size_t kb = n * (ng > 0 ? ng : 1) * 8, ab = n * (na > 0 ? na : 1) * 8, nb = (n * (ng + na) + 15) & ~(size_t) 15;
     GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d, kb + ab + nb));
@@ -3848,7 +3989,7 @@ extern "C" int gx_result_fetch(gx_result *r, int64_t max_groups, int64_t *key_ou
     if (ng == 0 && r->ngroups == 0) {
         GX_CHECK_ARG(ctx, max_groups >= 1, "result_fetch: buffer too small");
         for (int a = 0; a < na; a++) {
-            int fn = r->plan.aggs[a].fn;
+            int fn = final_fn(r->plan.aggs[a].fn);
             bool is_count = fn == GX_AGG_COUNT_STAR || fn == GX_AGG_COUNT;
             long long zero = 0; memcpy(&agg_out[a], &zero, 8);
             if (null_out) null_out[a] = is_count ? 0 : 1;
@@ -3880,7 +4021,7 @@ extern "C" int gx_result_fetch(gx_result *r, int64_t max_groups, int64_t *key_ou
             if (null_out) null_out[g * (ng + na) + c] = isnull;
         }
         for (int a = 0; a < na; a++) {
-            int fn = r->plan.aggs[a].fn, word = r->agg_word[a], cw = r->agg_cnt_word[a];
+            int fn = final_fn(r->plan.aggs[a].fn), word = r->agg_word[a], cw = r->agg_cnt_word[a];
             // cw == 0: the argument cannot be NULL, so a group that exists has input;
             // w0 (rows per group) is only maintained when count(*)/avg need it
             long long cnt = cw ? (long long) w[cw] : (r->need_w0 ? (long long) w[0] : 1);
@@ -3912,6 +4053,7 @@ extern "C" int gx_result_fetch_states(gx_result *r, int64_t max_groups, int64_t 
     if (!r || !key_out || !val_out || !cnt_out) return GX_ERR_ARG;
     gx_ctx *ctx = r->ctx;
     const int ng = r->plan.n_group_cols, na = r->plan.n_aggs, RW = r->rec_words;
+    GX_CHECK_ARG(ctx, !gx_result_has_distinct(r), "result_fetch_states: a count(DISTINCT) result has no partial state");
     if (ng == 0 && r->ngroups == 0) {                           // plain aggregate over zero rows: initial states
         GX_CHECK_ARG(ctx, max_groups >= 1, "result_fetch_states: buffer too small");
         for (int a = 0; a < na; a++) {

@@ -156,6 +156,8 @@ struct gx_result {
     int need_w0;                     // w0 (rows per group) is maintained
 };
 
+bool gx_result_has_distinct(const gx_result *r);      // some aggregate is GX_AGG_COUNT_DISTINCT: no partial states
+
 #define GX_SET_ERR(ctx, ...) do { if (ctx) snprintf((ctx)->err, sizeof((ctx)->err), __VA_ARGS__); \
                                   gx_set_global_err(__VA_ARGS__); } while (0)
 void gx_set_global_err(const char *fmt, ...);

@@ -72,6 +72,7 @@
 #include "utils/guc.h"
 #include "utils/memutils.h"
 #include "utils/rel.h"
+#include "utils/selfuncs.h"
 #include "utils/resowner.h"
 #include "utils/snapmgr.h"
 #include "utils/syscache.h"
@@ -877,12 +878,26 @@ static void
 gpuexec_explain(CustomScanState *node, List *ancestors, ExplainState *es)
 {
 	GpuExecState *st = (GpuExecState *) node;
+	int			i;
 
 	ExplainPropertyText("GPU Strategy", st->n_joins ? "hash build + fused probe/aggregate" : "scan + hash aggregate", es);
 	if (st->n_joins)
 		ExplainPropertyText("GPU Join Type", st->plan.join_type == GX_JOIN_SEMI ? "Semi" : st->plan.join_type == GX_JOIN_ANTI ? "Anti" : "Inner", es);
 	if (st->n_joins > 1)
 		ExplainPropertyInteger("GPU Joins", NULL, st->n_joins, es);
+	for (i = 0; i < st->plan.n_aggs; i++)
+		if (st->plan.aggs[i].fn == GX_AGG_COUNT_DISTINCT)
+		{
+			int			att = st->outer.attnums[st->plan.aggs[i].arg.ops[0].col];
+			char		name[NAMEDATALEN + 16];
+
+			if (st->outer_rel && st->outer_rel->rd_att && att < st->outer_rel->rd_att->natts)
+				snprintf(name, sizeof(name), "%s", NameStr(TupleDescAttr(st->outer_rel->rd_att, att)->attname));
+			else
+				snprintf(name, sizeof(name), "attribute %d", att + 1);
+			ExplainPropertyText("GPU Distinct Column", name, es);
+			break;
+		}
 	ExplainPropertyText("GPU Output", st->partial ? "partial states (Finalize above the redistribute)" : "final values (GROUP BY covers the distribution key)", es);
 	if (es->analyze && st->done_exec)
 	{
@@ -1363,8 +1378,11 @@ match_joins(PlannerInfo *root, HashPath *top, GpuExecState *out, double *est_byt
 
 static bool
 gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_rel, GpuExecState *out,
-				   List **agg_refs, double *est_rows, double *est_groups, double *est_bytes, double *est_pages)
+				   List **agg_refs, double *est_rows, double *est_groups, double *est_bytes, double *est_pages,
+				   double *est_pairs)
 {
+	Var		   *distinct_arg = NULL;	/* the column of the query's count(DISTINCT) aggregates, */
+	int			distinct_c = -1;		/* and its outer column number */
 	Query	   *parse = root->parse;
 	Path	   *in = input_rel->cheapest_total_path;
 	gx_agg_plan *plan = &out->plan;
@@ -1481,9 +1499,39 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 				return false;	/* functionally dependent column: not carried */
 			continue;
 		}
-		if (!IsA(a, Aggref) || a->aggdistinct || a->aggorder || a->aggfilter || a->aggdirectargs || plan->n_aggs >= GX_MAX_AGGS)
+		if (!IsA(a, Aggref) || a->aggorder || a->aggfilter || a->aggdirectargs || plan->n_aggs >= GX_MAX_AGGS)
 			return false;
 		g = &plan->aggs[plan->n_aggs];
+		if (a->aggdistinct)
+		{
+			/* count(DISTINCT col) over a plain int4 / int8 / date column of the outer relation (GX_AGG_COUNT_DISTINCT):
+			 * one sort clause, over the argument, and the same column in every DISTINCT aggregate of the query */
+			TargetEntry *arg;
+			SortGroupClause *sgc;
+			Var		   *v;
+			int			c;
+
+			if (a->aggfnoid != AGG_COUNT_ANY || list_length(a->args) != 1 || list_length(a->aggdistinct) != 1)
+				return false;
+			arg = (TargetEntry *) linitial(a->args);
+			sgc = (SortGroupClause *) linitial(a->aggdistinct);
+			v = (Var *) arg->expr;
+			if (sgc->tleSortGroupRef != arg->ressortgroupref || !IsA(v, Var) || v->varlevelsup != 0 || v->varno != out->outer.rti ||
+				(v->vartype != INT4OID && v->vartype != INT8OID && v->vartype != DATEOID))
+				return false;
+			c = rel_column(&out->outer, v->varno, v->varattno, v->vartype, v->vartypmod);
+			if (c < 0 || (distinct_arg != NULL && !equal(distinct_arg, v)))
+				return false;
+			distinct_arg = v;
+			distinct_c = c;
+			g->fn = GX_AGG_COUNT_DISTINCT;
+			g->arg.nops = 1;
+			g->arg.ops[0].op = GX_OP_COL;
+			g->arg.ops[0].col = c;
+			*agg_refs = lappend(*agg_refs, a);
+			plan->n_aggs++;
+			continue;
+		}
 		switch (a->aggfnoid)
 		{
 			case AGG_COUNT_STAR:
@@ -1530,6 +1578,42 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 	*est_rows = in->rows;
 	*est_groups = output_rel->rows > 0 ? output_rel->rows : 1;
 	plan->est_groups = (int64) *est_groups;
+	if (distinct_arg)
+	{
+		/* the library groups by the key plus the DISTINCT column first: that key must fit too (first fit, the column
+		 * packed last), and est_groups is read as the number of distinct (group, value) pairs */
+		List	   *exprs = NIL;
+		int			used[2] = {0, 0},
+					b;
+		double		pairs;
+
+		if (plan->n_group_cols >= GX_MAX_GROUP_COLS)
+			return false;
+		for (i = 0; i <= plan->n_group_cols; i++)
+		{
+			const gx_colref *gc = i < plan->n_group_cols ? &plan->group_cols[i] : NULL;
+			int32		t = gc == NULL ? out->outer.types[distinct_c]
+				: gc->side == 0 ? out->outer.types[gc->col]
+				: out->join[gc->side - 1].rel.types[out->join[gc->side - 1].payload_cols[gc->col]];
+			int			w;
+
+			b = staged_type_bytes(t);
+			w = used[0] + b <= 8 ? 0 : 1;
+			if (used[w] + b > 8)
+				return false;
+			used[w] += b;
+		}
+		foreach(lc, parse->groupClause)
+			exprs = lappend(exprs, get_sortgroupclause_tle((SortGroupClause *) lfirst(lc), parse->targetList)->expr);
+		exprs = lappend(exprs, distinct_arg);
+		pairs = estimate_num_groups(root, exprs, in->rows, NULL);
+		if (pairs > in->rows)
+			pairs = in->rows;
+		if (pairs < 1)
+			pairs = 1;
+		plan->est_groups = (int64) pairs;
+		*est_pairs = pairs;
+	}
 	/* HBM the plan needs: the referenced columns of every row, plus 16 B x 2 per build row */
 	{
 		double		bytes = 0;
@@ -1546,6 +1630,10 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 				bytes += j->tuples * staged_type_bytes(j->rel.types[k]);
 			bytes += j->tuples * 32;
 		}
+		/* count(DISTINCT): one record of (3 + state words) 8-byte words per pair, held about three times over while the
+		 * fold reads the stage-1 records and partitions its copy of them (csrc/gx_agg.cu, count_distinct_run) */
+		if (distinct_arg)
+			bytes += *est_pairs * 8.0 * (3 + 1 + 2 * plan->n_aggs) * 3;
 		*est_bytes = bytes * 1.25;
 	}
 	return true;
@@ -1561,7 +1649,8 @@ gpuexec_upper_paths_hook(PlannerInfo *root, UpperRelationKind stage, RelOptInfo 
 	double		rows,
 				groups,
 				bytes = 0,
-				pages = 0;
+				pages = 0,
+				pairs = 0;
 	ListCell   *lc;
 
 	if (prev_upper_paths_hook)
@@ -1569,7 +1658,7 @@ gpuexec_upper_paths_hook(PlannerInfo *root, UpperRelationKind stage, RelOptInfo 
 	if (!gpuexec_enabled || stage != UPPERREL_GROUP_AGG)
 		return;
 	memset(&desc, 0, sizeof(desc));
-	if (!gpuexec_match_plan(root, input_rel, output_rel, &desc, &agg_refs, &rows, &groups, &bytes, &pages))
+	if (!gpuexec_match_plan(root, input_rel, output_rel, &desc, &agg_refs, &rows, &groups, &bytes, &pages, &pairs))
 		return;					/* decline: the CPU paths stay as they are */
 	/* capacity (the analogue of ExecChooseHashTableSize deciding on batches, nodeHash.c:864): there is
 	 * no spill path on the device, so a plan that would not fit is left to the CPU executor */
@@ -1582,6 +1671,9 @@ gpuexec_upper_paths_hook(PlannerInfo *root, UpperRelationKind stage, RelOptInfo 
 		PathTarget *scan_target;
 
 		desc.partial = !pushdown;
+		/* a count(DISTINCT) result has no partial state, and distinct counts do not add across datanodes */
+		if (desc.partial && pairs > 0)
+			return;
 		/* the scan tuple: GROUP BY expressions, then the aggregates (partial Aggrefs in two-phase mode) */
 		scan_target = create_empty_pathtarget();
 		foreach(lc, parse->groupClause)

@@ -199,6 +199,10 @@ void DefineCustomRealVariable(const char *n, const char *s, const char *l, doubl
 double		seq_page_cost = 1.0, cpu_tuple_cost = 0.01;		/* costsize.c:100-104 */
 static double fake_datanodes = 1;
 double path_count_datanodes(Path *p) { return fake_datanodes; }
+/* selfuncs.c:3349 estimates from column statistics the harness does not have: the scenario's "pairs N" line stands in for
+ * them (count(DISTINCT) asks for the GROUP BY columns plus its argument), else every input row is its own group */
+static double fake_pairs = 0;
+double estimate_num_groups(PlannerInfo *root, List *groupExprs, double input_rows, List **pgset) { return fake_pairs > 0 ? fake_pairs : input_rows; }
 void DefineCustomIntVariable(const char *n, const char *s, const char *l, int *v, int b, int mn, int mx, GucContext c, int f, GucIntCheckHook a, GucIntAssignHook g, GucShowHook h) { }
 static const CustomScanMethods *registered_methods = NULL;
 void RegisterCustomScanMethods(const CustomScanMethods *m) { registered_methods = m; }
@@ -566,8 +570,13 @@ static int plan_main(const char *path)
 			for (i = 0; i < (int) lengthof(tab); i++) if (!strcmp(tab[i].n, w)) break;
 			if (i == (int) lengthof(tab)) { fprintf(stderr, "harness: aggregate %s\n", w); return 2; }
 			ag->aggfnoid = tab[i].fn; ag->aggtype = tab[i].ty; ag->aggtranstype = tab[i].tr; ag->aggsplit = AGGSPLIT_SIMPLE; ag->aggkind = 'n';
-			if (strstr(line + n, "distinct")) ag->aggdistinct = list_make1(makeNode(SortGroupClause));
-			else if (tab[i].fn == 2803) ag->aggstar = true;
+			if (strstr(line + n, "distinct"))
+			{
+				/* "target agg count v1.2 distinct": the argument, and one sort clause over it (parse_agg.c transformAggregateCall) */
+				*strstr(line + n, "distinct") = '\0';
+				ag->aggdistinct = list_make1(makeNode(SortGroupClause));
+			}
+			if (tab[i].fn == 2803) ag->aggstar = true;
 			else { Node *e = plan_expr(line + n); if (!e) { fprintf(stderr, "harness: bad expression\n"); return 2; } ag->args = list_make1(makeTargetEntry((Expr *) e, 1, NULL, false)); }
 			parse->targetList = lappend(parse->targetList, makeTargetEntry((Expr *) ag, list_length(parse->targetList) + 1, NULL, false));
 		}
@@ -587,6 +596,7 @@ static int plan_main(const char *path)
 		else if (!strncmp(line, "having", 6)) parse->havingQual = (Node *) plan_const(INT4OID, "1");
 		else if (!strncmp(line, "groupingsets", 12)) parse->groupingSets = list_make1(makeNode(GroupingSet));
 		else if (sscanf(line, "groups %lf", &t) == 1) output_rel->rows = t;
+		else if (sscanf(line, "pairs %lf", &t) == 1) fake_pairs = t;
 		else if (!strncmp(line, "protected", 9)) { g_enable_cls = true; fake_cls_policy = true; }
 		else { fprintf(stderr, "harness: scenario line not understood: %s", line); return 2; }
 	}
