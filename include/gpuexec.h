@@ -72,8 +72,12 @@ enum {
     GX_AGG_MAX_F8     = 7, /* float8larger                                   */
     GX_AGG_SUM_I8     = 8, /* sum(int8): declined with GX_ERR_ARG, the reference
                               returns numeric (see DESIGN.md §3.2)            */
-    GX_AGG_COUNT_DISTINCT = 9 /* count(DISTINCT col): process_ordered_aggregate_single
+    GX_AGG_COUNT_DISTINCT = 9, /* count(DISTINCT col): process_ordered_aggregate_single
                               (executor/nodeAgg.c:888) with int8inc_any; see below */
+    GX_AGG_VAR_POP_F8     = 10, /* float8_accum/float8_var_pop     (float.c:3010)  */
+    GX_AGG_VAR_SAMP_F8    = 11, /* float8_accum/float8_var_samp    (float.c:3032); variance() */
+    GX_AGG_STDDEV_POP_F8  = 12, /* float8_accum/float8_stddev_pop  (float.c:3054)  */
+    GX_AGG_STDDEV_SAMP_F8 = 13  /* float8_accum/float8_stddev_samp (float.c:3076); stddev() */
 };
 /* GX_AGG_COUNT_DISTINCT counts the distinct non-NULL values of one column per group.  Its argument is a single
  * GX_OP_COL over an outer column of type INT4, INT8, DATE or CHAR, compared as int4eq / int8eq / date_eq do
@@ -88,6 +92,15 @@ enum {
  * does not fit 16 bytes with the argument packed after it (first fit, GX_MAX_GROUP_COLS columns at most).  Such a
  * result has no partial states: gx_result_fetch_states is GX_ERR_ARG, and so is gx_result_combine with more than
  * one rank (distinct counts do not add across datanodes). */
+/* GX_AGG_VAR_POP_F8 .. GX_AGG_STDDEV_SAMP_F8 take the float8 expression argument of GX_AGG_SUM_F8 / GX_AGG_AVG_F8 and
+ * skip NULL inputs.  gx_result_fetch returns the finalized float8: NULL when N == 0 (pop) or N <= 1 (samp).  A group
+ * with an infinite or NaN input gives NaN (float8_accum makes its Sxx NaN); a finite input whose state overflows is
+ * GX_ERR_OVERFLOW.  The device keeps the sum of squared deviations as sums shifted by the group's first value, merged
+ * with re-centring (DESIGN.md §3.2), so Sxx matches the exact value within 2^-30 Sxx + 16 N^2 2^-52 D^2, D the largest
+ * deviation from the group mean; Sxx is never negative and a constant group gives exactly 0.  gx_result_fetch_states
+ * returns {N, Sx} as for GX_AGG_AVG_F8 (never NULL, {0, 0} over zero rows) and gx_result_fetch_sxx the Sxx that
+ * completes float8_combine's {N, Sx, Sxx}.  A plan whose state words exceed the library's limit is GX_ERR_ARG, and so
+ * is gx_result_combine with more than one rank (a two-phase plan combines the states in the reference's Finalize). */
 
 /* expression opcodes: tiny postfix VM over float8 (the provider pattern-matches
  * Var/Const/+,-,* trees from the reference's expression tree and declines
@@ -414,6 +427,9 @@ int  gx_result_fetch(gx_result *r, int64_t max_groups, int64_t *key_out,
  * int8 sum bit-cast; null_out = 1 while the transition value is NULL. */
 int  gx_result_fetch_states(gx_result *r, int64_t max_groups, int64_t *key_out,
                             double *val_out, int64_t *cnt_out, uint8_t *null_out);
+/* Sxx of the float8_accum state {N, Sx, Sxx} per group and aggregate, groups in the order of gx_result_fetch_states:
+ * sxx_out[g*n_aggs + a] is the group's Sxx for GX_AGG_VAR_* / GX_AGG_STDDEV_* and 0 for any other aggregate. */
+int  gx_result_fetch_sxx(gx_result *r, int64_t max_groups, double *sxx_out);
 void gx_result_free(gx_result *r);
 
 /* One-call form used by the provider and by bench.py's e2e leg: HOST column

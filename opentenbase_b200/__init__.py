@@ -24,6 +24,7 @@ GX_INT4, GX_INT8, GX_FLOAT8, GX_DATE, GX_CHAR = 1, 2, 3, 4, 5
 GX_LT, GX_LE, GX_EQ, GX_GE, GX_GT, GX_NE = 1, 2, 3, 4, 5, 6
 (GX_AGG_COUNT_STAR, GX_AGG_COUNT, GX_AGG_SUM_F8, GX_AGG_AVG_F8, GX_AGG_SUM_I4,
  GX_AGG_MIN_F8, GX_AGG_MAX_F8, GX_AGG_SUM_I8, GX_AGG_COUNT_DISTINCT) = 1, 2, 3, 4, 5, 6, 7, 8, 9
+(GX_AGG_VAR_POP_F8, GX_AGG_VAR_SAMP_F8, GX_AGG_STDDEV_POP_F8, GX_AGG_STDDEV_SAMP_F8) = 10, 11, 12, 13
 GX_OP_COL, GX_OP_CONST, GX_OP_ADD, GX_OP_SUB, GX_OP_MUL = 1, 2, 3, 4, 5
 GX_JOIN_INNER, GX_JOIN_LEFT, GX_JOIN_SEMI, GX_JOIN_ANTI = 0, 1, 4, 5
 T_ORDERS, T_LINEITEM, T_CUSTOMER = 1, 2, 3
@@ -178,6 +179,7 @@ def _declare(L):
         "gx_result_ngroups": (i64, [vp]),
         "gx_result_fetch": (C.c_int, [vp, i64, vp, vp, vp]),
         "gx_result_fetch_states": (C.c_int, [vp, i64, vp, vp, vp, vp]),
+        "gx_result_fetch_sxx": (C.c_int, [vp, i64, vp]),
         "gx_result_free": (None, [vp]),
         "gx_exec_host": (C.c_int, [vp, C.POINTER(GxHostTable), C.POINTER(GxHostTable), C.c_int, C.c_int,
                                    C.POINTER(GxPred), C.c_int, C.POINTER(i32), C.c_int, C.POINTER(GxAggPlan), pp]),
@@ -381,6 +383,14 @@ class Result:
         cnts = np.zeros((n, na), np.int64); nulls = np.zeros((n, ng + na), np.uint8)
         self.ctx._chk(lib().gx_result_fetch_states(self.h, n, keys.ctypes.data, vals.ctypes.data, cnts.ctypes.data, nulls.ctypes.data))
         return keys, vals, cnts, nulls
+
+    def fetch_sxx(self):
+        """Sxx of each variance aggregate's {N, Sx, Sxx} state, float64[n, na] (0 for other aggregates), groups in
+        the order of fetch_states"""
+        n, na = self.ngroups, self.plan.n_aggs
+        sxx = np.zeros((n, na), np.float64)
+        self.ctx._chk(lib().gx_result_fetch_sxx(self.h, n, sxx.ctypes.data))
+        return sxx
 
     def free(self):
         if self.h and self.ctx.h:          # handles die with their context (stream-ordered frees need its stream)

@@ -29,7 +29,11 @@
 
 int gx_fill_dpreds(gx_ctx *ctx, const gx_table *t, int n_preds, const gx_pred *preds, gx_dpred *out);
 
-enum { WK_ADD_I64 = 0, WK_ADD_F64 = 1, WK_MIN_F64 = 2, WK_MAX_F64 = 3 };
+enum { WK_ADD_I64 = 0, WK_ADD_F64 = 1, WK_MIN_F64 = 2, WK_MAX_F64 = 3, WK_VAR_C = 4, WK_VAR_S = 5 };
+// A variance state is three words {C, S1, S2}: S1 = sum(x - C) and S2 = sum((x - C)^2) around a shift C that the
+// state's first value sets.  They merge together (var_merge), so the C word's kind carries the word that counts the
+// state's inputs: wkind = WK_VAR_C | count word << 8 (0: w0); S1 and S2 are WK_VAR_S and never merged on their own.
+#define GX_VAR_UNSET_BITS 0x7FF4000000000001ULL      // C before the first value: a NaN no float8 arithmetic produces
 // initial value of every float8 sum (state words and register accumulators): -0.0 is the exact additive identity,
 // so a group whose inputs are all -0.0 sums to -0.0 as float8pl does when the first input becomes the state
 #define GX_NEG_ZERO_BITS 0x8000000000000000ULL
@@ -72,7 +76,7 @@ struct gx_agg_dev {
     int chain_n; int _pad2;
     gx_chain_step chain[GX_MAX_JOINS - 1];
 };
-// gx_k_agg takes gx_agg_dev by value (__grid_constant__): 2832 bytes with the chain steps, 3112 with gx_k_runagg's second
+// gx_k_agg takes gx_agg_dev by value (__grid_constant__): 2896 bytes with the chain steps, 3176 with gx_k_runagg's second
 // argument, inside the 4 KB of kernel parameters every architecture accepts
 static_assert(sizeof(gx_agg_dev) <= 4096, "gx_agg_dev outgrew the kernel parameter space");
 
@@ -107,6 +111,41 @@ __device__ __forceinline__ void merge_word(unsigned long long *addr, int kind, u
         case WK_ADD_F64: atomicAdd((double *) addr, __longlong_as_double((long long) v)); break;
         case WK_MIN_F64: atomic_min_f64(addr, __longlong_as_double((long long) v), true); break;
         default:         atomic_min_f64(addr, __longlong_as_double((long long) v), false); break;
+    }
+}
+// Merge a variance state {cs, s1, s2} of n inputs into the words at dst = {C, S1, S2} of another.  The target's C is
+// set once, from the unset value; then the source is re-centred on it: with d = cs - C,
+// S1 += s1 + n d and S2 += s2 + 2 d s1 + n d^2 (independent atomics: C no longer changes).  An input NaN that happens
+// to carry GX_VAR_UNSET_BITS leaves C unset, but its own d is NaN, so the state is NaN as it must be.
+__device__ __forceinline__ void var_merge(unsigned long long *dst, double cs, double s1, double s2, long long n)
+{
+    if (n == 0) return;
+    const unsigned long long old = atomicCAS(dst, GX_VAR_UNSET_BITS, (unsigned long long) __double_as_longlong(cs));
+    const double c = old == GX_VAR_UNSET_BITS ? cs : __longlong_as_double((long long) old);
+    const double d = __dsub_rn(cs, c), nd = __dmul_rn((double) n, d);
+    atomicAdd((double *) &dst[1], __dadd_rn(s1, nd));
+    atomicAdd((double *) &dst[2], __dadd_rn(__dadd_rn(s2, __dmul_rn(__dmul_rn(2.0, d), s1)), __dmul_rn(nd, d)));
+}
+// the same merge in registers: state a (na inputs) takes state b (nb inputs), keeping a's shift
+__device__ __forceinline__ void var_combine(double &ac, double &a1, double &a2, long long &na, double bc, double b1, double b2, long long nb)
+{
+    if (nb == 0) return;
+    if (na == 0) { ac = bc; a1 = b1; a2 = b2; na = nb; return; }
+    const double d = __dsub_rn(bc, ac), nd = __dmul_rn((double) nb, d);
+    a2 = __dadd_rn(a2, __dadd_rn(__dadd_rn(b2, __dmul_rn(__dmul_rn(2.0, d), b1)), __dmul_rn(nd, d)));
+    a1 = __dadd_rn(a1, __dadd_rn(b1, nd));
+    na += nb;
+}
+// merge the state words src[0, nwords) of one group into dst (w0 first in both)
+__device__ __forceinline__ void merge_words(unsigned long long *dst, const unsigned long long *src, const int *wkind, int nwords)
+{
+    for (int j = 0; j < nwords; j++) {
+        const int k = wkind[j];
+        if ((k & 0xFF) == WK_VAR_C) {
+            var_merge(&dst[j], __longlong_as_double((long long) src[j]), __longlong_as_double((long long) src[j + 1]),
+                      __longlong_as_double((long long) src[j + 2]), (long long) src[k >> 8]);
+            j += 2;
+        } else merge_word(&dst[j], k, src[j]);
     }
 }
 
@@ -224,6 +263,19 @@ struct Sink {
         else if (SINK == SINK_SMEM_LP) { double *p = (double *) at(word); *p = __dadd_rn(*p, v); }
         else atomicAdd((double *) at(word), v);
     }
+    // one value into the variance state at words {word, word + 1, word + 2} = {C, S1, S2}
+    __device__ __forceinline__ void var_f64(int word, double x)
+    {
+        unsigned long long *pc = at(word);
+        const unsigned long long xb = (unsigned long long) __double_as_longlong(x);
+        double c = x;
+        if (SINK == SINK_RECORD) *pc = xb;
+        else if (SINK == SINK_SMEM_LP) { if (*pc == GX_VAR_UNSET_BITS) *pc = xb; else c = __longlong_as_double((long long) *pc); }
+        else { const unsigned long long old = atomicCAS(pc, GX_VAR_UNSET_BITS, xb); if (old != GX_VAR_UNSET_BITS) c = __longlong_as_double((long long) old); }
+        const double d = __dsub_rn(x, c);
+        add_f64(word + 1, d);
+        add_f64(word + 2, __dmul_rn(d, d));
+    }
     __device__ __forceinline__ void minmax_f64(int word, double v, bool want_min)
     {
         if (SINK == SINK_RECORD) *at(word) = (unsigned long long) __double_as_longlong(v);
@@ -276,7 +328,7 @@ __device__ __forceinline__ void apply_aggs(const gx_dplan &P, bool need_w0, long
             bool isnull = false;
             double v = gx_eval_expr(g.expr, r, isnull);
             if (isnull) continue;                             // strict transition function
-            if (g.kind == GXU_ADD_F64) sink.add_f64(g.word, v);
+            if (g.kind == GXU_ADD_F64) { sink.add_f64(g.word, v); if (g.var_word) sink.var_f64(g.var_word, v); }
             else sink.minmax_f64(g.word, v, g.kind == GXU_MIN_F64);
             if (g.cnt_word) sink.inc(g.cnt_word);
         }
@@ -372,7 +424,7 @@ __device__ __forceinline__ void smem_dense_merge(const SmemTable &T, const gx_ag
         unsigned long long k0 = T.tagkey ? (t & 0x00FFFFFFFFFFFFFFULL) : T.k0[i];
         unsigned long long *rec = global_upsert(A, k0, (!T.tagkey && T.nkw > 1) ? T.k1[i] : 0ULL, nullmask);
         if (!rec) { atomicOr((unsigned long long *) &A.counters[1], 2ULL); continue; }
-        for (int j = 0; j < T.nwords; j++) merge_word(&rec[3 + j], A.wkind[j], T.w[(size_t) i * T.nwords + j]);
+        merge_words(&rec[3], &T.w[(size_t) i * T.nwords], A.wkind, T.nwords);
     }
 }
 
@@ -401,6 +453,24 @@ __device__ __forceinline__ unsigned long long lp_reduce_word(const SmemTable &T,
         }
     }
     return acc;                                   // valid in lane 0
+}
+// the same for the variance state at words {word, word + 1, word + 2} whose inputs word cw counts; lane 0 merges it into rec
+__device__ __forceinline__ void lp_var_merge(const SmemTable &T, int nwarps, int word, int cw, unsigned int gi, int lane, unsigned long long *rec)
+{
+    double c = 0.0, s1 = 0.0, s2 = 0.0; long long n = 0;
+    for (int wp = 0; wp < nwarps; wp++) {
+        const unsigned long long *v = &T.w[(((size_t) wp * T.nwords + word) * T.gmax + gi) * 32 + lane];
+        const size_t ws = (size_t) T.gmax * 32;
+        var_combine(c, s1, s2, n, __longlong_as_double((long long) v[0]), __longlong_as_double((long long) v[ws]),
+                    __longlong_as_double((long long) v[2 * ws]), (long long) T.w[(((size_t) wp * T.nwords + cw) * T.gmax + gi) * 32 + lane]);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const double bc = __shfl_down_sync(0xffffffffu, c, o), b1 = __shfl_down_sync(0xffffffffu, s1, o), b2 = __shfl_down_sync(0xffffffffu, s2, o);
+        const long long bn = __shfl_down_sync(0xffffffffu, n, o);
+        if (lane + o < 32) var_combine(c, s1, s2, n, bc, b1, b2, bn);
+    }
+    if (lane == 0 && rec) var_merge(&rec[3 + word], c, s1, s2, n);
 }
 
 // XF < 0: no join, or an INNER join walked row by row over the 16-byte table.  XF = GX_SLOTS_*: a SEMI / ANTI join
@@ -568,6 +638,11 @@ __global__ void __launch_bounds__(1024, 1) gx_k_agg(const __grid_constant__ gx_a
             unsigned long long *rec = nullptr;
             if (lane == 0) rec = global_upsert(A, k0, (!T.tagkey && T.nkw > 1) ? T.k1[i] : 0ULL, nullmask);
             for (int j = 0; j < T.nwords; j++) {
+                if ((A.wkind[j] & 0xFF) == WK_VAR_C) {
+                    lp_var_merge(T, nwarps, j, A.wkind[j] >> 8, gi, lane, rec);
+                    if (lane == 0 && !rec) atomicOr((unsigned long long *) &A.counters[1], 2ULL);
+                    j += 2; continue;
+                }
                 unsigned long long v = lp_reduce_word(T, nwarps, j, gi, A.wkind[j], lane);
                 if (lane == 0) { if (rec) merge_word(&rec[3 + j], A.wkind[j], v); else atomicOr((unsigned long long *) &A.counters[1], 2ULL); }
             }
@@ -2369,7 +2444,7 @@ __global__ void __launch_bounds__(512) gx_k_radix_agg(const gx_agg_dev A, const 
             const unsigned long long *rec = recs + i * RW;
             int s = smem_upsert<false>(T, rec[1], rec[2], (unsigned int) rec[0]);
             if (s < 0) { s_over = 1; continue; }
-            for (int j = 0; j < T.nwords; j++) merge_word(&T.w[(size_t) s * T.nwords + j], A.wkind[j], rec[3 + j]);
+            merge_words(&T.w[(size_t) s * T.nwords], &rec[3], A.wkind, T.nwords);
         }
         __syncthreads();
         if (s_over) { if (threadIdx.x == 0) overflowed[part] = 1; __syncthreads(); continue; }
@@ -2402,7 +2477,7 @@ __global__ void gx_k_merge_records(const gx_agg_dev A, const unsigned long long 
             const unsigned long long *rec = recs + i * RW;
             unsigned long long *g = global_upsert(A, rec[1], rec[2], (unsigned int) rec[0]);
             if (!g) { atomicOr((unsigned long long *) &A.counters[1], 2ULL); continue; }
-            for (int j = 0; j < A.P.nwords; j++) merge_word(&g[3 + j], A.wkind[j], rec[3 + j]);
+            merge_words(&g[3], &rec[3], A.wkind, A.P.nwords);
         }
         return;
     }
@@ -2414,7 +2489,7 @@ __global__ void gx_k_merge_records(const gx_agg_dev A, const unsigned long long 
             const unsigned long long *rec = recs + i * RW;
             unsigned long long *g = global_upsert(A, rec[1], rec[2], (unsigned int) rec[0]);
             if (!g) { atomicOr((unsigned long long *) &A.counters[1], 2ULL); continue; }
-            for (int j = 0; j < A.P.nwords; j++) merge_word(&g[3 + j], A.wkind[j], rec[3 + j]);
+            merge_words(&g[3], &rec[3], A.wkind, A.P.nwords);
         }
     }
 }
@@ -2440,7 +2515,7 @@ __global__ void gx_k_merge_gathered(const gx_agg_dev A, const unsigned long long
         if ((int) (h % (unsigned long long) nranks) != rank) continue;
         unsigned long long *g = global_upsert(A, rec[1], rec[2], (unsigned int) rec[0]);
         if (!g) { atomicOr((unsigned long long *) &A.counters[1], 2ULL); continue; }
-        for (int w = 0; w < A.P.nwords; w++) merge_word(&g[3 + w], A.wkind[w], rec[3 + w]);
+        merge_words(&g[3], &rec[3], A.wkind, A.P.nwords);
     }
 }
 __global__ void gx_k_pack_partial(const unsigned long long *recs, long long n, long long cap, int RW, unsigned long long *out)
@@ -2516,8 +2591,9 @@ struct compiled_plan {
     gx_agg_dev A;
     int32_t group_types[GX_MAX_GROUP_COLS];
     int gword[GX_MAX_GROUP_COLS], gshift[GX_MAX_GROUP_COLS], gbytes[GX_MAX_GROUP_COLS];
-    int agg_word[GX_MAX_AGGS], agg_cnt_word[GX_MAX_AGGS];
+    int agg_word[GX_MAX_AGGS], agg_cnt_word[GX_MAX_AGGS], agg_var_word[GX_MAX_AGGS];
     int need_w0;
+    bool has_var;                    // some aggregate keeps a variance state: the specialised kernels do not
 };
 
 // LEFT is not among them: its inner-side group columns would have to turn NULL on a miss in every sink
@@ -2611,7 +2687,16 @@ static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
         const gx_agg &src = plan->aggs[a];
         bool nullable = false;
         auto new_word = [&](int kind, long long init) { cp->A.wkind[nw] = kind; cp->A.winit[nw] = init; return nw++; };
-        if (nw + 2 > GX_MAX_WORDS) { GX_SET_ERR(ctx, "agg plan: too many state words"); return GX_ERR_ARG; }
+        const bool var = gx_is_var_fn(src.fn);
+        // {C, S1, S2} of a variance over the same value as an earlier sum / avg / variance, or all of its words
+        auto new_var = [&](gx_dagg &owner) {
+            if (!owner.var_word) {
+                owner.var_word = new_word(WK_VAR_C | (owner.cnt_word << 8), (long long) GX_VAR_UNSET_BITS);
+                new_word(WK_VAR_S, 0); new_word(WK_VAR_S, 0);
+            }
+            cp->agg_var_word[a] = owner.var_word; cp->has_var = true;
+        };
+        if (nw + (var ? 5 : 2) > GX_MAX_WORDS) { GX_SET_ERR(ctx, "agg plan: too many state words"); return GX_ERR_ARG; }
         switch (src.fn) {
             case GX_AGG_COUNT_STAR: g.kind = GXU_NONE; cp->agg_word[a] = 0; cp->need_w0 = 1; break;
             case GX_AGG_SUM_I8:
@@ -2633,15 +2718,17 @@ static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
                 }
                 break;
             }
-            case GX_AGG_SUM_F8: case GX_AGG_AVG_F8: case GX_AGG_MIN_F8: case GX_AGG_MAX_F8: {
+            case GX_AGG_SUM_F8: case GX_AGG_AVG_F8: case GX_AGG_MIN_F8: case GX_AGG_MAX_F8:
+            case GX_AGG_VAR_POP_F8: case GX_AGG_VAR_SAMP_F8: case GX_AGG_STDDEV_POP_F8: case GX_AGG_STDDEV_SAMP_F8: {
                 GX_CHECK_ARG(ctx, src.arg.nops >= 1 && src.arg.nops <= GX_MAX_EXPR_OPS, "agg %d: missing argument expression", a);
-                // sum(x) and avg(x) over the same argument keep ONE running sum (float8pl and float8_accum
-                // add the same values in the same order: float.c:970, :2823) — Q1 has two such pairs
-                if (src.fn == GX_AGG_SUM_F8 || src.fn == GX_AGG_AVG_F8) {
+                // sum(x), avg(x) and the variances of x keep ONE running sum and count (float8pl and float8_accum
+                // add the same values in the same order: float.c:970, :2823) — Q1 has two such pairs; the
+                // variances of x share one {C, S1, S2} too.  The first of them owns the words and updates them all.
+                if (src.fn == GX_AGG_SUM_F8 || src.fn == GX_AGG_AVG_F8 || var) {
                     int twin = -1;
                     for (int b = 0; b < a && twin < 0; b++) {
                         const gx_agg &o = plan->aggs[b];
-                        if ((o.fn != GX_AGG_SUM_F8 && o.fn != GX_AGG_AVG_F8) || o.arg.nops != src.arg.nops) continue;
+                        if ((o.fn != GX_AGG_SUM_F8 && o.fn != GX_AGG_AVG_F8 && !gx_is_var_fn(o.fn)) || o.arg.nops != src.arg.nops) continue;
                         bool same = true;
                         for (int k = 0; k < src.arg.nops && same; k++)
                             same = o.arg.ops[k].op == src.arg.ops[k].op && o.arg.ops[k].col == src.arg.ops[k].col &&
@@ -2650,7 +2737,8 @@ static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
                     }
                     if (twin >= 0) {
                         g.kind = GXU_NONE; cp->agg_word[a] = cp->agg_word[twin]; cp->agg_cnt_word[a] = cp->agg_cnt_word[twin];
-                        if (cp->agg_cnt_word[a] == 0 && src.fn == GX_AGG_AVG_F8) cp->need_w0 = 1;
+                        if (cp->agg_cnt_word[a] == 0 && (src.fn == GX_AGG_AVG_F8 || var)) cp->need_w0 = 1;
+                        if (var) new_var(P.aggs[twin]);
                         break;
                     }
                 }
@@ -2664,7 +2752,8 @@ static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
                 } else { g.kind = GXU_ADD_F64; g.word = new_word(WK_ADD_F64, (long long) GX_NEG_ZERO_BITS); }   // -0: x + -0 == x for every x, -0 included
                 cp->agg_word[a] = g.word;
                 g.cnt_word = nullable ? new_word(WK_ADD_I64, 0) : 0; cp->agg_cnt_word[a] = g.cnt_word;
-                if (!nullable && src.fn == GX_AGG_AVG_F8) cp->need_w0 = 1;    // N of float8_avg
+                if (!nullable && (src.fn == GX_AGG_AVG_F8 || var)) cp->need_w0 = 1;    // N of float8_avg / float8_accum
+                if (var) new_var(g);
                 break;
             }
             default: GX_SET_ERR(ctx, "agg %d: unknown aggregate function %d", a, src.fn); return GX_ERR_ARG;
@@ -2994,7 +3083,7 @@ static int table_to_result(gx_ctx *ctx, compiled_plan *cp, const gx_agg_plan *pl
     const int RW = 3 + cp->A.P.nwords;
     gx_result *r; gx_result_alloc(ctx, plan, cp->group_types, ngroups, &r);
     r->nkw = cp->A.P.nkw; r->nwords = cp->A.P.nwords; r->rec_words = RW; r->need_w0 = cp->need_w0;
-    for (int a = 0; a < plan->n_aggs; a++) { r->agg_word[a] = cp->agg_word[a]; r->agg_cnt_word[a] = cp->agg_cnt_word[a]; }
+    for (int a = 0; a < plan->n_aggs; a++) { r->agg_word[a] = cp->agg_word[a]; r->agg_cnt_word[a] = cp->agg_cnt_word[a]; r->agg_var_word[a] = cp->agg_var_word[a]; }
     cudaError_t e = gx_tmp_alloc(ctx, (void **) &r->d_recs, (size_t) r->cap * RW * 8);
     if (e != cudaSuccess) { gx_result_free(r); GX_SET_ERR(ctx, "result: %s", cudaGetErrorString(e)); return GX_ERR_NOMEM; }
     GX_CUDA(ctx, cudaMemsetAsync(ctx->d_scratch + 12, 0, sizeof(long long), ctx->stream));
@@ -3054,7 +3143,8 @@ static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
     // the specialised kernels below join one table and know one payload word; a SEMI / ANTI plan takes gx_k_agg's
     // existence probe, a join chain its chain probe (both read the first table in the format its build wrote)
     const bool exist = A.P.join_type != GX_JOIN_INNER || A.chain_n > 1;
-    bool fast_ok = !exist && plan->n_preds == 0 && plan->n_group_cols == 1 && tagkey && outer->nrows > 0;
+    // a variance state is only updated by gx_k_agg: every specialised kernel below is ruled out by cp.has_var
+    bool fast_ok = !exist && !cp.has_var && plan->n_preds == 0 && plan->n_group_cols == 1 && tagkey && outer->nrows > 0;
     if (fast_ok) {
         const gx_dgroupcol &gc = A.P.gcols[0];
         if (A.P.has_join) {
@@ -3087,7 +3177,7 @@ static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
     const bool runjoin_env = !(norun && norun[0] == '1');
 
     // the tile-at-a-time lane-private kernel: no join, count(*) and float8 sums over NOT-NULL float8 columns
-    bool lptile_ok = !A.P.has_join;
+    bool lptile_ok = !A.P.has_join && !cp.has_var;
     for (int a = 0; a < A.P.nagg && lptile_ok; a++) {
         const gx_dagg &ga = A.P.aggs[a];
         if (ga.kind == GXU_NONE) continue;
@@ -3126,7 +3216,7 @@ static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
         gx_runagg_args RA; memset(&RA, 0, sizeof(RA));
         { const char *pf = getenv("GX_RUNAGG_PF"); RA.pf = pf ? atoi(pf) : 1; }     // bit 0: rows two tiles ahead into L2, bit 1: the tile's join-table lines
         const char *e = getenv("GX_NO_RUNAGG");
-        bool ok = !(e && e[0] == '1') && !exist && plan->strategy == 0 && A.P.has_join && h->unique && A.P.key_type == GX_INT8 && A.P.okey.nulls == nullptr &&
+        bool ok = !(e && e[0] == '1') && !exist && !cp.has_var && plan->strategy == 0 && A.P.has_join && h->unique && A.P.key_type == GX_INT8 && A.P.okey.nulls == nullptr &&
                   outer->nrows > 0 && plan->n_group_cols >= 1;
         bool has_key = false;
         for (int c = 0; c < plan->n_group_cols && ok; c++) {
@@ -3217,7 +3307,7 @@ static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
                 gx_tmp_free(ctx, g_tab);
                 gx_result *r; gx_result_alloc(ctx, plan, cp.group_types, direct + c[0], &r);
                 r->nkw = A.P.nkw; r->nwords = nwords; r->rec_words = RW; r->need_w0 = 1;
-                for (int a = 0; a < plan->n_aggs; a++) { r->agg_word[a] = cp.agg_word[a]; r->agg_cnt_word[a] = cp.agg_cnt_word[a]; }
+                for (int a = 0; a < plan->n_aggs; a++) { r->agg_word[a] = cp.agg_word[a]; r->agg_cnt_word[a] = cp.agg_cnt_word[a]; r->agg_var_word[a] = cp.agg_var_word[a]; }
                 r->d_recs = (long long *) d_out; r->ngroups = direct + c[0]; r->cap = out_cap;
                 remember_layout(r, &cp);
                 *out = r;
@@ -3330,7 +3420,10 @@ static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
 // Not seen (DESIGN.md §7): an overflow whose infinity does not survive to the state (min(x*x) with other rows finite,
 // x*x - x*x ending as NaN), and any overflow in an argument with a non-finite constant (every row has an infinite
 // or NaN input there).
-struct gx_infscan_args { const unsigned long long *recs; long long n; int RW, nchk, need_w0, _pad; int word[GX_MAX_AGGS], cw[GX_MAX_AGGS]; int *flag; };
+// nf[i]: word i is a variance's S1 or S2, where an overflow can also end as NaN (the re-centring merge adds 2 d S1 and
+// n d^2 of opposite signs, Inf + -Inf): there every non-finite value is a candidate, not only an infinite one
+struct gx_infscan_args { const unsigned long long *recs; long long n; int RW, nchk, need_w0, _pad; int word[GX_MAX_WORDS], cw[GX_MAX_WORDS], nf[GX_MAX_WORDS]; int *flag; };
+__host__ __device__ __forceinline__ bool overflow_candidate(double x, bool nf) { return nf ? !isfinite(x) : isinf(x); }
 __global__ void gx_k_inf_scan(const gx_infscan_args S)
 {
     const long long stride = (long long) gridDim.x * blockDim.x;
@@ -3338,7 +3431,7 @@ __global__ void gx_k_inf_scan(const gx_infscan_args S)
         const unsigned long long *w = S.recs + (size_t) gI * S.RW + 3;
         for (int a = 0; a < S.nchk; a++) {
             const long long cnt = S.cw[a] ? (long long) w[S.cw[a]] : (S.need_w0 ? (long long) w[0] : 1);
-            if (cnt != 0 && isinf(__longlong_as_double((long long) w[S.word[a]]))) *S.flag = 1;
+            if (cnt != 0 && overflow_candidate(__longlong_as_double((long long) w[S.word[a]]), S.nf[a])) *S.flag = 1;
         }
     }
 }
@@ -3349,15 +3442,21 @@ struct gx_group_key {
 };
 struct gx_group_key_hash { size_t operator()(const gx_group_key &k) const { return (size_t) (k.k0 * 0x9E3779B97F4A7C15ULL ^ k.k1 * 0xC2B2AE3D27D4EB4FULL ^ k.m); } };
 
-// the float8 state words of r's aggregates that can overflow (chk[i] = aggregate number); sums_only: SUM/AVG
-static void f8_checked_words(const gx_result *r, bool sums_only, gx_infscan_args *S, int *chk)
+// the float8 state words of r's aggregates that can overflow, each once (chk[i] = aggregate number, the entries of
+// one aggregate adjacent); sums_only: SUM/AVG and the variances' Sx, S1, S2
+static void f8_checked_words(const gx_result *r, bool sums_only, gx_infscan_args *S, int *chk /* GX_MAX_WORDS */)
 {
     memset(S, 0, sizeof(*S));
+    auto add = [&](int a, int word, int nf) {
+        for (int i = 0; i < S->nchk; i++) if (S->word[i] == word) return;
+        chk[S->nchk] = a; S->word[S->nchk] = word; S->cw[S->nchk] = r->agg_cnt_word[a]; S->nf[S->nchk] = nf; S->nchk++;
+    };
     for (int a = 0; a < r->plan.n_aggs; a++) {
         const int fn = r->plan.aggs[a].fn;
-        const bool sum = fn == GX_AGG_SUM_F8 || fn == GX_AGG_AVG_F8;
+        const bool sum = fn == GX_AGG_SUM_F8 || fn == GX_AGG_AVG_F8 || gx_is_var_fn(fn);
         if (!sum && (sums_only || (fn != GX_AGG_MIN_F8 && fn != GX_AGG_MAX_F8))) continue;
-        chk[S->nchk] = a; S->word[S->nchk] = r->agg_word[a]; S->cw[S->nchk] = r->agg_cnt_word[a]; S->nchk++;
+        add(a, r->agg_word[a], 0);
+        if (gx_is_var_fn(fn)) { add(a, r->agg_var_word[a] + 1, 1); add(a, r->agg_var_word[a] + 2, 1); }
     }
     S->RW = r->rec_words; S->need_w0 = r->need_w0;
 }
@@ -3387,7 +3486,7 @@ static long long rec_count(const gx_infscan_args &S, const unsigned long long *w
 static int check_f8_overflow(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, gx_result *r,
                              const chain_spec *ch = nullptr)
 {
-    gx_infscan_args S; int chk[GX_MAX_AGGS];
+    gx_infscan_args S; int chk[GX_MAX_WORDS];
     f8_checked_words(r, false, &S, chk);
     // an argument with a non-finite constant has an infinite (or NaN) input in every row: never an overflow
     int keep = 0;
@@ -3395,19 +3494,22 @@ static int check_f8_overflow(gx_ctx *ctx, const gx_table *outer, const gx_hash *
         const gx_expr &src = plan->aggs[chk[i]].arg;
         bool finite = true;
         for (int j = 0; j < src.nops; j++) if (src.ops[j].op == GX_OP_CONST && !std::isfinite(src.ops[j].k)) finite = false;
-        if (finite) { chk[keep] = chk[i]; S.word[keep] = S.word[i]; S.cw[keep] = S.cw[i]; keep++; }
+        if (finite) { chk[keep] = chk[i]; S.word[keep] = S.word[i]; S.cw[keep] = S.cw[i]; S.nf[keep] = S.nf[i]; keep++; }
     }
     S.nchk = keep;
     bool any;
     int rc = any_inf_word(ctx, S, (const unsigned long long *) r->d_recs, r->ngroups, &any);
     if (rc != GX_OK || !any) return rc;
 
-    // the verification aggregate: one sum(0 * c1 * c2 * ...) per checked argument
+    // the verification aggregate: one sum(0 * c1 * c2 * ...) per checked aggregate (vi[i]: that of word i)
     gx_agg_plan vp = *plan;
-    vp.n_aggs = S.nchk;
+    int vi[GX_MAX_WORDS];
+    vp.n_aggs = 0;
     for (int i = 0; i < S.nchk; i++) {
+        vi[i] = (i > 0 && chk[i] == chk[i - 1]) ? vi[i - 1] : vp.n_aggs++;
+        if (i > 0 && chk[i] == chk[i - 1]) continue;
         const gx_expr &src = plan->aggs[chk[i]].arg;
-        gx_agg &va = vp.aggs[i]; memset(&va, 0, sizeof(va));
+        gx_agg &va = vp.aggs[vi[i]]; memset(&va, 0, sizeof(va));
         va.fn = GX_AGG_SUM_F8;
         gx_expr &e = va.arg;
         e.ops[e.nops].op = GX_OP_CONST; e.ops[e.nops].k = 0.0; e.nops++;
@@ -3439,10 +3541,10 @@ static int check_f8_overflow(gx_ctx *ctx, const gx_table *outer, const gx_hash *
         const unsigned long long *rec = hr.data() + (size_t) gI * r->rec_words, *w = rec + 3;
         for (int i = 0; i < S.nchk && rc == GX_OK; i++) {
             double x; memcpy(&x, &w[S.word[i]], 8);
-            if (rec_count(S, w, i) == 0 || !std::isinf(x)) continue;
+            if (rec_count(S, w, i) == 0 || !overflow_candidate(x, S.nf[i])) continue;
             auto it = at.find({ rec[0] & mmask, rec[1], rec[2] });
             if (it == at.end()) { GX_SET_ERR(ctx, "hash_agg: overflow check lost a group"); rc = GX_ERR_STATE; break; }
-            double nonfinite; memcpy(&nonfinite, &hv[(size_t) it->second * v->rec_words + 3 + v->agg_word[i]], 8);
+            double nonfinite; memcpy(&nonfinite, &hv[(size_t) it->second * v->rec_words + 3 + v->agg_word[vi[i]]], 8);
             if (!std::isnan(nonfinite)) { GX_SET_ERR(ctx, "value out of range: overflow"); rc = GX_ERR_OVERFLOW; }
         }
     }
@@ -3452,12 +3554,13 @@ static int check_f8_overflow(gx_ctx *ctx, const gx_table *outer, const gx_hash *
 
 // The same rule for the Finalize step across datanodes (float8pl / float8_combine, float.c:2725): every datanode's
 // gx_hash_agg already rejected its own finite overflows, so an infinite partial sum comes from an infinite input.
-// A merged SUM/AVG word that is infinite while none of the partial records merged into it was is an overflow of
+// A merged SUM/AVG word that is infinite (a variance's S1 / S2: not finite) while none of the partial records merged
+// into it was is an overflow of
 // the combine itself.  spans: the partial records (device), merged: the merged groups (device).
 static int check_combine_overflow(gx_ctx *ctx, const gx_result *r, const std::vector<std::pair<const unsigned long long *, long long>> &spans,
                                   const unsigned long long *merged, long long nmerged)
 {
-    gx_infscan_args S; int chk[GX_MAX_AGGS];
+    gx_infscan_args S; int chk[GX_MAX_WORDS];
     f8_checked_words(r, true, &S, chk);
     bool any;
     int rc = any_inf_word(ctx, S, merged, nmerged, &any);
@@ -3480,14 +3583,14 @@ static int check_combine_overflow(gx_ctx *ctx, const gx_result *r, const std::ve
     for (long long k = 0; k < nin; k++) {
         const unsigned long long *rec = hin.data() + (size_t) k * RW, *w = rec + 3;
         unsigned int bits = 0;
-        for (int i = 0; i < S.nchk; i++) { double x; memcpy(&x, &w[S.word[i]], 8); if (std::isinf(x)) bits |= 1u << i; }
+        for (int i = 0; i < S.nchk; i++) { double x; memcpy(&x, &w[S.word[i]], 8); if (overflow_candidate(x, S.nf[i])) bits |= 1u << i; }
         if (bits) inf_in[{ rec[0] & mmask, rec[1], rec[2] }] |= bits;
     }
     for (long long gI = 0; gI < nmerged; gI++) {
         const unsigned long long *rec = hm.data() + (size_t) gI * RW, *w = rec + 3;
         for (int i = 0; i < S.nchk; i++) {
             double x; memcpy(&x, &w[S.word[i]], 8);
-            if (rec_count(S, w, i) == 0 || !std::isinf(x)) continue;
+            if (rec_count(S, w, i) == 0 || !overflow_candidate(x, S.nf[i])) continue;
             auto it = inf_in.find({ rec[0] & mmask, rec[1], rec[2] });
             if (it == inf_in.end() || !((it->second >> i) & 1u)) { GX_SET_ERR(ctx, "value out of range: overflow"); return GX_ERR_OVERFLOW; }
         }
@@ -3584,6 +3687,7 @@ static int count_distinct_run(gx_ctx *ctx, const gx_table *outer, const gx_hash 
     for (int a = 0; a < plan->n_aggs; a++) {
         r->agg_word[a] = map[a] < 0 ? s1->nwords : s1->agg_word[map[a]];
         r->agg_cnt_word[a] = map[a] < 0 ? 0 : s1->agg_cnt_word[map[a]];
+        r->agg_var_word[a] = map[a] < 0 ? 0 : s1->agg_var_word[map[a]];
     }
     result_layout L = L1;
     L.wkind[s1->nwords] = WK_ADD_I64; L.winit[s1->nwords] = 0;
@@ -3867,7 +3971,7 @@ static int run_radix(gx_ctx *ctx, compiled_plan *cp, const gx_agg_plan *plan, lo
     if (rc) return rc;
     gx_result *r; gx_result_alloc(ctx, plan, cp->group_types, ngroups, &r);
     r->nkw = A.P.nkw; r->nwords = nwords; r->rec_words = RW; r->need_w0 = cp->need_w0;
-    for (int a = 0; a < plan->n_aggs; a++) { r->agg_word[a] = cp->agg_word[a]; r->agg_cnt_word[a] = cp->agg_cnt_word[a]; }
+    for (int a = 0; a < plan->n_aggs; a++) { r->agg_word[a] = cp->agg_word[a]; r->agg_cnt_word[a] = cp->agg_cnt_word[a]; r->agg_var_word[a] = cp->agg_var_word[a]; }
     r->d_recs = (long long *) d_groups; r->ngroups = ngroups; r->cap = ngroups;
     if (!d_groups) { GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &r->d_recs, 64)); }
     *out = r;
@@ -3898,6 +4002,11 @@ bool gx_result_has_distinct(const gx_result *r)
     for (int a = 0; a < r->plan.n_aggs; a++) if (r->plan.aggs[a].fn == GX_AGG_COUNT_DISTINCT) return true;
     return false;
 }
+bool gx_result_has_variance(const gx_result *r)
+{
+    for (int a = 0; a < r->plan.n_aggs; a++) if (gx_is_var_fn(r->plan.aggs[a].fn)) return true;
+    return false;
+}
 int gx_result_layout_words(gx_result *r, int *wkind, long long *winit)
 {
     if (!g_layouts || !g_layouts->count(r)) return GX_ERR_STATE;
@@ -3906,13 +4015,31 @@ int gx_result_layout_words(gx_result *r, int *wkind, long long *winit)
     return GX_OK;
 }
 
+// Sxx of a variance state {C, S1, S2} of n > 0 inputs: S2 - S1^2 / n, never negative (float8_accum's Sxx is not);
+// NaN stays NaN (a non-finite input)
+__host__ __device__ __forceinline__ double var_sxx(double s1, double s2, long long n)
+{
+    const double v = s2 - s1 * (s1 / (double) n);            // S1^2 / N <= S2 is finite even where S1^2 is not
+    return (v < 0.0 || v == 0.0) ? 0.0 : v;
+}
+// float8_var_pop / _var_samp / _stddev_pop / _stddev_samp (float.c:3010-3096); *isnull for N == 0 (pop) or N <= 1 (samp)
+__host__ __device__ __forceinline__ double var_final(int fn, const unsigned long long *w, int vw, long long n, bool *isnull)
+{
+    const bool pop = fn == GX_AGG_VAR_POP_F8 || fn == GX_AGG_STDDEV_POP_F8;
+    *isnull = pop ? n == 0 : n <= 1;
+    if (*isnull) return 0.0;
+    double s1, s2; memcpy(&s1, &w[vw + 1], 8); memcpy(&s2, &w[vw + 2], 8);
+    const double v = var_sxx(s1, s2, n) / (pop ? (double) n : (double) n - 1.0);
+    return fn == GX_AGG_STDDEV_POP_F8 || fn == GX_AGG_STDDEV_SAMP_F8 ? sqrt(v) : v;
+}
+
 // finalize_aggregates (nodeAgg.c:1363).  float8_avg = Sx / N, NULL when N == 0 (float.c:2991-3008).
 // Small results are finalized on the host from the raw records; large ones (Q3: millions of
 // groups) on the device, straight into the caller's column layout, so the host only copies.
 struct gx_final_args {
     const unsigned long long *recs; long long ngroups; int RW, ng, na, need_w0;
     int gword[GX_MAX_GROUP_COLS], gshift[GX_MAX_GROUP_COLS], gtype[GX_MAX_GROUP_COLS];
-    int fn[GX_MAX_AGGS], word[GX_MAX_AGGS], cw[GX_MAX_AGGS];
+    int fn[GX_MAX_AGGS], word[GX_MAX_AGGS], cw[GX_MAX_AGGS], vw[GX_MAX_AGGS];
     long long *key_out; double *agg_out; unsigned char *null_out;
 };
 __global__ void gx_k_finalize(const gx_final_args F)
@@ -3942,6 +4069,8 @@ __global__ void gx_k_finalize(const gx_final_args F)
                 case GX_AGG_COUNT: ires = (long long) w[word]; is_int = true; break;
                 case GX_AGG_SUM_I4: case GX_AGG_SUM_I8: ires = (long long) w[word]; is_int = true; isnull = cnt == 0; break;
                 case GX_AGG_AVG_F8: { const double sx = __longlong_as_double((long long) w[word]) + 0.0; if (cnt == 0) isnull = true; else res = sx / (double) cnt; break; }
+                case GX_AGG_VAR_POP_F8: case GX_AGG_VAR_SAMP_F8: case GX_AGG_STDDEV_POP_F8: case GX_AGG_STDDEV_SAMP_F8:
+                    res = var_final(fn, w, F.vw[a], cnt, &isnull); break;
                 default: res = __longlong_as_double((long long) w[word]); isnull = cnt == 0; break;
             }
             if (isnull) { res = 0.0; ires = 0; }
@@ -3962,7 +4091,7 @@ static int fetch_on_device(gx_result *r, const result_layout &L, int64_t *key_ou
     gx_final_args F; memset(&F, 0, sizeof(F));
     F.recs = (const unsigned long long *) r->d_recs; F.ngroups = r->ngroups; F.RW = r->rec_words; F.ng = ng; F.na = na; F.need_w0 = r->need_w0;
     for (int c = 0; c < ng; c++) { F.gword[c] = L.gword[c]; F.gshift[c] = L.gshift[c]; F.gtype[c] = r->group_types[c]; }
-    for (int a = 0; a < na; a++) { F.fn[a] = final_fn(r->plan.aggs[a].fn); F.word[a] = r->agg_word[a]; F.cw[a] = r->agg_cnt_word[a]; }
+    for (int a = 0; a < na; a++) { F.fn[a] = final_fn(r->plan.aggs[a].fn); F.word[a] = r->agg_word[a]; F.cw[a] = r->agg_cnt_word[a]; F.vw[a] = r->agg_var_word[a]; }
     char *d = nullptr;
     const size_t kb = n * (ng > 0 ? ng : 1) * 8, ab = n * (na > 0 ? na : 1) * 8, nb = (n * (ng + na) + 15) & ~(size_t) 15;
     GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d, kb + ab + nb));
@@ -4031,6 +4160,9 @@ extern "C" int gx_result_fetch(gx_result *r, int64_t max_groups, int64_t *key_ou
                 case GX_AGG_COUNT: ires = (long long) w[word]; is_int = true; break;
                 case GX_AGG_SUM_I4: case GX_AGG_SUM_I8: ires = (long long) w[word]; is_int = true; isnull = cnt == 0; break;
                 case GX_AGG_AVG_F8: { double sx; memcpy(&sx, &w[word], 8); sx += 0.0; if (cnt == 0) isnull = 1; else res = sx / (double) cnt; break; }
+                case GX_AGG_VAR_POP_F8: case GX_AGG_VAR_SAMP_F8: case GX_AGG_STDDEV_POP_F8: case GX_AGG_STDDEV_SAMP_F8: {
+                    bool vn; res = var_final(fn, w, r->agg_var_word[a], cnt, &vn); isnull = vn; break;
+                }
                 default: { memcpy(&res, &w[word], 8); isnull = cnt == 0; break; }
             }
             if (isnull) { res = 0.0; ires = 0; }
@@ -4059,7 +4191,7 @@ extern "C" int gx_result_fetch_states(gx_result *r, int64_t max_groups, int64_t 
         for (int a = 0; a < na; a++) {
             const int fn = r->plan.aggs[a].fn;
             val_out[a] = 0.0; cnt_out[a] = 0;
-            if (null_out) null_out[a] = (fn == GX_AGG_COUNT_STAR || fn == GX_AGG_COUNT || fn == GX_AGG_AVG_F8) ? 0 : 1;
+            if (null_out) null_out[a] = (fn == GX_AGG_COUNT_STAR || fn == GX_AGG_COUNT || fn == GX_AGG_AVG_F8 || gx_is_var_fn(fn)) ? 0 : 1;
         }
         return GX_OK;
     }
@@ -4095,7 +4227,8 @@ extern "C" int gx_result_fetch_states(gx_result *r, int64_t max_groups, int64_t 
                 case GX_AGG_COUNT_STAR: n = rows; break;
                 case GX_AGG_COUNT: n = (long long) w[word]; break;
                 case GX_AGG_SUM_I4: case GX_AGG_SUM_I8: memcpy(&v, &w[word], 8); isnull = cnt == 0; break;
-                case GX_AGG_AVG_F8: memcpy(&v, &w[word], 8); v += 0.0; break;    // {N, Sx}: never NULL; Sx starts at +0 ('{0,0,0}')
+                case GX_AGG_AVG_F8: case GX_AGG_VAR_POP_F8: case GX_AGG_VAR_SAMP_F8: case GX_AGG_STDDEV_POP_F8: case GX_AGG_STDDEV_SAMP_F8:
+                    memcpy(&v, &w[word], 8); v += 0.0; break;    // {N, Sx}: never NULL; Sx starts at +0 ('{0,0,0}')
                 default: memcpy(&v, &w[word], 8); isnull = cnt == 0; break;      // sum / min / max: strict, NULL until the first input
             }
             val_out[gI * na + a] = isnull ? 0.0 : v; cnt_out[gI * na + a] = n;
@@ -4103,5 +4236,39 @@ extern "C" int gx_result_fetch_states(gx_result *r, int64_t max_groups, int64_t 
         }
     }
     free(h);
+    return GX_OK;
+}
+
+// Sxx completing the {N, Sx} of gx_result_fetch_states for a variance aggregate, in the same group order
+extern "C" int gx_result_fetch_sxx(gx_result *r, int64_t max_groups, double *sxx_out)
+{
+    if (!r || !sxx_out) return GX_ERR_ARG;
+    gx_ctx *ctx = r->ctx;
+    const int na = r->plan.n_aggs, RW = r->rec_words;
+    GX_CHECK_ARG(ctx, !gx_result_has_distinct(r), "result_fetch_sxx: a count(DISTINCT) result has no partial state");
+    if (r->plan.n_group_cols == 0 && r->ngroups == 0) {              // plain aggregate over zero rows: '{0,0,0}'
+        GX_CHECK_ARG(ctx, max_groups >= 1, "result_fetch_sxx: buffer too small");
+        for (int a = 0; a < na; a++) sxx_out[a] = 0.0;
+        return GX_OK;
+    }
+    GX_CHECK_ARG(ctx, max_groups >= r->ngroups, "result_fetch_sxx: buffer holds %lld groups, result has %lld", (long long) max_groups, (long long) r->ngroups);
+    if (r->ngroups == 0) return GX_OK;
+    std::vector<unsigned long long> h((size_t) r->ngroups * RW);
+    cudaError_t e = cudaMemcpyAsync(h.data(), r->d_recs, h.size() * 8, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) { GX_SET_ERR(ctx, "result_fetch_sxx: %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
+    for (int64_t gI = 0; gI < r->ngroups; gI++) {
+        const unsigned long long *w = h.data() + (size_t) gI * RW + 3;
+        for (int a = 0; a < na; a++) {
+            double sxx = 0.0;
+            if (gx_is_var_fn(r->plan.aggs[a].fn)) {
+                const int cw = r->agg_cnt_word[a], vw = r->agg_var_word[a];
+                const long long n = cw ? (long long) w[cw] : (long long) w[0];
+                double s1, s2; memcpy(&s1, &w[vw + 1], 8); memcpy(&s2, &w[vw + 2], 8);
+                if (n > 0) sxx = var_sxx(s1, s2, n);
+            }
+            sxx_out[gI * na + a] = sxx;
+        }
+    }
     return GX_OK;
 }

@@ -877,6 +877,7 @@ extern "C" int gx_result_combine(gx_ctx *ctx, gx_result *r)
     if (!ctx || !r) return GX_ERR_ARG;
     const int N = ctx->nranks;
     GX_CHECK_ARG(ctx, N == 1 || !gx_result_has_distinct(r), "combine: count(DISTINCT) counts do not add across %d ranks", N);
+    GX_CHECK_ARG(ctx, N == 1 || !gx_result_has_variance(r), "combine: variance states are not combined across %d ranks", N);
     if (N == 1 || !ctx->comm || r->finalized_across) return GX_OK;
     const int RW = r->rec_words;
     long long nrec = r->ngroups;

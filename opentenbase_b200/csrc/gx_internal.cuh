@@ -149,6 +149,7 @@ struct gx_result {
     // per-agg state layout
     int agg_word[GX_MAX_AGGS];       // first word of the aggregate's state
     int agg_cnt_word[GX_MAX_AGGS];   // word holding its non-NULL input count (may be 0 = row count)
+    int agg_var_word[GX_MAX_AGGS];   // variance aggregates: the shift C, followed by S1 and S2 (0 = none)
     long long *d_recs;               // ngroups * rec_words (dense, partial states)
     unsigned int *d_nullmask;        // ngroups (group-key null bits)
     int64_t ngroups, cap;
@@ -157,6 +158,8 @@ struct gx_result {
 };
 
 bool gx_result_has_distinct(const gx_result *r);      // some aggregate is GX_AGG_COUNT_DISTINCT: no partial states
+bool gx_result_has_variance(const gx_result *r);      // some aggregate is GX_AGG_VAR_* / GX_AGG_STDDEV_*
+static inline bool gx_is_var_fn(int fn) { return fn >= GX_AGG_VAR_POP_F8 && fn <= GX_AGG_STDDEV_SAMP_F8; }
 
 #define GX_SET_ERR(ctx, ...) do { if (ctx) snprintf((ctx)->err, sizeof((ctx)->err), __VA_ARGS__); \
                                   gx_set_global_err(__VA_ARGS__); } while (0)
@@ -218,6 +221,8 @@ struct gx_dagg {
     int word;          // state word receiving the value
     int cnt_word;      // word receiving +1 per non-NULL input (0 = none: w0 row count serves)
     int is_int;        // value is an integer column (SUM_I4/I8, COUNT(col))
+    int var_word;      // GXU_ADD_F64 only: first of the words {C, S1, S2} of a variance over the same value (0 = none)
+    int _pad;
     gx_dexpr expr;     // float8 argument (kind F64) ...
     gx_dcol icol;      // ... or integer argument column
 };

@@ -151,6 +151,7 @@ typedef struct GpuExecState
 	int64	   *keys;
 	double	   *aggs;
 	int64	   *cnts;			/* partial mode: N of every transition state */
+	double	   *sxx;			/* partial mode: Sxx of every variance state */
 	uint8	   *nulls;
 	double		load_ms,
 				exec_ms;
@@ -655,6 +656,9 @@ gpuexec_begin(CustomScanState *node, EState *estate, int eflags)
 	live_handles = h;
 }
 
+static bool is_variance_fn(int fn);
+static bool plan_has_variance(const gx_agg_plan *plan);
+
 static void
 gpuexec_run(GpuExecState *st, EState *estate)
 {
@@ -712,6 +716,11 @@ gpuexec_run(GpuExecState *st, EState *estate)
 	{
 		st->cnts = (int64 *) palloc(sizeof(int64) * Max(n * na, 1));
 		GX_CHECK(gx_result_fetch_states(st->result, n, st->keys, st->aggs, st->cnts, st->nulls));
+		if (plan_has_variance(&st->plan))
+		{
+			st->sxx = (double *) palloc(sizeof(double) * Max(n * na, 1));
+			GX_CHECK(gx_result_fetch_sxx(st->result, n, st->sxx));
+		}
 	}
 	else
 		GX_CHECK(gx_result_fetch(st->result, n, st->keys, st->aggs, st->nulls));
@@ -731,7 +740,8 @@ gpuexec_run(GpuExecState *st, EState *estate)
  * plan's targetlist is projected over it (ExecAssignScanProjectionInfoWithVarno,
  * nodeCustom.c:100-101) below.  In partial mode an aggregate column carries the transition
  * value the reference's combine function expects (pg_aggregate.h:178-252): int8 for
- * count/sum(int4), float8 for sum/min/max(float8), float8[3] {N, Sx, Sxx} for avg(float8). */
+ * count/sum(int4), float8 for sum/min/max(float8), float8[3] {N, Sx, Sxx} for avg(float8) and the
+ * variances and standard deviations of float8. */
 static TupleTableSlot *
 gpuexec_exec(CustomScanState *node)
 {
@@ -804,16 +814,16 @@ gpuexec_exec(CustomScanState *node)
 			double		d = st->aggs[g * na + a];
 			int			fn = st->plan.aggs[a].fn;
 
-			if (st->partial && fn == GX_AGG_AVG_F8)
+			if (st->partial && (fn == GX_AGG_AVG_F8 || is_variance_fn(fn)))
 			{
-				/* float8_accum's transition value {N, Sx, Sxx}; Sxx is not carried (only
+				/* float8_accum's transition value {N, Sx, Sxx}; avg's Sxx is not carried (only
 				 * var/stddev read it; float8_combine, float.c:2725, keeps it finite) */
 				MemoryContext old = MemoryContextSwitchTo(econtext->ecxt_per_tuple_memory);
 				Datum		elems[3];
 
 				elems[0] = Float8GetDatum((double) st->cnts[g * na + a]);
 				elems[1] = Float8GetDatum(d);
-				elems[2] = Float8GetDatum(0.0);
+				elems[2] = Float8GetDatum(fn == GX_AGG_AVG_F8 ? 0.0 : st->sxx[g * na + a]);
 				slot->tts_values[i] = PointerGetDatum(construct_array(elems, 3, FLOAT8OID, sizeof(float8), FLOAT8PASSBYVAL, 'd'));
 				MemoryContextSwitchTo(old);
 			}
@@ -966,6 +976,12 @@ gpuexec_plan_path(PlannerInfo *root, RelOptInfo *rel, CustomPath *best_path,
 #define AGG_MAX_F8     2120
 #define AGG_MIN_F8     2136
 #define AGG_SUM_I4     2108
+#define AGG_VAR_POP_F8     2722
+#define AGG_VAR_SAMP_F8    2645
+#define AGG_VARIANCE_F8    2152
+#define AGG_STDDEV_POP_F8  2728
+#define AGG_STDDEV_SAMP_F8 2716
+#define AGG_STDDEV_F8      2158
 
 /* column number of (rti, attno) in the descriptor, appended on first use */
 static int
@@ -989,6 +1005,23 @@ rel_column(GpuRelInfo *r, Index rti, AttrNumber attno, Oid typid, int32 typmod)
 }
 
 /* float8 expression -> postfix program over outer columns */
+static bool
+is_variance_fn(int fn)
+{
+	return fn == GX_AGG_VAR_POP_F8 || fn == GX_AGG_VAR_SAMP_F8 || fn == GX_AGG_STDDEV_POP_F8 || fn == GX_AGG_STDDEV_SAMP_F8;
+}
+
+static bool
+plan_has_variance(const gx_agg_plan *plan)
+{
+	int			a;
+
+	for (a = 0; a < plan->n_aggs; a++)
+		if (is_variance_fn(plan->aggs[a].fn))
+			return true;
+	return false;
+}
+
 static bool
 match_f8_expr(Node *n, GpuRelInfo *outer, gx_expr *e)
 {
@@ -1225,6 +1258,88 @@ column_is_not_null(PlannerInfo *root, Index rti, AttrNumber attno)
 		ReleaseSysCache(tp);
 	}
 	return res;
+}
+
+/*
+ * The library's state words per group (csrc/gx_agg.cu, compile_plan), restated so that a variance plan the library
+ * would refuse with "too many state words" is declined here, at plan time.  Word 0 counts the group's rows; a count
+ * of a nullable column takes one word, a sum(int4) two when its column is nullable; sum, avg, min and max of float8
+ * take a value word and, over a nullable argument, a count word; sum, avg and the variances of one argument share
+ * these, and the variances of one argument share three more {C, S1, S2}.  Before each aggregate the library wants
+ * room for two words, or five for a variance; count(DISTINCT) is no aggregate of its first stage, and its fold adds
+ * one word at the end.
+ */
+#define GPUEXEC_MAX_STATE_WORDS 18		/* GX_MAX_WORDS, csrc/gx_internal.cuh */
+
+static bool
+same_f8_expr(const gx_expr *x, const gx_expr *y)
+{
+	int			k;
+
+	if (x->nops != y->nops)
+		return false;
+	for (k = 0; k < x->nops; k++)
+		if (x->ops[k].op != y->ops[k].op || x->ops[k].col != y->ops[k].col || memcmp(&x->ops[k].k, &y->ops[k].k, sizeof(double)) != 0)
+			return false;
+	return true;
+}
+
+static bool
+state_words_fit(PlannerInfo *root, const GpuRelInfo *outer, const gx_agg_plan *plan)
+{
+	bool		var_words[GX_MAX_AGGS] = {false};
+	bool		distinct = false;
+	int			nw = 1,
+				a,
+				b,
+				k;
+
+	for (a = 0; a < plan->n_aggs; a++)
+	{
+		const gx_agg *g = &plan->aggs[a];
+		bool		var = is_variance_fn(g->fn),
+					nullable = false;
+		int			twin = -1;
+
+		if (g->fn != GX_AGG_COUNT_DISTINCT && nw + (var ? 5 : 2) > GPUEXEC_MAX_STATE_WORDS)
+			return false;
+		for (k = 0; k < g->arg.nops; k++)
+			if (g->arg.ops[k].op == GX_OP_COL && !column_is_not_null(root, outer->rti, outer->attnums[g->arg.ops[k].col] + 1))
+				nullable = true;
+		switch (g->fn)
+		{
+			case GX_AGG_COUNT_STAR:
+				break;
+			case GX_AGG_COUNT_DISTINCT:
+				distinct = true;
+				break;
+			case GX_AGG_COUNT:
+				nw += nullable ? 1 : 0;
+				break;
+			case GX_AGG_SUM_I4:
+			case GX_AGG_MIN_F8:
+			case GX_AGG_MAX_F8:
+				nw += nullable ? 2 : 1;
+				break;
+			default:			/* sum, avg and the variances of float8 */
+				for (b = 0; b < a && twin < 0; b++)
+					if ((plan->aggs[b].fn == GX_AGG_SUM_F8 || plan->aggs[b].fn == GX_AGG_AVG_F8 || is_variance_fn(plan->aggs[b].fn)) &&
+						same_f8_expr(&plan->aggs[b].arg, &g->arg))
+						twin = b;
+				if (twin < 0)
+				{
+					twin = a;
+					nw += nullable ? 2 : 1;
+				}
+				if (var && !var_words[twin])
+				{
+					var_words[twin] = true;
+					nw += 3;
+				}
+				break;
+		}
+	}
+	return nw + (distinct ? 1 : 0) <= GPUEXEC_MAX_STATE_WORDS;
 }
 
 /* payload slot of column c of a join's build side, appended on first use: a probe key of a later step and a group column
@@ -1555,6 +1670,20 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 			case AGG_COUNT_ANY:
 				g->fn = GX_AGG_COUNT;
 				break;
+			case AGG_VAR_POP_F8:
+				g->fn = GX_AGG_VAR_POP_F8;
+				break;
+			case AGG_VAR_SAMP_F8:
+			case AGG_VARIANCE_F8:
+				g->fn = GX_AGG_VAR_SAMP_F8;
+				break;
+			case AGG_STDDEV_POP_F8:
+				g->fn = GX_AGG_STDDEV_POP_F8;
+				break;
+			case AGG_STDDEV_SAMP_F8:
+			case AGG_STDDEV_F8:
+				g->fn = GX_AGG_STDDEV_SAMP_F8;
+				break;
 			default:
 				return false;
 		}
@@ -1574,6 +1703,8 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 		plan->n_aggs++;
 	}
 	if (plan->n_aggs == 0 && plan->n_group_cols == 0)
+		return false;
+	if (plan_has_variance(plan) && !state_words_fit(root, &out->outer, plan))
 		return false;
 	*est_rows = in->rows;
 	*est_groups = output_rel->rows > 0 ? output_rel->rows : 1;

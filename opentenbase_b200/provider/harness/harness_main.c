@@ -564,7 +564,10 @@ static int plan_main(const char *path)
 			static const struct { const char *n; Oid fn, ty, tr; } tab[] = {
 				{"count_star", 2803, INT8OID, INT8OID}, {"count", 2147, INT8OID, INT8OID}, {"sum_f8", 2111, FLOAT8OID, FLOAT8OID}, {"avg_f8", 2105, FLOAT8OID, FLOAT8ARRAYOID},
 				{"min_f8", 2136, FLOAT8OID, FLOAT8OID}, {"max_f8", 2120, FLOAT8OID, FLOAT8OID}, {"sum_i4", 2108, INT8OID, INT8OID}, {"sum_numeric", 2114, NUMERICOID, INTERNALOID},
-				{"stddev_f8", 2158, FLOAT8OID, FLOAT8ARRAYOID},
+				{"stddev_f8", 2158, FLOAT8OID, FLOAT8ARRAYOID}, {"stddev_samp_f8", 2716, FLOAT8OID, FLOAT8ARRAYOID},
+				{"stddev_pop_f8", 2728, FLOAT8OID, FLOAT8ARRAYOID}, {"variance_f8", 2152, FLOAT8OID, FLOAT8ARRAYOID},
+				{"var_samp_f8", 2645, FLOAT8OID, FLOAT8ARRAYOID}, {"var_pop_f8", 2722, FLOAT8OID, FLOAT8ARRAYOID},
+				{"stddev_f4", 2157, FLOAT8OID, FLOAT8ARRAYOID}, {"stddev_i8", 2154, NUMERICOID, INTERNALOID},
 			};
 
 			for (i = 0; i < (int) lengthof(tab); i++) if (!strcmp(tab[i].n, w)) break;
