@@ -411,7 +411,10 @@ int  gx_hash_agg_joins(gx_ctx *ctx, const gx_table *outer, int n_steps, const gx
 
 /* Combine partial states across datanodes: redistribute groups on the group
  * key, then Finalize HashAggregate (xc_groupby.out:193-205; combine fns
- * int8pl / float8pl / float8_combine).  No-op when no communicator. */
+ * int8pl / float8pl / float8_combine).  No-op when no communicator.
+ * Afterwards every group is returned by exactly one rank, so the union of the
+ * ranks' rows is the answer.  A plain aggregate (no group columns) has its one
+ * row on rank 0; gx_result_ngroups is 0 on every other rank. */
 int  gx_result_combine(gx_ctx *ctx, gx_result *r);
 int64_t gx_result_ngroups(const gx_result *r);
 /* Fetch finalized rows (output order unspecified, as in the reference:
@@ -481,6 +484,12 @@ int  gx_partition_by_node(gx_ctx *ctx, const gx_table *in, int key_col,
  * 4 hashint8new (CRC32C), 5 murmurhash32(uint32 of low half) */
 int  gx_debug_hash(gx_ctx *ctx, int which, const int64_t *host_in, int64_t n,
                    uint32_t *host_out);
+/* gx_result_combine without a communicator, for tests on one GPU: parts[0..nparts-1] are the partial results of
+ * nparts datanodes (same plan).  parts[rank] is combined in place exactly as gx_result_combine combines it on rank
+ * `rank` of nparts ranks whose ranks hold those parts; the other parts are only read.  nparts 1..GX_MAX_NODES.
+ * GX_ERR_ARG, the context staying usable: the plans or record layouts of the parts differ, a part was combined
+ * already, or rank is out of range. */
+int  gx_debug_combine(gx_ctx *ctx, int nparts, gx_result *const *parts, int rank);
 
 #ifdef __cplusplus
 }

@@ -192,6 +192,7 @@ def _declare(L):
         "gx_redistribute": (C.c_int, [vp, vp, C.c_int, pp]),
         "gx_partition_by_node": (C.c_int, [vp, vp, C.c_int, pp, vp]),
         "gx_debug_hash": (C.c_int, [vp, C.c_int, vp, i64, vp]),
+        "gx_debug_combine": (C.c_int, [vp, C.c_int, pp, C.c_int]),
     }
     for name, (res, args) in sig.items():
         f = getattr(L, name)
@@ -635,6 +636,13 @@ class Context:
         out = np.empty(len(v), np.uint32)
         self._chk(lib().gx_debug_hash(self.h, which, v.ctypes.data, len(v), out.ctypes.data))
         return out
+
+    def debug_combine(self, parts, rank) -> Result:
+        """gx_debug_combine: combine parts[rank] in place as rank `rank` of len(parts) datanodes would, the other
+        parts standing for the other datanodes' partial results; returns parts[rank]"""
+        arr = (C.c_void_p * max(len(parts), 1))(*[p.h for p in parts])
+        self._chk(lib().gx_debug_combine(self.h, len(parts), arr, rank))
+        return parts[rank]
 
 
 def _exec_host(self, outer_types, outer_ptrs, outer_nrows, plan, inner_types=None, inner_ptrs=None, inner_nrows=0,

@@ -3306,7 +3306,7 @@ static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
                 }
                 gx_tmp_free(ctx, g_tab);
                 gx_result *r; gx_result_alloc(ctx, plan, cp.group_types, direct + c[0], &r);
-                r->nkw = A.P.nkw; r->nwords = nwords; r->rec_words = RW; r->need_w0 = 1;
+                r->nkw = A.P.nkw; r->nwords = nwords; r->rec_words = RW; r->need_w0 = cp.need_w0;
                 for (int a = 0; a < plan->n_aggs; a++) { r->agg_word[a] = cp.agg_word[a]; r->agg_cnt_word[a] = cp.agg_cnt_word[a]; r->agg_var_word[a] = cp.agg_var_word[a]; }
                 r->d_recs = (long long *) d_out; r->ngroups = direct + c[0]; r->cap = out_cap;
                 remember_layout(r, &cp);
@@ -3897,7 +3897,7 @@ int gx_pack_partial(gx_ctx *ctx, gx_result *r, long long cap, unsigned long long
     return GX_OK;
 }
 // ... and merge the all-gathered segments; *anybig = some rank did not fit (caller takes the general path)
-int gx_combine_gathered(gx_ctx *ctx, gx_result *r, const unsigned long long *d_gather, int nseg, long long cap,
+int gx_combine_gathered(gx_ctx *ctx, gx_result *r, const unsigned long long *d_gather, int nseg, long long cap, int rank, int nranks,
                         unsigned long long **d_out, long long *ngroups_out, int *anybig)
 {
     gx_agg_dev A; memset(&A, 0, sizeof(A));
@@ -3917,7 +3917,7 @@ int gx_combine_gathered(gx_ctx *ctx, gx_result *r, const unsigned long long *d_g
         gx_launch_scope ls(ctx, "combine_merge", 2);
         long long total = (long long) nseg * cap;
         unsigned grid = (unsigned) ((total + 255) / 256); if (grid > (unsigned) ctx->sm_count * 8) grid = (unsigned) ctx->sm_count * 8;
-        gx_k_merge_gathered<<<grid, 256, 0, ctx->stream>>>(A, d_gather, nseg, cap, ctx->rank, ctx->nranks);
+        gx_k_merge_gathered<<<grid, 256, 0, ctx->stream>>>(A, d_gather, nseg, cap, rank, nranks);
         gx_k_compact_groups<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(g_tab, g_cap, r->nwords, d_groups, ctx->d_scratch + 12);
     }
     GX_CUDA(ctx, cudaGetLastError());
@@ -3982,8 +3982,8 @@ static int run_radix(gx_ctx *ctx, compiled_plan *cp, const gx_agg_plan *plan, lo
 extern "C" int64_t gx_result_ngroups(const gx_result *r)
 {
     if (!r) return -1;
-    // a plain aggregate over zero rows still returns one row (agg_retrieve_direct)
-    if (r->plan.n_group_cols == 0 && r->ngroups == 0) return 1;
+    // a plain aggregate over zero rows still returns one row (agg_retrieve_direct), on one rank only
+    if (gx_result_plain_empty(r)) return 1;
     return r->ngroups;
 }
 
@@ -4115,7 +4115,7 @@ extern "C" int gx_result_fetch(gx_result *r, int64_t max_groups, int64_t *key_ou
     if (!r) return GX_ERR_ARG;
     gx_ctx *ctx = r->ctx;
     const int ng = r->plan.n_group_cols, na = r->plan.n_aggs, RW = r->rec_words;
-    if (ng == 0 && r->ngroups == 0) {
+    if (gx_result_plain_empty(r)) {
         GX_CHECK_ARG(ctx, max_groups >= 1, "result_fetch: buffer too small");
         for (int a = 0; a < na; a++) {
             int fn = final_fn(r->plan.aggs[a].fn);
@@ -4186,7 +4186,7 @@ extern "C" int gx_result_fetch_states(gx_result *r, int64_t max_groups, int64_t 
     gx_ctx *ctx = r->ctx;
     const int ng = r->plan.n_group_cols, na = r->plan.n_aggs, RW = r->rec_words;
     GX_CHECK_ARG(ctx, !gx_result_has_distinct(r), "result_fetch_states: a count(DISTINCT) result has no partial state");
-    if (ng == 0 && r->ngroups == 0) {                           // plain aggregate over zero rows: initial states
+    if (gx_result_plain_empty(r)) {                             // plain aggregate over zero rows: initial states
         GX_CHECK_ARG(ctx, max_groups >= 1, "result_fetch_states: buffer too small");
         for (int a = 0; a < na; a++) {
             const int fn = r->plan.aggs[a].fn;
@@ -4246,7 +4246,7 @@ extern "C" int gx_result_fetch_sxx(gx_result *r, int64_t max_groups, double *sxx
     gx_ctx *ctx = r->ctx;
     const int na = r->plan.n_aggs, RW = r->rec_words;
     GX_CHECK_ARG(ctx, !gx_result_has_distinct(r), "result_fetch_sxx: a count(DISTINCT) result has no partial state");
-    if (r->plan.n_group_cols == 0 && r->ngroups == 0) {              // plain aggregate over zero rows: '{0,0,0}'
+    if (gx_result_plain_empty(r)) {                                  // plain aggregate over zero rows: '{0,0,0}'
         GX_CHECK_ARG(ctx, max_groups >= 1, "result_fetch_sxx: buffer too small");
         for (int a = 0; a < na; a++) sxx_out[a] = 0.0;
         return GX_OK;

@@ -836,7 +836,7 @@ int gx_result_layout_words(gx_result *r, int *wkind, long long *winit);
 int gx_combine_records(gx_ctx *ctx, gx_result *r, unsigned long long *d_recs, long long nrec,
                        unsigned long long **d_out, long long *ngroups_out);   // gx_agg.cu
 int gx_pack_partial(gx_ctx *ctx, gx_result *r, long long cap, unsigned long long *d_seg);
-int gx_combine_gathered(gx_ctx *ctx, gx_result *r, const unsigned long long *d_gather, int nseg, long long cap,
+int gx_combine_gathered(gx_ctx *ctx, gx_result *r, const unsigned long long *d_gather, int nseg, long long cap, int rank, int nranks,
                         unsigned long long **d_out, long long *ngroups_out, int *anybig);
 
 __global__ void gx_k_rec_dest_hist(const unsigned long long *recs, long long nrec, int RW, int nranks,
@@ -872,15 +872,120 @@ __global__ void gx_k_rec_scatter(const unsigned long long *recs, long long nrec,
     }
 }
 
-extern "C" int gx_result_combine(gx_ctx *ctx, gx_result *r)
+// Records -> a send buffer grouped by destination rank (the owner of each record's key, by the hash
+// gx_k_merge_gathered uses), with the offset and the number of records of every destination.
+static int partition_records(gx_ctx *ctx, const unsigned long long *recs, long long nrec, int RW, int N,
+                             unsigned long long **d_send_out, int64_t *sendoff, int64_t *counts)
 {
-    if (!ctx || !r) return GX_ERR_ARG;
-    const int N = ctx->nranks;
+    unsigned nblk = (unsigned) ctx->sm_count;
+    if ((long long) nblk * 256 > nrec) nblk = (unsigned) ((nrec + 255) / 256);
+    if (nblk == 0) nblk = 1;
+    unsigned char *d_dest; long long *d_hist; unsigned long long *d_send;
+    GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d_dest, (size_t) (nrec > 0 ? nrec : 1)));
+    GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d_hist, (size_t) N * nblk * 8));
+    GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d_send, (size_t) (nrec > 0 ? nrec : 1) * RW * 8));
+    long long h_offs[GX_MAX_NODES];
+    {
+        gx_launch_scope ls(ctx, "combine_partition", 3);
+        gx_k_rec_dest_hist<<<nblk, 256, 0, ctx->stream>>>(recs, nrec, RW, N, d_dest, d_hist);
+        gx_k_scan_i64<<<1, 1024, 0, ctx->stream>>>(d_hist, (long long) N * nblk, nullptr);
+        cudaMemcpy2DAsync(h_offs, 8, d_hist, (size_t) nblk * 8, 8, N, cudaMemcpyDeviceToHost, ctx->stream);
+        gx_k_rec_scatter<<<nblk, 256, 0, ctx->stream>>>(recs, nrec, RW, d_dest, d_hist, d_send);
+    }
+    cudaError_t e = cudaStreamSynchronize(ctx->stream);
+    gx_tmp_free(ctx, d_dest); gx_tmp_free(ctx, d_hist);
+    if (e != cudaSuccess) { gx_tmp_free(ctx, d_send); GX_SET_ERR(ctx, "combine: %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
+    for (int p = 0; p < N; p++) { sendoff[p] = h_offs[p]; counts[p] = ((p + 1 < N) ? h_offs[p + 1] : nrec) - h_offs[p]; }
+    *d_send_out = d_send;
+    return GX_OK;
+}
+
+// What the Finalize exchanges between ranks.  combine_run makes every decision and runs every device step; a
+// transport only moves bytes: over NCCL between processes, or in one process on one GPU, where it builds from
+// the partial results of all ranks what NCCL would have delivered to one of them (gx_debug_combine).
+struct gx_combine_transport {
+    int rank, nranks;
+    // every rank's segment of seg_bytes, in rank order, into d_all; d_seg is this rank's, packed with capacity cap
+    virtual int gather_segments(gx_ctx *ctx, const unsigned long long *d_seg, unsigned long long *d_all, long long cap, size_t seg_bytes) = 0;
+    // all[p * nranks + q] = the number of records rank p sends to rank q; mine = this rank's row
+    virtual int gather_counts(gx_ctx *ctx, const int64_t *mine, int64_t *all) = 0;
+    // the records every rank addressed to this one, rank p's at record recvoff[p] of d_recv; d_send, sendoff and
+    // counts are this rank's partitioned records
+    virtual int exchange_records(gx_ctx *ctx, const unsigned long long *d_send, const int64_t *sendoff, const int64_t *counts, int RW,
+                                 unsigned long long *d_recv, const int64_t *recvoff, const int64_t *recvcnt) = 0;
+};
+
+struct gx_nccl_transport : gx_combine_transport {
+    int gather_segments(gx_ctx *ctx, const unsigned long long *d_seg, unsigned long long *d_all, long long, size_t seg_bytes) override
+    {
+        gx_launch_scope ls(ctx, "allgather");
+        int nr = g_nccl.AllGather(d_seg, d_all, seg_bytes, GX_NCCL_INT8, ctx->comm, ctx->stream);
+        if (nr != 0) { GX_SET_ERR(ctx, "NCCL error %d in ncclAllGather: %s", nr, g_nccl.GetErrorString(nr)); return GX_ERR_NCCL; }
+        return GX_OK;
+    }
+    int gather_counts(gx_ctx *ctx, const int64_t *mine, int64_t *all) override { return allgather_i64(ctx, mine, nranks, all); }
+    int exchange_records(gx_ctx *ctx, const unsigned long long *d_send, const int64_t *sendoff, const int64_t *counts, int RW,
+                         unsigned long long *d_recv, const int64_t *recvoff, const int64_t *recvcnt) override
+    {
+        int64_t so[GX_MAX_NODES], sc[GX_MAX_NODES], ro[GX_MAX_NODES], rcn[GX_MAX_NODES];
+        for (int p = 0; p < nranks; p++) { so[p] = sendoff[p] * RW * 8; sc[p] = counts[p] * RW * 8; ro[p] = recvoff[p] * RW * 8; rcn[p] = recvcnt[p] * RW * 8; }
+        gx_launch_scope ls(ctx, "alltoall");
+        return alltoallv_bytes(ctx, (const char *) d_send, so, sc, (char *) d_recv, ro, rcn);
+    }
+};
+
+// parts[p] is the partial result of rank p; only parts[rank] is combined, the others are read
+struct gx_inproc_transport : gx_combine_transport {
+    gx_result *const *parts;
+    unsigned long long *send[GX_MAX_NODES];
+    int64_t sendoff[GX_MAX_NODES][GX_MAX_NODES];
+    gx_ctx *ctx;
+    gx_inproc_transport(gx_ctx *c, gx_result *const *p) : parts(p), ctx(c) { memset(send, 0, sizeof(send)); }
+    ~gx_inproc_transport() { for (int p = 0; p < GX_MAX_NODES; p++) gx_tmp_free(ctx, send[p]); }
+    int gather_segments(gx_ctx *ctx, const unsigned long long *, unsigned long long *d_all, long long cap, size_t seg_bytes) override
+    {
+        for (int p = 0; p < nranks; p++) { int rc = gx_pack_partial(ctx, parts[p], cap, d_all + (size_t) p * (seg_bytes / 8)); if (rc) return rc; }
+        return GX_OK;
+    }
+    int gather_counts(gx_ctx *ctx, const int64_t *mine, int64_t *all) override
+    {
+        for (int p = 0; p < nranks; p++) {
+            if (p == rank) { memcpy(all + (size_t) p * nranks, mine, (size_t) nranks * 8); continue; }
+            int rc = partition_records(ctx, (const unsigned long long *) parts[p]->d_recs, parts[p]->ngroups, parts[p]->rec_words, nranks,
+                                       &send[p], sendoff[p], all + (size_t) p * nranks);
+            if (rc) return rc;
+        }
+        return GX_OK;
+    }
+    int exchange_records(gx_ctx *ctx, const unsigned long long *d_send, const int64_t *own_off, const int64_t *, int RW,
+                         unsigned long long *d_recv, const int64_t *recvoff, const int64_t *recvcnt) override
+    {
+        gx_launch_scope ls(ctx, "alltoall");
+        for (int p = 0; p < nranks; p++) {
+            if (!recvcnt[p]) continue;
+            const unsigned long long *src = p == rank ? d_send + own_off[rank] * RW : send[p] + sendoff[p][rank] * RW;
+            GX_CUDA(ctx, cudaMemcpyAsync(d_recv + recvoff[p] * RW, src, (size_t) recvcnt[p] * RW * 8, cudaMemcpyDeviceToDevice, ctx->stream));
+        }
+        return GX_OK;
+    }
+};
+
+// The Finalize of rank T.rank of T.nranks over r, its partial result.  The groups of the ranks' results
+// partition the combined groups: each group is returned by the one rank that owns its key.  A plain aggregate's
+// one row is returned by rank 0, which owns the empty key (it hashes to 0); every other rank returns no row.
+static int combine_run(gx_ctx *ctx, gx_result *r, gx_combine_transport &T)
+{
+    const int N = T.nranks;
     GX_CHECK_ARG(ctx, N == 1 || !gx_result_has_distinct(r), "combine: count(DISTINCT) counts do not add across %d ranks", N);
     GX_CHECK_ARG(ctx, N == 1 || !gx_result_has_variance(r), "combine: variance states are not combined across %d ranks", N);
-    if (N == 1 || !ctx->comm || r->finalized_across) return GX_OK;
+    if (N == 1 || r->finalized_across) return GX_OK;
     const int RW = r->rec_words;
     long long nrec = r->ngroups;
+    auto finish = [&](unsigned long long *d_groups, long long ngroups, long long cap) {
+        gx_tmp_free(ctx, r->d_recs);
+        r->d_recs = (long long *) d_groups; r->ngroups = ngroups; r->cap = cap; r->finalized_across = 1;
+        r->plain_row_elsewhere = r->plan.n_group_cols == 0 && T.rank != 0;
+    };
     // ---- few groups (Q1, GROUP BY date): one ncclAllGather of fixed-capacity segments and a
     // device-side merge; no partition, no count exchange, one host synchronisation (the group
     // count).  The capacity comes from the planner's estimate, which every datanode shares
@@ -896,65 +1001,67 @@ extern "C" int gx_result_combine(gx_ctx *ctx, gx_result *r)
             GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d_seg, seg_bytes));
             GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d_all, seg_bytes * N));
             int rc = gx_pack_partial(ctx, r, cap, d_seg);
-            if (rc == GX_OK) {
-                gx_launch_scope ls(ctx, "allgather");
-                int nr = g_nccl.AllGather(d_seg, d_all, seg_bytes, GX_NCCL_INT8, ctx->comm, ctx->stream);
-                if (nr != 0) { GX_SET_ERR(ctx, "NCCL error %d in ncclAllGather: %s", nr, g_nccl.GetErrorString(nr)); rc = GX_ERR_NCCL; }
-            }
+            if (rc == GX_OK) rc = T.gather_segments(ctx, d_seg, d_all, cap, seg_bytes);
             unsigned long long *d_groups = nullptr; long long ngroups = 0; int anybig = 0;
-            if (rc == GX_OK) rc = gx_combine_gathered(ctx, r, d_all, N, cap, &d_groups, &ngroups, &anybig);
+            if (rc == GX_OK) rc = gx_combine_gathered(ctx, r, d_all, N, cap, T.rank, N, &d_groups, &ngroups, &anybig);
             gx_tmp_free(ctx, d_seg); gx_tmp_free(ctx, d_all);
             if (rc) return rc;
-            if (!anybig) {
-                gx_tmp_free(ctx, r->d_recs);
-                r->d_recs = (long long *) d_groups; r->ngroups = ngroups; r->cap = ngroups > 0 ? ngroups : 1; r->finalized_across = 1;
-                return GX_OK;
-            }
+            if (!anybig) { finish(d_groups, ngroups, ngroups > 0 ? ngroups : 1); return GX_OK; }
         }
     }
-    unsigned nblk = (unsigned) ctx->sm_count;
-    if ((long long) nblk * 256 > nrec) nblk = (unsigned) ((nrec + 255) / 256);
-    if (nblk == 0) nblk = 1;
-    unsigned char *d_dest; long long *d_hist; unsigned long long *d_send;
-    GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d_dest, (size_t) (nrec > 0 ? nrec : 1)));
-    GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d_hist, (size_t) N * nblk * 8));
-    GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d_send, (size_t) (nrec > 0 ? nrec : 1) * RW * 8));
-    long long h_offs[GX_MAX_NODES];
-    {
-        gx_launch_scope ls(ctx, "combine_partition", 3);
-        gx_k_rec_dest_hist<<<nblk, 256, 0, ctx->stream>>>((const unsigned long long *) r->d_recs, nrec, RW, N, d_dest, d_hist);
-        gx_k_scan_i64<<<1, 1024, 0, ctx->stream>>>(d_hist, (long long) N * nblk, nullptr);
-        cudaMemcpy2DAsync(h_offs, 8, d_hist, (size_t) nblk * 8, 8, N, cudaMemcpyDeviceToHost, ctx->stream);
-        gx_k_rec_scatter<<<nblk, 256, 0, ctx->stream>>>((const unsigned long long *) r->d_recs, nrec, RW, d_dest, d_hist, d_send);
-    }
-    GX_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    unsigned long long *d_send;
     int64_t counts[GX_MAX_NODES], sendoff[GX_MAX_NODES], recvcnt[GX_MAX_NODES], recvoff[GX_MAX_NODES], total = 0;
-    for (int p = 0; p < N; p++) { sendoff[p] = h_offs[p]; counts[p] = ((p + 1 < N) ? h_offs[p + 1] : nrec) - h_offs[p]; }
+    int rc = partition_records(ctx, (const unsigned long long *) r->d_recs, nrec, RW, N, &d_send, sendoff, counts);
+    if (rc) return rc;
     int64_t *all = (int64_t *) malloc((size_t) N * N * 8);
-    int rc = allgather_i64(ctx, counts, N, all);
+    rc = T.gather_counts(ctx, counts, all);
     if (rc == GX_OK) {
-        for (int p = 0; p < N; p++) { recvcnt[p] = all[(size_t) p * N + ctx->rank]; recvoff[p] = total; total += recvcnt[p]; }
+        for (int p = 0; p < N; p++) { recvcnt[p] = all[(size_t) p * N + T.rank]; recvoff[p] = total; total += recvcnt[p]; }
     }
     free(all);
     unsigned long long *d_recv = nullptr;
     if (rc == GX_OK) {
-        GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d_recv, (size_t) (total > 0 ? total : 1) * RW * 8));
-        int64_t so[GX_MAX_NODES], sc[GX_MAX_NODES], ro[GX_MAX_NODES], rcn[GX_MAX_NODES];
-        for (int p = 0; p < N; p++) { so[p] = sendoff[p] * RW * 8; sc[p] = counts[p] * RW * 8; ro[p] = recvoff[p] * RW * 8; rcn[p] = recvcnt[p] * RW * 8; }
-        gx_launch_scope ls(ctx, "alltoall");
-        rc = alltoallv_bytes(ctx, (const char *) d_send, so, sc, (char *) d_recv, ro, rcn);
+        cudaError_t e = gx_tmp_alloc(ctx, (void **) &d_recv, (size_t) (total > 0 ? total : 1) * RW * 8);
+        if (e != cudaSuccess) { d_recv = nullptr; GX_SET_ERR(ctx, "combine: %s", cudaGetErrorString(e)); rc = GX_ERR_NOMEM; }
     }
+    if (rc == GX_OK) rc = T.exchange_records(ctx, d_send, sendoff, counts, RW, d_recv, recvoff, recvcnt);
     if (rc == GX_OK) { cudaError_t e = cudaStreamSynchronize(ctx->stream); if (e != cudaSuccess) { GX_SET_ERR(ctx, "combine: %s", cudaGetErrorString(e)); rc = GX_ERR_CUDA; } }
-    gx_tmp_free(ctx, d_dest); gx_tmp_free(ctx, d_hist); gx_tmp_free(ctx, d_send);
+    gx_tmp_free(ctx, d_send);
     if (rc) { if (d_recv) gx_tmp_free(ctx, d_recv); return rc; }
     unsigned long long *d_groups; long long ngroups;
     rc = gx_combine_records(ctx, r, d_recv, total, &d_groups, &ngroups);
     gx_tmp_free(ctx, d_recv);
     if (rc) return rc;
-    gx_tmp_free(ctx, r->d_recs);
     if (!d_groups) { GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d_groups, 64)); }
-    r->d_recs = (long long *) d_groups; r->ngroups = ngroups; r->cap = ngroups; r->finalized_across = 1;
+    finish(d_groups, ngroups, ngroups);
     return GX_OK;
+}
+
+extern "C" int gx_result_combine(gx_ctx *ctx, gx_result *r)
+{
+    if (!ctx || !r) return GX_ERR_ARG;
+    gx_nccl_transport T;
+    T.rank = ctx->rank; T.nranks = ctx->comm ? ctx->nranks : 1;
+    return combine_run(ctx, r, T);
+}
+
+extern "C" int gx_debug_combine(gx_ctx *ctx, int nparts, gx_result *const *parts, int rank)
+{
+    if (!ctx || !parts) return GX_ERR_ARG;
+    GX_CHECK_ARG(ctx, nparts >= 1 && nparts <= GX_MAX_NODES, "debug_combine: %d parts (1..%d)", nparts, GX_MAX_NODES);
+    GX_CHECK_ARG(ctx, rank >= 0 && rank < nparts, "debug_combine: rank %d of %d parts", rank, nparts);
+    for (int p = 0; p < nparts; p++) {
+        const gx_result *a = parts[p], *b = parts[0];
+        GX_CHECK_ARG(ctx, a != nullptr, "debug_combine: part %d is NULL", p);
+        GX_CHECK_ARG(ctx, !a->finalized_across, "debug_combine: part %d was combined already", p);
+        GX_CHECK_ARG(ctx, memcmp(&a->plan, &b->plan, sizeof(a->plan)) == 0, "debug_combine: part %d has another plan than part 0", p);
+        GX_CHECK_ARG(ctx, a->rec_words == b->rec_words && memcmp(a->agg_word, b->agg_word, sizeof(a->agg_word)) == 0 &&
+                     memcmp(a->agg_cnt_word, b->agg_cnt_word, sizeof(a->agg_cnt_word)) == 0,
+                     "debug_combine: part %d has another record layout than part 0", p);
+    }
+    gx_inproc_transport T(ctx, parts);
+    T.rank = rank; T.nranks = nparts;
+    return combine_run(ctx, parts[rank], T);
 }
 
 // ------------------------------------------------- debug hash entry point

@@ -154,8 +154,11 @@ struct gx_result {
     unsigned int *d_nullmask;        // ngroups (group-key null bits)
     int64_t ngroups, cap;
     int finalized_across;            // combined over the communicator already
+    int plain_row_elsewhere;         // combined plain aggregate: another rank returns its one row
     int need_w0;                     // w0 (rows per group) is maintained
 };
+// a plain aggregate over zero rows: this result returns the one row of initial states
+static inline bool gx_result_plain_empty(const gx_result *r) { return r->plan.n_group_cols == 0 && r->ngroups == 0 && !r->plain_row_elsewhere; }
 
 bool gx_result_has_distinct(const gx_result *r);      // some aggregate is GX_AGG_COUNT_DISTINCT: no partial states
 bool gx_result_has_variance(const gx_result *r);      // some aggregate is GX_AGG_VAR_* / GX_AGG_STDDEV_*
