@@ -77,7 +77,20 @@ enum {
     GX_AGG_VAR_POP_F8     = 10, /* float8_accum/float8_var_pop     (float.c:3010)  */
     GX_AGG_VAR_SAMP_F8    = 11, /* float8_accum/float8_var_samp    (float.c:3032); variance() */
     GX_AGG_STDDEV_POP_F8  = 12, /* float8_accum/float8_stddev_pop  (float.c:3054)  */
-    GX_AGG_STDDEV_SAMP_F8 = 13  /* float8_accum/float8_stddev_samp (float.c:3076); stddev() */
+    GX_AGG_STDDEV_SAMP_F8 = 13, /* float8_accum/float8_stddev_samp (float.c:3076); stddev() */
+    /* SQL:2003 binary aggregates (pg_aggregate.h:304-316): two float8 arguments (Y, X), see below */
+    GX_AGG_REGR_COUNT        = 14, /* int8inc_float8_float8 (int8.c:805), bit-cast as GX_AGG_COUNT */
+    GX_AGG_REGR_SXX_F8       = 15, /* float8_regr_accum/float8_regr_sxx       (float.c:3386)  */
+    GX_AGG_REGR_SYY_F8       = 16, /* float8_regr_accum/float8_regr_syy       (float.c:3407)  */
+    GX_AGG_REGR_SXY_F8       = 17, /* float8_regr_accum/float8_regr_sxy       (float.c:3428)  */
+    GX_AGG_REGR_AVGX_F8      = 18, /* float8_regr_accum/float8_regr_avgx      (float.c:3449)  */
+    GX_AGG_REGR_AVGY_F8      = 19, /* float8_regr_accum/float8_regr_avgy      (float.c:3468)  */
+    GX_AGG_REGR_R2_F8        = 20, /* float8_regr_accum/float8_regr_r2        (float.c:3554)  */
+    GX_AGG_REGR_SLOPE_F8     = 21, /* float8_regr_accum/float8_regr_slope     (float.c:3587)  */
+    GX_AGG_REGR_INTERCEPT_F8 = 22, /* float8_regr_accum/float8_regr_intercept (float.c:3614)  */
+    GX_AGG_COVAR_POP_F8      = 23, /* float8_regr_accum/float8_covar_pop      (float.c:3487)  */
+    GX_AGG_COVAR_SAMP_F8     = 24, /* float8_regr_accum/float8_covar_samp     (float.c:3506)  */
+    GX_AGG_CORR_F8           = 25  /* float8_regr_accum/float8_corr           (float.c:3525)  */
 };
 /* GX_AGG_COUNT_DISTINCT counts the distinct non-NULL values of one column per group.  Its argument is a single
  * GX_OP_COL over an outer column of type INT4, INT8, DATE or CHAR, compared as int4eq / int8eq / date_eq do
@@ -101,6 +114,23 @@ enum {
  * returns {N, Sx} as for GX_AGG_AVG_F8 (never NULL, {0, 0} over zero rows) and gx_result_fetch_sxx the Sxx that
  * completes float8_combine's {N, Sx, Sxx}.  A plan whose state words exceed the library's limit is GX_ERR_ARG, and so
  * is gx_result_combine with more than one rank (a two-phase plan combines the states in the reference's Finalize). */
+/* GX_AGG_REGR_COUNT .. GX_AGG_CORR_F8 take two float8 expressions in one gx_expr: the ops before GX_OP_ARG2 are Y,
+ * the first SQL argument, the ops after it X (each a program a one-argument aggregate would take; GX_MAX_EXPR_OPS
+ * counts both and the separator).  GX_OP_ARG2 in a one-argument aggregate, twice, with an empty side, or missing in
+ * a two-argument aggregate is GX_ERR_ARG.  A row whose Y or X is NULL is skipped (the transition function is strict
+ * in both); N counts the remaining pairs.  gx_result_fetch returns the final of float.c:3386-3642: NULL when N < 1
+ * (N < 2 for covar_samp) and for a vertical line (Sxx == 0: regr_slope, regr_intercept, regr_r2); corr is NULL when
+ * Sxx == 0 or Syy == 0, regr_r2 is 1.0 when Syy == 0.  regr_count is never NULL.  As float8_regr_accum does, a
+ * non-finite X makes Sxx and Sxy NaN, a non-finite Y makes Syy and Sxy NaN, and Sx, Sy are ordinary sums; a finite
+ * input whose state overflows is GX_ERR_OVERFLOW (the rule of the variances above, both arguments' inputs counting).
+ * The device keeps {C, S1, S2} shifted sums for X and for Y plus the cross term sum((x - Cx)(y - Cy)), merged with
+ * re-centring (DESIGN.md §3.2): Sxx and Syy meet the variance bound, Sxy is within
+ * 2^-30 sqrt(Sxx Syy) + 16 N^2 2^-52 Dx Dy, and a constant X (Y) gives Sxx (Syy) exactly 0.
+ * The regression aggregates over one (Y, X) pair share one state; a plan with two different pairs is GX_ERR_ARG
+ * (two states do not fit the library's state words), and so is a plan whose state words exceed the limit.
+ * gx_result_fetch_states returns cnt_out = N (never NULL; val_out = Sx, 0 for regr_count) and gx_result_fetch_regr
+ * float8_regr_accum's six-element state.  gx_result_combine with more than one rank is GX_ERR_ARG for such a plan
+ * (a two-phase plan combines the states in the reference's Finalize with float8_regr_combine / int8pl). */
 
 /* expression opcodes: tiny postfix VM over float8 (the provider pattern-matches
  * Var/Const/+,-,* trees from the reference's expression tree and declines
@@ -110,7 +140,8 @@ enum {
     GX_OP_CONST = 2,  /* push k                                             */
     GX_OP_ADD   = 3,  /* float8pl  */
     GX_OP_SUB   = 4,  /* float8mi  */
-    GX_OP_MUL   = 5   /* float8mul */
+    GX_OP_MUL   = 5,  /* float8mul */
+    GX_OP_ARG2  = 6   /* two-argument aggregates only: ends Y's program, X's follows */
 };
 
 #define GX_MAX_PREDS      4
@@ -433,6 +464,10 @@ int  gx_result_fetch_states(gx_result *r, int64_t max_groups, int64_t *key_out,
 /* Sxx of the float8_accum state {N, Sx, Sxx} per group and aggregate, groups in the order of gx_result_fetch_states:
  * sxx_out[g*n_aggs + a] is the group's Sxx for GX_AGG_VAR_* / GX_AGG_STDDEV_* and 0 for any other aggregate. */
 int  gx_result_fetch_sxx(gx_result *r, int64_t max_groups, double *sxx_out);
+/* float8_regr_accum's state {N, Sx, Sxx, Sy, Syy, Sxy} per group and aggregate, groups in the order of
+ * gx_result_fetch_states: out[(g*n_aggs + a)*6 .. +5] for GX_AGG_REGR_SXX_F8 .. GX_AGG_CORR_F8, zeros for any other
+ * aggregate (regr_count's partial state is the int8 count of gx_result_fetch_states). */
+int  gx_result_fetch_regr(gx_result *r, int64_t max_groups, double *out);
 void gx_result_free(gx_result *r);
 
 /* One-call form used by the provider and by bench.py's e2e leg: HOST column

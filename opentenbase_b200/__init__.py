@@ -25,7 +25,10 @@ GX_LT, GX_LE, GX_EQ, GX_GE, GX_GT, GX_NE = 1, 2, 3, 4, 5, 6
 (GX_AGG_COUNT_STAR, GX_AGG_COUNT, GX_AGG_SUM_F8, GX_AGG_AVG_F8, GX_AGG_SUM_I4,
  GX_AGG_MIN_F8, GX_AGG_MAX_F8, GX_AGG_SUM_I8, GX_AGG_COUNT_DISTINCT) = 1, 2, 3, 4, 5, 6, 7, 8, 9
 (GX_AGG_VAR_POP_F8, GX_AGG_VAR_SAMP_F8, GX_AGG_STDDEV_POP_F8, GX_AGG_STDDEV_SAMP_F8) = 10, 11, 12, 13
-GX_OP_COL, GX_OP_CONST, GX_OP_ADD, GX_OP_SUB, GX_OP_MUL = 1, 2, 3, 4, 5
+(GX_AGG_REGR_COUNT, GX_AGG_REGR_SXX_F8, GX_AGG_REGR_SYY_F8, GX_AGG_REGR_SXY_F8, GX_AGG_REGR_AVGX_F8,
+ GX_AGG_REGR_AVGY_F8, GX_AGG_REGR_R2_F8, GX_AGG_REGR_SLOPE_F8, GX_AGG_REGR_INTERCEPT_F8, GX_AGG_COVAR_POP_F8,
+ GX_AGG_COVAR_SAMP_F8, GX_AGG_CORR_F8) = range(14, 26)
+GX_OP_COL, GX_OP_CONST, GX_OP_ADD, GX_OP_SUB, GX_OP_MUL, GX_OP_ARG2 = 1, 2, 3, 4, 5, 6
 GX_JOIN_INNER, GX_JOIN_LEFT, GX_JOIN_SEMI, GX_JOIN_ANTI = 0, 1, 4, 5
 T_ORDERS, T_LINEITEM, T_CUSTOMER = 1, 2, 3
 # fixed schemas of include/gx_tpch_gen.h
@@ -180,6 +183,7 @@ def _declare(L):
         "gx_result_fetch": (C.c_int, [vp, i64, vp, vp, vp]),
         "gx_result_fetch_states": (C.c_int, [vp, i64, vp, vp, vp, vp]),
         "gx_result_fetch_sxx": (C.c_int, [vp, i64, vp]),
+        "gx_result_fetch_regr": (C.c_int, [vp, i64, vp]),
         "gx_result_free": (None, [vp]),
         "gx_exec_host": (C.c_int, [vp, C.POINTER(GxHostTable), C.POINTER(GxHostTable), C.c_int, C.c_int,
                                    C.POINTER(GxPred), C.c_int, C.POINTER(i32), C.c_int, C.POINTER(GxAggPlan), pp]),
@@ -392,6 +396,14 @@ class Result:
         sxx = np.zeros((n, na), np.float64)
         self.ctx._chk(lib().gx_result_fetch_sxx(self.h, n, sxx.ctypes.data))
         return sxx
+
+    def fetch_regr(self):
+        """float8_regr_accum's {N, Sx, Sxx, Sy, Syy, Sxy} of each regression aggregate, float64[n, na, 6] (zeros for
+        other aggregates and regr_count), groups in the order of fetch_states"""
+        n, na = self.ngroups, self.plan.n_aggs
+        st = np.zeros((n, na, 6), np.float64)
+        self.ctx._chk(lib().gx_result_fetch_regr(self.h, n, st.ctypes.data))
+        return st
 
     def free(self):
         if self.h and self.ctx.h:          # handles die with their context (stream-ordered frees need its stream)

@@ -29,10 +29,14 @@
 
 int gx_fill_dpreds(gx_ctx *ctx, const gx_table *t, int n_preds, const gx_pred *preds, gx_dpred *out);
 
-enum { WK_ADD_I64 = 0, WK_ADD_F64 = 1, WK_MIN_F64 = 2, WK_MAX_F64 = 3, WK_VAR_C = 4, WK_VAR_S = 5 };
+enum { WK_ADD_I64 = 0, WK_ADD_F64 = 1, WK_MIN_F64 = 2, WK_MAX_F64 = 3, WK_VAR_C = 4, WK_VAR_S = 5, WK_REGR_C = 6 };
 // A variance state is three words {C, S1, S2}: S1 = sum(x - C) and S2 = sum((x - C)^2) around a shift C that the
 // state's first value sets.  They merge together (var_merge), so the C word's kind carries the word that counts the
 // state's inputs: wkind = WK_VAR_C | count word << 8 (0: w0); S1 and S2 are WK_VAR_S and never merged on their own.
+// A regression state (the two-argument aggregates, gx_dregr) is seven words {Cx, S1x, S2x, Cy, S1y, S2y, Sxy'}: one
+// such triple for X and one for Y, and the cross term Sxy' = sum((x - Cx)(y - Cy)).  They merge together
+// (regr_merge): Cx's kind is WK_REGR_C | count word << 8, the other six are WK_VAR_S.  Its Sx and Sy are two ordinary
+// WK_ADD_F64 words in front of it.
 #define GX_VAR_UNSET_BITS 0x7FF4000000000001ULL      // C before the first value: a NaN no float8 arithmetic produces
 // initial value of every float8 sum (state words and register accumulators): -0.0 is the exact additive identity,
 // so a group whose inputs are all -0.0 sums to -0.0 as float8pl does when the first input becomes the state
@@ -117,14 +121,16 @@ __device__ __forceinline__ void merge_word(unsigned long long *addr, int kind, u
 // set once, from the unset value; then the source is re-centred on it: with d = cs - C,
 // S1 += s1 + n d and S2 += s2 + 2 d s1 + n d^2 (independent atomics: C no longer changes).  An input NaN that happens
 // to carry GX_VAR_UNSET_BITS leaves C unset, but its own d is NaN, so the state is NaN as it must be.
-__device__ __forceinline__ void var_merge(unsigned long long *dst, double cs, double s1, double s2, long long n)
+// Returns d.
+__device__ __forceinline__ double var_merge(unsigned long long *dst, double cs, double s1, double s2, long long n)
 {
-    if (n == 0) return;
+    if (n == 0) return 0.0;
     const unsigned long long old = atomicCAS(dst, GX_VAR_UNSET_BITS, (unsigned long long) __double_as_longlong(cs));
     const double c = old == GX_VAR_UNSET_BITS ? cs : __longlong_as_double((long long) old);
     const double d = __dsub_rn(cs, c), nd = __dmul_rn((double) n, d);
     atomicAdd((double *) &dst[1], __dadd_rn(s1, nd));
     atomicAdd((double *) &dst[2], __dadd_rn(__dadd_rn(s2, __dmul_rn(__dmul_rn(2.0, d), s1)), __dmul_rn(nd, d)));
+    return d;
 }
 // the same merge in registers: state a (na inputs) takes state b (nb inputs), keeping a's shift
 __device__ __forceinline__ void var_combine(double &ac, double &a1, double &a2, long long &na, double bc, double b1, double b2, long long nb)
@@ -136,7 +142,38 @@ __device__ __forceinline__ void var_combine(double &ac, double &a1, double &a2, 
     a1 = __dadd_rn(a1, __dadd_rn(b1, nd));
     na += nb;
 }
-// merge the state words src[0, nwords) of one group into dst (w0 first in both)
+// the cross term a source regression state s = {Cx, S1x, S2x, Cy, S1y, S2y, Sxy'} of n inputs adds to a target whose
+// shifts lie dx = Cx_s - Cx_t and dy = Cy_s - Cy_t below s's: sum((x - Cx_t)(y - Cy_t)) over s's inputs
+// = Sxy'_s + dx S1y_s + dy S1x_s + n dx dy
+__device__ __forceinline__ double regr_cross(const double (&s)[7], long long n, double dx, double dy)
+{
+    return __dadd_rn(__dadd_rn(__dadd_rn(s[6], __dmul_rn(dx, s[4])), __dmul_rn(dy, s[1])), __dmul_rn(__dmul_rn((double) n, dx), dy));
+}
+// Merge the regression state s of n inputs into the words dst = {Cx, .., Sxy'} of another: each triple as var_merge
+// (which sets the target's shift once and re-centres), the cross term in the same call on the shifts it used
+__device__ __forceinline__ void regr_merge(unsigned long long *dst, const double (&s)[7], long long n)
+{
+    if (n == 0) return;
+    const double dx = var_merge(&dst[0], s[0], s[1], s[2], n), dy = var_merge(&dst[3], s[3], s[4], s[5], n);
+    atomicAdd((double *) &dst[6], regr_cross(s, n, dx, dy));
+}
+// the same merge in registers: state a (na inputs) takes state b (nb inputs), keeping a's shifts
+__device__ __forceinline__ void regr_combine(double (&a)[7], long long &na, const double (&b)[7], long long nb)
+{
+    if (nb == 0) return;
+    if (na == 0) {
+#pragma unroll
+        for (int i = 0; i < 7; i++) a[i] = b[i];
+        na = nb; return;
+    }
+    a[6] = __dadd_rn(a[6], regr_cross(b, nb, __dsub_rn(b[0], a[0]), __dsub_rn(b[3], a[3])));
+    long long n1 = na; var_combine(a[0], a[1], a[2], n1, b[0], b[1], b[2], nb);
+    n1 = na;           var_combine(a[3], a[4], a[5], n1, b[3], b[4], b[5], nb);
+    na += nb;
+}
+// merge the state words src[0, nwords) of one group into dst (w0 first in both).  REGR: the plan may keep a
+// regression state (gx_k_agg's plain instantiations and the specialised kernels never see one, and leave its merge out)
+template <bool REGR>
 __device__ __forceinline__ void merge_words(unsigned long long *dst, const unsigned long long *src, const int *wkind, int nwords)
 {
     for (int j = 0; j < nwords; j++) {
@@ -145,6 +182,12 @@ __device__ __forceinline__ void merge_words(unsigned long long *dst, const unsig
             var_merge(&dst[j], __longlong_as_double((long long) src[j]), __longlong_as_double((long long) src[j + 1]),
                       __longlong_as_double((long long) src[j + 2]), (long long) src[k >> 8]);
             j += 2;
+        } else if (REGR && (k & 0xFF) == WK_REGR_C) {
+            double s[7];
+#pragma unroll
+            for (int i = 0; i < 7; i++) s[i] = __longlong_as_double((long long) src[j + i]);
+            regr_merge(&dst[j], s, (long long) src[k >> 8]);
+            j += 6;
         } else merge_word(&dst[j], k, src[j]);
     }
 }
@@ -263,8 +306,8 @@ struct Sink {
         else if (SINK == SINK_SMEM_LP) { double *p = (double *) at(word); *p = __dadd_rn(*p, v); }
         else atomicAdd((double *) at(word), v);
     }
-    // one value into the variance state at words {word, word + 1, word + 2} = {C, S1, S2}
-    __device__ __forceinline__ void var_f64(int word, double x)
+    // x - C for the shift C at `word`, which the state's first value sets
+    __device__ __forceinline__ double shifted(int word, double x)
     {
         unsigned long long *pc = at(word);
         const unsigned long long xb = (unsigned long long) __double_as_longlong(x);
@@ -272,9 +315,26 @@ struct Sink {
         if (SINK == SINK_RECORD) *pc = xb;
         else if (SINK == SINK_SMEM_LP) { if (*pc == GX_VAR_UNSET_BITS) *pc = xb; else c = __longlong_as_double((long long) *pc); }
         else { const unsigned long long old = atomicCAS(pc, GX_VAR_UNSET_BITS, xb); if (old != GX_VAR_UNSET_BITS) c = __longlong_as_double((long long) old); }
-        const double d = __dsub_rn(x, c);
+        return __dsub_rn(x, c);
+    }
+    // one value into the variance state at words {word, word + 1, word + 2} = {C, S1, S2}
+    __device__ __forceinline__ void var_f64(int word, double x)
+    {
+        const double d = shifted(word, x);
         add_f64(word + 1, d);
         add_f64(word + 2, __dmul_rn(d, d));
+    }
+    // one (y, x) pair into the regression words {Sx, Sy, Cx, S1x, S2x, Cy, S1y, S2y, Sxy'} from `word` on
+    __device__ __forceinline__ void regr_f64(int word, double x, double y)
+    {
+        add_f64(word, x);
+        add_f64(word + 1, y);
+        const double dx = shifted(word + 2, x), dy = shifted(word + 5, y);
+        add_f64(word + 3, dx);
+        add_f64(word + 4, __dmul_rn(dx, dx));
+        add_f64(word + 6, dy);
+        add_f64(word + 7, __dmul_rn(dy, dy));
+        add_f64(word + 8, __dmul_rn(dx, dy));
     }
     __device__ __forceinline__ void minmax_f64(int word, double v, bool want_min)
     {
@@ -310,7 +370,7 @@ __device__ __forceinline__ void pack_group_key(const gx_dplan &P, long long r, u
     }
 }
 
-template <int SINK>
+template <int SINK, bool REGR>
 __device__ __forceinline__ void apply_aggs(const gx_dplan &P, bool need_w0, long long r, Sink<SINK> &sink)
 {
     if (need_w0 || SINK == SINK_RECORD) sink.inc(0);          // w0: rows in the group (count(*))
@@ -331,6 +391,14 @@ __device__ __forceinline__ void apply_aggs(const gx_dplan &P, bool need_w0, long
             if (g.kind == GXU_ADD_F64) { sink.add_f64(g.word, v); if (g.var_word) sink.var_f64(g.var_word, v); }
             else sink.minmax_f64(g.word, v, g.kind == GXU_MIN_F64);
             if (g.cnt_word) sink.inc(g.cnt_word);
+        }
+    }
+    if (REGR && P.regr.on) {                                  // the two-argument aggregates' one (Y, X) pair
+        bool isnull = false;
+        const double y = gx_eval_expr(P.regr.y, r, isnull), x = gx_eval_expr(P.regr.x, r, isnull);
+        if (!isnull) {                                        // strict in both arguments (float8_regr_accum)
+            if (P.regr.word) sink.regr_f64(P.regr.word, x, y);
+            if (P.regr.cnt_word) sink.inc(P.regr.cnt_word);
         }
     }
 }
@@ -357,20 +425,20 @@ __device__ __forceinline__ void pack_chain_key(const gx_dplan &P, long long r, c
     }
 }
 
-template <int SINK>
+template <int SINK, bool REGR>
 __device__ __forceinline__ void consume_key(const gx_agg_dev &A, const SmemTable &T, long long r, unsigned long long k0, unsigned long long k1,
                                             unsigned int nullmask, unsigned int cm);
 
-template <int SINK>
+template <int SINK, bool REGR>
 __device__ __forceinline__ void consume_row(const gx_agg_dev &A, const SmemTable &T, long long r, unsigned long long payload, unsigned int cm = 0)
 {
     unsigned long long k0, k1; unsigned int nullmask;
     pack_group_key(A.P, r, payload, k0, k1, nullmask);
-    consume_key<SINK>(A, T, r, k0, k1, nullmask, cm);
+    consume_key<SINK, REGR>(A, T, r, k0, k1, nullmask, cm);
 }
 
 // one row with its packed group key into the sink
-template <int SINK>
+template <int SINK, bool REGR>
 __device__ __forceinline__ void consume_key(const gx_agg_dev &A, const SmemTable &T, long long r, unsigned long long k0, unsigned long long k1,
                                             unsigned int nullmask, unsigned int cm)
 {
@@ -411,10 +479,11 @@ __device__ __forceinline__ void consume_key(const gx_agg_dev &A, const SmemTable
         for (int i = 0; i < A.P.nwords; i++) rec[3 + i] = (unsigned long long) A.winit[i];
         sink.w = rec + 3;
     }
-    apply_aggs<SINK>(A.P, A.need_w0 != 0, r, sink);
+    apply_aggs<SINK, REGR>(A.P, A.need_w0 != 0, r, sink);
 }
 
 // merge a CTA's dense shared-memory table into the global table
+template <bool REGR = false>
 __device__ __forceinline__ void smem_dense_merge(const SmemTable &T, const gx_agg_dev &A)
 {
     for (int i = threadIdx.x; i < T.S; i += blockDim.x) {
@@ -424,7 +493,7 @@ __device__ __forceinline__ void smem_dense_merge(const SmemTable &T, const gx_ag
         unsigned long long k0 = T.tagkey ? (t & 0x00FFFFFFFFFFFFFFULL) : T.k0[i];
         unsigned long long *rec = global_upsert(A, k0, (!T.tagkey && T.nkw > 1) ? T.k1[i] : 0ULL, nullmask);
         if (!rec) { atomicOr((unsigned long long *) &A.counters[1], 2ULL); continue; }
-        merge_words(&rec[3], &T.w[(size_t) i * T.nwords], A.wkind, T.nwords);
+        merge_words<REGR>(&rec[3], &T.w[(size_t) i * T.nwords], A.wkind, T.nwords);
     }
 }
 
@@ -472,6 +541,28 @@ __device__ __forceinline__ void lp_var_merge(const SmemTable &T, int nwarps, int
     }
     if (lane == 0 && rec) var_merge(&rec[3 + word], c, s1, s2, n);
 }
+// the same for the regression state at words [word, word + 7) whose pairs word cw counts
+__device__ __forceinline__ void lp_regr_merge(const SmemTable &T, int nwarps, int word, int cw, unsigned int gi, int lane, unsigned long long *rec)
+{
+    double a[7] = { 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0 }; long long n = 0;
+    const size_t ws = (size_t) T.gmax * 32;
+    for (int wp = 0; wp < nwarps; wp++) {
+        const unsigned long long *v = &T.w[(((size_t) wp * T.nwords + word) * T.gmax + gi) * 32 + lane];
+        double b[7];
+#pragma unroll
+        for (int i = 0; i < 7; i++) b[i] = __longlong_as_double((long long) v[i * ws]);
+        regr_combine(a, n, b, (long long) T.w[(((size_t) wp * T.nwords + cw) * T.gmax + gi) * 32 + lane]);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        double b[7];
+#pragma unroll
+        for (int i = 0; i < 7; i++) b[i] = __shfl_down_sync(0xffffffffu, a[i], o);
+        const long long bn = __shfl_down_sync(0xffffffffu, n, o);
+        if (lane + o < 32) regr_combine(a, n, b, bn);
+    }
+    if (lane == 0 && rec) regr_merge(&rec[3 + word], a, n);
+}
 
 // XF < 0: no join, or an INNER join walked row by row over the 16-byte table.  XF = GX_SLOTS_*: a SEMI / ANTI join
 // (nodeHashjoin.c:569-634), an existence test per outer row in the format the build wrote: PT_K x 32 rows per warp and
@@ -481,7 +572,9 @@ __device__ __forceinline__ void lp_var_merge(const SmemTable &T, int nwarps, int
 // XF = GX_XF_CHAIN + GX_SLOTS_*: a chain of unique INNER joins (gx_hash_agg_joins), step 1 probed in the format its build
 // wrote, steps 2.. in their 16-byte form, each with a key from the outer row or from an earlier step's payload; a row that
 // every step matches is consumed once, its group key packed from the outer row and the steps' payload words.
-template <int SINK, int XF>
+// REGR: the plan keeps a regression state (gx_dregr).  The instantiations without it leave its update and merge out,
+// so plans without a two-argument aggregate run the code they ran before it existed.
+template <int SINK, int XF, bool REGR>
 __global__ void __launch_bounds__(1024, 1) gx_k_agg(const __grid_constant__ gx_agg_dev A)
 {
     extern __shared__ unsigned long long smem[];
@@ -564,7 +657,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_agg(const __grid_constant__ gx_a
                 unsigned long long k0, k1; unsigned int nullmask;
                 const long long row = base + j * 32 + lane;
                 pack_chain_key(P, row, pj, k0, k1, nullmask);
-                consume_key<SINK>(A, T, row, k0, k1, nullmask, m);
+                consume_key<SINK, REGR>(A, T, row, k0, k1, nullmask, m);
             }
         }
     } else if constexpr (XF >= 0) {
@@ -588,7 +681,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_agg(const __grid_constant__ gx_a
             for (int j = 0; j < PT_K; j++) {
                 const bool take = (pass >> j) & 1u;
                 const unsigned int m = P.nwords >= 3 ? __ballot_sync(0xffffffffu, take) : 0u;
-                if (take) consume_row<SINK>(A, T, base + j * 32 + lane, 0ULL, m);
+                if (take) consume_row<SINK, REGR>(A, T, base + j * 32 + lane, 0ULL, m);
             }
         }
     } else {
@@ -602,21 +695,21 @@ __global__ void __launch_bounds__(1024, 1) gx_k_agg(const __grid_constant__ gx_a
                 // exactly the lanes that consume a row now; the barrier only pays when a row has several
                 // state words to update (with one counter it cost 20 % on the config-1 shape)
                 const unsigned int m = P.nwords >= 3 ? __ballot_sync(0xffffffffu, ok) : 0u;
-                if (ok) consume_row<SINK>(A, T, r, 0ULL, m);
+                if (ok) consume_row<SINK, REGR>(A, T, r, 0ULL, m);
                 continue;
             }
             if (!ok) continue;
             if (gx_is_null(P.okey, r)) continue;                  // NULL outer key never joins
             long long key = gx_load_int(P.okey, r);
             if (key == GX_EMPTY_KEY) {
-                for (int i = 0; i < A.special_count; i++) { consume_row<SINK>(A, T, r, A.special[i]); if (P.unique) break; }
+                for (int i = 0; i < A.special_count; i++) { consume_row<SINK, REGR>(A, T, r, A.special[i]); if (P.unique) break; }
                 continue;
             }
             unsigned long long s = gx_slot_index(key, A.sf);
             for (;;) {
                 gx_slot sl = A.slots[s];
                 if (sl.key == GX_EMPTY_KEY) break;
-                if (sl.key == key) { consume_row<SINK>(A, T, r, sl.payload); if (P.unique) break; }
+                if (sl.key == key) { consume_row<SINK, REGR>(A, T, r, sl.payload); if (P.unique) break; }
                 s = gx_next_slot(s, A.mask);
             }
         }
@@ -625,7 +718,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_agg(const __grid_constant__ gx_a
     __syncthreads();
     // merge the CTA's table into the global one
     if (SINK == SINK_SMEM) {
-        smem_dense_merge(T, A);
+        smem_dense_merge<REGR>(T, A);
     } else {
         const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
         for (int i = wid; i < T.S; i += nwarps) {              // one warp per directory slot
@@ -642,6 +735,11 @@ __global__ void __launch_bounds__(1024, 1) gx_k_agg(const __grid_constant__ gx_a
                     lp_var_merge(T, nwarps, j, A.wkind[j] >> 8, gi, lane, rec);
                     if (lane == 0 && !rec) atomicOr((unsigned long long *) &A.counters[1], 2ULL);
                     j += 2; continue;
+                }
+                if (REGR && (A.wkind[j] & 0xFF) == WK_REGR_C) {
+                    lp_regr_merge(T, nwarps, j, A.wkind[j] >> 8, gi, lane, rec);
+                    if (lane == 0 && !rec) atomicOr((unsigned long long *) &A.counters[1], 2ULL);
+                    j += 6; continue;
                 }
                 unsigned long long v = lp_reduce_word(T, nwarps, j, gi, A.wkind[j], lane);
                 if (lane == 0) { if (rec) merge_word(&rec[3 + j], A.wkind[j], v); else atomicOr((unsigned long long *) &A.counters[1], 2ULL); }
@@ -2444,7 +2542,7 @@ __global__ void __launch_bounds__(512) gx_k_radix_agg(const gx_agg_dev A, const 
             const unsigned long long *rec = recs + i * RW;
             int s = smem_upsert<false>(T, rec[1], rec[2], (unsigned int) rec[0]);
             if (s < 0) { s_over = 1; continue; }
-            merge_words(&T.w[(size_t) s * T.nwords], &rec[3], A.wkind, T.nwords);
+            merge_words<true>(&T.w[(size_t) s * T.nwords], &rec[3], A.wkind, T.nwords);
         }
         __syncthreads();
         if (s_over) { if (threadIdx.x == 0) overflowed[part] = 1; __syncthreads(); continue; }
@@ -2477,7 +2575,7 @@ __global__ void gx_k_merge_records(const gx_agg_dev A, const unsigned long long 
             const unsigned long long *rec = recs + i * RW;
             unsigned long long *g = global_upsert(A, rec[1], rec[2], (unsigned int) rec[0]);
             if (!g) { atomicOr((unsigned long long *) &A.counters[1], 2ULL); continue; }
-            merge_words(&g[3], &rec[3], A.wkind, A.P.nwords);
+            merge_words<true>(&g[3], &rec[3], A.wkind, A.P.nwords);
         }
         return;
     }
@@ -2489,7 +2587,7 @@ __global__ void gx_k_merge_records(const gx_agg_dev A, const unsigned long long 
             const unsigned long long *rec = recs + i * RW;
             unsigned long long *g = global_upsert(A, rec[1], rec[2], (unsigned int) rec[0]);
             if (!g) { atomicOr((unsigned long long *) &A.counters[1], 2ULL); continue; }
-            merge_words(&g[3], &rec[3], A.wkind, A.P.nwords);
+            merge_words<true>(&g[3], &rec[3], A.wkind, A.P.nwords);
         }
     }
 }
@@ -2515,7 +2613,7 @@ __global__ void gx_k_merge_gathered(const gx_agg_dev A, const unsigned long long
         if ((int) (h % (unsigned long long) nranks) != rank) continue;
         unsigned long long *g = global_upsert(A, rec[1], rec[2], (unsigned int) rec[0]);
         if (!g) { atomicOr((unsigned long long *) &A.counters[1], 2ULL); continue; }
-        merge_words(&g[3], &rec[3], A.wkind, A.P.nwords);
+        merge_words<true>(&g[3], &rec[3], A.wkind, A.P.nwords);
     }
 }
 __global__ void gx_k_pack_partial(const unsigned long long *recs, long long n, long long cap, int RW, unsigned long long *out)
@@ -2593,8 +2691,25 @@ struct compiled_plan {
     int gword[GX_MAX_GROUP_COLS], gshift[GX_MAX_GROUP_COLS], gbytes[GX_MAX_GROUP_COLS];
     int agg_word[GX_MAX_AGGS], agg_cnt_word[GX_MAX_AGGS], agg_var_word[GX_MAX_AGGS];
     int need_w0;
-    bool has_var;                    // some aggregate keeps a variance state: the specialised kernels do not
+    bool has_var;                    // some aggregate keeps a variance or regression state: the specialised kernels do not
 };
+
+// the same program, op by op (constants compared by their bits)
+static bool same_expr(const gx_expr &a, const gx_expr &b)
+{
+    if (a.nops != b.nops) return false;
+    for (int k = 0; k < a.nops; k++)
+        if (a.ops[k].op != b.ops[k].op || a.ops[k].col != b.ops[k].col || memcmp(&a.ops[k].k, &b.ops[k].k, sizeof(double)) != 0) return false;
+    return true;
+}
+// where GX_OP_ARG2 splits a two-argument aggregate's program into Y (ops before it) and X (ops after it); -1 when it
+// does not appear exactly once with a non-empty program on each side.  *nsep: how often it appears
+static int arg2_split(const gx_expr &e, int *nsep)
+{
+    int sep = -1; *nsep = 0;
+    for (int k = 0; k < e.nops && k < GX_MAX_EXPR_OPS; k++) if (e.ops[k].op == GX_OP_ARG2) { sep = k; (*nsep)++; }
+    return (*nsep == 1 && sep > 0 && sep < e.nops - 1 && e.nops <= GX_MAX_EXPR_OPS) ? sep : -1;
+}
 
 // LEFT is not among them: its inner-side group columns would have to turn NULL on a miss in every sink
 int gx_check_agg_join_type(gx_ctx *ctx, const gx_agg_plan *plan)
@@ -2682,6 +2797,20 @@ static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
     int nw = 1;                                     // w0 = row count
     cp->A.wkind[0] = WK_ADD_I64; cp->A.winit[0] = 0;
     P.nagg = plan->n_aggs;
+    // the two-argument aggregates: their (Y, X) programs, the same in all of them (one state per plan), the first of
+    // them owns the state; regr_count alone needs only the count of pairs
+    int regr_owner = -1; bool regr_full = false;
+    for (int a = 0; a < plan->n_aggs; a++) {
+        const gx_agg &src = plan->aggs[a];
+        if (src.fn == GX_AGG_COUNT_STAR) continue;                  // takes no argument: its program is not read
+        int nsep; const int sep = arg2_split(src.arg, &nsep);
+        if (!gx_is_regr_fn(src.fn)) { GX_CHECK_ARG(ctx, nsep == 0, "agg %d: GX_OP_ARG2 in a one-argument aggregate", a); continue; }
+        GX_CHECK_ARG(ctx, sep > 0, "agg %d: a two-argument aggregate takes Y's program, one GX_OP_ARG2 and X's program", a);
+        if (src.fn != GX_AGG_REGR_COUNT) regr_full = true;
+        if (regr_owner < 0) regr_owner = a;
+        else GX_CHECK_ARG(ctx, same_expr(src.arg, plan->aggs[regr_owner].arg),
+                          "agg %d: a second (Y, X) pair: two regression states do not fit the library's state words", a);
+    }
     for (int a = 0; a < plan->n_aggs; a++) {
         gx_dagg &g = P.aggs[a];
         const gx_agg &src = plan->aggs[a];
@@ -2696,7 +2825,7 @@ static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
             }
             cp->agg_var_word[a] = owner.var_word; cp->has_var = true;
         };
-        if (nw + (var ? 5 : 2) > GX_MAX_WORDS) { GX_SET_ERR(ctx, "agg plan: too many state words"); return GX_ERR_ARG; }
+        if (!gx_is_regr_fn(src.fn) && nw + (var ? 5 : 2) > GX_MAX_WORDS) { GX_SET_ERR(ctx, "agg plan: too many state words"); return GX_ERR_ARG; }
         switch (src.fn) {
             case GX_AGG_COUNT_STAR: g.kind = GXU_NONE; cp->agg_word[a] = 0; cp->need_w0 = 1; break;
             case GX_AGG_SUM_I8:
@@ -2756,6 +2885,35 @@ static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
                 if (var) new_var(g);
                 break;
             }
+            case GX_AGG_REGR_COUNT: case GX_AGG_REGR_SXX_F8: case GX_AGG_REGR_SYY_F8: case GX_AGG_REGR_SXY_F8:
+            case GX_AGG_REGR_AVGX_F8: case GX_AGG_REGR_AVGY_F8: case GX_AGG_REGR_R2_F8: case GX_AGG_REGR_SLOPE_F8:
+            case GX_AGG_REGR_INTERCEPT_F8: case GX_AGG_COVAR_POP_F8: case GX_AGG_COVAR_SAMP_F8: case GX_AGG_CORR_F8: {
+                // every row goes through P.regr (apply_aggs); the aggregates only read its words.  Not shared with
+                // sum(x) / avg(x): a row whose other argument is NULL is not among the pairs
+                g.kind = GXU_NONE; cp->has_var = true;
+                if (a == regr_owner) {
+                    int nsep; const int sep = arg2_split(src.arg, &nsep);
+                    gx_expr ey, ex; memset(&ey, 0, sizeof(ey)); memset(&ex, 0, sizeof(ex));
+                    ey.nops = sep; memcpy(ey.ops, src.arg.ops, (size_t) sep * sizeof(gx_expr_op));
+                    ex.nops = src.arg.nops - sep - 1; memcpy(ex.ops, &src.arg.ops[sep + 1], (size_t) ex.nops * sizeof(gx_expr_op));
+                    bool ny = false, nx = false;
+                    if (!compile_expr(ctx, outer, &ey, &P.regr.y, &ny) || !compile_expr(ctx, outer, &ex, &P.regr.x, &nx)) return GX_ERR_ARG;
+                    if (nw + ((ny || nx) ? 1 : 0) + (regr_full ? 9 : 0) > GX_MAX_WORDS) { GX_SET_ERR(ctx, "agg plan: too many state words"); return GX_ERR_ARG; }
+                    P.regr.on = 1;
+                    P.regr.cnt_word = (ny || nx) ? new_word(WK_ADD_I64, 0) : 0;
+                    if (!P.regr.cnt_word) cp->need_w0 = 1;                       // N = rows
+                    if (regr_full) {                       // {Sx, Sy, Cx, S1x, S2x, Cy, S1y, S2y, Sxy'}
+                        P.regr.word = new_word(WK_ADD_F64, (long long) GX_NEG_ZERO_BITS);
+                        new_word(WK_ADD_F64, (long long) GX_NEG_ZERO_BITS);
+                        new_word(WK_REGR_C | (P.regr.cnt_word << 8), (long long) GX_VAR_UNSET_BITS);
+                        new_word(WK_VAR_S, 0); new_word(WK_VAR_S, 0);
+                        new_word(WK_VAR_S, (long long) GX_VAR_UNSET_BITS);
+                        new_word(WK_VAR_S, 0); new_word(WK_VAR_S, 0); new_word(WK_VAR_S, 0);
+                    }
+                }
+                cp->agg_word[a] = P.regr.word; cp->agg_cnt_word[a] = P.regr.cnt_word;
+                break;
+            }
             default: GX_SET_ERR(ctx, "agg %d: unknown aggregate function %d", a, src.fn); return GX_ERR_ARG;
         }
     }
@@ -2785,12 +2943,12 @@ template <class FN> static int with_slot_format(const gx_agg_dev &A, FN fn)
     return fn(std::integral_constant<int, GX_SLOTS_WIDE>());
 }
 
-template <int SINK, int XF>
-static int launch_agg_k(gx_ctx *ctx, const gx_agg_dev &A, size_t smem, const char *name, int threads)
+template <int SINK, int XF, bool REGR>
+static int launch_agg_kr(gx_ctx *ctx, const gx_agg_dev &A, size_t smem, const char *name, int threads)
 {
     static bool attr_set = false;
     if (!attr_set) {
-        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_agg<SINK, XF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
+        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_agg<SINK, XF, REGR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
         attr_set = true;
     }
     long long nrows = A.row1 - A.row0;
@@ -2805,9 +2963,15 @@ static int launch_agg_k(gx_ctx *ctx, const gx_agg_dev &A, size_t smem, const cha
     gx_launch_scope fmt(ctx, XF == GX_SLOTS_NARROW ? "probe_agg_exist_narrow" : XF == GX_SLOTS_COMPACT ? "probe_agg_exist_compact" :
                              XF == GX_SLOTS_WIDE ? "probe_agg_exist_wide" : XF == GX_XF_CHAIN + GX_SLOTS_NARROW ? "probe_agg_chain_narrow" :
                              XF == GX_XF_CHAIN + GX_SLOTS_COMPACT ? "probe_agg_chain_compact" : XF == GX_XF_CHAIN + GX_SLOTS_WIDE ? "probe_agg_chain_wide" : nullptr, 0);
-    gx_k_agg<SINK, XF><<<grid, threads, smem, ctx->stream>>>(A);
+    gx_k_agg<SINK, XF, REGR><<<grid, threads, smem, ctx->stream>>>(A);
     GX_CUDA(ctx, cudaGetLastError());
     return GX_OK;
+}
+// a plan with a regression state takes the instantiation that updates and merges it
+template <int SINK, int XF>
+static int launch_agg_k(gx_ctx *ctx, const gx_agg_dev &A, size_t smem, const char *name, int threads)
+{
+    return A.P.regr.on ? launch_agg_kr<SINK, XF, true>(ctx, A, smem, name, threads) : launch_agg_kr<SINK, XF, false>(ctx, A, smem, name, threads);
 }
 // the kernel of the plan's join type: row by row (no join, INNER), the existence probe or the join chain in the (first)
 // table's own format
@@ -3134,6 +3298,9 @@ static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
     long long smax = 16; while (dense_bytes(smax * 2) <= budget) smax *= 2;
     int strategy = plan->strategy;
     if (strategy == 0) strategy = (est * 3 / 2 <= smax) ? 1 : 2;
+    // a regression state makes a record of 12 words or more: one per row (the radix path) is 100 B per row and more, so
+    // a plan with one whose groups outgrow the shared table but fit L2's share of the global table takes that table
+    if (plan->strategy == 0 && strategy == 2 && A.P.regr.on && est <= 65536) strategy = 3;
     GX_CHECK_ARG(ctx, strategy >= 1 && strategy <= 3, "agg plan: unknown strategy %d", strategy);
     A.need_w0 = cp.need_w0;
 
@@ -3443,7 +3610,9 @@ struct gx_group_key {
 struct gx_group_key_hash { size_t operator()(const gx_group_key &k) const { return (size_t) (k.k0 * 0x9E3779B97F4A7C15ULL ^ k.k1 * 0xC2B2AE3D27D4EB4FULL ^ k.m); } };
 
 // the float8 state words of r's aggregates that can overflow, each once (chk[i] = aggregate number, the entries of
-// one aggregate adjacent); sums_only: SUM/AVG and the variances' Sx, S1, S2
+// one aggregate adjacent); sums_only: SUM/AVG, the variances' Sx, S1, S2 and the regression words.  A regression
+// state's words are checked against the inputs of both its arguments (the verification aggregate reads every column
+// of the program): a group with a non-finite X or Y is not an overflow anywhere in its state.
 static void f8_checked_words(const gx_result *r, bool sums_only, gx_infscan_args *S, int *chk /* GX_MAX_WORDS */)
 {
     memset(S, 0, sizeof(*S));
@@ -3453,8 +3622,15 @@ static void f8_checked_words(const gx_result *r, bool sums_only, gx_infscan_args
     };
     for (int a = 0; a < r->plan.n_aggs; a++) {
         const int fn = r->plan.aggs[a].fn;
-        const bool sum = fn == GX_AGG_SUM_F8 || fn == GX_AGG_AVG_F8 || gx_is_var_fn(fn);
+        const bool sum = fn == GX_AGG_SUM_F8 || fn == GX_AGG_AVG_F8 || gx_is_var_fn(fn) || gx_is_regr_fn(fn);
         if (!sum && (sums_only || (fn != GX_AGG_MIN_F8 && fn != GX_AGG_MAX_F8))) continue;
+        if (gx_is_regr_fn(fn)) {             // Sx, Sy; S1x, S2x, S1y, S2y and the cross term
+            if (fn == GX_AGG_REGR_COUNT || !r->agg_word[a]) continue;
+            const int R = r->agg_word[a];
+            add(a, R, 0); add(a, R + 1, 0);
+            add(a, R + 3, 1); add(a, R + 4, 1); add(a, R + 6, 1); add(a, R + 7, 1); add(a, R + 8, 1);
+            continue;
+        }
         add(a, r->agg_word[a], 0);
         if (gx_is_var_fn(fn)) { add(a, r->agg_var_word[a] + 1, 1); add(a, r->agg_var_word[a] + 2, 1); }
     }
@@ -4007,6 +4183,11 @@ bool gx_result_has_variance(const gx_result *r)
     for (int a = 0; a < r->plan.n_aggs; a++) if (gx_is_var_fn(r->plan.aggs[a].fn)) return true;
     return false;
 }
+bool gx_result_has_regr(const gx_result *r)
+{
+    for (int a = 0; a < r->plan.n_aggs; a++) if (gx_is_regr_fn(r->plan.aggs[a].fn)) return true;
+    return false;
+}
 int gx_result_layout_words(gx_result *r, int *wkind, long long *winit)
 {
     if (!g_layouts || !g_layouts->count(r)) return GX_ERR_STATE;
@@ -4031,6 +4212,47 @@ __host__ __device__ __forceinline__ double var_final(int fn, const unsigned long
     double s1, s2; memcpy(&s1, &w[vw + 1], 8); memcpy(&s2, &w[vw + 2], 8);
     const double v = var_sxx(s1, s2, n) / (pop ? (double) n : (double) n - 1.0);
     return fn == GX_AGG_STDDEV_POP_F8 || fn == GX_AGG_STDDEV_SAMP_F8 ? sqrt(v) : v;
+}
+
+// float8_regr_accum's {N, Sx, Sxx, Sy, Syy, Sxy} (st[0..5]) of the regression words {Sx, Sy, Cx, S1x, S2x, Cy, S1y,
+// S2y, Sxy'} at w[R..] over n pairs: Sxx and Syy as var_sxx, Sxy = Sxy' - S1x (S1y / n).  float8_regr_accum makes Sxy
+// NaN with Sxx or Syy (a non-finite X or Y); the shifted sums need not (inf - (-inf) is +inf), so it is set here.
+// n == 0: '{0,0,0,0,0,0}'.
+__host__ __device__ __forceinline__ void regr_state(const unsigned long long *w, int R, long long n, double *st)
+{
+    double v[9];
+    memcpy(v, &w[R], sizeof(v));
+    st[0] = (double) n; st[1] = 0.0; st[2] = 0.0; st[3] = 0.0; st[4] = 0.0; st[5] = 0.0;
+    if (n == 0) return;
+    st[1] = v[0] + 0.0; st[3] = v[1] + 0.0;                   // the sums start at -0: float8pl from '{0,...}' gives +0
+    st[2] = var_sxx(v[3], v[4], n); st[4] = var_sxx(v[6], v[7], n);
+    st[5] = (isnan(st[2]) || isnan(st[4])) ? NAN : v[8] - v[3] * (v[6] / (double) n);
+}
+// the twelve finals of float.c:3386-3642 and int8.c:805 over the state of aggregate fn: is_int for regr_count
+__host__ __device__ __forceinline__ double regr_final(int fn, const unsigned long long *w, int R, long long n, bool *isnull, long long *ires)
+{
+    *isnull = false;
+    if (fn == GX_AGG_REGR_COUNT) { *ires = n; return 0.0; }
+    *isnull = fn == GX_AGG_COVAR_SAMP_F8 ? n < 2 : n < 1;
+    if (*isnull) return 0.0;
+    double st[6]; regr_state(w, R, n, st);
+    const double N = st[0], Sx = st[1], Sxx = st[2], Sy = st[3], Syy = st[4], Sxy = st[5];
+    switch (fn) {
+        case GX_AGG_REGR_SXX_F8: return Sxx;
+        case GX_AGG_REGR_SYY_F8: return Syy;
+        case GX_AGG_REGR_SXY_F8: return Sxy;
+        case GX_AGG_REGR_AVGX_F8: return Sx / N;
+        case GX_AGG_REGR_AVGY_F8: return Sy / N;
+        case GX_AGG_COVAR_POP_F8: return Sxy / N;
+        case GX_AGG_COVAR_SAMP_F8: return Sxy / (N - 1.0);
+        case GX_AGG_CORR_F8: if (Sxx == 0 || Syy == 0) { *isnull = true; return 0.0; } return Sxy / sqrt(Sxx * Syy);
+        case GX_AGG_REGR_R2_F8:
+            if (Sxx == 0) { *isnull = true; return 0.0; }
+            if (Syy == 0) return 1.0;
+            return (Sxy * Sxy) / (Sxx * Syy);
+        case GX_AGG_REGR_SLOPE_F8: if (Sxx == 0) { *isnull = true; return 0.0; } return Sxy / Sxx;
+        default: if (Sxx == 0) { *isnull = true; return 0.0; } return (Sy - Sx * Sxy / Sxx) / N;     // regr_intercept
+    }
 }
 
 // finalize_aggregates (nodeAgg.c:1363).  float8_avg = Sx / N, NULL when N == 0 (float.c:2991-3008).
@@ -4071,7 +4293,9 @@ __global__ void gx_k_finalize(const gx_final_args F)
                 case GX_AGG_AVG_F8: { const double sx = __longlong_as_double((long long) w[word]) + 0.0; if (cnt == 0) isnull = true; else res = sx / (double) cnt; break; }
                 case GX_AGG_VAR_POP_F8: case GX_AGG_VAR_SAMP_F8: case GX_AGG_STDDEV_POP_F8: case GX_AGG_STDDEV_SAMP_F8:
                     res = var_final(fn, w, F.vw[a], cnt, &isnull); break;
-                default: res = __longlong_as_double((long long) w[word]); isnull = cnt == 0; break;
+                default:
+                    if (gx_is_regr_fn(fn)) { res = regr_final(fn, w, word, cnt, &isnull, &ires); is_int = fn == GX_AGG_REGR_COUNT; break; }
+                    res = __longlong_as_double((long long) w[word]); isnull = cnt == 0; break;
             }
             if (isnull) { res = 0.0; ires = 0; }
             F.agg_out[gI * F.na + a] = is_int ? __longlong_as_double(ires) : res;
@@ -4119,7 +4343,7 @@ extern "C" int gx_result_fetch(gx_result *r, int64_t max_groups, int64_t *key_ou
         GX_CHECK_ARG(ctx, max_groups >= 1, "result_fetch: buffer too small");
         for (int a = 0; a < na; a++) {
             int fn = final_fn(r->plan.aggs[a].fn);
-            bool is_count = fn == GX_AGG_COUNT_STAR || fn == GX_AGG_COUNT;
+            bool is_count = fn == GX_AGG_COUNT_STAR || fn == GX_AGG_COUNT || fn == GX_AGG_REGR_COUNT;
             long long zero = 0; memcpy(&agg_out[a], &zero, 8);
             if (null_out) null_out[a] = is_count ? 0 : 1;
         }
@@ -4163,7 +4387,10 @@ extern "C" int gx_result_fetch(gx_result *r, int64_t max_groups, int64_t *key_ou
                 case GX_AGG_VAR_POP_F8: case GX_AGG_VAR_SAMP_F8: case GX_AGG_STDDEV_POP_F8: case GX_AGG_STDDEV_SAMP_F8: {
                     bool vn; res = var_final(fn, w, r->agg_var_word[a], cnt, &vn); isnull = vn; break;
                 }
-                default: { memcpy(&res, &w[word], 8); isnull = cnt == 0; break; }
+                default: {
+                    if (gx_is_regr_fn(fn)) { bool rn; res = regr_final(fn, w, word, cnt, &rn, &ires); isnull = rn; is_int = fn == GX_AGG_REGR_COUNT; break; }
+                    memcpy(&res, &w[word], 8); isnull = cnt == 0; break;
+                }
             }
             if (isnull) { res = 0.0; ires = 0; }
             if (is_int) memcpy(&agg_out[g * na + a], &ires, 8); else agg_out[g * na + a] = res;
@@ -4191,7 +4418,7 @@ extern "C" int gx_result_fetch_states(gx_result *r, int64_t max_groups, int64_t 
         for (int a = 0; a < na; a++) {
             const int fn = r->plan.aggs[a].fn;
             val_out[a] = 0.0; cnt_out[a] = 0;
-            if (null_out) null_out[a] = (fn == GX_AGG_COUNT_STAR || fn == GX_AGG_COUNT || fn == GX_AGG_AVG_F8 || gx_is_var_fn(fn)) ? 0 : 1;
+            if (null_out) null_out[a] = (fn == GX_AGG_COUNT_STAR || fn == GX_AGG_COUNT || fn == GX_AGG_AVG_F8 || gx_is_var_fn(fn) || gx_is_regr_fn(fn)) ? 0 : 1;
         }
         return GX_OK;
     }
@@ -4229,7 +4456,10 @@ extern "C" int gx_result_fetch_states(gx_result *r, int64_t max_groups, int64_t 
                 case GX_AGG_SUM_I4: case GX_AGG_SUM_I8: memcpy(&v, &w[word], 8); isnull = cnt == 0; break;
                 case GX_AGG_AVG_F8: case GX_AGG_VAR_POP_F8: case GX_AGG_VAR_SAMP_F8: case GX_AGG_STDDEV_POP_F8: case GX_AGG_STDDEV_SAMP_F8:
                     memcpy(&v, &w[word], 8); v += 0.0; break;    // {N, Sx}: never NULL; Sx starts at +0 ('{0,0,0}')
-                default: memcpy(&v, &w[word], 8); isnull = cnt == 0; break;      // sum / min / max: strict, NULL until the first input
+                case GX_AGG_REGR_COUNT: break;                               // int8pl's count; never NULL ('0')
+                default:
+                    if (gx_is_regr_fn(fn)) { memcpy(&v, &w[word], 8); v += 0.0; break; }   // {N, Sx}, never NULL ('{0,...}')
+                    memcpy(&v, &w[word], 8); isnull = cnt == 0; break;      // sum / min / max: strict, NULL until the first input
             }
             val_out[gI * na + a] = isnull ? 0.0 : v; cnt_out[gI * na + a] = n;
             if (null_out) null_out[gI * (ng + na) + ng + a] = isnull;
@@ -4268,6 +4498,38 @@ extern "C" int gx_result_fetch_sxx(gx_result *r, int64_t max_groups, double *sxx
                 if (n > 0) sxx = var_sxx(s1, s2, n);
             }
             sxx_out[gI * na + a] = sxx;
+        }
+    }
+    return GX_OK;
+}
+
+// float8_regr_accum's state of every regression aggregate (GX_AGG_REGR_SXX_F8 .. GX_AGG_CORR_F8), in the group order of
+// gx_result_fetch_states: out[(g * n_aggs + a) * 6 ..] = {N, Sx, Sxx, Sy, Syy, Sxy}, zeros for any other aggregate
+extern "C" int gx_result_fetch_regr(gx_result *r, int64_t max_groups, double *out)
+{
+    if (!r || !out) return GX_ERR_ARG;
+    gx_ctx *ctx = r->ctx;
+    const int na = r->plan.n_aggs, RW = r->rec_words;
+    GX_CHECK_ARG(ctx, !gx_result_has_distinct(r), "result_fetch_regr: a count(DISTINCT) result has no partial state");
+    if (gx_result_plain_empty(r)) {                                  // plain aggregate over zero rows: '{0,0,0,0,0,0}'
+        GX_CHECK_ARG(ctx, max_groups >= 1, "result_fetch_regr: buffer too small");
+        for (int i = 0; i < na * 6; i++) out[i] = 0.0;
+        return GX_OK;
+    }
+    GX_CHECK_ARG(ctx, max_groups >= r->ngroups, "result_fetch_regr: buffer holds %lld groups, result has %lld", (long long) max_groups, (long long) r->ngroups);
+    if (r->ngroups == 0) return GX_OK;
+    std::vector<unsigned long long> h((size_t) r->ngroups * RW);
+    cudaError_t e = cudaMemcpyAsync(h.data(), r->d_recs, h.size() * 8, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) { GX_SET_ERR(ctx, "result_fetch_regr: %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
+    for (int64_t gI = 0; gI < r->ngroups; gI++) {
+        const unsigned long long *w = h.data() + (size_t) gI * RW + 3;
+        for (int a = 0; a < na; a++) {
+            double *st = out + ((size_t) gI * na + a) * 6;
+            const int fn = r->plan.aggs[a].fn;
+            if (!gx_is_regr_fn(fn) || fn == GX_AGG_REGR_COUNT) { for (int i = 0; i < 6; i++) st[i] = 0.0; continue; }
+            const int cw = r->agg_cnt_word[a];
+            regr_state(w, r->agg_word[a], cw ? (long long) w[cw] : (long long) w[0], st);
         }
     }
     return GX_OK;

@@ -978,6 +978,7 @@ static int combine_run(gx_ctx *ctx, gx_result *r, gx_combine_transport &T)
     const int N = T.nranks;
     GX_CHECK_ARG(ctx, N == 1 || !gx_result_has_distinct(r), "combine: count(DISTINCT) counts do not add across %d ranks", N);
     GX_CHECK_ARG(ctx, N == 1 || !gx_result_has_variance(r), "combine: variance states are not combined across %d ranks", N);
+    GX_CHECK_ARG(ctx, N == 1 || !gx_result_has_regr(r), "combine: regression states are not combined across %d ranks", N);
     if (N == 1 || r->finalized_across) return GX_OK;
     const int RW = r->rec_words;
     long long nrec = r->ngroups;

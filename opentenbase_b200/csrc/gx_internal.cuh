@@ -162,7 +162,9 @@ static inline bool gx_result_plain_empty(const gx_result *r) { return r->plan.n_
 
 bool gx_result_has_distinct(const gx_result *r);      // some aggregate is GX_AGG_COUNT_DISTINCT: no partial states
 bool gx_result_has_variance(const gx_result *r);      // some aggregate is GX_AGG_VAR_* / GX_AGG_STDDEV_*
+bool gx_result_has_regr(const gx_result *r);          // some aggregate is GX_AGG_REGR_COUNT .. GX_AGG_CORR_F8
 static inline bool gx_is_var_fn(int fn) { return fn >= GX_AGG_VAR_POP_F8 && fn <= GX_AGG_STDDEV_SAMP_F8; }
+__host__ __device__ static inline bool gx_is_regr_fn(int fn) { return fn >= GX_AGG_REGR_COUNT && fn <= GX_AGG_CORR_F8; }
 
 #define GX_SET_ERR(ctx, ...) do { if (ctx) snprintf((ctx)->err, sizeof((ctx)->err), __VA_ARGS__); \
                                   gx_set_global_err(__VA_ARGS__); } while (0)
@@ -230,6 +232,11 @@ struct gx_dagg {
     gx_dcol icol;      // ... or integer argument column
 };
 
+// The state every two-argument aggregate of a plan shares (one (Y, X) pair per plan): a row whose y and x are both
+// non-NULL adds +1 to cnt_word (0: w0 counts the rows) and, when word != 0, updates the nine words from `word` on:
+// {Sx, Sy, Cx, S1x, S2x, Cy, S1y, S2y, Sxy'} (gx_agg.cu, WK_REGR_C).  on == 0: the plan has no such aggregate.
+struct gx_dregr { int on, word, cnt_word, _pad; gx_dexpr y, x; };
+
 struct gx_dgroupcol { int side; int type; gx_dcol col; int payload_idx; int word; int shift; int bytes; int _pad; };
 
 struct gx_dplan {
@@ -241,6 +248,7 @@ struct gx_dplan {
     gx_dagg aggs[GX_MAX_AGGS];
     int payload_types[GX_MAX_PAYLOAD];
     int n_payload; int join_type;       // GX_JOIN_INNER / _SEMI / _ANTI
+    gx_dregr regr;                      // the plan's one (Y, X) pair of the two-argument aggregates
 };
 
 #ifdef __CUDACC__

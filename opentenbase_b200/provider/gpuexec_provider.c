@@ -152,6 +152,7 @@ typedef struct GpuExecState
 	double	   *aggs;
 	int64	   *cnts;			/* partial mode: N of every transition state */
 	double	   *sxx;			/* partial mode: Sxx of every variance state */
+	double	   *regr;			/* partial mode: float8_regr_accum's six values of every regression state */
 	uint8	   *nulls;
 	double		load_ms,
 				exec_ms;
@@ -658,6 +659,8 @@ gpuexec_begin(CustomScanState *node, EState *estate, int eflags)
 
 static bool is_variance_fn(int fn);
 static bool plan_has_variance(const gx_agg_plan *plan);
+static bool is_regr_fn(int fn);
+static bool plan_has_regr(const gx_agg_plan *plan);
 
 static void
 gpuexec_run(GpuExecState *st, EState *estate)
@@ -721,6 +724,11 @@ gpuexec_run(GpuExecState *st, EState *estate)
 			st->sxx = (double *) palloc(sizeof(double) * Max(n * na, 1));
 			GX_CHECK(gx_result_fetch_sxx(st->result, n, st->sxx));
 		}
+		if (plan_has_regr(&st->plan))
+		{
+			st->regr = (double *) palloc(sizeof(double) * 6 * Max(n * na, 1));
+			GX_CHECK(gx_result_fetch_regr(st->result, n, st->regr));
+		}
 	}
 	else
 		GX_CHECK(gx_result_fetch(st->result, n, st->keys, st->aggs, st->nulls));
@@ -741,7 +749,8 @@ gpuexec_run(GpuExecState *st, EState *estate)
  * nodeCustom.c:100-101) below.  In partial mode an aggregate column carries the transition
  * value the reference's combine function expects (pg_aggregate.h:178-252): int8 for
  * count/sum(int4), float8 for sum/min/max(float8), float8[3] {N, Sx, Sxx} for avg(float8) and the
- * variances and standard deviations of float8. */
+ * variances and standard deviations of float8, float8[6] {N, Sx, Sxx, Sy, Syy, Sxy} for the regression aggregates
+ * (float8_regr_combine, float.c:3244) and int8 for regr_count (int8pl). */
 static TupleTableSlot *
 gpuexec_exec(CustomScanState *node)
 {
@@ -827,7 +836,18 @@ gpuexec_exec(CustomScanState *node)
 				slot->tts_values[i] = PointerGetDatum(construct_array(elems, 3, FLOAT8OID, sizeof(float8), FLOAT8PASSBYVAL, 'd'));
 				MemoryContextSwitchTo(old);
 			}
-			else if (st->partial && (fn == GX_AGG_COUNT_STAR || fn == GX_AGG_COUNT))
+			else if (st->partial && is_regr_fn(fn) && fn != GX_AGG_REGR_COUNT)
+			{
+				MemoryContext old = MemoryContextSwitchTo(econtext->ecxt_per_tuple_memory);
+				Datum		elems[6];
+				int			k;
+
+				for (k = 0; k < 6; k++)
+					elems[k] = Float8GetDatum(st->regr[(g * na + a) * 6 + k]);
+				slot->tts_values[i] = PointerGetDatum(construct_array(elems, 6, FLOAT8OID, sizeof(float8), FLOAT8PASSBYVAL, 'd'));
+				MemoryContextSwitchTo(old);
+			}
+			else if (st->partial && (fn == GX_AGG_COUNT_STAR || fn == GX_AGG_COUNT || fn == GX_AGG_REGR_COUNT))
 				slot->tts_values[i] = Int64GetDatum(st->cnts[g * na + a]);
 			else if (typid == INT8OID)
 			{
@@ -982,6 +1002,9 @@ gpuexec_plan_path(PlannerInfo *root, RelOptInfo *rel, CustomPath *best_path,
 #define AGG_STDDEV_POP_F8  2728
 #define AGG_STDDEV_SAMP_F8 2716
 #define AGG_STDDEV_F8      2158
+/* the SQL:2003 binary aggregates over (float8, float8), pg_aggregate.h:305-316: aggfnoid - AGG_REGR_COUNT + GX_AGG_REGR_COUNT */
+#define AGG_REGR_COUNT     2818
+#define AGG_CORR           2829
 
 /* column number of (rti, attno) in the descriptor, appended on first use */
 static int
@@ -1018,6 +1041,23 @@ plan_has_variance(const gx_agg_plan *plan)
 
 	for (a = 0; a < plan->n_aggs; a++)
 		if (is_variance_fn(plan->aggs[a].fn))
+			return true;
+	return false;
+}
+
+static bool
+is_regr_fn(int fn)
+{
+	return fn >= GX_AGG_REGR_COUNT && fn <= GX_AGG_CORR_F8;
+}
+
+static bool
+plan_has_regr(const gx_agg_plan *plan)
+{
+	int			a;
+
+	for (a = 0; a < plan->n_aggs; a++)
+		if (is_regr_fn(plan->aggs[a].fn))
 			return true;
 	return false;
 }
@@ -1288,11 +1328,26 @@ static bool
 state_words_fit(PlannerInfo *root, const GpuRelInfo *outer, const gx_agg_plan *plan)
 {
 	bool		var_words[GX_MAX_AGGS] = {false};
-	bool		distinct = false;
+	bool		distinct = false,
+				regr_full = false;
 	int			nw = 1,
+				regr_owner = -1,
 				a,
 				b,
 				k;
+
+	/* the two-argument aggregates share one state, over one (Y, X) pair: a second pair is declined */
+	for (a = 0; a < plan->n_aggs; a++)
+	{
+		if (!is_regr_fn(plan->aggs[a].fn))
+			continue;
+		if (plan->aggs[a].fn != GX_AGG_REGR_COUNT)
+			regr_full = true;
+		if (regr_owner < 0)
+			regr_owner = a;
+		else if (!same_f8_expr(&plan->aggs[a].arg, &plan->aggs[regr_owner].arg))
+			return false;
+	}
 
 	for (a = 0; a < plan->n_aggs; a++)
 	{
@@ -1301,7 +1356,7 @@ state_words_fit(PlannerInfo *root, const GpuRelInfo *outer, const gx_agg_plan *p
 					nullable = false;
 		int			twin = -1;
 
-		if (g->fn != GX_AGG_COUNT_DISTINCT && nw + (var ? 5 : 2) > GPUEXEC_MAX_STATE_WORDS)
+		if (g->fn != GX_AGG_COUNT_DISTINCT && !is_regr_fn(g->fn) && nw + (var ? 5 : 2) > GPUEXEC_MAX_STATE_WORDS)
 			return false;
 		for (k = 0; k < g->arg.nops; k++)
 			if (g->arg.ops[k].op == GX_OP_COL && !column_is_not_null(root, outer->rti, outer->attnums[g->arg.ops[k].col] + 1))
@@ -1312,6 +1367,26 @@ state_words_fit(PlannerInfo *root, const GpuRelInfo *outer, const gx_agg_plan *p
 				break;
 			case GX_AGG_COUNT_DISTINCT:
 				distinct = true;
+				break;
+			case GX_AGG_REGR_COUNT:
+			case GX_AGG_REGR_SXX_F8:
+			case GX_AGG_REGR_SYY_F8:
+			case GX_AGG_REGR_SXY_F8:
+			case GX_AGG_REGR_AVGX_F8:
+			case GX_AGG_REGR_AVGY_F8:
+			case GX_AGG_REGR_R2_F8:
+			case GX_AGG_REGR_SLOPE_F8:
+			case GX_AGG_REGR_INTERCEPT_F8:
+			case GX_AGG_COVAR_POP_F8:
+			case GX_AGG_COVAR_SAMP_F8:
+			case GX_AGG_CORR_F8:
+				/* the first of them owns the pair count (when a side is nullable) and, unless all are regr_count,
+				 * {Sx, Sy, Cx, S1x, S2x, Cy, S1y, S2y, Sxy'}; never shared with sum / avg */
+				if (a != regr_owner)
+					break;
+				nw += (nullable ? 1 : 0) + (regr_full ? 9 : 0);
+				if (nw > GPUEXEC_MAX_STATE_WORDS)
+					return false;
 				break;
 			case GX_AGG_COUNT:
 				nw += nullable ? 1 : 0;
@@ -1685,9 +1760,23 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 				g->fn = GX_AGG_STDDEV_SAMP_F8;
 				break;
 			default:
+				if (a->aggfnoid < AGG_REGR_COUNT || a->aggfnoid > AGG_CORR)
+					return false;
+				break;
+		}
+		if (a->aggfnoid >= AGG_REGR_COUNT && a->aggfnoid <= AGG_CORR)
+		{
+			/* regr_* / covar_* / corr (Y, X): Y's program, GX_OP_ARG2, X's program, within GX_MAX_EXPR_OPS */
+			g->fn = GX_AGG_REGR_COUNT + (int) (a->aggfnoid - AGG_REGR_COUNT);
+			if (list_length(a->args) != 2 ||
+				!match_f8_expr((Node *) ((TargetEntry *) linitial(a->args))->expr, &out->outer, &g->arg) ||
+				g->arg.nops >= GX_MAX_EXPR_OPS)
+				return false;
+			g->arg.ops[g->arg.nops++].op = GX_OP_ARG2;
+			if (!match_f8_expr((Node *) ((TargetEntry *) lsecond(a->args))->expr, &out->outer, &g->arg))
 				return false;
 		}
-		if (g->fn != GX_AGG_COUNT_STAR)
+		else if (g->fn != GX_AGG_COUNT_STAR)
 		{
 			TargetEntry *arg;
 
@@ -1704,7 +1793,7 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 	}
 	if (plan->n_aggs == 0 && plan->n_group_cols == 0)
 		return false;
-	if (plan_has_variance(plan) && !state_words_fit(root, &out->outer, plan))
+	if ((plan_has_variance(plan) || plan_has_regr(plan)) && !state_words_fit(root, &out->outer, plan))
 		return false;
 	*est_rows = in->rows;
 	*est_groups = output_rel->rows > 0 ? output_rel->rows : 1;

@@ -21,7 +21,7 @@
 struct gx_ctx { int dummy; };
 struct gx_table { int ncols; int32_t types[GX_MAX_COLS]; int64_t pages, rows, batches, est_rows; int finished; };
 struct gx_hash { int key_col, n_payload, unique, n_preds; };
-struct gx_result { int64_t ngroups; int ng, na; int64_t *keys; double *aggs; int64_t *cnts; uint8_t *nulls; double *sxx; };
+struct gx_result { int64_t ngroups; int ng, na; int64_t *keys; double *aggs; int64_t *cnts; uint8_t *nulls; double *sxx, *regr; };
 
 static char last_error[256] = "";
 static void *stage[2];
@@ -128,7 +128,7 @@ int gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col, int n_preds, 
 void gx_hash_free(gx_hash *h) { if (h) { live_hashes--; free(h); } }
 
 /* file: int64 ngroups, int32 ng, int32 na, keys[ngroups*ng] int64, aggs[ngroups*na] double, cnts[ngroups*na] int64, nulls[ngroups*(ng+na)],
- * then optionally sxx[ngroups*na] double (zeros when absent) */
+ * then optionally sxx[ngroups*na] double and regr[ngroups*na*6] double (zeros when absent) */
 int gx_hash_agg(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, gx_result **out)
 {
 	const char *path = getenv("GX_DOUBLE_RESULT");
@@ -149,9 +149,11 @@ int gx_hash_agg(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_a
 	r->cnts = (int64_t *) calloc((size_t) r->ngroups * na + 1, 8);
 	r->nulls = (uint8_t *) calloc((size_t) r->ngroups * (ng + na) + 1, 1);
 	r->sxx = (double *) calloc((size_t) r->ngroups * na + 1, 8);
+	r->regr = (double *) calloc((size_t) r->ngroups * na * 6 + 1, 8);
 	n = fread(r->keys, 8, (size_t) r->ngroups * ng, f); n = fread(r->aggs, 8, (size_t) r->ngroups * na, f);
 	n = fread(r->cnts, 8, (size_t) r->ngroups * na, f); n = fread(r->nulls, 1, (size_t) r->ngroups * (ng + na), f);
 	n = fread(r->sxx, 8, (size_t) r->ngroups * na, f);
+	n = fread(r->regr, 8, (size_t) r->ngroups * na * 6, f);
 	fclose(f);
 	fprintf(stderr, "double: hash_agg outer rows %lld join %d groups %d aggs %d preds %d outer_key %d est_groups %lld\n", (long long) outer->rows, h != NULL,
 			plan->n_group_cols, plan->n_aggs, plan->n_preds, plan->outer_key_col, (long long) plan->est_groups);
@@ -198,9 +200,15 @@ int gx_result_fetch_sxx(gx_result *r, int64_t max_groups, double *sxx_out)
 	fprintf(stderr, "double: result_fetch_sxx\n");
 	return GX_OK;
 }
+int gx_result_fetch_regr(gx_result *r, int64_t max_groups, double *out)
+{
+	memcpy(out, r->regr, (size_t) r->ngroups * r->na * 6 * 8);
+	fprintf(stderr, "double: result_fetch_regr\n");
+	return GX_OK;
+}
 void gx_result_free(gx_result *r)
 {
 	if (!r) return;
 	live_results--;
-	free(r->keys); free(r->aggs); free(r->cnts); free(r->nulls); free(r->sxx); free(r);
+	free(r->keys); free(r->aggs); free(r->cnts); free(r->nulls); free(r->sxx); free(r->regr); free(r);
 }

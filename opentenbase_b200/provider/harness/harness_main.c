@@ -568,11 +568,24 @@ static int plan_main(const char *path)
 				{"stddev_pop_f8", 2728, FLOAT8OID, FLOAT8ARRAYOID}, {"variance_f8", 2152, FLOAT8OID, FLOAT8ARRAYOID},
 				{"var_samp_f8", 2645, FLOAT8OID, FLOAT8ARRAYOID}, {"var_pop_f8", 2722, FLOAT8OID, FLOAT8ARRAYOID},
 				{"stddev_f4", 2157, FLOAT8OID, FLOAT8ARRAYOID}, {"stddev_i8", 2154, NUMERICOID, INTERNALOID},
+				{"regr_count", 2818, INT8OID, INT8OID}, {"regr_sxx", 2819, FLOAT8OID, FLOAT8ARRAYOID}, {"regr_syy", 2820, FLOAT8OID, FLOAT8ARRAYOID},
+				{"regr_sxy", 2821, FLOAT8OID, FLOAT8ARRAYOID}, {"regr_avgx", 2822, FLOAT8OID, FLOAT8ARRAYOID}, {"regr_avgy", 2823, FLOAT8OID, FLOAT8ARRAYOID},
+				{"regr_r2", 2824, FLOAT8OID, FLOAT8ARRAYOID}, {"regr_slope", 2825, FLOAT8OID, FLOAT8ARRAYOID}, {"regr_intercept", 2826, FLOAT8OID, FLOAT8ARRAYOID},
+				{"covar_pop", 2827, FLOAT8OID, FLOAT8ARRAYOID}, {"covar_samp", 2828, FLOAT8OID, FLOAT8ARRAYOID}, {"corr", 2829, FLOAT8OID, FLOAT8ARRAYOID},
 			};
 
 			for (i = 0; i < (int) lengthof(tab); i++) if (!strcmp(tab[i].n, w)) break;
 			if (i == (int) lengthof(tab)) { fprintf(stderr, "harness: aggregate %s\n", w); return 2; }
 			ag->aggfnoid = tab[i].fn; ag->aggtype = tab[i].ty; ag->aggtranstype = tab[i].tr; ag->aggsplit = AGGSPLIT_SIMPLE; ag->aggkind = 'n';
+			{
+				/* "... filter" / "... order" after the arguments: a FILTER clause or an ORDER BY inside the call */
+				char	   *kf = strstr(line + n, " filter"), *ko = strstr(line + n, " order");
+
+				if (kf) ag->aggfilter = (Expr *) plan_const(INT4OID, "1");
+				if (ko) ag->aggorder = list_make1(makeNode(SortGroupClause));
+				if (kf) *kf = '\0';
+				if (ko) *ko = '\0';
+			}
 			if (strstr(line + n, "distinct"))
 			{
 				/* "target agg count v1.2 distinct": the argument, and one sort clause over it (parse_agg.c transformAggregateCall) */
@@ -580,6 +593,17 @@ static int plan_main(const char *path)
 				ag->aggdistinct = list_make1(makeNode(SortGroupClause));
 			}
 			if (tab[i].fn == 2803) ag->aggstar = true;
+			else if (strstr(line + n, " , "))
+			{
+				/* "target agg corr Y , X": the two arguments of a binary aggregate, Y first */
+				char	   *x = strstr(line + n, " , ");
+				Node	   *ey, *ex;
+
+				*x = '\0';
+				ey = plan_expr(line + n); ex = plan_expr(x + 3);
+				if (!ey || !ex) { fprintf(stderr, "harness: bad expression\n"); return 2; }
+				ag->args = list_make2(makeTargetEntry((Expr *) ey, 1, NULL, false), makeTargetEntry((Expr *) ex, 2, NULL, false));
+			}
 			else { Node *e = plan_expr(line + n); if (!e) { fprintf(stderr, "harness: bad expression\n"); return 2; } ag->args = list_make1(makeTargetEntry((Expr *) e, 1, NULL, false)); }
 			parse->targetList = lappend(parse->targetList, makeTargetEntry((Expr *) ag, list_length(parse->targetList) + 1, NULL, false));
 		}
@@ -817,8 +841,11 @@ int main(int argc, char **argv)
 					{
 						ArrayType  *a = (ArrayType *) DatumGetPointer(res->tts_values[i]);
 						double	   *v = (double *) ARR_DATA_PTR(a);
+						int			k;
 
-						printf("{%.17g,%.17g,%.17g}", v[0], v[1], v[2]);
+						for (k = 0; k < ARR_DIMS(a)[0]; k++)
+							printf("%c%.17g", k ? ',' : '{', v[k]);
+						putchar('}');
 						break;
 					}
 				default: printf("%d", DatumGetInt32(res->tts_values[i])); break;
