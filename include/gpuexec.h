@@ -525,6 +525,15 @@ int  gx_debug_hash(gx_ctx *ctx, int which, const int64_t *host_in, int64_t n,
  * GX_ERR_ARG, the context staying usable: the plans or record layouts of the parts differ, a part was combined
  * already, or rank is out of range. */
 int  gx_debug_combine(gx_ctx *ctx, int nparts, gx_result *const *parts, int rank);
+/* gx_redistribute of rank `rank` of nparts, on one GPU: parts[p] is the input table of datanode p (same column
+ * count and types).  window_bytes > 0 runs the peer-window path with windows of that size per rank, 0 the NCCL
+ * path.  The context's shard map must cover nparts nodes.  *out receives the rows rank `rank` would receive;
+ * *path_out (may be NULL) = 0 peer windows, 1 NCCL path with one-pass regions, 2 NCCL path with the two-pass
+ * partition (this rank's own part).  GX_ERR_ARG, the context staying usable: nparts outside 1..GX_MAX_NODES,
+ * rank out of range, parts whose column count or types differ, a key column out of range or not INT4/INT8/DATE,
+ * a shard map for another node count, window_bytes * nparts above 4 GiB. */
+int  gx_debug_redistribute(gx_ctx *ctx, int nparts, const gx_table *const *parts, int key_col, int rank,
+                           size_t window_bytes, gx_table **out, int *path_out);
 
 #ifdef __cplusplus
 }

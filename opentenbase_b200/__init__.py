@@ -197,6 +197,7 @@ def _declare(L):
         "gx_partition_by_node": (C.c_int, [vp, vp, C.c_int, pp, vp]),
         "gx_debug_hash": (C.c_int, [vp, C.c_int, vp, i64, vp]),
         "gx_debug_combine": (C.c_int, [vp, C.c_int, pp, C.c_int]),
+        "gx_debug_redistribute": (C.c_int, [vp, C.c_int, pp, C.c_int, C.c_int, sz, pp, C.POINTER(C.c_int)]),
     }
     for name, (res, args) in sig.items():
         f = getattr(L, name)
@@ -655,6 +656,15 @@ class Context:
         arr = (C.c_void_p * max(len(parts), 1))(*[p.h for p in parts])
         self._chk(lib().gx_debug_combine(self.h, len(parts), arr, rank))
         return parts[rank]
+
+    def debug_redistribute(self, parts, key_col, rank, window_bytes=0):
+        """gx_debug_redistribute: the rows rank `rank` of len(parts) datanodes would receive from gx_redistribute, the
+        parts standing for the datanodes' input tables; window_bytes > 0 takes the peer-window path with windows of
+        that size, 0 the NCCL path.  Returns (Table, path): 0 peer windows, 1 one-pass regions, 2 two-pass partition."""
+        arr = (C.c_void_p * max(len(parts), 1))(*[p.h for p in parts])
+        h, path = C.c_void_p(), C.c_int(-1)
+        self._chk(lib().gx_debug_redistribute(self.h, len(parts), arr, key_col, rank, window_bytes, C.byref(h), C.byref(path)))
+        return Table(self, h, parts[rank].types), path.value
 
 
 def _exec_host(self, outer_types, outer_ptrs, outer_nrows, plan, inner_types=None, inner_ptrs=None, inner_nrows=0,

@@ -683,31 +683,41 @@ __global__ void __launch_bounds__(256) gx_k_peer_gather(const __grid_constant__ 
     }
 }
 
-// Returns GX_OK with *done = 1 and *out set when the rows travelled through the windows; *done = 0 when the ranks
-// agreed (through the headers) that this call must take the NCCL path.
-static int redistribute_peer(gx_ctx *ctx, const gx_table *in, int key_col, gx_table **out, int *done)
+// What the redistribute of table rows exchanges between ranks.  redistribute_run makes every decision and runs every
+// device step; a transport only moves bytes and headers: through the peer windows and NCCL between processes, or in
+// one process on one GPU, where it builds from the input tables of all ranks what the other ranks would have delivered
+// to one of them (gx_debug_redistribute).
+struct gx_redist_transport {
+    int rank, nranks;
+    size_t window_bytes;            // window of every rank; 0: no peer windows, every call takes the NCCL path
+    // dst[d] = this rank's region in the window of rank d, once the rows of the previous call have left it
+    virtual int window_open(gx_ctx *ctx, long long region_stride, char **dst) = 0;
+    // after this rank's rows are in the windows (d_cur: its cursor, see peer_route): the header of every source s of
+    // this rank's window, hdr[s * 3 + {0, 1, 2}] = {rows (PEER_FALLBACK: s cannot use the windows), cap, nullbits};
+    // *win = this rank's window, region s at s * region_stride
+    virtual int window_headers(gx_ctx *ctx, const unsigned long long *d_cur, int feasible, long long cap, unsigned long long nullbits,
+                               unsigned long long *hdr, const char **win) = 0;
+    // nothing more of this call is read from this rank's window
+    virtual void window_release(gx_ctx *ctx) = 0;
+    // all[p * n + i] = word i of rank p's `mine`
+    virtual int gather_counts(gx_ctx *ctx, const int64_t *mine, int n, int64_t *all) = 0;
+    // the bytes of column c (want_null: its NULL bytes) every rank addressed to this one, rank p's at ro[p] of recvbuf;
+    // sendbuf, so and sc are this rank's
+    virtual int exchange_column(gx_ctx *ctx, int c, int want_null, const char *sendbuf, const int64_t *so, const int64_t *sc,
+                                char *recvbuf, const int64_t *ro, const int64_t *rcn) = 0;
+};
+
+// One rank's rows into its regions of the N destinations' windows (dst[d]).  d_cur[GX_MAX_NODES + 1], zeroed by the
+// caller, receives the rows per destination and the overflow flag.  The rank chooses the layout of its regions itself
+// (*cap, *nullbits); *feasible = 0 when a region of that layout does not fit region_stride, and nothing is routed.
+static int peer_route(gx_ctx *ctx, const gx_table *in, int key_col, int N, long long region_stride, char *const *dst,
+                      unsigned long long *d_cur, long long *cap_out, unsigned long long *nullbits_out, int *feasible_out)
 {
-    *done = 0;
-    const int N = ctx->nranks, kt = in->types[key_col];
-    GX_CHECK_ARG(ctx, kt == GX_INT4 || kt == GX_INT8 || kt == GX_DATE, "route: distribution column type %d not supported (int4/int8/date)", kt);
-    const unsigned long long epoch = ++ctx->peer_epoch;
-    const char *tmo = getenv("GX_PEER_TIMEOUT_MS");
-    const unsigned long long timeout_ns = (unsigned long long) (tmo ? atoll(tmo) : 60000) * 1000000ULL;
-    gx_peer_ptrs P; memset(&P, 0, sizeof(P));
-    for (int p = 0; p < N; p++) P.base[p] = ctx->peer_base[p];
-    char *own = ctx->peer_base[ctx->rank];
-    const long long region_stride = (long long) (ctx->peer_win_bytes / N) & ~255LL;
+    const int kt = in->types[key_col];
     int sizes[GX_MAX_COLS]; unsigned long long nullbits = 0;
     for (int c = 0; c < in->ncols; c++) { sizes[c] = gx_type_size(in->types[c]); if (in->nulls[c]) nullbits |= 1ULL << c; }
     const long long cap = in->nrows / N + in->nrows / (4 * N) + 4096;
     const int feasible = peer_layout(cap, in->ncols, sizes, nullbits, in->ncols, 0) <= region_stride;
-
-    unsigned long long *d_cur; int *d_flag; unsigned long long *d_hdr;
-    GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d_cur, (GX_MAX_NODES + 2) * 8 + (size_t) GX_MAX_NODES * 3 * 8));
-    GX_CUDA(ctx, cudaMemsetAsync(d_cur, 0, (GX_MAX_NODES + 2) * 8, ctx->stream));
-    d_flag = (int *) (d_cur + GX_MAX_NODES + 1); d_hdr = d_cur + GX_MAX_NODES + 2;
-    // the regions this rank owns in the peers' windows must have been emptied (previous call)
-    { gx_launch_scope ls(ctx, "peer_wait_ack"); gx_k_peer_wait<<<1, GX_MAX_NODES, 0, ctx->stream>>>(PEER_ACK(own, 0), 1, N, epoch - 1, timeout_ns, d_flag, nullptr); }
     if (feasible && in->nrows > 0) {
         gx_peer_route_args a; memset(&a, 0, sizeof(a));
         a.key.data = in->cols[key_col]; a.key.nulls = in->nulls[key_col]; a.key.type = kt;
@@ -717,47 +727,59 @@ static int redistribute_peer(gx_ctx *ctx, const gx_table *in, int key_col, gx_ta
             a.coff[c] = peer_layout(cap, in->ncols, sizes, nullbits, c, 0);
             a.noff[c] = in->nulls[c] ? peer_layout(cap, in->ncols, sizes, nullbits, c, 1) : -1;
         }
-        for (int p = 0; p < N; p++) a.dst[p] = ctx->peer_base[p] + PEER_CTL_BYTES + (long long) ctx->rank * region_stride;
+        for (int p = 0; p < N; p++) a.dst[p] = dst[p];
         const long long tiles = (in->nrows + PR_THREADS * PR_K - 1) / (PR_THREADS * PR_K), maxb = (long long) ctx->sm_count * 8;
         gx_launch_scope ls(ctx, "peer_scatter");
         gx_k_route_peer<<<(unsigned) (tiles < maxb ? tiles : maxb), PR_THREADS, 0, ctx->stream>>>(a);
     }
-    { gx_launch_scope ls(ctx, "peer_publish"); gx_k_peer_publish<<<1, GX_MAX_NODES, 0, ctx->stream>>>(P, N, ctx->rank, epoch, d_cur, feasible, (unsigned long long) cap, nullbits); }
-    { gx_launch_scope ls(ctx, "peer_wait"); gx_k_peer_wait<<<1, GX_MAX_NODES, 0, ctx->stream>>>(PEER_HDR(own, 0), 4, N, epoch, timeout_ns, d_flag, d_hdr); }
-    unsigned long long h_hdr[GX_MAX_NODES * 3]; int h_flag = 0;
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(h_hdr, d_hdr, (size_t) N * 3 * 8, cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&h_flag, d_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    *cap_out = cap; *nullbits_out = nullbits; *feasible_out = feasible;
+    return GX_OK;
+}
+
+// Returns GX_OK with *done = 1 and *out set when the rows travelled through the windows; *done = 0 when the ranks
+// agreed (through the headers) that this call must take the NCCL path.
+static int redistribute_peer(gx_ctx *ctx, const gx_table *in, int key_col, gx_redist_transport &T, gx_table **out, int *done)
+{
+    *done = 0;
+    const int N = T.nranks;
+    const long long region_stride = (long long) (T.window_bytes / N) & ~255LL;
+    char *dst[GX_MAX_NODES];
+    int rc = T.window_open(ctx, region_stride, dst); if (rc) return rc;
+    unsigned long long *d_cur;
+    GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d_cur, (GX_MAX_NODES + 1) * 8));
+    GX_CUDA(ctx, cudaMemsetAsync(d_cur, 0, (GX_MAX_NODES + 1) * 8, ctx->stream));
+    long long cap = 0; unsigned long long nullbits = 0; int feasible = 0;
+    rc = peer_route(ctx, in, key_col, N, region_stride, dst, d_cur, &cap, &nullbits, &feasible);
+    unsigned long long h_hdr[GX_MAX_NODES * 3]; const char *win = nullptr;
+    if (rc == GX_OK) rc = T.window_headers(ctx, d_cur, feasible, cap, nullbits, h_hdr, &win);
     gx_tmp_free(ctx, d_cur);
-    if (e != cudaSuccess) { GX_SET_ERR(ctx, "redistribute (peer windows): %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
-    if (h_flag) { GX_SET_ERR(ctx, "redistribute (peer windows): rank %d waited %llu ms for its peers", ctx->rank, timeout_ns / 1000000ULL); return GX_ERR_NCCL; }
+    if (rc) return rc;
     bool fallback = false; long long total = 0; unsigned long long anynull = 0;
     for (int s = 0; s < N; s++) {
         if (h_hdr[s * 3] == PEER_FALLBACK) fallback = true; else total += (long long) h_hdr[s * 3];
         anynull |= h_hdr[s * 3 + 2];
     }
     if (fallback) {
-        // nothing of this epoch will be read from the windows: release them and let the caller take the NCCL path
-        gx_launch_scope ls(ctx, "peer_ack"); gx_k_peer_ack<<<1, GX_MAX_NODES, 0, ctx->stream>>>(P, N, ctx->rank, epoch);
+        // nothing of this call will be read from the windows: release them and let the caller take the NCCL path
+        T.window_release(ctx);
         return GX_OK;
     }
     bool hn[GX_MAX_COLS];
     for (int c = 0; c < in->ncols; c++) hn[c] = (anynull >> c) & 1ULL;
     gx_table *t;
-    int rc = gx_table_alloc_like(ctx, in->ncols, in->types, hn, total, &t);
+    rc = gx_table_alloc_like(ctx, in->ncols, in->types, hn, total, &t);
     if (rc == GX_OK && total > 0) {
         gx_peer_gather_args g; memset(&g, 0, sizeof(g));
-        g.nnodes = N; g.ncols = in->ncols; g.win = own + PEER_CTL_BYTES; g.region_stride = region_stride;
+        g.nnodes = N; g.ncols = in->ncols; g.win = win; g.region_stride = region_stride;
         long long most = 0;
         for (int s = 0; s < N; s++) { g.count[s] = (long long) h_hdr[s * 3]; g.cap[s] = (long long) h_hdr[s * 3 + 1]; g.nullbits[s] = h_hdr[s * 3 + 2]; if (g.count[s] > most) most = g.count[s]; }
-        for (int c = 0; c < in->ncols; c++) { g.sizes[c] = sizes[c]; g.out[c] = t->cols[c]; g.out_nulls[c] = t->nulls[c]; }
+        for (int c = 0; c < in->ncols; c++) { g.sizes[c] = gx_type_size(in->types[c]); g.out[c] = t->cols[c]; g.out_nulls[c] = t->nulls[c]; }
         long long bx = (most + 256 * 8 - 1) / (256 * 8); if (bx < 1) bx = 1; if (bx > ctx->sm_count * 2) bx = ctx->sm_count * 2;
         gx_launch_scope ls(ctx, "peer_gather");
         gx_k_peer_gather<<<dim3((unsigned) bx, (unsigned) N, (unsigned) (anynull ? 2 * in->ncols : in->ncols)), 256, 0, ctx->stream>>>(g);
     }
-    // the ack goes out even when the allocation failed: the peers must not wait for this rank
-    { gx_launch_scope ls(ctx, "peer_ack"); gx_k_peer_ack<<<1, GX_MAX_NODES, 0, ctx->stream>>>(P, N, ctx->rank, epoch); }
+    // the release goes out even when the allocation failed: the peers must not wait for this rank
+    T.window_release(ctx);
     if (rc) return rc;
     GX_CUDA(ctx, cudaGetLastError());
     t->nrows = total;
@@ -765,36 +787,68 @@ static int redistribute_peer(gx_ctx *ctx, const gx_table *in, int key_col, gx_ta
     return GX_OK;
 }
 
-extern "C" int gx_redistribute(gx_ctx *ctx, const gx_table *in, int key_col, gx_table **out)
+// One rank's rows partitioned by destination for the NCCL path: the one-pass regions of `cap` rows per destination, or
+// (GX_PARTITION_TWO_PASS=1, or a region overflowed) the exact two-pass form, densely packed.  counts[N] tells which
+// columns have a NULL array, so that every rank agrees on the columns of the result.
+struct gx_redist_part {
+    gx_table *t;
+    int64_t counts[GX_MAX_NODES + 1], sendoff[GX_MAX_NODES];
+    int path;                       // 1 one-pass regions, 2 two-pass
+};
+static int redist_partition(gx_ctx *ctx, const gx_table *in, int key_col, int N, gx_redist_part *s)
 {
-    if (!ctx || !in || !out) return GX_ERR_ARG;
-    const int N = ctx->nranks;
-    GX_CHECK_ARG(ctx, ctx->nnodes == N, "redistribute: shard map covers %d nodes but the communicator has %d ranks", ctx->nnodes, N);
-    int64_t counts[GX_MAX_NODES + 1];
-    gx_table *part = nullptr;
-    long long cap = 0; int overflowed = 0;
     const char *two = getenv("GX_PARTITION_TWO_PASS");
-    int rc = GX_OK;
-    if (N > 1 && ctx->comm && ctx->peer_ready == 1) {
-        GX_CHECK_ARG(ctx, key_col >= 0 && key_col < in->ncols, "route: key column %d out of range", key_col);
-        int done = 0;
-        rc = redistribute_peer(ctx, in, key_col, out, &done);
-        if (rc || done) return rc;
-    }
-    if (!(two && two[0] == '1') && (N == 1 || ctx->comm)) { rc = partition_regions(ctx, in, key_col, &part, counts, &cap, &overflowed); if (rc) return rc; }
-    if (!part) { rc = partition_impl(ctx, in, key_col, &part, counts); if (rc) return rc; cap = 0; }
-    if (N == 1 || !ctx->comm) { *out = part; return GX_OK; }
-    // counts first (+ which columns carry NULL arrays, so every rank agrees)
+    long long cap = 0; int overflowed = 0, rc;
+    s->t = nullptr;
+    if (!(two && two[0] == '1')) { rc = partition_regions(ctx, in, key_col, &s->t, s->counts, &cap, &overflowed); if (rc) return rc; }
+    if (!s->t) { rc = partition_impl(ctx, in, key_col, &s->t, s->counts); if (rc) return rc; cap = 0; }
     int64_t nullbits = 0;
     for (int c = 0; c < in->ncols; c++) if (in->nulls[c]) nullbits |= 1LL << c;
-    counts[N] = nullbits;
+    s->counts[N] = nullbits;
+    for (int p = 0; p < N; p++)
+        s->sendoff[p] = cap ? (int64_t) p * cap : (p ? s->sendoff[p - 1] + s->counts[p - 1] : 0);   // regions, or densely packed
+    s->path = cap ? 1 : 2;
+    return GX_OK;
+}
+
+// the NULL bytes a partitioned part sends for column c: its own, or zeros when it has no NULL array for c but another
+// rank has one (*tmp: the zeros, for the caller to free)
+static int send_nulls(gx_ctx *ctx, const gx_table *part, int c, const uint8_t **src, uint8_t **tmp)
+{
+    *tmp = nullptr; *src = part->nulls[c];
+    if (*src) return GX_OK;
+    GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) tmp, (size_t) (part->nrows > 0 ? part->nrows : 1)));
+    GX_CUDA(ctx, cudaMemsetAsync(*tmp, 0, (size_t) part->nrows, ctx->stream));
+    *src = *tmp;
+    return GX_OK;
+}
+
+// The redistribute of rank T.rank of T.nranks: *out receives the rows of every rank whose key routes to this rank.
+// *path (may be NULL): 0 the rows travelled through the peer windows, 1 the NCCL path with this rank's rows in one-pass
+// regions, 2 the NCCL path with them in the two-pass form.
+static int redistribute_run(gx_ctx *ctx, const gx_table *in, int key_col, gx_redist_transport &T, gx_table **out, int *path)
+{
+    const int N = T.nranks;
+    GX_CHECK_ARG(ctx, ctx->nnodes == N, "redistribute: shard map covers %d nodes but the communicator has %d ranks", ctx->nnodes, N);
+    GX_CHECK_ARG(ctx, key_col >= 0 && key_col < in->ncols, "route: key column %d out of range", key_col);
+    const int kt = in->types[key_col];
+    GX_CHECK_ARG(ctx, kt == GX_INT4 || kt == GX_INT8 || kt == GX_DATE, "route: distribution column type %d not supported (int4/int8/date)", kt);
+    int rc = GX_OK;
+    if (N > 1 && T.window_bytes > 0) {
+        int done = 0;
+        rc = redistribute_peer(ctx, in, key_col, T, out, &done);
+        if (rc || done) { if (path && done) *path = 0; return rc; }
+    }
+    gx_redist_part s;
+    rc = redist_partition(ctx, in, key_col, N, &s); if (rc) return rc;
+    if (path) *path = s.path;
+    if (N == 1) { *out = s.t; return GX_OK; }
     int64_t *all = (int64_t *) malloc((size_t) N * (N + 1) * 8);
-    rc = allgather_i64(ctx, counts, N + 1, all);
-    if (rc) { free(all); gx_table_free(part); return rc; }
-    int64_t sendoff[GX_MAX_NODES], recvcnt[GX_MAX_NODES], recvoff[GX_MAX_NODES], total = 0, anynull = 0;
+    rc = T.gather_counts(ctx, s.counts, N + 1, all);
+    if (rc) { free(all); gx_table_free(s.t); return rc; }
+    int64_t recvcnt[GX_MAX_NODES], recvoff[GX_MAX_NODES], total = 0, anynull = 0;
     for (int p = 0; p < N; p++) {
-        sendoff[p] = cap ? (int64_t) p * cap : (p ? sendoff[p - 1] + counts[p - 1] : 0);   // regions, or densely packed (two-pass)
-        recvcnt[p] = all[(size_t) p * (N + 1) + ctx->rank];
+        recvcnt[p] = all[(size_t) p * (N + 1) + T.rank];
         recvoff[p] = total; total += recvcnt[p];
         anynull |= all[(size_t) p * (N + 1) + N];
     }
@@ -803,31 +857,200 @@ extern "C" int gx_redistribute(gx_ctx *ctx, const gx_table *in, int key_col, gx_
     for (int c = 0; c < in->ncols; c++) hn[c] = (anynull >> c) & 1;
     gx_table *t;
     rc = gx_table_alloc_like(ctx, in->ncols, in->types, hn, total, &t);
-    if (rc) { gx_table_free(part); return rc; }
+    if (rc) { gx_table_free(s.t); return rc; }
     {
         gx_launch_scope ls(ctx, "alltoall", in->ncols);
         for (int c = 0; c < in->ncols && rc == GX_OK; c++) {
             int sz = gx_type_size(in->types[c]);
             int64_t so[GX_MAX_NODES], sc[GX_MAX_NODES], ro[GX_MAX_NODES], rcn[GX_MAX_NODES];
-            for (int p = 0; p < N; p++) { so[p] = sendoff[p] * sz; sc[p] = counts[p] * sz; ro[p] = recvoff[p] * sz; rcn[p] = recvcnt[p] * sz; }
-            rc = alltoallv_bytes(ctx, (const char *) part->cols[c], so, sc, (char *) t->cols[c], ro, rcn);
+            for (int p = 0; p < N; p++) { so[p] = s.sendoff[p] * sz; sc[p] = s.counts[p] * sz; ro[p] = recvoff[p] * sz; rcn[p] = recvcnt[p] * sz; }
+            rc = T.exchange_column(ctx, c, 0, (const char *) s.t->cols[c], so, sc, (char *) t->cols[c], ro, rcn);
             if (rc == GX_OK && hn[c]) {
-                // a rank without a NULL array for this column sends zeros
-                uint8_t *src = part->nulls[c];
-                uint8_t *tmp = nullptr;
-                if (!src) { gx_tmp_alloc(ctx, (void **) &tmp, (size_t) (part->nrows > 0 ? part->nrows : 1)); cudaMemsetAsync(tmp, 0, (size_t) part->nrows, ctx->stream); src = tmp; }
-                rc = alltoallv_bytes(ctx, (const char *) src, sendoff, counts, (char *) t->nulls[c], recvoff, recvcnt);
+                const uint8_t *src; uint8_t *tmp;
+                rc = send_nulls(ctx, s.t, c, &src, &tmp);
+                if (rc == GX_OK) rc = T.exchange_column(ctx, c, 1, (const char *) src, s.sendoff, s.counts, (char *) t->nulls[c], recvoff, recvcnt);
                 if (tmp) { cudaStreamSynchronize(ctx->stream); gx_tmp_free(ctx, tmp); }
             }
         }
     }
     cudaError_t e = cudaStreamSynchronize(ctx->stream);
-    gx_table_free(part);
+    gx_table_free(s.t);
     if (rc) { gx_table_free(t); return rc; }
     if (e != cudaSuccess) { gx_table_free(t); GX_SET_ERR(ctx, "redistribute: %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
     t->nrows = total;
     *out = t;
     return GX_OK;
+}
+
+// Between processes: the peer windows mapped through CUDA IPC, their headers and acknowledgements, and NCCL.
+struct gx_nccl_redist_transport : gx_redist_transport {
+    unsigned long long epoch = 0, timeout_ns = 0;
+    unsigned long long *d_ctl = nullptr;            // [0] timed-out flag, [1 ..] the headers of the sources
+    int window_open(gx_ctx *ctx, long long region_stride, char **dst) override
+    {
+        epoch = ++ctx->peer_epoch;
+        const char *tmo = getenv("GX_PEER_TIMEOUT_MS");
+        timeout_ns = (unsigned long long) (tmo ? atoll(tmo) : 60000) * 1000000ULL;
+        GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d_ctl, 8 + (size_t) GX_MAX_NODES * 3 * 8));
+        GX_CUDA(ctx, cudaMemsetAsync(d_ctl, 0, 8, ctx->stream));
+        // the regions this rank owns in the peers' windows must have been emptied (previous call)
+        { gx_launch_scope ls(ctx, "peer_wait_ack"); gx_k_peer_wait<<<1, GX_MAX_NODES, 0, ctx->stream>>>(PEER_ACK(ctx->peer_base[rank], 0), 1, nranks, epoch - 1, timeout_ns, (int *) d_ctl, nullptr); }
+        for (int p = 0; p < nranks; p++) dst[p] = ctx->peer_base[p] + PEER_CTL_BYTES + (long long) rank * region_stride;
+        return GX_OK;
+    }
+    int window_headers(gx_ctx *ctx, const unsigned long long *d_cur, int feasible, long long cap, unsigned long long nullbits,
+                       unsigned long long *hdr, const char **win) override
+    {
+        gx_peer_ptrs P; memset(&P, 0, sizeof(P));
+        for (int p = 0; p < nranks; p++) P.base[p] = ctx->peer_base[p];
+        char *own = ctx->peer_base[rank];
+        { gx_launch_scope ls(ctx, "peer_publish"); gx_k_peer_publish<<<1, GX_MAX_NODES, 0, ctx->stream>>>(P, nranks, rank, epoch, d_cur, feasible, (unsigned long long) cap, nullbits); }
+        { gx_launch_scope ls(ctx, "peer_wait"); gx_k_peer_wait<<<1, GX_MAX_NODES, 0, ctx->stream>>>(PEER_HDR(own, 0), 4, nranks, epoch, timeout_ns, (int *) d_ctl, d_ctl + 1); }
+        int h_flag = 0;
+        cudaError_t e = cudaGetLastError();
+        if (e == cudaSuccess) e = cudaMemcpyAsync(hdr, d_ctl + 1, (size_t) nranks * 3 * 8, cudaMemcpyDeviceToHost, ctx->stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(&h_flag, d_ctl, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+        gx_tmp_free(ctx, d_ctl); d_ctl = nullptr;
+        if (e != cudaSuccess) { GX_SET_ERR(ctx, "redistribute (peer windows): %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
+        if (h_flag) { GX_SET_ERR(ctx, "redistribute (peer windows): rank %d waited %llu ms for its peers", rank, timeout_ns / 1000000ULL); return GX_ERR_NCCL; }
+        *win = own + PEER_CTL_BYTES;
+        return GX_OK;
+    }
+    void window_release(gx_ctx *ctx) override
+    {
+        gx_peer_ptrs P; memset(&P, 0, sizeof(P));
+        for (int p = 0; p < nranks; p++) P.base[p] = ctx->peer_base[p];
+        gx_launch_scope ls(ctx, "peer_ack"); gx_k_peer_ack<<<1, GX_MAX_NODES, 0, ctx->stream>>>(P, nranks, rank, epoch);
+    }
+    int gather_counts(gx_ctx *ctx, const int64_t *mine, int n, int64_t *all) override { return allgather_i64(ctx, mine, n, all); }
+    int exchange_column(gx_ctx *ctx, int, int, const char *sendbuf, const int64_t *so, const int64_t *sc,
+                        char *recvbuf, const int64_t *ro, const int64_t *rcn) override
+    {
+        return alltoallv_bytes(ctx, sendbuf, so, sc, recvbuf, ro, rcn);
+    }
+};
+
+// In one process: parts[p] is the input table of rank p.  The body redistributes parts[rank]; the other parts are
+// routed or partitioned here by the body's own steps, as their ranks would, and what they address to this rank is
+// copied out of their buffers.  The windows of all ranks are allocated here; no header is published or awaited.
+struct gx_inproc_redist_transport : gx_redist_transport {
+    const gx_table *const *parts; int key_col; gx_ctx *ctx;
+    char *win[GX_MAX_NODES]; long long region_stride = 0;
+    gx_redist_part sent[GX_MAX_NODES];              // what every other rank sends on the NCCL path
+    gx_inproc_redist_transport(gx_ctx *c, const gx_table *const *p, int k) : parts(p), key_col(k), ctx(c)
+    {
+        memset(win, 0, sizeof(win));
+        for (int i = 0; i < GX_MAX_NODES; i++) sent[i].t = nullptr;
+    }
+    ~gx_inproc_redist_transport()
+    {
+        window_release(ctx);
+        for (int i = 0; i < GX_MAX_NODES; i++) if (sent[i].t) gx_table_free(sent[i].t);
+    }
+    int window_open(gx_ctx *ctx, long long stride, char **dst) override
+    {
+        region_stride = stride;
+        for (int d = 0; d < nranks; d++) {
+            GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &win[d], window_bytes));
+            dst[d] = win[d] + (long long) rank * region_stride;
+        }
+        return GX_OK;
+    }
+    int window_headers(gx_ctx *ctx, const unsigned long long *d_cur, int feasible, long long cap, unsigned long long nullbits,
+                       unsigned long long *hdr, const char **own) override
+    {
+        unsigned long long *d_src = nullptr;
+        GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d_src, (GX_MAX_NODES + 1) * 8));
+        int rc = GX_OK;
+        for (int s = 0; s < nranks && rc == GX_OK; s++) {
+            long long c = cap; unsigned long long nb = nullbits; int f = feasible;
+            const unsigned long long *cur = d_cur;
+            if (s != rank) {
+                char *dst[GX_MAX_NODES];
+                for (int d = 0; d < nranks; d++) dst[d] = win[d] + (long long) s * region_stride;
+                cudaError_t e = cudaMemsetAsync(d_src, 0, (GX_MAX_NODES + 1) * 8, ctx->stream);
+                if (e != cudaSuccess) { GX_SET_ERR(ctx, "debug_redistribute: %s", cudaGetErrorString(e)); rc = GX_ERR_CUDA; break; }
+                rc = peer_route(ctx, parts[s], key_col, nranks, region_stride, dst, d_src, &c, &nb, &f);
+                cur = d_src;
+            }
+            unsigned long long h[GX_MAX_NODES + 1];
+            cudaError_t e = cudaGetLastError();
+            if (e == cudaSuccess) e = cudaMemcpyAsync(h, cur, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream);
+            if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+            if (rc == GX_OK && e != cudaSuccess) { GX_SET_ERR(ctx, "debug_redistribute: %s", cudaGetErrorString(e)); rc = GX_ERR_CUDA; }
+            // what gx_k_peer_publish of rank s writes into the header of this rank's window
+            hdr[s * 3] = !f || h[GX_MAX_NODES] != 0 ? PEER_FALLBACK : h[rank]; hdr[s * 3 + 1] = (unsigned long long) c; hdr[s * 3 + 2] = nb;
+        }
+        gx_tmp_free(ctx, d_src);
+        *own = win[rank];
+        return rc;
+    }
+    void window_release(gx_ctx *ctx) override
+    {
+        for (int d = 0; d < GX_MAX_NODES; d++) { gx_tmp_free(ctx, win[d]); win[d] = nullptr; }
+    }
+    int gather_counts(gx_ctx *ctx, const int64_t *mine, int n, int64_t *all) override
+    {
+        for (int p = 0; p < nranks; p++) {
+            if (p != rank) { int rc = redist_partition(ctx, parts[p], key_col, nranks, &sent[p]); if (rc) return rc; }
+            memcpy(all + (size_t) p * n, p == rank ? mine : sent[p].counts, (size_t) n * 8);
+        }
+        return GX_OK;
+    }
+    int exchange_column(gx_ctx *ctx, int c, int want_null, const char *sendbuf, const int64_t *so, const int64_t *,
+                        char *recvbuf, const int64_t *ro, const int64_t *rcn) override
+    {
+        for (int p = 0; p < nranks; p++) {
+            if (!rcn[p]) continue;
+            const char *src = sendbuf + so[rank];
+            uint8_t *tmp = nullptr;
+            if (p != rank) {
+                const gx_table *part = sent[p].t;
+                if (want_null) {
+                    const uint8_t *nb;
+                    int rc = send_nulls(ctx, part, c, &nb, &tmp); if (rc) return rc;
+                    src = (const char *) nb + sent[p].sendoff[rank];
+                } else {
+                    src = (const char *) part->cols[c] + sent[p].sendoff[rank] * gx_type_size(part->types[c]);
+                }
+            }
+            cudaError_t e = cudaMemcpyAsync(recvbuf + ro[p], src, (size_t) rcn[p], cudaMemcpyDeviceToDevice, ctx->stream);
+            gx_tmp_free(ctx, tmp);
+            if (e != cudaSuccess) { GX_SET_ERR(ctx, "debug_redistribute: %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
+        }
+        return GX_OK;
+    }
+};
+
+extern "C" int gx_redistribute(gx_ctx *ctx, const gx_table *in, int key_col, gx_table **out)
+{
+    if (!ctx || !in || !out) return GX_ERR_ARG;
+    gx_nccl_redist_transport T;
+    T.rank = ctx->rank; T.nranks = ctx->nranks;
+    T.window_bytes = ctx->comm && ctx->peer_ready == 1 ? ctx->peer_win_bytes : 0;
+    return redistribute_run(ctx, in, key_col, T, out, nullptr);
+}
+
+#define GX_DEBUG_WINDOW_LIMIT (4ULL << 30)      // window_bytes * nparts of gx_debug_redistribute
+
+extern "C" int gx_debug_redistribute(gx_ctx *ctx, int nparts, const gx_table *const *parts, int key_col, int rank,
+                                     size_t window_bytes, gx_table **out, int *path_out)
+{
+    if (!ctx || !parts || !out) return GX_ERR_ARG;
+    GX_CHECK_ARG(ctx, nparts >= 1 && nparts <= GX_MAX_NODES, "debug_redistribute: %d parts (1..%d)", nparts, GX_MAX_NODES);
+    GX_CHECK_ARG(ctx, rank >= 0 && rank < nparts, "debug_redistribute: rank %d of %d parts", rank, nparts);
+    for (int p = 0; p < nparts; p++) {
+        const gx_table *a = parts[p], *b = parts[0];
+        GX_CHECK_ARG(ctx, a != nullptr, "debug_redistribute: part %d is NULL", p);
+        GX_CHECK_ARG(ctx, a->ncols == b->ncols && memcmp(a->types, b->types, sizeof(a->types[0]) * a->ncols) == 0,
+                     "debug_redistribute: part %d has other columns than part 0", p);
+    }
+    GX_CHECK_ARG(ctx, window_bytes <= GX_DEBUG_WINDOW_LIMIT / (size_t) nparts, "debug_redistribute: %d windows of %zu bytes exceed %llu bytes",
+                 nparts, window_bytes, GX_DEBUG_WINDOW_LIMIT);
+    gx_inproc_redist_transport T(ctx, parts, key_col);
+    T.rank = rank; T.nranks = nparts; T.window_bytes = window_bytes;
+    return redistribute_run(ctx, parts[rank], key_col, T, out, path_out);
 }
 
 // ------------------------------------------- Finalize across datanodes
