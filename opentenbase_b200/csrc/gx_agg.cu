@@ -2687,11 +2687,8 @@ static bool compile_expr(gx_ctx *ctx, const gx_table *t, const gx_expr *in, gx_d
 
 struct compiled_plan {
     gx_agg_dev A;
-    int32_t group_types[GX_MAX_GROUP_COLS];
-    int gword[GX_MAX_GROUP_COLS], gshift[GX_MAX_GROUP_COLS], gbytes[GX_MAX_GROUP_COLS];
-    int agg_word[GX_MAX_AGGS], agg_cnt_word[GX_MAX_AGGS], agg_var_word[GX_MAX_AGGS];
-    int need_w0;
-    bool has_var;                    // some aggregate keeps a variance or regression state: the specialised kernels do not
+    gx_rec_layout L;                 // of the plan's records; A carries its wkind, winit and need_w0
+    bool has_var;                   // some aggregate keeps a variance or regression state: the specialised kernels do not
 };
 
 // the same program, op by op (constants compared by their bits)
@@ -2728,6 +2725,7 @@ static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
 {
     memset(cp, 0, sizeof(*cp));
     gx_dplan &P = cp->A.P;
+    gx_rec_layout &L = cp->L;
     GX_CHECK_ARG(ctx, plan->n_aggs >= 0 && plan->n_aggs <= GX_MAX_AGGS, "agg plan: n_aggs %d", plan->n_aggs);
     GX_CHECK_ARG(ctx, plan->n_group_cols >= 0 && plan->n_group_cols <= GX_MAX_GROUP_COLS, "agg plan: n_group_cols %d", plan->n_group_cols);
     int rc = gx_check_agg_join_type(ctx, plan); if (rc) return rc;
@@ -2790,12 +2788,12 @@ static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
         int w = (used[0] + g.bytes <= 8) ? 0 : 1;
         GX_CHECK_ARG(ctx, used[w] + g.bytes <= 8, "agg plan: group key wider than 16 bytes");
         g.word = w; g.shift = 8 * used[w]; used[w] += g.bytes;
-        cp->group_types[c] = type; cp->gword[c] = g.word; cp->gshift[c] = g.shift; cp->gbytes[c] = g.bytes;
+        L.group_types[c] = type; L.gword[c] = g.word; L.gshift[c] = g.shift; L.gbytes[c] = g.bytes;
     }
     P.nkw = used[1] ? 2 : 1;
     // aggregates
     int nw = 1;                                     // w0 = row count
-    cp->A.wkind[0] = WK_ADD_I64; cp->A.winit[0] = 0;
+    L.wkind[0] = WK_ADD_I64; L.winit[0] = 0;
     P.nagg = plan->n_aggs;
     // the two-argument aggregates: their (Y, X) programs, the same in all of them (one state per plan), the first of
     // them owns the state; regr_count alone needs only the count of pairs
@@ -2815,7 +2813,7 @@ static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
         gx_dagg &g = P.aggs[a];
         const gx_agg &src = plan->aggs[a];
         bool nullable = false;
-        auto new_word = [&](int kind, long long init) { cp->A.wkind[nw] = kind; cp->A.winit[nw] = init; return nw++; };
+        auto new_word = [&](int kind, long long init) { L.wkind[nw] = kind; L.winit[nw] = init; return nw++; };
         const bool var = gx_is_var_fn(src.fn);
         // {C, S1, S2} of a variance over the same value as an earlier sum / avg / variance, or all of its words
         auto new_var = [&](gx_dagg &owner) {
@@ -2823,11 +2821,11 @@ static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
                 owner.var_word = new_word(WK_VAR_C | (owner.cnt_word << 8), (long long) GX_VAR_UNSET_BITS);
                 new_word(WK_VAR_S, 0); new_word(WK_VAR_S, 0);
             }
-            cp->agg_var_word[a] = owner.var_word; cp->has_var = true;
+            L.agg_var_word[a] = owner.var_word; cp->has_var = true;
         };
         if (!gx_is_regr_fn(src.fn) && nw + (var ? 5 : 2) > GX_MAX_WORDS) { GX_SET_ERR(ctx, "agg plan: too many state words"); return GX_ERR_ARG; }
         switch (src.fn) {
-            case GX_AGG_COUNT_STAR: g.kind = GXU_NONE; cp->agg_word[a] = 0; cp->need_w0 = 1; break;
+            case GX_AGG_COUNT_STAR: g.kind = GXU_NONE; L.agg_word[a] = 0; L.need_w0 = 1; break;
             case GX_AGG_SUM_I8:
                 // the int64 accumulators wrap, and the reference's sum(int8) is numeric (never overflows)
                 GX_SET_ERR(ctx, "agg %d: sum(int8) is not supported", a); return GX_ERR_ARG;
@@ -2839,11 +2837,11 @@ static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
                 if (src.fn == GX_AGG_SUM_I4) GX_CHECK_ARG(ctx, t == GX_INT4, "agg %d: sum(int4) needs an int4 column", a);
                 g.is_int = 1; g.icol = dcol_of(outer, col); nullable = outer->nulls[col] != nullptr;
                 if (src.fn == GX_AGG_COUNT) {
-                    if (nullable) { g.kind = GXU_CNT; g.word = new_word(WK_ADD_I64, 0); cp->agg_word[a] = g.word; }
-                    else { g.kind = GXU_NONE; cp->agg_word[a] = 0; cp->need_w0 = 1; }
+                    if (nullable) { g.kind = GXU_CNT; g.word = new_word(WK_ADD_I64, 0); L.agg_word[a] = g.word; }
+                    else { g.kind = GXU_NONE; L.agg_word[a] = 0; L.need_w0 = 1; }
                 } else {
-                    g.kind = GXU_ADD_I64; g.word = new_word(WK_ADD_I64, 0); cp->agg_word[a] = g.word;
-                    g.cnt_word = nullable ? new_word(WK_ADD_I64, 0) : 0; cp->agg_cnt_word[a] = g.cnt_word;
+                    g.kind = GXU_ADD_I64; g.word = new_word(WK_ADD_I64, 0); L.agg_word[a] = g.word;
+                    g.cnt_word = nullable ? new_word(WK_ADD_I64, 0) : 0; L.agg_cnt_word[a] = g.cnt_word;
                 }
                 break;
             }
@@ -2857,16 +2855,11 @@ static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
                     int twin = -1;
                     for (int b = 0; b < a && twin < 0; b++) {
                         const gx_agg &o = plan->aggs[b];
-                        if ((o.fn != GX_AGG_SUM_F8 && o.fn != GX_AGG_AVG_F8 && !gx_is_var_fn(o.fn)) || o.arg.nops != src.arg.nops) continue;
-                        bool same = true;
-                        for (int k = 0; k < src.arg.nops && same; k++)
-                            same = o.arg.ops[k].op == src.arg.ops[k].op && o.arg.ops[k].col == src.arg.ops[k].col &&
-                                   memcmp(&o.arg.ops[k].k, &src.arg.ops[k].k, sizeof(double)) == 0;
-                        if (same) twin = b;
+                        if ((o.fn == GX_AGG_SUM_F8 || o.fn == GX_AGG_AVG_F8 || gx_is_var_fn(o.fn)) && same_expr(o.arg, src.arg)) twin = b;
                     }
                     if (twin >= 0) {
-                        g.kind = GXU_NONE; cp->agg_word[a] = cp->agg_word[twin]; cp->agg_cnt_word[a] = cp->agg_cnt_word[twin];
-                        if (cp->agg_cnt_word[a] == 0 && (src.fn == GX_AGG_AVG_F8 || var)) cp->need_w0 = 1;
+                        g.kind = GXU_NONE; L.agg_word[a] = L.agg_word[twin]; L.agg_cnt_word[a] = L.agg_cnt_word[twin];
+                        if (L.agg_cnt_word[a] == 0 && (src.fn == GX_AGG_AVG_F8 || var)) L.need_w0 = 1;
                         if (var) new_var(P.aggs[twin]);
                         break;
                     }
@@ -2879,9 +2872,9 @@ static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
                     double ninf = -__builtin_inf(); long long bits; memcpy(&bits, &ninf, 8);
                     g.kind = GXU_MAX_F64; g.word = new_word(WK_MAX_F64, bits);
                 } else { g.kind = GXU_ADD_F64; g.word = new_word(WK_ADD_F64, (long long) GX_NEG_ZERO_BITS); }   // -0: x + -0 == x for every x, -0 included
-                cp->agg_word[a] = g.word;
-                g.cnt_word = nullable ? new_word(WK_ADD_I64, 0) : 0; cp->agg_cnt_word[a] = g.cnt_word;
-                if (!nullable && (src.fn == GX_AGG_AVG_F8 || var)) cp->need_w0 = 1;    // N of float8_avg / float8_accum
+                L.agg_word[a] = g.word;
+                g.cnt_word = nullable ? new_word(WK_ADD_I64, 0) : 0; L.agg_cnt_word[a] = g.cnt_word;
+                if (!nullable && (src.fn == GX_AGG_AVG_F8 || var)) L.need_w0 = 1;    // N of float8_avg / float8_accum
                 if (var) new_var(g);
                 break;
             }
@@ -2901,7 +2894,7 @@ static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
                     if (nw + ((ny || nx) ? 1 : 0) + (regr_full ? 9 : 0) > GX_MAX_WORDS) { GX_SET_ERR(ctx, "agg plan: too many state words"); return GX_ERR_ARG; }
                     P.regr.on = 1;
                     P.regr.cnt_word = (ny || nx) ? new_word(WK_ADD_I64, 0) : 0;
-                    if (!P.regr.cnt_word) cp->need_w0 = 1;                       // N = rows
+                    if (!P.regr.cnt_word) L.need_w0 = 1;                       // N = rows
                     if (regr_full) {                       // {Sx, Sy, Cx, S1x, S2x, Cy, S1y, S2y, Sxy'}
                         P.regr.word = new_word(WK_ADD_F64, (long long) GX_NEG_ZERO_BITS);
                         new_word(WK_ADD_F64, (long long) GX_NEG_ZERO_BITS);
@@ -2911,25 +2904,38 @@ static int compile_plan(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
                         new_word(WK_VAR_S, 0); new_word(WK_VAR_S, 0); new_word(WK_VAR_S, 0);
                     }
                 }
-                cp->agg_word[a] = P.regr.word; cp->agg_cnt_word[a] = P.regr.cnt_word;
+                L.agg_word[a] = P.regr.word; L.agg_cnt_word[a] = P.regr.cnt_word;
                 break;
             }
             default: GX_SET_ERR(ctx, "agg %d: unknown aggregate function %d", a, src.fn); return GX_ERR_ARG;
         }
     }
     P.nwords = nw;
+    L.nkw = P.nkw; L.nwords = nw; L.rec_words = 3 + nw;
+    memcpy(cp->A.wkind, L.wkind, sizeof(L.wkind)); memcpy(cp->A.winit, L.winit, sizeof(L.winit));
+    cp->A.need_w0 = L.need_w0;
     cp->A.row0 = 0; cp->A.row1 = outer->nrows;
     cp->A.counters = ctx->d_scratch + 8;
     return GX_OK;
 }
 
-int gx_result_alloc(gx_ctx *ctx, const gx_agg_plan *plan, const int32_t *group_types, int64_t cap, gx_result **out)
+// a result over the ngroups records of layout L at d_recs (room for cap), which it owns from here on
+static gx_result *new_result(gx_ctx *ctx, const gx_agg_plan *plan, const gx_rec_layout &L, void *d_recs, int64_t ngroups, int64_t cap)
 {
     gx_result *r = (gx_result *) calloc(1, sizeof(gx_result));
-    r->ctx = ctx; r->plan = *plan; r->cap = cap < 1 ? 1 : cap;
-    for (int c = 0; c < plan->n_group_cols; c++) r->group_types[c] = group_types[c];
-    *out = r;
-    return GX_OK;
+    r->ctx = ctx; r->plan = *plan; r->L = L;
+    r->d_recs = (long long *) d_recs; r->ngroups = ngroups; r->cap = cap;
+    return r;
+}
+
+// the parameter block of a merge of records of layout L by their whole key (gx_aggregate_records, gx_k_merge_gathered)
+static gx_agg_dev merge_params(gx_ctx *ctx, const gx_rec_layout &L)
+{
+    gx_agg_dev A; memset(&A, 0, sizeof(A));
+    A.P.nwords = L.nwords; A.P.nkw = 2;
+    memcpy(A.wkind, L.wkind, sizeof(A.wkind)); memcpy(A.winit, L.winit, sizeof(A.winit));
+    A.counters = ctx->d_scratch + 8;
+    return A;
 }
 
 static size_t smem_bytes_for(int S, int nkw, int nwords) { return (size_t) S * 8 * (1 + nkw + nwords); }
@@ -3241,40 +3247,24 @@ static int read_counters(gx_ctx *ctx, long long *c /* 4 */, long long *cursor = 
 }
 
 // global table -> result (dense)
-static int table_to_result(gx_ctx *ctx, compiled_plan *cp, const gx_agg_plan *plan, unsigned long long *g_tab, long long g_cap,
+static int table_to_result(gx_ctx *ctx, const compiled_plan *cp, const gx_agg_plan *plan, unsigned long long *g_tab, long long g_cap,
                            long long ngroups, gx_result **out)
 {
-    const int RW = 3 + cp->A.P.nwords;
-    gx_result *r; gx_result_alloc(ctx, plan, cp->group_types, ngroups, &r);
-    r->nkw = cp->A.P.nkw; r->nwords = cp->A.P.nwords; r->rec_words = RW; r->need_w0 = cp->need_w0;
-    for (int a = 0; a < plan->n_aggs; a++) { r->agg_word[a] = cp->agg_word[a]; r->agg_cnt_word[a] = cp->agg_cnt_word[a]; r->agg_var_word[a] = cp->agg_var_word[a]; }
-    cudaError_t e = gx_tmp_alloc(ctx, (void **) &r->d_recs, (size_t) r->cap * RW * 8);
-    if (e != cudaSuccess) { gx_result_free(r); GX_SET_ERR(ctx, "result: %s", cudaGetErrorString(e)); return GX_ERR_NOMEM; }
+    const long long cap = ngroups > 0 ? ngroups : 1;
+    unsigned long long *d_recs;
+    cudaError_t e = gx_tmp_alloc(ctx, (void **) &d_recs, (size_t) cap * cp->L.rec_words * 8);
+    if (e != cudaSuccess) { GX_SET_ERR(ctx, "result: %s", cudaGetErrorString(e)); return GX_ERR_NOMEM; }
     GX_CUDA(ctx, cudaMemsetAsync(ctx->d_scratch + 12, 0, sizeof(long long), ctx->stream));
     if (ngroups > 0) {
         gx_launch_scope ls(ctx, "agg_compact");
-        gx_k_compact_groups<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(g_tab, g_cap, cp->A.P.nwords, (unsigned long long *) r->d_recs, ctx->d_scratch + 12);
+        gx_k_compact_groups<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(g_tab, g_cap, cp->A.P.nwords, d_recs, ctx->d_scratch + 12);
     }
     GX_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    r->ngroups = ngroups;
-    *out = r;
+    *out = new_result(ctx, plan, cp->L, d_recs, ngroups, cap);
     return GX_OK;
 }
 
-// keep the compiled layout around for fetch/combine
-struct result_layout { int gword[GX_MAX_GROUP_COLS], gshift[GX_MAX_GROUP_COLS], gbytes[GX_MAX_GROUP_COLS]; int wkind[GX_MAX_WORDS]; long long winit[GX_MAX_WORDS]; };
-static std::map<gx_result *, result_layout> *g_layouts;
-static void remember_layout(gx_result *r, const compiled_plan *cp)
-{
-    if (!g_layouts) g_layouts = new std::map<gx_result *, result_layout>();
-    result_layout L; memset(&L, 0, sizeof(L));
-    for (int c = 0; c < GX_MAX_GROUP_COLS; c++) { L.gword[c] = cp->gword[c]; L.gshift[c] = cp->gshift[c]; L.gbytes[c] = cp->gbytes[c]; }
-    for (int i = 0; i < GX_MAX_WORDS; i++) { L.wkind[i] = cp->A.wkind[i]; L.winit[i] = cp->A.winit[i]; }
-    (*g_layouts)[r] = L;
-}
-
 static int run_radix(gx_ctx *ctx, compiled_plan *cp, const gx_agg_plan *plan, long long nrows_in, gx_result **out);
-int gx_result_layout_words(gx_result *r, int *wkind, long long *winit);
 int gx_aggregate_records(gx_ctx *ctx, gx_agg_dev A, unsigned long long *d_recs, long long nrec,
                          unsigned long long **d_out, long long *ngroups_out);
 
@@ -3291,7 +3281,7 @@ static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
     // ---- shared-memory plan (strategy 1) -----------------------------------
     // key bytes <= 7 and one key word: the tag word carries the key itself
     int keybytes = 0;
-    for (int c = 0; c < plan->n_group_cols; c++) keybytes += cp.gbytes[c];
+    for (int c = 0; c < plan->n_group_cols; c++) keybytes += cp.L.gbytes[c];
     const int tagkey = (A.P.nkw == 1 && keybytes <= 7) ? 1 : 0;
     const size_t budget = ctx->smem_optin - 1024;
     auto dense_bytes = [&](long long S) { return (size_t) S * 8 * (1 + (tagkey ? 0 : A.P.nkw) + nwords); };
@@ -3302,7 +3292,6 @@ static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
     // a plan with one whose groups outgrow the shared table but fit L2's share of the global table takes that table
     if (plan->strategy == 0 && strategy == 2 && A.P.regr.on && est <= 65536) strategy = 3;
     GX_CHECK_ARG(ctx, strategy >= 1 && strategy <= 3, "agg plan: unknown strategy %d", strategy);
-    A.need_w0 = cp.need_w0;
 
     // ---- does the plan have the shape the specialised kernel was written for?
     gx_fast_args FA; memset(&FA, 0, sizeof(FA));
@@ -3472,12 +3461,7 @@ static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
                     GX_CUDA(ctx, cudaGetLastError());
                 }
                 gx_tmp_free(ctx, g_tab);
-                gx_result *r; gx_result_alloc(ctx, plan, cp.group_types, direct + c[0], &r);
-                r->nkw = A.P.nkw; r->nwords = nwords; r->rec_words = RW; r->need_w0 = cp.need_w0;
-                for (int a = 0; a < plan->n_aggs; a++) { r->agg_word[a] = cp.agg_word[a]; r->agg_cnt_word[a] = cp.agg_cnt_word[a]; r->agg_var_word[a] = cp.agg_var_word[a]; }
-                r->d_recs = (long long *) d_out; r->ngroups = direct + c[0]; r->cap = out_cap;
-                remember_layout(r, &cp);
-                *out = r;
+                *out = new_result(ctx, plan, cp.L, d_out, direct + c[0], out_cap);
                 return GX_OK;
             }
             gx_tmp_free(ctx, g_tab); gx_tmp_free(ctx, d_out);      // keys descend somewhere: general path
@@ -3486,7 +3470,7 @@ static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
     }
 
     for (int attempt = 0; attempt < 8; attempt++) {
-        if (strategy == 2) { rc = need_wide(); if (rc) return rc; rc = run_radix(ctx, &cp, plan, outer->nrows, out); if (rc == GX_OK) remember_layout(*out, &cp); return rc; }
+        if (strategy == 2) { rc = need_wide(); if (rc) return rc; return run_radix(ctx, &cp, plan, outer->nrows, out); }
         long long S = 16; while (S * 2 < est * 3 && S < smax) S *= 2;     // load factor <= 0.67
         // lane-private mode for a handful of groups: [warp][word][group][lane]
         int gmax = 0, lp_warps = 0; size_t lp_bytes = 0;
@@ -3520,7 +3504,7 @@ static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
               fprintf(stderr, "gpuexec: hash_agg attempt %d strategy %d S %lld gmax %d fast_ok %d use_fast %d use_run %d cslots %d narrow %d slot mode %d seg %d tma %d rows %lld\n",
                       attempt, strategy, S, gmax, (int) fast_ok, (int) use_fast, (int) use_run, A.cslots != nullptr, A.narrow != nullptr, A.sf.mode,
                       (int) gx_runjoin_seg_enabled(), (int) gx_runjoin_tma_enabled(), (long long) outer->nrows); }
-        if (use_fast) rc = launch_fast(ctx, A, FA, A.P.has_join != 0, cp.need_w0 != 0, FA.vcol != nullptr, dense_bytes(S), kname, use_run);
+        if (use_fast) rc = launch_fast(ctx, A, FA, A.P.has_join != 0, A.need_w0 != 0, FA.vcol != nullptr, dense_bytes(S), kname, use_run);
         else if (use_few && countchar_ok) {
             gx_launch_scope ls(ctx, kname);
             gx_launch_scope which(ctx, "agg_count_char", 0);
@@ -3560,7 +3544,6 @@ static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
         if (c[1] == 0) {
             rc = table_to_result(ctx, &cp, plan, g_tab, g_cap, c[0], out);
             gx_tmp_free(ctx, g_tab);
-            if (rc == GX_OK) remember_layout(*out, &cp);
             return rc;
         }
         gx_tmp_free(ctx, g_tab);
@@ -3618,23 +3601,23 @@ static void f8_checked_words(const gx_result *r, bool sums_only, gx_infscan_args
     memset(S, 0, sizeof(*S));
     auto add = [&](int a, int word, int nf) {
         for (int i = 0; i < S->nchk; i++) if (S->word[i] == word) return;
-        chk[S->nchk] = a; S->word[S->nchk] = word; S->cw[S->nchk] = r->agg_cnt_word[a]; S->nf[S->nchk] = nf; S->nchk++;
+        chk[S->nchk] = a; S->word[S->nchk] = word; S->cw[S->nchk] = r->L.agg_cnt_word[a]; S->nf[S->nchk] = nf; S->nchk++;
     };
     for (int a = 0; a < r->plan.n_aggs; a++) {
         const int fn = r->plan.aggs[a].fn;
         const bool sum = fn == GX_AGG_SUM_F8 || fn == GX_AGG_AVG_F8 || gx_is_var_fn(fn) || gx_is_regr_fn(fn);
         if (!sum && (sums_only || (fn != GX_AGG_MIN_F8 && fn != GX_AGG_MAX_F8))) continue;
         if (gx_is_regr_fn(fn)) {             // Sx, Sy; S1x, S2x, S1y, S2y and the cross term
-            if (fn == GX_AGG_REGR_COUNT || !r->agg_word[a]) continue;
-            const int R = r->agg_word[a];
+            if (fn == GX_AGG_REGR_COUNT || !r->L.agg_word[a]) continue;
+            const int R = r->L.agg_word[a];
             add(a, R, 0); add(a, R + 1, 0);
             add(a, R + 3, 1); add(a, R + 4, 1); add(a, R + 6, 1); add(a, R + 7, 1); add(a, R + 8, 1);
             continue;
         }
-        add(a, r->agg_word[a], 0);
-        if (gx_is_var_fn(fn)) { add(a, r->agg_var_word[a] + 1, 1); add(a, r->agg_var_word[a] + 2, 1); }
+        add(a, r->L.agg_word[a], 0);
+        if (gx_is_var_fn(fn)) { add(a, r->L.agg_var_word[a] + 1, 1); add(a, r->L.agg_var_word[a] + 2, 1); }
     }
-    S->RW = r->rec_words; S->need_w0 = r->need_w0;
+    S->RW = r->L.rec_words; S->need_w0 = r->L.need_w0;
 }
 // does any group of recs[0, n) hold a non-empty infinite checked word?
 static int any_inf_word(gx_ctx *ctx, gx_infscan_args S, const unsigned long long *recs, long long n, bool *any)
@@ -3701,26 +3684,26 @@ static int check_f8_overflow(gx_ctx *ctx, const gx_table *outer, const gx_hash *
     if (rc != GX_OK) return rc;
     const int ng = plan->n_group_cols;
     const unsigned long long mmask = (1ULL << ng) - 1;
-    std::vector<unsigned long long> hr((size_t) r->ngroups * r->rec_words), hv((size_t) v->ngroups * v->rec_words + 1);
+    std::vector<unsigned long long> hr((size_t) r->ngroups * r->L.rec_words), hv((size_t) v->ngroups * v->L.rec_words + 1);
     cudaError_t e = cudaMemcpyAsync(hr.data(), r->d_recs, hr.size() * 8, cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess && v->ngroups) e = cudaMemcpyAsync(hv.data(), v->d_recs, (size_t) v->ngroups * v->rec_words * 8, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess && v->ngroups) e = cudaMemcpyAsync(hv.data(), v->d_recs, (size_t) v->ngroups * v->L.rec_words * 8, cudaMemcpyDeviceToHost, ctx->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
     if (e != cudaSuccess) { gx_result_free(v); GX_SET_ERR(ctx, "hash_agg: %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
     std::unordered_map<gx_group_key, long long, gx_group_key_hash> at;
     at.reserve((size_t) v->ngroups);
     for (long long gI = 0; gI < v->ngroups; gI++) {
-        const unsigned long long *rec = hv.data() + (size_t) gI * v->rec_words;
+        const unsigned long long *rec = hv.data() + (size_t) gI * v->L.rec_words;
         at[{ rec[0] & mmask, rec[1], rec[2] }] = gI;
     }
     rc = GX_OK;
     for (long long gI = 0; gI < r->ngroups && rc == GX_OK; gI++) {
-        const unsigned long long *rec = hr.data() + (size_t) gI * r->rec_words, *w = rec + 3;
+        const unsigned long long *rec = hr.data() + (size_t) gI * r->L.rec_words, *w = rec + 3;
         for (int i = 0; i < S.nchk && rc == GX_OK; i++) {
             double x; memcpy(&x, &w[S.word[i]], 8);
             if (rec_count(S, w, i) == 0 || !overflow_candidate(x, S.nf[i])) continue;
             auto it = at.find({ rec[0] & mmask, rec[1], rec[2] });
             if (it == at.end()) { GX_SET_ERR(ctx, "hash_agg: overflow check lost a group"); rc = GX_ERR_STATE; break; }
-            double nonfinite; memcpy(&nonfinite, &hv[(size_t) it->second * v->rec_words + 3 + v->agg_word[vi[i]]], 8);
+            double nonfinite; memcpy(&nonfinite, &hv[(size_t) it->second * v->L.rec_words + 3 + v->L.agg_word[vi[i]]], 8);
             if (!std::isnan(nonfinite)) { GX_SET_ERR(ctx, "value out of range: overflow"); rc = GX_ERR_OVERFLOW; }
         }
     }
@@ -3741,7 +3724,7 @@ static int check_combine_overflow(gx_ctx *ctx, const gx_result *r, const std::ve
     bool any;
     int rc = any_inf_word(ctx, S, merged, nmerged, &any);
     if (rc != GX_OK || !any) return rc;
-    const int RW = r->rec_words;
+    const int RW = r->L.rec_words;
     const unsigned long long mmask = (1ULL << r->plan.n_group_cols) - 1;
     long long nin = 0;
     for (auto &sp : spans) nin += sp.second;
@@ -3849,26 +3832,25 @@ static int count_distinct_run(gx_ctx *ctx, const gx_table *outer, const gx_hash 
     gx_result *s1 = nullptr;
     int rc = hash_agg_checked(ctx, outer, h, &p1, &s1, ch);
     if (rc != GX_OK) return rc;
-    const result_layout L1 = (*g_layouts)[s1];
-    const int RW1 = s1->rec_words, nw = s1->nwords + 1;
+    const gx_rec_layout &L1 = s1->L;
+    const int RW1 = L1.rec_words, nw = L1.nwords + 1;
     if (nw > GX_MAX_WORDS) { gx_result_free(s1); GX_SET_ERR(ctx, "agg plan: too many state words"); return GX_ERR_ARG; }
 
-    gx_result *r; gx_result_alloc(ctx, plan, s1->group_types, 0, &r);
-    r->nkw = 1; r->nwords = nw; r->rec_words = RW1 + 1; r->need_w0 = s1->need_w0;
+    // the fold's records: stage 1's without the argument in the key, and the DISTINCT word appended
+    gx_rec_layout L = L1;
+    L.nkw = 1; L.nwords = nw; L.rec_words = RW1 + 1;
+    L.wkind[L1.nwords] = WK_ADD_I64; L.winit[L1.nwords] = 0;
     gx_distinct_args D; memset(&D, 0, sizeof(D));
     for (int c = 0; c < ng; c++) {
         const unsigned long long bits = (L1.gbytes[c] < 8 ? (1ULL << (8 * L1.gbytes[c])) - 1 : ~0ULL) << L1.gshift[c];
-        if (L1.gword[c] == 0) D.keep0 |= bits; else { D.keep1 |= bits; r->nkw = 2; }
+        if (L1.gword[c] == 0) D.keep0 |= bits; else { D.keep1 |= bits; L.nkw = 2; }
     }
     for (int a = 0; a < plan->n_aggs; a++) {
-        r->agg_word[a] = map[a] < 0 ? s1->nwords : s1->agg_word[map[a]];
-        r->agg_cnt_word[a] = map[a] < 0 ? 0 : s1->agg_cnt_word[map[a]];
-        r->agg_var_word[a] = map[a] < 0 ? 0 : s1->agg_var_word[map[a]];
+        L.agg_word[a] = map[a] < 0 ? L1.nwords : L1.agg_word[map[a]];
+        L.agg_cnt_word[a] = map[a] < 0 ? 0 : L1.agg_cnt_word[map[a]];
+        L.agg_var_word[a] = map[a] < 0 ? 0 : L1.agg_var_word[map[a]];
     }
-    result_layout L = L1;
-    L.wkind[s1->nwords] = WK_ADD_I64; L.winit[s1->nwords] = 0;
-    if (!g_layouts) g_layouts = new std::map<gx_result *, result_layout>();
-    (*g_layouts)[r] = L;
+    gx_result *r = new_result(ctx, plan, L, nullptr, 0, 0);        // its records once the fold has merged them
 
     const long long nrec = s1->ngroups;
     unsigned long long *d_fold = nullptr, *d_out = nullptr; long long ngroups = 0;
@@ -3886,13 +3868,7 @@ static int count_distinct_run(gx_ctx *ctx, const gx_table *outer, const gx_hash 
             if (e != cudaSuccess) { rc = GX_ERR_CUDA; GX_SET_ERR(ctx, "count(DISTINCT) fold: %s", cudaGetErrorString(e)); }
         }
         gx_result_free(s1);
-        if (rc == GX_OK) {
-            gx_agg_dev A; memset(&A, 0, sizeof(A));
-            A.P.nwords = nw; A.P.nkw = 2;
-            for (int i = 0; i < GX_MAX_WORDS; i++) { A.wkind[i] = L.wkind[i]; A.winit[i] = L.winit[i]; }
-            A.counters = ctx->d_scratch + 8;
-            rc = gx_aggregate_records(ctx, A, d_fold, nrec, &d_out, &ngroups);
-        }
+        if (rc == GX_OK) rc = gx_aggregate_records(ctx, merge_params(ctx, L), d_fold, nrec, &d_out, &ngroups);
         if (rc == GX_OK) rc = check_combine_overflow(ctx, r, { { d_fold, nrec } }, d_out, ngroups);
     }
     gx_tmp_free(ctx, d_fold);
@@ -4052,11 +4028,7 @@ int gx_aggregate_records(gx_ctx *ctx, gx_agg_dev A, unsigned long long *d_recs, 
 int gx_combine_records(gx_ctx *ctx, gx_result *r, unsigned long long *d_recs, long long nrec,
                        unsigned long long **d_out, long long *ngroups_out)
 {
-    gx_agg_dev A; memset(&A, 0, sizeof(A));
-    A.P.nwords = r->nwords; A.P.nkw = 2;
-    int rc = gx_result_layout_words(r, A.wkind, A.winit); if (rc) { GX_SET_ERR(ctx, "combine: unknown result"); return rc; }
-    A.counters = ctx->d_scratch + 8;
-    rc = gx_aggregate_records(ctx, A, d_recs, nrec, d_out, ngroups_out);
+    int rc = gx_aggregate_records(ctx, merge_params(ctx, r->L), d_recs, nrec, d_out, ngroups_out);
     if (rc == GX_OK) rc = check_combine_overflow(ctx, r, { { d_recs, nrec } }, *d_out, *ngroups_out);
     if (rc != GX_OK && *d_out) { gx_tmp_free(ctx, *d_out); *d_out = nullptr; *ngroups_out = 0; }
     return rc;
@@ -4066,9 +4038,9 @@ int gx_combine_records(gx_ctx *ctx, gx_result *r, unsigned long long *d_recs, lo
 int gx_pack_partial(gx_ctx *ctx, gx_result *r, long long cap, unsigned long long *d_seg)
 {
     gx_launch_scope ls(ctx, "combine_pack");
-    long long words = r->ngroups * r->rec_words;
+    long long words = r->ngroups * r->L.rec_words;
     unsigned grid = (unsigned) ((words + 255) / 256); if (grid < 1) grid = 1; if (grid > (unsigned) ctx->sm_count * 4) grid = (unsigned) ctx->sm_count * 4;
-    gx_k_pack_partial<<<grid, 256, 0, ctx->stream>>>((const unsigned long long *) r->d_recs, r->ngroups, cap, r->rec_words, d_seg);
+    gx_k_pack_partial<<<grid, 256, 0, ctx->stream>>>((const unsigned long long *) r->d_recs, r->ngroups, cap, r->L.rec_words, d_seg);
     GX_CUDA(ctx, cudaGetLastError());
     return GX_OK;
 }
@@ -4076,11 +4048,8 @@ int gx_pack_partial(gx_ctx *ctx, gx_result *r, long long cap, unsigned long long
 int gx_combine_gathered(gx_ctx *ctx, gx_result *r, const unsigned long long *d_gather, int nseg, long long cap, int rank, int nranks,
                         unsigned long long **d_out, long long *ngroups_out, int *anybig)
 {
-    gx_agg_dev A; memset(&A, 0, sizeof(A));
-    A.P.nwords = r->nwords; A.P.nkw = 2;
-    int rc = gx_result_layout_words(r, A.wkind, A.winit); if (rc) { GX_SET_ERR(ctx, "combine: unknown result"); return rc; }
-    A.counters = ctx->d_scratch + 8;
-    const int RW = 3 + r->nwords;
+    gx_agg_dev A = merge_params(ctx, r->L);
+    const int RW = r->L.rec_words;
     long long g_cap = gx_pow2_ceil(2 * (long long) nseg * cap + 1024);
     unsigned long long *g_tab, *d_groups;
     GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &g_tab, (size_t) g_cap * RW * 8));
@@ -4094,11 +4063,11 @@ int gx_combine_gathered(gx_ctx *ctx, gx_result *r, const unsigned long long *d_g
         long long total = (long long) nseg * cap;
         unsigned grid = (unsigned) ((total + 255) / 256); if (grid > (unsigned) ctx->sm_count * 8) grid = (unsigned) ctx->sm_count * 8;
         gx_k_merge_gathered<<<grid, 256, 0, ctx->stream>>>(A, d_gather, nseg, cap, rank, nranks);
-        gx_k_compact_groups<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(g_tab, g_cap, r->nwords, d_groups, ctx->d_scratch + 12);
+        gx_k_compact_groups<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(g_tab, g_cap, r->L.nwords, d_groups, ctx->d_scratch + 12);
     }
     GX_CUDA(ctx, cudaGetLastError());
     long long c[4];
-    rc = read_counters(ctx, c);
+    int rc = read_counters(ctx, c);
     gx_tmp_free(ctx, g_tab);
     if (rc == GX_OK && c[1]) { GX_SET_ERR(ctx, "combine: merge table overflowed"); rc = GX_ERR_STATE; }
     if (rc != GX_OK) { gx_tmp_free(ctx, d_groups); return rc; }
@@ -4145,12 +4114,8 @@ static int run_radix(gx_ctx *ctx, compiled_plan *cp, const gx_agg_plan *plan, lo
     int rc = gx_aggregate_records(ctx, A, d_recs, cap, &d_groups, &ngroups);
     gx_tmp_free(ctx, d_recs);
     if (rc) return rc;
-    gx_result *r; gx_result_alloc(ctx, plan, cp->group_types, ngroups, &r);
-    r->nkw = A.P.nkw; r->nwords = nwords; r->rec_words = RW; r->need_w0 = cp->need_w0;
-    for (int a = 0; a < plan->n_aggs; a++) { r->agg_word[a] = cp->agg_word[a]; r->agg_cnt_word[a] = cp->agg_cnt_word[a]; r->agg_var_word[a] = cp->agg_var_word[a]; }
-    r->d_recs = (long long *) d_groups; r->ngroups = ngroups; r->cap = ngroups;
-    if (!d_groups) { GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &r->d_recs, 64)); }
-    *out = r;
+    if (!d_groups) { GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d_groups, 64)); }
+    *out = new_result(ctx, plan, cp->L, d_groups, ngroups, ngroups);
     return GX_OK;
 }
 
@@ -4166,7 +4131,6 @@ extern "C" int64_t gx_result_ngroups(const gx_result *r)
 extern "C" void gx_result_free(gx_result *r)
 {
     if (!r) return;
-    if (g_layouts) g_layouts->erase(r);
     gx_tmp_free(r->ctx, r->d_recs);
     gx_tmp_free(r->ctx, r->d_nullmask);
     free(r);
@@ -4187,13 +4151,6 @@ bool gx_result_has_regr(const gx_result *r)
 {
     for (int a = 0; a < r->plan.n_aggs; a++) if (gx_is_regr_fn(r->plan.aggs[a].fn)) return true;
     return false;
-}
-int gx_result_layout_words(gx_result *r, int *wkind, long long *winit)
-{
-    if (!g_layouts || !g_layouts->count(r)) return GX_ERR_STATE;
-    const result_layout &L = (*g_layouts)[r];
-    for (int i = 0; i < GX_MAX_WORDS; i++) { wkind[i] = L.wkind[i]; winit[i] = L.winit[i]; }
-    return GX_OK;
 }
 
 // Sxx of a variance state {C, S1, S2} of n > 0 inputs: S2 - S1^2 / n, never negative (float8_accum's Sxx is not);
@@ -4255,71 +4212,101 @@ __host__ __device__ __forceinline__ double regr_final(int fn, const unsigned lon
     }
 }
 
-// finalize_aggregates (nodeAgg.c:1363).  float8_avg = Sx / N, NULL when N == 0 (float.c:2991-3008).
-// Small results are finalized on the host from the raw records; large ones (Q3: millions of
-// groups) on the device, straight into the caller's column layout, so the host only copies.
-struct gx_final_args {
-    const unsigned long long *recs; long long ngroups; int RW, ng, na, need_w0;
-    int gword[GX_MAX_GROUP_COLS], gshift[GX_MAX_GROUP_COLS], gtype[GX_MAX_GROUP_COLS];
-    int fn[GX_MAX_AGGS], word[GX_MAX_AGGS], cw[GX_MAX_AGGS], vw[GX_MAX_AGGS];
-    long long *key_out; double *agg_out; unsigned char *null_out;
-};
-__global__ void gx_k_finalize(const gx_final_args F)
+// a count(DISTINCT) word holds the count itself once folded: it finalizes as count(col)
+__host__ __device__ __forceinline__ int final_fn(int fn) { return fn == GX_AGG_COUNT_DISTINCT ? GX_AGG_COUNT : fn; }
+
+// group column c of a record, 0 when NULL (*isnull)
+__host__ __device__ __forceinline__ long long rec_key(const gx_rec_layout &L, const unsigned long long *rec, int c, bool *isnull)
 {
-    const long long stride = (long long) gridDim.x * blockDim.x;
-    for (long long gI = (long long) blockIdx.x * blockDim.x + threadIdx.x; gI < F.ngroups; gI += stride) {
-        const unsigned long long *rec = F.recs + (size_t) gI * F.RW, *w = rec + 3;
-        const unsigned int nullmask = (unsigned int) rec[0];
-        for (int c = 0; c < F.ng; c++) {
-            const bool isnull = (nullmask >> c) & 1;
-            const unsigned long long v = (F.gword[c] == 0 ? rec[1] : rec[2]) >> F.gshift[c];
-            long long sv;
-            switch (F.gtype[c]) {
-                case GX_INT4: case GX_DATE: sv = (long long) (int) (unsigned int) v; break;
-                case GX_CHAR: sv = (long long) (signed char) (unsigned char) v; break;
-                default: sv = (long long) v; break;
-            }
-            F.key_out[gI * F.ng + c] = isnull ? 0 : sv;
-            if (F.null_out) F.null_out[gI * (F.ng + F.na) + c] = isnull;
-        }
-        for (int a = 0; a < F.na; a++) {
-            const int fn = F.fn[a], word = F.word[a], cw = F.cw[a];
-            const long long cnt = cw ? (long long) w[cw] : (F.need_w0 ? (long long) w[0] : 1);
-            bool isnull = false, is_int = false; double res = 0.0; long long ires = 0;
-            switch (fn) {
-                case GX_AGG_COUNT_STAR: ires = (long long) w[0]; is_int = true; break;
-                case GX_AGG_COUNT: ires = (long long) w[word]; is_int = true; break;
-                case GX_AGG_SUM_I4: case GX_AGG_SUM_I8: ires = (long long) w[word]; is_int = true; isnull = cnt == 0; break;
-                case GX_AGG_AVG_F8: { const double sx = __longlong_as_double((long long) w[word]) + 0.0; if (cnt == 0) isnull = true; else res = sx / (double) cnt; break; }
-                case GX_AGG_VAR_POP_F8: case GX_AGG_VAR_SAMP_F8: case GX_AGG_STDDEV_POP_F8: case GX_AGG_STDDEV_SAMP_F8:
-                    res = var_final(fn, w, F.vw[a], cnt, &isnull); break;
-                default:
-                    if (gx_is_regr_fn(fn)) { res = regr_final(fn, w, word, cnt, &isnull, &ires); is_int = fn == GX_AGG_REGR_COUNT; break; }
-                    res = __longlong_as_double((long long) w[word]); isnull = cnt == 0; break;
-            }
-            if (isnull) { res = 0.0; ires = 0; }
-            F.agg_out[gI * F.na + a] = is_int ? __longlong_as_double(ires) : res;
-            if (F.null_out) F.null_out[gI * (F.ng + F.na) + F.ng + a] = isnull;
-        }
+    *isnull = ((unsigned int) rec[0] >> c) & 1;
+    if (*isnull) return 0;
+    const unsigned long long v = (L.gword[c] == 0 ? rec[1] : rec[2]) >> L.gshift[c];
+    switch (L.group_types[c]) {
+        case GX_INT4: case GX_DATE: return (long long) (int) (unsigned int) v;
+        case GX_CHAR: return (long long) (signed char) (unsigned char) v;
+        default: return (long long) v;
     }
 }
 
-// a count(DISTINCT) word holds the count itself once folded: it finalizes as count(col)
-static int final_fn(int fn) { return fn == GX_AGG_COUNT_DISTINCT ? GX_AGG_COUNT : fn; }
+// finalize_aggregates (nodeAgg.c:1363) of aggregate a, function fn, from its group's state words w: the 8 bytes of the
+// value (an integer result bit-cast), 0 when NULL (*isnull).  float8_avg = Sx / N, NULL when N == 0 (float.c:2991-3008).
+__host__ __device__ __forceinline__ long long agg_final(const gx_rec_layout &L, int a, int fn, const unsigned long long *w, bool *isnull)
+{
+    fn = final_fn(fn);
+    const int word = L.agg_word[a], cw = L.agg_cnt_word[a];
+    // cw == 0: the argument cannot be NULL, so a group that exists has input;
+    // w0 (rows per group) is only maintained when count(*)/avg need it
+    const long long cnt = cw ? (long long) w[cw] : (L.need_w0 ? (long long) w[0] : 1);
+    bool is_int = false; double res = 0.0; long long ires = 0;
+    *isnull = false;
+    switch (fn) {
+        case GX_AGG_COUNT_STAR: ires = (long long) w[0]; is_int = true; break;
+        case GX_AGG_COUNT: ires = (long long) w[word]; is_int = true; break;
+        case GX_AGG_SUM_I4: case GX_AGG_SUM_I8: ires = (long long) w[word]; is_int = true; *isnull = cnt == 0; break;
+        case GX_AGG_AVG_F8: { double sx; memcpy(&sx, &w[word], 8); sx += 0.0; if (cnt == 0) *isnull = true; else res = sx / (double) cnt; break; }
+        case GX_AGG_VAR_POP_F8: case GX_AGG_VAR_SAMP_F8: case GX_AGG_STDDEV_POP_F8: case GX_AGG_STDDEV_SAMP_F8:
+            res = var_final(fn, w, L.agg_var_word[a], cnt, isnull); break;
+        default:
+            if (gx_is_regr_fn(fn)) { res = regr_final(fn, w, word, cnt, isnull, &ires); is_int = fn == GX_AGG_REGR_COUNT; break; }
+            memcpy(&res, &w[word], 8); *isnull = cnt == 0; break;
+    }
+    if (*isnull) return 0;
+    if (!is_int) memcpy(&ires, &res, 8);
+    return ires;
+}
 
-static int fetch_on_device(gx_result *r, const result_layout &L, int64_t *key_out, double *agg_out, uint8_t *null_out)
+// Small results are finalized on the host from the raw records; large ones (Q3: millions of groups) on the device,
+// straight into the caller's column layout, so the host only copies.  Both run finalize_group over every group.
+struct gx_final_args {
+    const unsigned long long *recs; long long ngroups; int ng, na;
+    gx_rec_layout L;
+    int fn[GX_MAX_AGGS];
+    int64_t *key_out; double *agg_out; uint8_t *null_out;
+};
+__host__ __device__ __forceinline__ void finalize_group(const gx_final_args &F, long long gI)
+{
+    const unsigned long long *rec = F.recs + (size_t) gI * F.L.rec_words;
+    bool isnull;
+    for (int c = 0; c < F.ng; c++) {
+        F.key_out[gI * F.ng + c] = rec_key(F.L, rec, c, &isnull);
+        if (F.null_out) F.null_out[gI * (F.ng + F.na) + c] = isnull;
+    }
+    for (int a = 0; a < F.na; a++) {
+        const long long v = agg_final(F.L, a, F.fn[a], rec + 3, &isnull);
+        memcpy(&F.agg_out[gI * F.na + a], &v, 8);
+        if (F.null_out) F.null_out[gI * (F.ng + F.na) + F.ng + a] = isnull;
+    }
+}
+__global__ void gx_k_finalize(const gx_final_args F)
+{
+    const long long stride = (long long) gridDim.x * blockDim.x;
+    for (long long gI = (long long) blockIdx.x * blockDim.x + threadIdx.x; gI < F.ngroups; gI += stride) finalize_group(F, gI);
+}
+
+// What every fetch does once the result has groups to return: the caller's buffer must hold them all, then the
+// records come to the host in *h (h == nullptr: not copied).  who: the fetch's name in its error messages.
+static int fetch_records(gx_result *r, int64_t max_groups, const char *who, std::vector<unsigned long long> *h)
 {
     gx_ctx *ctx = r->ctx;
-    const int ng = r->plan.n_group_cols, na = r->plan.n_aggs;
+    GX_CHECK_ARG(ctx, max_groups >= r->ngroups, "%s: buffer holds %lld groups, result has %lld", who, (long long) max_groups, (long long) r->ngroups);
+    if (!h || r->ngroups == 0) return GX_OK;
+    h->resize((size_t) r->ngroups * r->L.rec_words);
+    cudaError_t e = cudaMemcpyAsync(h->data(), r->d_recs, h->size() * 8, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) { GX_SET_ERR(ctx, "%s: %s", who, cudaGetErrorString(e)); return GX_ERR_CUDA; }
+    return GX_OK;
+}
+
+static int fetch_on_device(gx_result *r, gx_final_args F, int64_t *key_out, double *agg_out, uint8_t *null_out)
+{
+    gx_ctx *ctx = r->ctx;
+    const int ng = F.ng, na = F.na;
     const size_t n = (size_t) r->ngroups;
-    gx_final_args F; memset(&F, 0, sizeof(F));
-    F.recs = (const unsigned long long *) r->d_recs; F.ngroups = r->ngroups; F.RW = r->rec_words; F.ng = ng; F.na = na; F.need_w0 = r->need_w0;
-    for (int c = 0; c < ng; c++) { F.gword[c] = L.gword[c]; F.gshift[c] = L.gshift[c]; F.gtype[c] = r->group_types[c]; }
-    for (int a = 0; a < na; a++) { F.fn[a] = final_fn(r->plan.aggs[a].fn); F.word[a] = r->agg_word[a]; F.cw[a] = r->agg_cnt_word[a]; F.vw[a] = r->agg_var_word[a]; }
     char *d = nullptr;
     const size_t kb = n * (ng > 0 ? ng : 1) * 8, ab = n * (na > 0 ? na : 1) * 8, nb = (n * (ng + na) + 15) & ~(size_t) 15;
     GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d, kb + ab + nb));
-    F.key_out = (long long *) d; F.agg_out = (double *) (d + kb); F.null_out = null_out ? (unsigned char *) (d + kb + ab) : nullptr;
+    F.recs = (const unsigned long long *) r->d_recs;
+    F.key_out = (int64_t *) d; F.agg_out = (double *) (d + kb); F.null_out = null_out ? (uint8_t *) (d + kb + ab) : nullptr;
     {
         gx_launch_scope ls(ctx, "finalize");
         gx_k_finalize<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(F);
@@ -4338,7 +4325,7 @@ extern "C" int gx_result_fetch(gx_result *r, int64_t max_groups, int64_t *key_ou
 {
     if (!r) return GX_ERR_ARG;
     gx_ctx *ctx = r->ctx;
-    const int ng = r->plan.n_group_cols, na = r->plan.n_aggs, RW = r->rec_words;
+    const int ng = r->plan.n_group_cols, na = r->plan.n_aggs;
     if (gx_result_plain_empty(r)) {
         GX_CHECK_ARG(ctx, max_groups >= 1, "result_fetch: buffer too small");
         for (int a = 0; a < na; a++) {
@@ -4349,55 +4336,16 @@ extern "C" int gx_result_fetch(gx_result *r, int64_t max_groups, int64_t *key_ou
         }
         return GX_OK;
     }
-    GX_CHECK_ARG(ctx, max_groups >= r->ngroups, "result_fetch: buffer holds %lld groups, result has %lld", (long long) max_groups, (long long) r->ngroups);
-    if (r->ngroups == 0) return GX_OK;
-    GX_CHECK_ARG(ctx, g_layouts && g_layouts->count(r), "result_fetch: unknown result");
-    const result_layout &L = (*g_layouts)[r];
-    if (r->ngroups > 8192) return fetch_on_device(r, L, key_out, agg_out, null_out);
-    unsigned long long *h = (unsigned long long *) malloc((size_t) r->ngroups * RW * 8);
-    cudaError_t e = cudaMemcpyAsync(h, r->d_recs, (size_t) r->ngroups * RW * 8, cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) { free(h); GX_SET_ERR(ctx, "result_fetch: %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
-    for (int64_t g = 0; g < r->ngroups; g++) {
-        const unsigned long long *rec = h + (size_t) g * RW, *w = rec + 3;
-        unsigned int nullmask = (unsigned int) rec[0];
-        for (int c = 0; c < ng; c++) {
-            bool isnull = (nullmask >> c) & 1;
-            unsigned long long v = (L.gword[c] == 0 ? rec[1] : rec[2]) >> L.gshift[c];
-            long long sv;
-            switch (r->group_types[c]) {
-                case GX_INT4: case GX_DATE: sv = (long long) (int32_t) (uint32_t) v; break;
-                case GX_CHAR: sv = (long long) (int8_t) (uint8_t) v; break;
-                default: sv = (long long) v; break;
-            }
-            key_out[g * ng + c] = isnull ? 0 : sv;
-            if (null_out) null_out[g * (ng + na) + c] = isnull;
-        }
-        for (int a = 0; a < na; a++) {
-            int fn = final_fn(r->plan.aggs[a].fn), word = r->agg_word[a], cw = r->agg_cnt_word[a];
-            // cw == 0: the argument cannot be NULL, so a group that exists has input;
-            // w0 (rows per group) is only maintained when count(*)/avg need it
-            long long cnt = cw ? (long long) w[cw] : (r->need_w0 ? (long long) w[0] : 1);
-            uint8_t isnull = 0; double res = 0.0; long long ires = 0; bool is_int = false;
-            switch (fn) {
-                case GX_AGG_COUNT_STAR: ires = (long long) w[0]; is_int = true; break;
-                case GX_AGG_COUNT: ires = (long long) w[word]; is_int = true; break;
-                case GX_AGG_SUM_I4: case GX_AGG_SUM_I8: ires = (long long) w[word]; is_int = true; isnull = cnt == 0; break;
-                case GX_AGG_AVG_F8: { double sx; memcpy(&sx, &w[word], 8); sx += 0.0; if (cnt == 0) isnull = 1; else res = sx / (double) cnt; break; }
-                case GX_AGG_VAR_POP_F8: case GX_AGG_VAR_SAMP_F8: case GX_AGG_STDDEV_POP_F8: case GX_AGG_STDDEV_SAMP_F8: {
-                    bool vn; res = var_final(fn, w, r->agg_var_word[a], cnt, &vn); isnull = vn; break;
-                }
-                default: {
-                    if (gx_is_regr_fn(fn)) { bool rn; res = regr_final(fn, w, word, cnt, &rn, &ires); isnull = rn; is_int = fn == GX_AGG_REGR_COUNT; break; }
-                    memcpy(&res, &w[word], 8); isnull = cnt == 0; break;
-                }
-            }
-            if (isnull) { res = 0.0; ires = 0; }
-            if (is_int) memcpy(&agg_out[g * na + a], &ires, 8); else agg_out[g * na + a] = res;
-            if (null_out) null_out[g * (ng + na) + ng + a] = isnull;
-        }
-    }
-    free(h);
+    const bool on_device = r->ngroups > 8192;
+    std::vector<unsigned long long> h;
+    int rc = fetch_records(r, max_groups, "result_fetch", on_device ? nullptr : &h);
+    if (rc != GX_OK) return rc;
+    gx_final_args F; memset(&F, 0, sizeof(F));
+    F.ngroups = r->ngroups; F.ng = ng; F.na = na; F.L = r->L;
+    for (int a = 0; a < na; a++) F.fn[a] = r->plan.aggs[a].fn;
+    if (on_device) return fetch_on_device(r, F, key_out, agg_out, null_out);
+    F.recs = h.data(); F.key_out = key_out; F.agg_out = agg_out; F.null_out = null_out;
+    for (int64_t gI = 0; gI < r->ngroups; gI++) finalize_group(F, gI);
     return GX_OK;
 }
 
@@ -4411,7 +4359,7 @@ extern "C" int gx_result_fetch_states(gx_result *r, int64_t max_groups, int64_t 
 {
     if (!r || !key_out || !val_out || !cnt_out) return GX_ERR_ARG;
     gx_ctx *ctx = r->ctx;
-    const int ng = r->plan.n_group_cols, na = r->plan.n_aggs, RW = r->rec_words;
+    const int ng = r->plan.n_group_cols, na = r->plan.n_aggs, RW = r->L.rec_words;
     GX_CHECK_ARG(ctx, !gx_result_has_distinct(r), "result_fetch_states: a count(DISTINCT) result has no partial state");
     if (gx_result_plain_empty(r)) {                             // plain aggregate over zero rows: initial states
         GX_CHECK_ARG(ctx, max_groups >= 1, "result_fetch_states: buffer too small");
@@ -4422,33 +4370,20 @@ extern "C" int gx_result_fetch_states(gx_result *r, int64_t max_groups, int64_t 
         }
         return GX_OK;
     }
-    GX_CHECK_ARG(ctx, max_groups >= r->ngroups, "result_fetch_states: buffer holds %lld groups, result has %lld", (long long) max_groups, (long long) r->ngroups);
-    if (r->ngroups == 0) return GX_OK;
-    GX_CHECK_ARG(ctx, g_layouts && g_layouts->count(r), "result_fetch_states: unknown result");
-    const result_layout &L = (*g_layouts)[r];
-    unsigned long long *h = (unsigned long long *) malloc((size_t) r->ngroups * RW * 8);
-    cudaError_t e = cudaMemcpyAsync(h, r->d_recs, (size_t) r->ngroups * RW * 8, cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) { free(h); GX_SET_ERR(ctx, "result_fetch_states: %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
+    std::vector<unsigned long long> h;
+    int rc = fetch_records(r, max_groups, "result_fetch_states", &h);
+    if (rc != GX_OK) return rc;
     for (int64_t gI = 0; gI < r->ngroups; gI++) {
-        const unsigned long long *rec = h + (size_t) gI * RW, *w = rec + 3;
-        const unsigned int nullmask = (unsigned int) rec[0];
+        const unsigned long long *rec = h.data() + (size_t) gI * RW, *w = rec + 3;
         for (int c = 0; c < ng; c++) {
-            const bool isnull = (nullmask >> c) & 1;
-            const unsigned long long v = (L.gword[c] == 0 ? rec[1] : rec[2]) >> L.gshift[c];
-            long long sv;
-            switch (r->group_types[c]) {
-                case GX_INT4: case GX_DATE: sv = (long long) (int32_t) (uint32_t) v; break;
-                case GX_CHAR: sv = (long long) (int8_t) (uint8_t) v; break;
-                default: sv = (long long) v; break;
-            }
-            key_out[gI * ng + c] = isnull ? 0 : sv;
+            bool isnull;
+            key_out[gI * ng + c] = rec_key(r->L, rec, c, &isnull);
             if (null_out) null_out[gI * (ng + na) + c] = isnull;
         }
         for (int a = 0; a < na; a++) {
-            const int fn = r->plan.aggs[a].fn, word = r->agg_word[a], cw = r->agg_cnt_word[a];
+            const int fn = r->plan.aggs[a].fn, word = r->L.agg_word[a], cw = r->L.agg_cnt_word[a];
             const long long rows = (long long) w[0];
-            const long long cnt = cw ? (long long) w[cw] : (r->need_w0 ? rows : 1);
+            const long long cnt = cw ? (long long) w[cw] : (r->L.need_w0 ? rows : 1);
             double v = 0.0; long long n = cnt; uint8_t isnull = 0;
             switch (fn) {
                 case GX_AGG_COUNT_STAR: n = rows; break;
@@ -4465,7 +4400,6 @@ extern "C" int gx_result_fetch_states(gx_result *r, int64_t max_groups, int64_t 
             if (null_out) null_out[gI * (ng + na) + ng + a] = isnull;
         }
     }
-    free(h);
     return GX_OK;
 }
 
@@ -4474,25 +4408,22 @@ extern "C" int gx_result_fetch_sxx(gx_result *r, int64_t max_groups, double *sxx
 {
     if (!r || !sxx_out) return GX_ERR_ARG;
     gx_ctx *ctx = r->ctx;
-    const int na = r->plan.n_aggs, RW = r->rec_words;
+    const int na = r->plan.n_aggs, RW = r->L.rec_words;
     GX_CHECK_ARG(ctx, !gx_result_has_distinct(r), "result_fetch_sxx: a count(DISTINCT) result has no partial state");
     if (gx_result_plain_empty(r)) {                                  // plain aggregate over zero rows: '{0,0,0}'
         GX_CHECK_ARG(ctx, max_groups >= 1, "result_fetch_sxx: buffer too small");
         for (int a = 0; a < na; a++) sxx_out[a] = 0.0;
         return GX_OK;
     }
-    GX_CHECK_ARG(ctx, max_groups >= r->ngroups, "result_fetch_sxx: buffer holds %lld groups, result has %lld", (long long) max_groups, (long long) r->ngroups);
-    if (r->ngroups == 0) return GX_OK;
-    std::vector<unsigned long long> h((size_t) r->ngroups * RW);
-    cudaError_t e = cudaMemcpyAsync(h.data(), r->d_recs, h.size() * 8, cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) { GX_SET_ERR(ctx, "result_fetch_sxx: %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
+    std::vector<unsigned long long> h;
+    int rc = fetch_records(r, max_groups, "result_fetch_sxx", &h);
+    if (rc != GX_OK) return rc;
     for (int64_t gI = 0; gI < r->ngroups; gI++) {
         const unsigned long long *w = h.data() + (size_t) gI * RW + 3;
         for (int a = 0; a < na; a++) {
             double sxx = 0.0;
             if (gx_is_var_fn(r->plan.aggs[a].fn)) {
-                const int cw = r->agg_cnt_word[a], vw = r->agg_var_word[a];
+                const int cw = r->L.agg_cnt_word[a], vw = r->L.agg_var_word[a];
                 const long long n = cw ? (long long) w[cw] : (long long) w[0];
                 double s1, s2; memcpy(&s1, &w[vw + 1], 8); memcpy(&s2, &w[vw + 2], 8);
                 if (n > 0) sxx = var_sxx(s1, s2, n);
@@ -4509,27 +4440,24 @@ extern "C" int gx_result_fetch_regr(gx_result *r, int64_t max_groups, double *ou
 {
     if (!r || !out) return GX_ERR_ARG;
     gx_ctx *ctx = r->ctx;
-    const int na = r->plan.n_aggs, RW = r->rec_words;
+    const int na = r->plan.n_aggs, RW = r->L.rec_words;
     GX_CHECK_ARG(ctx, !gx_result_has_distinct(r), "result_fetch_regr: a count(DISTINCT) result has no partial state");
     if (gx_result_plain_empty(r)) {                                  // plain aggregate over zero rows: '{0,0,0,0,0,0}'
         GX_CHECK_ARG(ctx, max_groups >= 1, "result_fetch_regr: buffer too small");
         for (int i = 0; i < na * 6; i++) out[i] = 0.0;
         return GX_OK;
     }
-    GX_CHECK_ARG(ctx, max_groups >= r->ngroups, "result_fetch_regr: buffer holds %lld groups, result has %lld", (long long) max_groups, (long long) r->ngroups);
-    if (r->ngroups == 0) return GX_OK;
-    std::vector<unsigned long long> h((size_t) r->ngroups * RW);
-    cudaError_t e = cudaMemcpyAsync(h.data(), r->d_recs, h.size() * 8, cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) { GX_SET_ERR(ctx, "result_fetch_regr: %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
+    std::vector<unsigned long long> h;
+    int rc = fetch_records(r, max_groups, "result_fetch_regr", &h);
+    if (rc != GX_OK) return rc;
     for (int64_t gI = 0; gI < r->ngroups; gI++) {
         const unsigned long long *w = h.data() + (size_t) gI * RW + 3;
         for (int a = 0; a < na; a++) {
             double *st = out + ((size_t) gI * na + a) * 6;
             const int fn = r->plan.aggs[a].fn;
             if (!gx_is_regr_fn(fn) || fn == GX_AGG_REGR_COUNT) { for (int i = 0; i < 6; i++) st[i] = 0.0; continue; }
-            const int cw = r->agg_cnt_word[a];
-            regr_state(w, r->agg_word[a], cw ? (long long) w[cw] : (long long) w[0], st);
+            const int cw = r->L.agg_cnt_word[a];
+            regr_state(w, r->L.agg_word[a], cw ? (long long) w[cw] : (long long) w[0], st);
         }
     }
     return GX_OK;

@@ -1054,8 +1054,6 @@ extern "C" int gx_debug_redistribute(gx_ctx *ctx, int nparts, const gx_table *co
 }
 
 // ------------------------------------------- Finalize across datanodes
-struct gx_agg_dev;
-int gx_result_layout_words(gx_result *r, int *wkind, long long *winit);
 int gx_combine_records(gx_ctx *ctx, gx_result *r, unsigned long long *d_recs, long long nrec,
                        unsigned long long **d_out, long long *ngroups_out);   // gx_agg.cu
 int gx_pack_partial(gx_ctx *ctx, gx_result *r, long long cap, unsigned long long *d_seg);
@@ -1174,7 +1172,7 @@ struct gx_inproc_transport : gx_combine_transport {
     {
         for (int p = 0; p < nranks; p++) {
             if (p == rank) { memcpy(all + (size_t) p * nranks, mine, (size_t) nranks * 8); continue; }
-            int rc = partition_records(ctx, (const unsigned long long *) parts[p]->d_recs, parts[p]->ngroups, parts[p]->rec_words, nranks,
+            int rc = partition_records(ctx, (const unsigned long long *) parts[p]->d_recs, parts[p]->ngroups, parts[p]->L.rec_words, nranks,
                                        &send[p], sendoff[p], all + (size_t) p * nranks);
             if (rc) return rc;
         }
@@ -1203,7 +1201,7 @@ static int combine_run(gx_ctx *ctx, gx_result *r, gx_combine_transport &T)
     GX_CHECK_ARG(ctx, N == 1 || !gx_result_has_variance(r), "combine: variance states are not combined across %d ranks", N);
     GX_CHECK_ARG(ctx, N == 1 || !gx_result_has_regr(r), "combine: regression states are not combined across %d ranks", N);
     if (N == 1 || r->finalized_across) return GX_OK;
-    const int RW = r->rec_words;
+    const int RW = r->L.rec_words;
     long long nrec = r->ngroups;
     auto finish = [&](unsigned long long *d_groups, long long ngroups, long long cap) {
         gx_tmp_free(ctx, r->d_recs);
@@ -1279,8 +1277,8 @@ extern "C" int gx_debug_combine(gx_ctx *ctx, int nparts, gx_result *const *parts
         GX_CHECK_ARG(ctx, a != nullptr, "debug_combine: part %d is NULL", p);
         GX_CHECK_ARG(ctx, !a->finalized_across, "debug_combine: part %d was combined already", p);
         GX_CHECK_ARG(ctx, memcmp(&a->plan, &b->plan, sizeof(a->plan)) == 0, "debug_combine: part %d has another plan than part 0", p);
-        GX_CHECK_ARG(ctx, a->rec_words == b->rec_words && memcmp(a->agg_word, b->agg_word, sizeof(a->agg_word)) == 0 &&
-                     memcmp(a->agg_cnt_word, b->agg_cnt_word, sizeof(a->agg_cnt_word)) == 0,
+        GX_CHECK_ARG(ctx, a->L.rec_words == b->L.rec_words && memcmp(a->L.agg_word, b->L.agg_word, sizeof(a->L.agg_word)) == 0 &&
+                     memcmp(a->L.agg_cnt_word, b->L.agg_cnt_word, sizeof(a->L.agg_cnt_word)) == 0,
                      "debug_combine: part %d has another record layout than part 0", p);
     }
     gx_inproc_transport T(ctx, parts);

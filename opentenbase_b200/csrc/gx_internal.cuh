@@ -135,27 +135,34 @@ static inline gx_slotfn gx_hash_slotfn(const gx_hash *h)
 }
 cudaError_t gx_stage_mark(gx_ctx *ctx, const void *host);   // gx_exec.cu: record "copy of this staging slot enqueued"   // materialise the 16-byte slot array of a compact table
 
-// A group-state record: [k0][k1][w0..w(nwords-1)], 8-byte words.
+// A group-state record: [null bits][k0][k1][w0..w(nwords-1)], 8-byte words.
 // w0 is always the group's row count.
 #define GX_MAX_WORDS 18
+
+// where a record keeps each group column and each aggregate's state, and how its state words merge
+struct gx_rec_layout {
+    int nkw;                         // key words (1 or 2)
+    int nwords;                      // state words
+    int rec_words;                   // 3 + nwords (the null bits, k0 and k1 are always present)
+    int need_w0;                     // w0 (rows per group) is maintained
+    int32_t group_types[GX_MAX_GROUP_COLS];
+    int gword[GX_MAX_GROUP_COLS], gshift[GX_MAX_GROUP_COLS], gbytes[GX_MAX_GROUP_COLS];   // k0 or k1, bit offset, width
+    int agg_word[GX_MAX_AGGS];       // first word of the aggregate's state
+    int agg_cnt_word[GX_MAX_AGGS];   // word holding its non-NULL input count (may be 0 = row count)
+    int agg_var_word[GX_MAX_AGGS];   // variance aggregates: the shift C, followed by S1 and S2 (0 = none)
+    int wkind[GX_MAX_WORDS];         // merge kind of each state word (gx_agg.cu, WK_*)
+    long long winit[GX_MAX_WORDS];   // initial value of each state word
+};
 
 struct gx_result {
     gx_ctx *ctx;
     gx_agg_plan plan;
-    int32_t group_types[GX_MAX_GROUP_COLS];
-    int nkw;                         // key words (1 or 2)
-    int nwords;                      // state words
-    int rec_words;                   // 2 + nwords (k0,k1 always present in records)
-    // per-agg state layout
-    int agg_word[GX_MAX_AGGS];       // first word of the aggregate's state
-    int agg_cnt_word[GX_MAX_AGGS];   // word holding its non-NULL input count (may be 0 = row count)
-    int agg_var_word[GX_MAX_AGGS];   // variance aggregates: the shift C, followed by S1 and S2 (0 = none)
-    long long *d_recs;               // ngroups * rec_words (dense, partial states)
+    gx_rec_layout L;
+    long long *d_recs;               // ngroups * L.rec_words (dense, partial states)
     unsigned int *d_nullmask;        // ngroups (group-key null bits)
     int64_t ngroups, cap;
     int finalized_across;            // combined over the communicator already
     int plain_row_elsewhere;         // combined plain aggregate: another rank returns its one row
-    int need_w0;                     // w0 (rows per group) is maintained
 };
 // a plain aggregate over zero rows: this result returns the one row of initial states
 static inline bool gx_result_plain_empty(const gx_result *r) { return r->plan.n_group_cols == 0 && r->ngroups == 0 && !r->plain_row_elsewhere; }
@@ -206,7 +213,6 @@ static inline void gx_tmp_free(gx_ctx *ctx, void *p) { if (p) cudaFreeAsync(p, c
 
 int gx_table_alloc_like(gx_ctx *ctx, int ncols, const int32_t *types, const bool *has_nulls,
                         int64_t capacity, gx_table **out);
-int gx_result_alloc(gx_ctx *ctx, const gx_agg_plan *plan, const int32_t *group_types, int64_t cap, gx_result **out);
 // GX_ERR_ARG unless the plan's join type is one gx_hash_agg runs (INNER, SEMI, ANTI)
 int gx_check_agg_join_type(gx_ctx *ctx, const gx_agg_plan *plan);
 

@@ -12,8 +12,11 @@ import pytest
 
 import opentenbase_b200 as g
 import oracle as O
+import distinct_ref as DR
 import exact_ref as X
 import fp_edge_data as D
+import regr_ref as R
+import var_ref as V
 from helpers import to_gpu_plan
 
 pytestmark = pytest.mark.gpu
@@ -223,6 +226,94 @@ def test_fetch_paths_see_special_values(gx, name, ngroups):
     groups = [D.SPECIAL_GROUPS[i % len(D.SPECIAL_GROUPS)] for i in range(ngroups)]
     gi, x, y = D.special(np.random.default_rng(5), groups)
     fam.check(gi, x, y, SHAPES["general"][0], gkey_of=lambda i: i * 3 - 9000)
+
+
+INF, NAN = float("inf"), float("nan")
+# test_finalize_paths_agree: group shapes as (x, y, v) rows, None for NULL; None for an ordinary group.  At most four
+# inputs of small dyadic values per group: every state is exact in whatever order the rows arrive, so two runs over
+# the same rows hold the same states
+FINAL_SHAPES = [
+    [(None, None, None)] * 2,                                            # all inputs NULL
+    [(1.5, -2.5, 7)],                                                    # one input: the _samp variances, covar_samp NULL
+    [(2.0, 1.0, 1), (2.0, 2.0, 1), (2.0, 4.0, 2), (2.0, 9.0, 3)],        # constant X: corr, regr_slope NULL
+    [(1.0, 5.0, 4), (2.0, 5.0, 4), (3.0, 5.0, 4), (6.0, 5.0, 5)],        # constant Y, varying X: regr_r2 = 1
+    [(INF, 1.0, 1), (1.0, 2.0, 2), (2.0, 3.0, 3), (3.0, 4.0, 4)],
+    [(1.0, -INF, 1), (2.0, 1.0, 1), (0.5, 1.0, 2), (4.0, 2.0, 2)],
+    [(NAN, 1.0, 6), (1.0, 1.0, 6), (2.0, NAN, 6), (3.0, 2.0, 6)],
+    [(-0.0, -0.0, 0), (-0.0, -0.0, 0)],                                  # sums that end at -0
+    None, None,
+]
+X1, Y2, V3 = [(C, 1, 0)], [(C, 2, 0)], [(C, 3, 0)]
+PAIR = Y2 + [(g.GX_OP_ARG2, 0, 0)] + X1
+# every aggregate function of the ABI but the declined sum(int8), in as many plans as GX_MAX_AGGS asks for
+FINAL_PLANS = [
+    [CNT, (g.GX_AGG_COUNT, V3), (g.GX_AGG_SUM_I4, V3), SX, AX, NX, MX],
+    [(fn, X1) for fn in V.VAR_FNS] + [(fn, PAIR) for fn in R.REGR_FNS[:4]],
+    [(fn, PAIR) for fn in R.REGR_FNS[4:]],
+    [(g.GX_AGG_COUNT_DISTINCT, V3), CNT, SX],
+]
+INT_RESULTS = {g.GX_AGG_COUNT_STAR, g.GX_AGG_COUNT, g.GX_AGG_SUM_I4, g.GX_AGG_REGR_COUNT, g.GX_AGG_COUNT_DISTINCT}
+
+
+def _final_bits(aggs, vals):
+    """the result bits, NaN payloads canonicalised in the float8 results: a NaN the final itself makes (inf - inf in a
+    variance's Sxx) is the default NaN of whichever processor finalized"""
+    b = vals.view(np.int64).copy()
+    for a, (fn, _) in enumerate(aggs):
+        if fn not in INT_RESULTS:
+            b[np.isnan(vals[:, a]), a] = np.float64(NAN).view(np.int64)
+    return b
+
+
+def test_finalize_paths_agree(gx):
+    """8193 groups are finalized on the device (gx_k_finalize), the same rows without one ordinary group on the host
+    (8192): every aggregate function over groups without input, with one input, a constant X or Y, +-inf, NaN and
+    sums ending at -0 gives the same bits and NULL flags on both paths, and both match the exact references"""
+    rng = np.random.default_rng(9)
+    gi, xs, ys, vs = [], [], [], []
+    for i in range(8193):
+        shape = FINAL_SHAPES[i % len(FINAL_SHAPES)]
+        if shape is None:
+            shape = [(rng.integers(-8, 9) / 4, rng.integers(-8, 9) / 4, int(rng.integers(0, 3))) for _ in range(4)]
+            if i % 3 == 0:
+                shape.append((None, None, None))
+        for x, y, v in shape:
+            gi.append(i); xs.append(x); ys.append(y); vs.append(v)
+    gi = np.array(gi)
+    drop = max(i for i in range(8193) if FINAL_SHAPES[i % len(FINAL_SHAPES)] is None)
+    gkeys = [(i * 3 - 9000,) for i in range(8193)]
+    types = [g.GX_INT4, g.GX_FLOAT8, g.GX_FLOAT8, g.GX_INT4]
+    runs = {}
+    for ngroups, rows in ((8193, np.arange(len(gi))), (8192, np.flatnonzero(gi != drop))):
+        key = (gi[rows] * 3 - 9000).astype(np.int32)
+        cols = [key] + [np.array([0 if vals[r] is None else vals[r] for r in rows], t) for vals, t in ((xs, np.float64), (ys, np.float64), (vs, np.int32))]
+        nulls = [None] + [np.array([vals[r] is None for r in rows], np.uint8) for vals in (xs, ys, vs)]
+        t = gx.table_from(types, cols, nulls)
+        runs[ngroups] = []
+        for aggs in FINAL_PLANS:
+            plan = g.make_plan(group_cols=[(0, 0)], aggs=aggs, est_groups=ngroups)
+            gx.profile(True)
+            got = gx.hash_agg(t, plan).fetch()
+            on_device = gx.profile_get("finalize")[1] > 0
+            gx.profile(False)
+            assert on_device == (ngroups > 8192) and len(got[0]) == ngroups
+            if aggs[0][0] == g.GX_AGG_COUNT_DISTINCT:
+                DR.check(plan, DR.expect_groups(plan, cols, types, np.arange(len(rows)), nulls), got, [g.GX_INT4])
+            elif aggs[0] == CNT:
+                X.check(plan, X.expect_groups(plan, cols, nulls, gindex=gi[rows], gkeys=gkeys), got, [g.GX_INT4])
+            else:
+                checked = R.check(plan, cols, nulls, key.astype(np.int64), got)
+                if aggs[0][0] in V.VAR_FNS:
+                    checked += V.check(plan, cols, nulls, key.astype(np.int64), got)
+                assert checked == ngroups * len(aggs)
+            runs[ngroups].append(got)
+        t.free()
+    for aggs, (k0, a0, n0), (k1, a1, n1) in zip(FINAL_PLANS, runs[8193], runs[8192]):
+        at = {int(k): i for i, k in enumerate(k0[:, 0])}
+        rows = np.array([at[int(k)] for k in k1[:, 0]])
+        assert (drop * 3 - 9000) not in set(k1[:, 0].tolist())
+        np.testing.assert_array_equal(_final_bits(aggs, a0[rows]), _final_bits(aggs, a1))
+        np.testing.assert_array_equal(n0[rows], n1)
 
 
 def test_sum_int8_is_declined(gx):
