@@ -2942,36 +2942,60 @@ static size_t smem_bytes_for(int S, int nkw, int nwords) { return (size_t) S * 8
 
 static int ilog2(long long x) { int l = 0; while ((1LL << l) < x) l++; return l; }
 
+// calls fn with the slot format of the plan's join table as a compile-time constant (std::integral_constant)
 template <class FN> static int with_slot_format(const gx_agg_dev &A, FN fn)
 {
     if (A.narrow) return fn(std::integral_constant<int, GX_SLOTS_NARROW>());
     if (A.cslots) return fn(std::integral_constant<int, GX_SLOTS_COMPACT>());
     return fn(std::integral_constant<int, GX_SLOTS_WIDE>());
 }
+// calls fn with what a specialised kernel accumulates, (count, sum), as compile-time constants (std::bool_constant):
+// both, the count only or the sum only
+template <class FN> static int with_cnt_sum(bool cnt, bool sum, FN fn)
+{
+    if (cnt && sum) return fn(std::true_type(), std::true_type());
+    if (cnt) return fn(std::true_type(), std::false_type());
+    return fn(std::false_type(), std::true_type());
+}
+
+// CTAs for `units` of work, `per_cta` to a CTA: at least 1, at most `cap`.  A kernel that counts a CTA's rows in
+// `bits`-bit counters gets a larger cap while a CTA's share of the `rows` would reach 2^bits.
+static unsigned agg_grid(long long units, long long per_cta, long long cap, long long rows = 0, int bits = 0)
+{
+    while (bits && (rows + cap - 1) / cap >= (1LL << bits)) cap *= 2;
+    const long long nb = (units + per_cta - 1) / per_cta;
+    return (unsigned) (nb < cap ? (nb > 0 ? nb : 1) : cap);
+}
+
+// One launch of the aggregate kernel K.  The first one raises K's dynamic shared-memory limit to smem_attr (< 0: left as
+// it is).  The launch counts under `name`, with `which` and `fmt` as second and third profile names (gx_profile_get;
+// nullptr: none).
+template <auto *K, class... Args>
+static int launch_kernel(gx_ctx *ctx, int smem_attr, unsigned grid, int threads, size_t smem, const char *name, const char *which,
+                         const char *fmt, const Args &... args)
+{
+    static bool attr_set = false;
+    if (smem_attr >= 0 && !attr_set) {
+        GX_CUDA(ctx, cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_attr));
+        attr_set = true;
+    }
+    gx_launch_scope ls(ctx, name), w(ctx, which, 0), f(ctx, fmt, 0);
+    K<<<grid, threads, smem, ctx->stream>>>(args...);
+    GX_CUDA(ctx, cudaGetLastError());
+    return GX_OK;
+}
 
 template <int SINK, int XF, bool REGR>
 static int launch_agg_kr(gx_ctx *ctx, const gx_agg_dev &A, size_t smem, const char *name, int threads)
 {
-    static bool attr_set = false;
-    if (!attr_set) {
-        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_agg<SINK, XF, REGR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
-        attr_set = true;
-    }
-    long long nrows = A.row1 - A.row0;
-    long long nb = (nrows + threads - 1) / threads, maxb = (long long) ctx->sm_count;
-    // the shared-memory counters are 32-bit per CTA
-    while ((nrows + maxb - 1) / maxb >= (1LL << 32)) maxb *= 2;
-    unsigned grid = (unsigned) (nb < maxb ? (nb > 0 ? nb : 1) : maxb);
-    gx_launch_scope ls(ctx, name);
-    // second profile name: which sink answered (gx_profile_get)
-    gx_launch_scope which(ctx, SINK == SINK_SMEM_LP ? "agg_smem_lp" : SINK == SINK_SMEM ? "agg_smem" : SINK == SINK_GLOBAL ? "agg_global" : "agg_records", 0);
-    // third profile name of a SEMI / ANTI plan or a join chain: the slot format its (first) probe read
-    gx_launch_scope fmt(ctx, XF == GX_SLOTS_NARROW ? "probe_agg_exist_narrow" : XF == GX_SLOTS_COMPACT ? "probe_agg_exist_compact" :
-                             XF == GX_SLOTS_WIDE ? "probe_agg_exist_wide" : XF == GX_XF_CHAIN + GX_SLOTS_NARROW ? "probe_agg_chain_narrow" :
-                             XF == GX_XF_CHAIN + GX_SLOTS_COMPACT ? "probe_agg_chain_compact" : XF == GX_XF_CHAIN + GX_SLOTS_WIDE ? "probe_agg_chain_wide" : nullptr, 0);
-    gx_k_agg<SINK, XF, REGR><<<grid, threads, smem, ctx->stream>>>(A);
-    GX_CUDA(ctx, cudaGetLastError());
-    return GX_OK;
+    const long long nrows = A.row1 - A.row0;
+    // second profile name: which sink answered; third, of a SEMI / ANTI plan or a join chain: the slot format its (first)
+    // probe read.  The shared-memory counters are 32-bit per CTA.
+    return launch_kernel<gx_k_agg<SINK, XF, REGR>>(ctx, (int) ctx->smem_optin, agg_grid(nrows, threads, ctx->sm_count, nrows, 32), threads, smem, name,
+        SINK == SINK_SMEM_LP ? "agg_smem_lp" : SINK == SINK_SMEM ? "agg_smem" : SINK == SINK_GLOBAL ? "agg_global" : "agg_records",
+        XF == GX_SLOTS_NARROW ? "probe_agg_exist_narrow" : XF == GX_SLOTS_COMPACT ? "probe_agg_exist_compact" :
+        XF == GX_SLOTS_WIDE ? "probe_agg_exist_wide" : XF == GX_XF_CHAIN + GX_SLOTS_NARROW ? "probe_agg_chain_narrow" :
+        XF == GX_XF_CHAIN + GX_SLOTS_COMPACT ? "probe_agg_chain_compact" : XF == GX_XF_CHAIN + GX_SLOTS_WIDE ? "probe_agg_chain_wide" : nullptr, A);
 }
 // a plan with a regression state takes the instantiation that updates and merges it
 template <int SINK, int XF>
@@ -2989,75 +3013,67 @@ static int launch_agg(gx_ctx *ctx, const gx_agg_dev &A, size_t smem, const char 
     return with_slot_format(A, [&](auto f) { return launch_agg_k<SINK, decltype(f)::value>(ctx, A, smem, name, threads); });
 }
 
-template <int K>
-static int launch_lptile_k(gx_ctx *ctx, const gx_agg_dev &A, size_t smem, const char *name, int threads)
-{
-    static bool attr_set = false;
-    if (!attr_set) {
-        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_agg_lptile<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
-        attr_set = true;
-    }
-    long long nrows = A.row1 - A.row0, per_block = (long long) (threads / 32) * 32 * K;
-    long long nb = (nrows + per_block - 1) / per_block, maxb = (long long) ctx->sm_count;
-    unsigned grid = (unsigned) (nb < maxb ? (nb > 0 ? nb : 1) : maxb);
-    gx_launch_scope ls(ctx, name);
-    gx_launch_scope which(ctx, K == 8 ? "agg_lptile8" : "agg_lptile4", 0);
-    gx_k_agg_lptile<K><<<grid, threads, smem, ctx->stream>>>(A);
-    GX_CUDA(ctx, cudaGetLastError());
-    return GX_OK;
-}
-static int launch_lptile(gx_ctx *ctx, const gx_agg_dev &A, size_t smem, const char *name, int threads)
-{
-    const char *k4 = getenv("GX_LPTILE_K4");
-    if (threads <= 640 && !(k4 && k4[0] == '1')) return launch_lptile_k<8>(ctx, A, smem, name, threads);
-    return launch_lptile_k<4>(ctx, A, smem, name, threads);
-}
-
-template <bool JOIN, bool HAS_CNT, bool HAS_SUM>
-static int launch_fast_t(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_args &FA, size_t smem, const char *name)
-{
-    static bool attr_set = false;
-    if (!attr_set) {
-        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_fast<JOIN, HAS_CNT, HAS_SUM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
-        attr_set = true;
-    }
-    long long nvec = (A.row1 - A.row0 + 3) / 4;
-    long long nb = (nvec + 1023) / 1024, maxb = (long long) ctx->sm_count;
-    while ((A.row1 - A.row0 + maxb - 1) / maxb >= (1LL << 32)) maxb *= 2;
-    unsigned grid = (unsigned) (nb < maxb ? (nb > 0 ? nb : 1) : maxb);
-    gx_launch_scope ls(ctx, name);
-    gx_launch_scope which(ctx, JOIN ? "probe_agg_fast" : "agg_fast", 0);
-    gx_k_fast<JOIN, HAS_CNT, HAS_SUM><<<grid, 1024, smem, ctx->stream>>>(A, FA);
-    GX_CUDA(ctx, cudaGetLastError());
-    return GX_OK;
-}
-template <bool HAS_CNT, bool HAS_SUM, int FMT>
-static int launch_runjoin_t(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_args &FA, size_t smem, const char *name)
-{
-    static bool attr_set = false;
-    if (!attr_set) {
-        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runjoin<HAS_CNT, HAS_SUM, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
-        attr_set = true;
-    }
-    long long nvec = (A.row1 - A.row0 + 3) / 4;
-    long long nb = (nvec + 1023) / 1024, maxb = (long long) ctx->sm_count;
-    while ((A.row1 - A.row0 + maxb - 1) / maxb >= (1LL << 32)) maxb *= 2;
-    unsigned grid = (unsigned) (nb < maxb ? (nb > 0 ? nb : 1) : maxb);
-    gx_launch_scope ls(ctx, name);
-    gx_launch_scope which(ctx, "probe_agg_run", 0);
-    gx_k_runjoin<HAS_CNT, HAS_SUM, FMT><<<grid, 1024, smem, ctx->stream>>>(A, FA);
-    GX_CUDA(ctx, cudaGetLastError());
-    return GX_OK;
-}
 // Probe kernel at SF100 on one H100 80GB HBM3 (700 W), bench.py, two runs each: gx_k_runjoin 4.256 / 4.258 ms,
 // gx_k_runjoin_tma 3.937 / 3.934 ms, with the branch-free fold 4.043 / 4.039 ms, + full probe rounds only 3.971 / 3.965 ms
 // -> 1 is the default; GX_RUNJOIN_TMA=0 restores gx_k_runjoin
 #define GX_RUNJOIN_TMA_DEFAULT 1         /* 0 off, 1 gx_k_runjoin_tma, 2 + branch-free fold, 3 + probe rounds of 32 lanes only */
+// GX_RUNJOIN_SEG=1/0 selects / forbids gx_k_runjoin_seg; a run that raised flag 16 (a bounded mbarrier wait gave up)
+// switches it and gx_k_runjoin_tma off for the rest of the process
+#define GX_RUNJOIN_SEG_DEFAULT 0
+static bool g_runjoin_seg_broken = false;
+
+// the aggregate path's environment switches (README), read once per gx_hash_agg call
+struct agg_switches {
+    bool no_runjoin, no_runagg, no_lptile, lptile_k4, no_fewgroups, fg_512, runjoin_carry, runjoin_v2, runjoin_seg, debug;
+    int runjoin_tma;                // 0: gx_k_runjoin; else the gx_k_runjoin_tma variant
+    int seg_bufs;                   // gx_k_runjoin_seg's ring depth; 0: by size
+    int runjoin_pf, runagg_pf;      // gx_fast_args::pf, gx_runagg_args::pf
+    bool runagg_dense;
+    bool seg_on() const { return runjoin_seg && !g_runjoin_seg_broken; }
+    bool tma_on() const { return runjoin_tma != 0 && !g_runjoin_seg_broken; }
+};
+static bool env_is(const char *name, char c) { const char *e = getenv(name); return e && e[0] == c; }
+static int env_int(const char *name, int dflt) { const char *e = getenv(name); return e ? atoi(e) : dflt; }
+// the first character's digit; dflt when unset or empty
+static int env_digit(const char *name, int dflt) { const char *e = getenv(name); return e && e[0] ? e[0] - '0' : dflt; }
+static agg_switches read_switches()
+{
+    agg_switches s;
+    s.no_runjoin = env_is("GX_NO_RUNJOIN", '1');
+    s.no_runagg = env_is("GX_NO_RUNAGG", '1');
+    s.no_lptile = env_is("GX_NO_LPTILE", '1');
+    s.lptile_k4 = env_is("GX_LPTILE_K4", '1');
+    s.no_fewgroups = env_is("GX_NO_FEWGROUPS", '1');
+    s.fg_512 = env_is("GX_FG_VARIANT", '0');
+    s.runjoin_carry = env_is("GX_RUNJOIN_CARRY", '1');
+    s.runjoin_v2 = env_is("GX_RUNJOIN_V2", '1');
+    s.runjoin_seg = env_digit("GX_RUNJOIN_SEG", GX_RUNJOIN_SEG_DEFAULT) != 0;
+    s.debug = env_is("GX_DEBUG_AGG", '1');
+    s.runjoin_tma = env_digit("GX_RUNJOIN_TMA", GX_RUNJOIN_TMA_DEFAULT);
+    const char *e = getenv("GX_RUNJOIN_SEG_BUFS");
+    s.seg_bufs = 0;
+    if (e && e[0]) { const int v = atoi(e); s.seg_bufs = v >= 2 && v <= GX_SEG_MAXBUF ? v : 2; }
+    s.runjoin_pf = env_int("GX_RUNJOIN_PF", 0);
+    s.runagg_pf = env_int("GX_RUNAGG_PF", 1);
+    s.runagg_dense = env_int("GX_RUNAGG_DENSE", 1) != 0;
+    return s;
+}
+
+static int launch_lptile(gx_ctx *ctx, const agg_switches &sw, const gx_agg_dev &A, size_t smem, const char *name, int threads)
+{
+    auto go = [&](auto k) {
+        return launch_kernel<gx_k_agg_lptile<k>>(ctx, (int) ctx->smem_optin, agg_grid(A.row1 - A.row0, (long long) (threads / 32) * 32 * k, ctx->sm_count),
+                                                 threads, smem, name, k == 8 ? "agg_lptile8" : "agg_lptile4", nullptr, A);
+    };
+    if (threads <= 640 && !sw.lptile_k4) return go(std::integral_constant<int, 8>());
+    return go(std::integral_constant<int, 4>());
+}
+
 // gx_k_runjoin_seg: 31 consumer warps + 1 producer warp, the rest of the CTA's shared memory is the two-deep ring of
 // join-table pieces.  0 slots = the ring does not fit next to this group table (the caller keeps gx_k_runjoin).
 // Ring depth 3 when three buffers of the size a chunk is expected to need fit (table slots per outer row x 3968 rows, + 15 %
 // and the two edge blocks), else 2 larger ones.
-static unsigned int runjoin_seg_slots(const gx_ctx *ctx, size_t table_bytes, const gx_agg_dev &A, int *nbuf)
+static unsigned int runjoin_seg_slots(const gx_ctx *ctx, const agg_switches &sw, size_t table_bytes, const gx_agg_dev &A, int *nbuf)
 {
     const size_t fixed = table_bytes + GX_SEG_CW * sizeof(gx_runlist) + sizeof(gx_seg_ctl) + 1024;
     *nbuf = 2;
@@ -3065,176 +3081,100 @@ static unsigned int runjoin_seg_slots(const gx_ctx *ctx, size_t table_bytes, con
     const size_t avail = (ctx->smem_optin - fixed) / 8;
     const long long nrows = A.row1 - A.row0 > 0 ? A.row1 - A.row0 : 1;
     const double need = 1.15 * (double) (A.mask + 1ULL) / (double) nrows * (GX_SEG_CW * 128) + 96.0;
-    const char *e = getenv("GX_RUNJOIN_SEG_BUFS");
-    if (e && e[0]) { int v = atoi(e); if (v >= 2 && v <= GX_SEG_MAXBUF) *nbuf = v; }
+    if (sw.seg_bufs) *nbuf = sw.seg_bufs;
     else if (need * 3.0 <= (double) avail) *nbuf = 3;
     size_t slots = avail / (size_t) *nbuf;
     if (slots > 4096) slots = 4096;                              // 32 KB per buffer
     return (unsigned int) (slots & ~(size_t) 31);
 }
-template <bool HAS_CNT, bool HAS_SUM, int FMT>
-static int launch_runjoin_seg_t(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_args &FA, size_t table_bytes, unsigned int seg_slots, int nbuf, const char *name)
+
+// the kernels for one join or group column, count(*) and one float8 sum: the run-folding join kernels (use_run) and gx_k_fast
+static int launch_fast(gx_ctx *ctx, const agg_switches &sw, const gx_agg_dev &A, const gx_fast_args &FA, bool join, bool cnt, bool sum,
+                       size_t smem, const char *name, bool use_run)
 {
-    static bool attr_set = false;
-    if (!attr_set) {
-        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runjoin_seg<HAS_CNT, HAS_SUM, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
-        attr_set = true;
-    }
-    const size_t smem = table_bytes + GX_SEG_CW * sizeof(gx_runlist) + (size_t) nbuf * seg_slots * 8 + sizeof(gx_seg_ctl);
-    const long long nvec = (A.row1 - A.row0) >> 2, cvec = (long long) GX_SEG_CW * 32;
-    long long nb = (nvec + cvec - 1) / cvec, maxb = (long long) ctx->sm_count;
-    while ((A.row1 - A.row0 + maxb - 1) / maxb >= (1LL << 32)) maxb *= 2;      // 32-bit row counters per CTA
-    unsigned grid = (unsigned) (nb < maxb ? (nb > 0 ? nb : 1) : maxb);
-    gx_launch_scope ls(ctx, name);
-    gx_launch_scope which(ctx, "probe_agg_seg", 0);              // same kernel under a second profile name: tells gx_profile_get() which variant ran
-    gx_k_runjoin_seg<HAS_CNT, HAS_SUM, FMT><<<grid, 1024, smem, ctx->stream>>>(A, FA, seg_slots, nbuf);
-    GX_CUDA(ctx, cudaGetLastError());
-    return GX_OK;
-}
-template <bool HAS_CNT, bool HAS_SUM, int FMT>
-static int launch_runjoin3_t(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_args &FA, size_t table_bytes, const char *name)
-{
-    static bool attr_set = false;
-    if (!attr_set) {
-        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runjoin3<HAS_CNT, HAS_SUM, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
-        attr_set = true;
-    }
-    long long nvec = (A.row1 - A.row0 + 3) / 4;
-    long long nb = (nvec + 1023) / 1024, maxb = (long long) ctx->sm_count;
-    while ((A.row1 - A.row0 + maxb - 1) / maxb >= (1LL << 32)) maxb *= 2;
-    unsigned grid = (unsigned) (nb < maxb ? (nb > 0 ? nb : 1) : maxb);
-    gx_launch_scope ls(ctx, name);
-    gx_launch_scope which(ctx, "probe_agg_run3", 0);
-    gx_k_runjoin3<HAS_CNT, HAS_SUM, FMT><<<grid, 1024, table_bytes + 32 * sizeof(gx_runlist3), ctx->stream>>>(A, FA);
-    GX_CUDA(ctx, cudaGetLastError());
-    return GX_OK;
-}
-template <bool HAS_SUM, int FMT>
-static int launch_runjoin_tma_t(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_args &FA, size_t smem, const char *name)
-{
-    static bool attr_set = false;
-    if (!attr_set) {
-        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runjoin_tma<HAS_SUM, FMT, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
-        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runjoin_tma<HAS_SUM, FMT, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
-        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runjoin_tma<HAS_SUM, FMT, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
-        attr_set = true;
-    }
-    const char *fv = getenv("GX_RUNJOIN_TMA");
-    const int variant = fv && fv[0] ? fv[0] - '0' : GX_RUNJOIN_TMA_DEFAULT;           // 2: the branch-free fold, 3: + full probe rounds only
-    long long nvec = (A.row1 - A.row0 + 3) / 4;
-    long long nb = (nvec + 1023) / 1024, maxb = (long long) ctx->sm_count;
-    while ((A.row1 - A.row0 + maxb - 1) / maxb >= (1LL << 31)) maxb *= 2;      // 31-bit row counters per CTA
-    unsigned grid = (unsigned) (nb < maxb ? (nb > 0 ? nb : 1) : maxb);
-    gx_launch_scope ls(ctx, name);
-    gx_launch_scope which(ctx, "probe_agg_tma", 0);              // second profile name: which variant ran
-    if (variant == 3) gx_k_runjoin_tma<HAS_SUM, FMT, true, true><<<grid, 1024, smem, ctx->stream>>>(A, FA);
-    else if (variant == 2) gx_k_runjoin_tma<HAS_SUM, FMT, true, false><<<grid, 1024, smem, ctx->stream>>>(A, FA);
-    else gx_k_runjoin_tma<HAS_SUM, FMT, false, false><<<grid, 1024, smem, ctx->stream>>>(A, FA);
-    GX_CUDA(ctx, cudaGetLastError());
-    return GX_OK;
-}
-template <bool HAS_SUM, int FMT>
-static int launch_runjoin2_t(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_args &FA, const char *name)
-{
-    static bool attr_set = false;
-    const size_t smem = (size_t) A.s_slots * 16 + 16 * sizeof(gx_runlist);
-    if (!attr_set) {
-        // once per instantiation, so for the largest group table launch_fast hands it (4096 slots), not the first caller's
-        const int smem_max = (int) (4096 * 16 + 16 * sizeof(gx_runlist));
-        GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runjoin2<HAS_SUM, FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
-        attr_set = true;
-    }
-    long long nvec = (A.row1 - A.row0 + 3) / 4;
-    long long nb = (nvec + 511) / 512, maxb = (long long) ctx->sm_count * 2;
-    while ((A.row1 - A.row0 + maxb - 1) / maxb >= (1LL << 31)) maxb *= 2;      // 31-bit row counters per CTA
-    unsigned grid = (unsigned) (nb < maxb ? (nb > 0 ? nb : 1) : maxb);
-    gx_launch_scope ls(ctx, name);
-    gx_launch_scope which(ctx, "probe_agg_run2", 0);
-    gx_k_runjoin2<HAS_SUM, FMT><<<grid, 512, smem, ctx->stream>>>(A, FA);
-    GX_CUDA(ctx, cudaGetLastError());
-    return GX_OK;
-}
-// GX_RUNJOIN_SEG=1/0 selects / forbids gx_k_runjoin_seg; a run that raised flag 16 (a bounded mbarrier wait gave up)
-// switches it off for the rest of the process
-#define GX_RUNJOIN_SEG_DEFAULT 0
-static bool g_runjoin_seg_broken = false;
-static bool gx_runjoin_seg_enabled()
-{
-    if (g_runjoin_seg_broken) return false;
-    const char *e = getenv("GX_RUNJOIN_SEG");
-    return e && e[0] ? e[0] != '0' : GX_RUNJOIN_SEG_DEFAULT != 0;
-}
-// GX_RUNJOIN_TMA=1/0 selects / forbids gx_k_runjoin_tma (same rules as GX_RUNJOIN_SEG)
-static bool gx_runjoin_tma_enabled()
-{
-    if (g_runjoin_seg_broken) return false;
-    const char *e = getenv("GX_RUNJOIN_TMA");
-    return e && e[0] ? e[0] != '0' : GX_RUNJOIN_TMA_DEFAULT != 0;
-}
-// calls fn with the slot format of the plan's join table as a compile-time constant (std::integral_constant)
-static int launch_fast(gx_ctx *ctx, const gx_agg_dev &A, const gx_fast_args &FA, bool join, bool cnt, bool sum, size_t smem, const char *name, bool use_run)
-{
+    const long long nrows = A.row1 - A.row0, nvec = (nrows + 3) / 4;
+    const int optin = (int) ctx->smem_optin;
+    // a CTA per 1024 vectors of 4 rows, with 32-bit row counters per CTA
+    const unsigned grid = agg_grid(nvec, 1024, ctx->sm_count, nrows, 32);
     // gx_k_runjoin3: finished runs wait for a full round of 32 (GX_RUNJOIN_CARRY=1; A/B against gx_k_runjoin)
-    {
-        const char *cv = getenv("GX_RUNJOIN_CARRY");
-        if (use_run && cv && cv[0] == '1' && smem + 32 * sizeof(gx_runlist3) <= ctx->smem_optin - 1024)
-            return with_slot_format(A, [&](auto f) {
-                constexpr int F = decltype(f)::value;
-                if (cnt && sum) return launch_runjoin3_t<true, true, F>(ctx, A, FA, smem, name);
-                if (cnt) return launch_runjoin3_t<true, false, F>(ctx, A, FA, smem, name);
-                return launch_runjoin3_t<false, true, F>(ctx, A, FA, smem, name);
-            });
-    }
+    if (use_run && sw.runjoin_carry && smem + 32 * sizeof(gx_runlist3) <= ctx->smem_optin - 1024)
+        return with_slot_format(A, [&](auto f) { return with_cnt_sum(cnt, sum, [&](auto c, auto s) {
+            return launch_kernel<gx_k_runjoin3<c, s, f>>(ctx, optin, grid, 1024, smem + 32 * sizeof(gx_runlist3), name, "probe_agg_run3", nullptr, A, FA);
+        }); });
+    // gx_k_runjoin2 and gx_k_runjoin_tma have the sum as their only such parameter: with_cnt_sum(true, sum, ...) picks it
     // gx_k_runjoin2: two CTAs of 512 threads per SM with 16-byte group slots (64 KB + 40 KB of run lists) instead of
-    // one CTA of 1024 threads with 24-byte slots; opt-in behind GX_RUNJOIN_V2=1.
-    {
-        const char *v2 = getenv("GX_RUNJOIN_V2");
-        if (use_run && v2 && v2[0] == '1' && A.s_slots <= 4096)
-            return with_slot_format(A, [&](auto f) {
-                constexpr int F = decltype(f)::value;
-                return sum ? launch_runjoin2_t<true, F>(ctx, A, FA, name) : launch_runjoin2_t<false, F>(ctx, A, FA, name);
-            });
-    }
-    // the run-folding join kernel keeps a per-warp run list next to the group table
-    const size_t run_bytes = 32 * sizeof(gx_runlist);
-    // rows through the copy engine (gx_k_runjoin_tma): packed group slots, so at most 4096 of them; 16-byte aligned columns
-    if (use_run && gx_runjoin_tma_enabled() && A.s_slots <= 4096 && (A.row0 & 1) == 0 &&
+    // one CTA of 1024 threads with 24-byte slots; opt-in behind GX_RUNJOIN_V2=1.  Its limit is set once per instantiation,
+    // so for the largest group table launch_fast hands it (4096 slots), not the first caller's; 31-bit row counters per CTA.
+    if (use_run && sw.runjoin_v2 && A.s_slots <= 4096)
+        return with_slot_format(A, [&](auto f) { return with_cnt_sum(true, sum, [&](auto, auto s) {
+            return launch_kernel<gx_k_runjoin2<s, f>>(ctx, (int) (4096 * 16 + 16 * sizeof(gx_runlist)), agg_grid(nvec, 512, 2LL * ctx->sm_count, nrows, 31), 512,
+                                                      (size_t) A.s_slots * 16 + 16 * sizeof(gx_runlist), name, "probe_agg_run2", nullptr, A, FA);
+        }); });
+    // rows through the copy engine (gx_k_runjoin_tma): packed group slots, so at most 4096 of them; 16-byte aligned columns;
+    // 31-bit row counters per CTA.  Second profile name: which variant ran.
+    if (use_run && sw.tma_on() && A.s_slots <= 4096 && (A.row0 & 1) == 0 &&
         ((uintptr_t) FA.okey & 15) == 0 && ((uintptr_t) FA.vcol & 15) == 0) {
         const size_t tma_smem = (size_t) A.s_slots * 16 + 32 * sizeof(gx_runlist) + 32 * sizeof(gx_rowstage) + 32 * 8;
+        const unsigned tma_grid = agg_grid(nvec, 1024, ctx->sm_count, nrows, 31);
         if (tma_smem + 1024 <= ctx->smem_optin)
-            return with_slot_format(A, [&](auto f) {
-                constexpr int F = decltype(f)::value;
-                return sum ? launch_runjoin_tma_t<true, F>(ctx, A, FA, tma_smem, name) : launch_runjoin_tma_t<false, F>(ctx, A, FA, tma_smem, name);
-            });
+            return with_slot_format(A, [&](auto f) { return with_cnt_sum(true, sum, [&](auto, auto s) {
+                if (sw.runjoin_tma == 3)
+                    return launch_kernel<gx_k_runjoin_tma<s, f, true, true>>(ctx, optin, tma_grid, 1024, tma_smem, name, "probe_agg_tma", nullptr, A, FA);
+                if (sw.runjoin_tma == 2)
+                    return launch_kernel<gx_k_runjoin_tma<s, f, true, false>>(ctx, optin, tma_grid, 1024, tma_smem, name, "probe_agg_tma", nullptr, A, FA);
+                return launch_kernel<gx_k_runjoin_tma<s, f, false, false>>(ctx, optin, tma_grid, 1024, tma_smem, name, "probe_agg_tma", nullptr, A, FA);
+            }); });
     }
-    // compact table + order-preserving slots: the streamed-table variant (gx_k_runjoin_seg)
-    if (use_run && (A.cslots || A.narrow) && A.sf.mode != 0 && gx_runjoin_seg_enabled()) {
+    // compact table + order-preserving slots: the streamed-table variant (gx_k_runjoin_seg); a CTA per GX_SEG_CW * 32 whole vectors
+    if (use_run && (A.cslots || A.narrow) && A.sf.mode != 0 && sw.seg_on()) {
         int nbuf = 2;
-        const unsigned int seg_slots = runjoin_seg_slots(ctx, smem, A, &nbuf);
-        auto seg = [&](auto f) {
-            constexpr int F = decltype(f)::value;
-            if (cnt && sum) return launch_runjoin_seg_t<true, true, F>(ctx, A, FA, smem, seg_slots, nbuf, name);
-            if (cnt) return launch_runjoin_seg_t<true, false, F>(ctx, A, FA, smem, seg_slots, nbuf, name);
-            return launch_runjoin_seg_t<false, true, F>(ctx, A, FA, smem, seg_slots, nbuf, name);
-        };
+        const unsigned int seg_slots = runjoin_seg_slots(ctx, sw, smem, A, &nbuf);
+        const size_t seg_smem = smem + GX_SEG_CW * sizeof(gx_runlist) + (size_t) nbuf * seg_slots * 8 + sizeof(gx_seg_ctl);
+        auto seg = [&](auto f) { return with_cnt_sum(cnt, sum, [&](auto c, auto s) {
+            return launch_kernel<gx_k_runjoin_seg<c, s, f>>(ctx, optin, agg_grid(nrows >> 2, (long long) GX_SEG_CW * 32, ctx->sm_count, nrows, 32), 1024,
+                                                            seg_smem, name, "probe_agg_seg", nullptr, A, FA, seg_slots, nbuf);
+        }); };
         if (seg_slots >= 512)
             return A.narrow ? seg(std::integral_constant<int, GX_SLOTS_NARROW>()) : seg(std::integral_constant<int, GX_SLOTS_COMPACT>());
     }
+    // the run-folding join kernel keeps a per-warp run list next to the group table
     if (use_run)
-        return with_slot_format(A, [&](auto f) {
-            constexpr int F = decltype(f)::value;
-            if (cnt && sum) return launch_runjoin_t<true, true, F>(ctx, A, FA, smem + run_bytes, name);
-            if (cnt) return launch_runjoin_t<true, false, F>(ctx, A, FA, smem + run_bytes, name);
-            return launch_runjoin_t<false, true, F>(ctx, A, FA, smem + run_bytes, name);
-        });
-    if (join) {
-        if (cnt && sum) return launch_fast_t<true, true, true>(ctx, A, FA, smem, name);
-        if (cnt) return launch_fast_t<true, true, false>(ctx, A, FA, smem, name);
-        return launch_fast_t<true, false, true>(ctx, A, FA, smem, name);
+        return with_slot_format(A, [&](auto f) { return with_cnt_sum(cnt, sum, [&](auto c, auto s) {
+            return launch_kernel<gx_k_runjoin<c, s, f>>(ctx, optin, grid, 1024, smem + 32 * sizeof(gx_runlist), name, "probe_agg_run", nullptr, A, FA);
+        }); });
+    return with_cnt_sum(cnt, sum, [&](auto c, auto s) {
+        if (join) return launch_kernel<gx_k_fast<true, c, s>>(ctx, optin, grid, 1024, smem, name, "probe_agg_fast", nullptr, A, FA);
+        return launch_kernel<gx_k_fast<false, c, s>>(ctx, optin, grid, 1024, smem, name, "agg_fast", nullptr, A, FA);
+    });
+}
+
+// Does every aggregate of the plan sum float8 terms (GXU_ADD_F64, not integer, no count word of its own), each term a
+// constant or a NOT NULL float8 column?  With V: also lists the distinct columns the terms read (col, nc) and, for each
+// such aggregate, its number, its state word and the column of each term (vagg, vword, tslot; -1: a constant); then
+// false when a value would go beyond max_nv or a column beyond FG_NC.
+template <class V = gx_fewgroups_args>
+static bool f8sum_shape(const gx_agg_dev &A, V *v = nullptr, int max_nv = 0)
+{
+    for (int a = 0; a < A.P.nagg; a++) {
+        const gx_dagg &ga = A.P.aggs[a];
+        if (ga.kind == GXU_NONE) continue;
+        if (ga.kind != GXU_ADD_F64 || ga.is_int || ga.cnt_word != 0 || ga.expr.nterms < 1) return false;
+        for (int t = 0; t < ga.expr.nterms; t++)
+            if (ga.expr.t[t].kind != GXT_CONST && (ga.expr.t[t].col.type != GX_FLOAT8 || ga.expr.t[t].col.nulls != nullptr)) return false;
+        if (!v) continue;
+        if (v->nv >= max_nv) return false;
+        for (int t = 0; t < ga.expr.nterms; t++) {
+            int slot = -1;
+            if (ga.expr.t[t].kind != GXT_CONST) {
+                const double *col = (const double *) ga.expr.t[t].col.data;
+                for (int c = 0; c < v->nc; c++) if (v->col[c] == col) slot = c;
+                if (slot < 0) { if (v->nc == FG_NC) return false; slot = v->nc; v->col[v->nc++] = col; }
+            }
+            v->tslot[v->nv][t] = (signed char) slot;
+        }
+        v->vagg[v->nv] = a; v->vword[v->nv] = ga.word; v->nv++;
     }
-    if (cnt && sum) return launch_fast_t<false, true, true>(ctx, A, FA, smem, name);
-    if (cnt) return launch_fast_t<false, true, false>(ctx, A, FA, smem, name);
-    return launch_fast_t<false, false, true>(ctx, A, FA, smem, name);
+    return true;
 }
 
 static int read_counters(gx_ctx *ctx, long long *c /* 4 */, long long *cursor = nullptr)
@@ -3268,281 +3208,246 @@ static int run_radix(gx_ctx *ctx, compiled_plan *cp, const gx_agg_plan *plan, lo
 int gx_aggregate_records(gx_ctx *ctx, gx_agg_dev A, unsigned long long *d_recs, long long nrec,
                          unsigned long long **d_out, long long *ngroups_out);
 
-static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, gx_result **out,
-                        const chain_spec *ch = nullptr)
-{
+// one gx_hash_agg call: its compiled plan, its switches, and the kernel families its plan's shape admits
+struct agg_call {
+    gx_ctx *ctx; const gx_table *outer; const gx_hash *h; const gx_agg_plan *plan;
     compiled_plan cp;
-    int rc = compile_plan(ctx, outer, h, plan, &cp, ch); if (rc) return rc;
-    gx_agg_dev &A = cp.A;
-    const int nwords = A.P.nwords, RW = 3 + nwords;
-    long long est = plan->est_groups > 0 ? plan->est_groups : 1024;
-    if (plan->n_group_cols == 0) est = 1;
+    agg_switches sw;
+    long long est, smax;            // groups expected; slots of the largest shared-memory group table
+    int strategy;                   // 1 shared-memory table, 2 radix, 3 global table (gx_agg_plan::strategy)
+    int tagkey;                     // key bytes <= 7 and one key word: the tag word carries the key itself
+    size_t budget;                  // shared memory of a group table
+    bool exist;                     // a SEMI / ANTI plan or a join chain (gx_k_agg's probes)
+    bool fast_ok, lptile_ok, fewgroups_ok, countchar_ok;
+    gx_fast_args FA;
+    gx_fewgroups_args FG;
+    size_t dense_bytes(long long S) const { return (size_t) S * 8 * (1 + (tagkey ? 0 : cp.A.P.nkw) + cp.A.P.nwords); }
+    // only gx_k_runjoin and the existence probe read the compact and narrow table forms; everything else needs the 16-byte slots
+    int need_wide()
+    {
+        if (!h || cp.A.slots || exist) return GX_OK;
+        int rc = gx_hash_wide(ctx, const_cast<gx_hash *>(h));
+        cp.A.slots = h->slots;
+        return rc;
+    }
+};
+
+// compiles the plan and decides the strategy and which kernel families its shape admits
+static int agg_prepare(agg_call &C, gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, const chain_spec *ch)
+{
+    C.ctx = ctx; C.outer = outer; C.h = h; C.plan = plan;
+    int rc = compile_plan(ctx, outer, h, plan, &C.cp, ch); if (rc) return rc;
+    C.sw = read_switches();
+    const gx_agg_dev &A = C.cp.A;
+    C.est = plan->est_groups > 0 ? plan->est_groups : 1024;
+    if (plan->n_group_cols == 0) C.est = 1;
 
     // ---- shared-memory plan (strategy 1) -----------------------------------
-    // key bytes <= 7 and one key word: the tag word carries the key itself
     int keybytes = 0;
-    for (int c = 0; c < plan->n_group_cols; c++) keybytes += cp.L.gbytes[c];
-    const int tagkey = (A.P.nkw == 1 && keybytes <= 7) ? 1 : 0;
-    const size_t budget = ctx->smem_optin - 1024;
-    auto dense_bytes = [&](long long S) { return (size_t) S * 8 * (1 + (tagkey ? 0 : A.P.nkw) + nwords); };
-    long long smax = 16; while (dense_bytes(smax * 2) <= budget) smax *= 2;
-    int strategy = plan->strategy;
-    if (strategy == 0) strategy = (est * 3 / 2 <= smax) ? 1 : 2;
+    for (int c = 0; c < plan->n_group_cols; c++) keybytes += C.cp.L.gbytes[c];
+    C.tagkey = (A.P.nkw == 1 && keybytes <= 7) ? 1 : 0;
+    C.budget = ctx->smem_optin - 1024;
+    C.smax = 16; while (C.dense_bytes(C.smax * 2) <= C.budget) C.smax *= 2;
+    C.strategy = plan->strategy;
+    if (C.strategy == 0) C.strategy = (C.est * 3 / 2 <= C.smax) ? 1 : 2;
     // a regression state makes a record of 12 words or more: one per row (the radix path) is 100 B per row and more, so
     // a plan with one whose groups outgrow the shared table but fit L2's share of the global table takes that table
-    if (plan->strategy == 0 && strategy == 2 && A.P.regr.on && est <= 65536) strategy = 3;
-    GX_CHECK_ARG(ctx, strategy >= 1 && strategy <= 3, "agg plan: unknown strategy %d", strategy);
+    if (plan->strategy == 0 && C.strategy == 2 && A.P.regr.on && C.est <= 65536) C.strategy = 3;
+    GX_CHECK_ARG(ctx, C.strategy >= 1 && C.strategy <= 3, "agg plan: unknown strategy %d", C.strategy);
 
     // ---- does the plan have the shape the specialised kernel was written for?
-    gx_fast_args FA; memset(&FA, 0, sizeof(FA));
-    { const char *pf = getenv("GX_RUNJOIN_PF"); FA.pf = pf ? atoi(pf) : 0; }
+    C.FA.pf = C.sw.runjoin_pf;
     // the specialised kernels below join one table and know one payload word; a SEMI / ANTI plan takes gx_k_agg's
     // existence probe, a join chain its chain probe (both read the first table in the format its build wrote)
-    const bool exist = A.P.join_type != GX_JOIN_INNER || A.chain_n > 1;
+    C.exist = A.P.join_type != GX_JOIN_INNER || A.chain_n > 1;
     // a variance state is only updated by gx_k_agg: every specialised kernel below is ruled out by cp.has_var
-    bool fast_ok = !exist && !cp.has_var && plan->n_preds == 0 && plan->n_group_cols == 1 && tagkey && outer->nrows > 0;
-    if (fast_ok) {
+    C.fast_ok = !C.exist && !C.cp.has_var && plan->n_preds == 0 && plan->n_group_cols == 1 && C.tagkey && outer->nrows > 0;
+    if (C.fast_ok) {
         const gx_dgroupcol &gc = A.P.gcols[0];
         if (A.P.has_join) {
-            fast_ok = gc.side == 1 && gc.payload_idx == 0 && gc.bytes == 4 && h->unique && A.P.key_type == GX_INT8 && A.P.okey.nulls == nullptr;
-            FA.okey = (const long long *) A.P.okey.data;
+            C.fast_ok = gc.side == 1 && gc.payload_idx == 0 && gc.bytes == 4 && h->unique && A.P.key_type == GX_INT8 && A.P.okey.nulls == nullptr;
+            C.FA.okey = (const long long *) A.P.okey.data;
         } else {
-            fast_ok = gc.side == 0 && gc.bytes == 4 && gc.col.nulls == nullptr;
-            FA.gcol = (const int *) gc.col.data;
+            C.fast_ok = gc.side == 0 && gc.bytes == 4 && gc.col.nulls == nullptr;
+            C.FA.gcol = (const int *) gc.col.data;
         }
         int nvalue = 0;
-        for (int a = 0; a < plan->n_aggs && fast_ok; a++) {
+        for (int a = 0; a < plan->n_aggs && C.fast_ok; a++) {
             const gx_dagg &ga = A.P.aggs[a];
             if (plan->aggs[a].fn == GX_AGG_COUNT_STAR) continue;
             if ((plan->aggs[a].fn == GX_AGG_SUM_F8 || plan->aggs[a].fn == GX_AGG_AVG_F8) && ga.expr.nterms == 1 && ga.expr.t[0].kind == GXT_COL &&
                 ga.expr.t[0].col.type == GX_FLOAT8 && ga.expr.t[0].col.nulls == nullptr && nvalue == 0) {
-                FA.vcol = (const double *) ga.expr.t[0].col.data; FA.sum_word = ga.word; nvalue++;
-            } else fast_ok = false;
+                C.FA.vcol = (const double *) ga.expr.t[0].col.data; C.FA.sum_word = ga.word; nvalue++;
+            } else C.fast_ok = false;
         }
     }
-
-    // only gx_k_runjoin and the existence probe read the compact and narrow table forms; everything else needs the 16-byte slots
-    auto need_wide = [&]() -> int {
-        if (!h || A.slots || exist) return GX_OK;
-        int wrc = gx_hash_wide(ctx, const_cast<gx_hash *>(h));
-        A.slots = h->slots;
-        return wrc;
-    };
-    const size_t run_bytes = 32 * sizeof(gx_runlist);
-    const char *norun = getenv("GX_NO_RUNJOIN");
-    const bool runjoin_env = !(norun && norun[0] == '1');
 
     // the tile-at-a-time lane-private kernel: no join, count(*) and float8 sums over NOT-NULL float8 columns
-    bool lptile_ok = !A.P.has_join && !cp.has_var;
-    for (int a = 0; a < A.P.nagg && lptile_ok; a++) {
-        const gx_dagg &ga = A.P.aggs[a];
-        if (ga.kind == GXU_NONE) continue;
-        lptile_ok = ga.kind == GXU_ADD_F64 && !ga.is_int && ga.cnt_word == 0 && ga.expr.nterms >= 1;
-        for (int t = 0; t < ga.expr.nterms && lptile_ok; t++)
-            lptile_ok = ga.expr.t[t].kind == GXT_CONST || (ga.expr.t[t].col.type == GX_FLOAT8 && ga.expr.t[t].col.nulls == nullptr);
-    }
-    { const char *e = getenv("GX_NO_LPTILE"); if (e && e[0] == '1') lptile_ok = false; }
+    C.lptile_ok = !A.P.has_join && !C.cp.has_var && f8sum_shape(A) && !C.sw.no_lptile;
     // register-accumulator kernels for <= FG_G groups (Q1, config 1): same plan shape as the tiled kernel,
     // key in one word without NULLs
-    gx_fewgroups_args FG; memset(&FG, 0, sizeof(FG));
-    bool fewgroups_ok = lptile_ok && A.P.nkw == 1 && plan->n_group_cols >= 1 && outer->nrows > 0;
-    for (int c = 0; c < plan->n_group_cols && fewgroups_ok; c++) fewgroups_ok = A.P.gcols[c].side == 0 && A.P.gcols[c].col.nulls == nullptr;
-    for (int a = 0; a < A.P.nagg && fewgroups_ok; a++) {
-        if (A.P.aggs[a].kind == GXU_NONE) continue;
-        if (FG.nv >= FG_NV) { fewgroups_ok = false; break; }
-        const gx_dexpr &e = A.P.aggs[a].expr;
-        for (int t = 0; t < e.nterms && fewgroups_ok; t++) {
-            int slot = -1;
-            if (e.t[t].kind != GXT_CONST) {
-                const double *cp = (const double *) e.t[t].col.data;
-                for (int c = 0; c < FG.nc; c++) if (FG.col[c] == cp) slot = c;
-                if (slot < 0) { if (FG.nc < FG_NC) { slot = FG.nc; FG.col[FG.nc++] = cp; } else fewgroups_ok = false; }
-            }
-            FG.tslot[FG.nv][t] = (signed char) slot;
-        }
-        FG.vagg[FG.nv] = a; FG.vword[FG.nv] = A.P.aggs[a].word; FG.nv++;
-    }
-    { const char *e = getenv("GX_NO_FEWGROUPS"); if (e && e[0] == '1') fewgroups_ok = false; }
-    bool countchar_ok = fewgroups_ok && FG.nv == 0 && plan->n_preds == 0 && plan->n_group_cols == 1 && A.P.gcols[0].type == GX_CHAR;
+    C.fewgroups_ok = C.lptile_ok && A.P.nkw == 1 && plan->n_group_cols >= 1 && outer->nrows > 0;
+    for (int c = 0; c < plan->n_group_cols && C.fewgroups_ok; c++) C.fewgroups_ok = A.P.gcols[c].side == 0 && A.P.gcols[c].col.nulls == nullptr;
+    C.fewgroups_ok = C.fewgroups_ok && f8sum_shape(A, &C.FG, FG_NV) && !C.sw.no_fewgroups;
+    C.countchar_ok = C.fewgroups_ok && C.FG.nv == 0 && plan->n_preds == 0 && plan->n_group_cols == 1 && A.P.gcols[0].type == GX_CHAR;
+    return GX_OK;
+}
 
-    // ---- GROUP BY contains the join key of a unique build side and the outer side is in key order:
-    // a run of equal keys is a group (gx_k_runagg).  Tried first; a raised "keys descend" flag sends the
-    // plan down the general path below.
+// GROUP BY contains the join key of a unique build side and the outer side is in key order: a run of equal keys is a
+// group (gx_k_runagg).  Tried first; *done stays false when the plan has another shape, or when a raised "keys descend"
+// flag sends it down the general path.
+static int try_runagg(agg_call &C, gx_result **out, bool *done)
+{
+    gx_ctx *ctx = C.ctx; gx_agg_dev &A = C.cp.A; const gx_agg_plan *plan = C.plan;
+    *done = false;
+    gx_runagg_args RA; memset(&RA, 0, sizeof(RA));
+    RA.pf = C.sw.runagg_pf;                                     // bit 0: rows two tiles ahead into L2, bit 1: the tile's join-table lines
+    bool ok = !C.sw.no_runagg && !C.exist && !C.cp.has_var && plan->strategy == 0 && A.P.has_join && C.h->unique && A.P.key_type == GX_INT8 &&
+              A.P.okey.nulls == nullptr && C.outer->nrows > 0 && plan->n_group_cols >= 1;
+    bool has_key = false;
+    for (int c = 0; c < plan->n_group_cols && ok; c++) {
+        const gx_dgroupcol &gc = A.P.gcols[c];
+        if (gc.side == 0) { ok = plan->group_cols[c].col == plan->outer_key_col; RA.gk_from_key[c] = 1; has_key = true; }
+        else RA.gk_pbit[c] = gc.payload_idx;
+        RA.gk_word[c] = gc.word; RA.gk_shift[c] = gc.shift; RA.gk_bytes[c] = gc.bytes;
+    }
+    RA.ngk = plan->n_group_cols;
+    if (!(ok && has_key && f8sum_shape(A, &RA, RA_NV))) return GX_OK;
+
+    int rc = C.need_wide(); if (rc) return rc;
+    const int RW = 3 + A.P.nwords;
+    const bool small = RA.nv <= 2 && RA.nc <= 2;           // two CTAs of 384 threads per SM (85 registers each)
+    const int dense = (small && RA.nv <= 1) ? C.sw.runagg_dense : 0;
+    const int threads = (small && !dense) ? 384 : 512, nwarps = threads / 32;
+    const size_t smem = (size_t) nwarps * ((size_t) RA_LIST * (1 + RA.nv) + RA_LIST / 2) * 8;
+    const long long nrows = C.outer->nrows, total_warps = (long long) ctx->sm_count * (small ? 2 : 1) * nwarps;
+    long long rpw = (nrows + total_warps - 1) / total_warps; rpw = (rpw + 31) / 32 * 32; if (rpw < 128) rpw = 128;
+    const long long nchunks = (nrows + rpw - 1) / rpw;
+    const unsigned grid = (unsigned) ((nchunks + nwarps - 1) / nwarps);
+    RA.rows_per_warp = rpw;
     {
-        gx_runagg_args RA; memset(&RA, 0, sizeof(RA));
-        { const char *pf = getenv("GX_RUNAGG_PF"); RA.pf = pf ? atoi(pf) : 1; }     // bit 0: rows two tiles ahead into L2, bit 1: the tile's join-table lines
-        const char *e = getenv("GX_NO_RUNAGG");
-        bool ok = !(e && e[0] == '1') && !exist && !cp.has_var && plan->strategy == 0 && A.P.has_join && h->unique && A.P.key_type == GX_INT8 && A.P.okey.nulls == nullptr &&
-                  outer->nrows > 0 && plan->n_group_cols >= 1;
-        bool has_key = false;
-        for (int c = 0; c < plan->n_group_cols && ok; c++) {
-            const gx_dgroupcol &gc = A.P.gcols[c];
-            if (gc.side == 0) { ok = plan->group_cols[c].col == plan->outer_key_col; RA.gk_from_key[c] = 1; has_key = true; }
-            else RA.gk_pbit[c] = gc.payload_idx;
-            RA.gk_word[c] = gc.word; RA.gk_shift[c] = gc.shift; RA.gk_bytes[c] = gc.bytes;
-        }
-        RA.ngk = plan->n_group_cols;
-        ok = ok && has_key;
-        for (int a = 0; a < A.P.nagg && ok; a++) {
-            const gx_dagg &ga = A.P.aggs[a];
-            if (ga.kind == GXU_NONE) continue;
-            ok = ga.kind == GXU_ADD_F64 && !ga.is_int && ga.cnt_word == 0 && RA.nv < RA_NV && ga.expr.nterms >= 1;
-            for (int t = 0; t < ga.expr.nterms && ok; t++)
-                ok = ga.expr.t[t].kind == GXT_CONST || (ga.expr.t[t].col.type == GX_FLOAT8 && ga.expr.t[t].col.nulls == nullptr);
-            for (int t = 0; t < ga.expr.nterms && ok; t++) {
-                int slot = -1;
-                if (ga.expr.t[t].kind != GXT_CONST) {
-                    const double *cp = (const double *) ga.expr.t[t].col.data;
-                    for (int c = 0; c < RA.nc; c++) if (RA.col[c] == cp) slot = c;
-                    if (slot < 0) { if (RA.nc < FG_NC) { slot = RA.nc; RA.col[RA.nc++] = cp; } else ok = false; }
-                }
-                RA.tslot[RA.nv][t] = (signed char) slot;
-            }
-            if (ok) { RA.vagg[RA.nv] = a; RA.vword[RA.nv] = ga.word; RA.nv++; }
-        }
-        if (ok) {
-            rc = need_wide(); if (rc) return rc;
-            static bool attr = false;
-            const bool small = RA.nv <= 2 && RA.nc <= 2;           // two CTAs of 384 threads per SM (85 registers each)
-            const char *dn = getenv("GX_RUNAGG_DENSE");
-            const int dense = (small && RA.nv <= 1) ? (dn ? atoi(dn) != 0 : 1) : 0;
-            const int threads = (small && !dense) ? 384 : 512, nwarps = threads / 32;
-            const size_t smem = (size_t) nwarps * ((size_t) RA_LIST * (1 + RA.nv) + RA_LIST / 2) * 8;
-            if (!attr) {
-                GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runagg<1, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
-                GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runagg<2, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
-                GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runagg<1, 2, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
-                GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_runagg<RA_NV, FG_NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin));
-                attr = true;
-            }
-            const long long nrows = outer->nrows, total_warps = (long long) ctx->sm_count * (small ? 2 : 1) * nwarps;
-            long long rpw = (nrows + total_warps - 1) / total_warps; rpw = (rpw + 31) / 32 * 32; if (rpw < 128) rpw = 128;
-            const long long nchunks = (nrows + rpw - 1) / rpw;
-            const unsigned grid = (unsigned) ((nchunks + nwarps - 1) / nwarps);
-            RA.rows_per_warp = rpw;
-            {
-                // what a tile reads, for the row prefetch: the key, the argument columns, the qual columns (first four)
-                auto list = [&](const void *ptr, int size) {
-                    if (RA.pf_n < 4 && ptr) { RA.pf_ptr[RA.pf_n] = (const char *) ptr; RA.pf_size[RA.pf_n] = size; RA.pf_lines[RA.pf_n] = size; RA.pf_n++; }
-                };
-                list(A.P.okey.data, 8);
-                for (int c = 0; c < RA.nc; c++) list(RA.col[c], 8);
-                for (int q = 0; q < A.P.npreds; q++) list(A.P.preds[q].col.data, gx_type_size(A.P.preds[q].col.type));
-            }
-            const long long out_cap = (h->nentries < nrows ? h->nentries : nrows) + 64;
-            const long long g_cap = gx_pow2_ceil(8 * nchunks + 1024);
-            unsigned long long *g_tab, *d_out;
-            GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &g_tab, (size_t) g_cap * RW * 8));
-            cudaError_t ae = gx_tmp_alloc(ctx, (void **) &d_out, (size_t) out_cap * RW * 8);
-            if (ae != cudaSuccess) { gx_tmp_free(ctx, g_tab); GX_SET_ERR(ctx, "hash_agg: %s", cudaGetErrorString(ae)); return GX_ERR_NOMEM; }
-            GX_CUDA(ctx, cudaMemsetAsync(g_tab, 0, (size_t) g_cap * RW * 8, ctx->stream));
-            GX_CUDA(ctx, cudaMemsetAsync(A.counters, 0, 5 * sizeof(long long), ctx->stream));
-            A.g_tab = g_tab; A.g_mask = (unsigned long long) g_cap - 1;
-            RA.out = d_out; RA.out_cap = out_cap; RA.cursor = ctx->d_scratch + 12;
-            {
-                gx_launch_scope ls(ctx, "runagg");
-                gx_launch_scope which(ctx, dense ? "runagg_dense" : (small && RA.nv <= 1) ? "runagg_small1" : small ? "runagg_small2" : "runagg_wide", 0);
-                if (dense) gx_k_runagg<1, 2, 1><<<grid, threads, smem, ctx->stream>>>(A, RA);
-                else if (small && RA.nv <= 1) gx_k_runagg<1, 2><<<grid, threads, smem, ctx->stream>>>(A, RA);
-                else if (small) gx_k_runagg<2, 2><<<grid, threads, smem, ctx->stream>>>(A, RA);
-                else gx_k_runagg<RA_NV, FG_NC><<<grid, threads, smem, ctx->stream>>>(A, RA);
-            }
-            GX_CUDA(ctx, cudaGetLastError());
-            long long c[4], direct = 0;
-            rc = read_counters(ctx, c, &direct);
-            // an out-of-order outer side (flag 8) may also overrun the output: the general path answers either way
-            if (rc == GX_OK && !(c[1] & 8) && (c[1] & 6)) { GX_SET_ERR(ctx, "hash_agg: run-aggregate output overflowed (flags %lld)", c[1]); rc = GX_ERR_STATE; }
-            if (rc != GX_OK) { gx_tmp_free(ctx, g_tab); gx_tmp_free(ctx, d_out); return rc; }
-            if (!(c[1] & 8)) {
-                if (c[0] > 0) {
-                    gx_launch_scope ls(ctx, "runagg_merge");
-                    gx_k_compact_groups<<<(unsigned) ((g_cap + 255) / 256 < (long long) ctx->sm_count * 4 ? (g_cap + 255) / 256 : (long long) ctx->sm_count * 4), 256, 0, ctx->stream>>>(
-                        g_tab, g_cap, nwords, d_out, ctx->d_scratch + 12);
-                    GX_CUDA(ctx, cudaGetLastError());
-                }
-                gx_tmp_free(ctx, g_tab);
-                *out = new_result(ctx, plan, cp.L, d_out, direct + c[0], out_cap);
-                return GX_OK;
-            }
-            gx_tmp_free(ctx, g_tab); gx_tmp_free(ctx, d_out);      // keys descend somewhere: general path
-            A.g_tab = nullptr;
-        }
+        // what a tile reads, for the row prefetch: the key, the argument columns, the qual columns (first four)
+        auto list = [&](const void *ptr, int size) {
+            if (RA.pf_n < 4 && ptr) { RA.pf_ptr[RA.pf_n] = (const char *) ptr; RA.pf_size[RA.pf_n] = size; RA.pf_lines[RA.pf_n] = size; RA.pf_n++; }
+        };
+        list(A.P.okey.data, 8);
+        for (int c = 0; c < RA.nc; c++) list(RA.col[c], 8);
+        for (int q = 0; q < A.P.npreds; q++) list(A.P.preds[q].col.data, gx_type_size(A.P.preds[q].col.type));
     }
+    const long long out_cap = (C.h->nentries < nrows ? C.h->nentries : nrows) + 64;
+    const long long g_cap = gx_pow2_ceil(8 * nchunks + 1024);
+    unsigned long long *g_tab, *d_out;
+    GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &g_tab, (size_t) g_cap * RW * 8));
+    cudaError_t ae = gx_tmp_alloc(ctx, (void **) &d_out, (size_t) out_cap * RW * 8);
+    if (ae != cudaSuccess) { gx_tmp_free(ctx, g_tab); GX_SET_ERR(ctx, "hash_agg: %s", cudaGetErrorString(ae)); return GX_ERR_NOMEM; }
+    GX_CUDA(ctx, cudaMemsetAsync(g_tab, 0, (size_t) g_cap * RW * 8, ctx->stream));
+    GX_CUDA(ctx, cudaMemsetAsync(A.counters, 0, 5 * sizeof(long long), ctx->stream));
+    A.g_tab = g_tab; A.g_mask = (unsigned long long) g_cap - 1;
+    RA.out = d_out; RA.out_cap = out_cap; RA.cursor = ctx->d_scratch + 12;
+    const int optin = (int) ctx->smem_optin;
+    if (dense) rc = launch_kernel<gx_k_runagg<1, 2, 1>>(ctx, optin, grid, threads, smem, "runagg", "runagg_dense", nullptr, A, RA);
+    else if (small && RA.nv <= 1) rc = launch_kernel<gx_k_runagg<1, 2>>(ctx, optin, grid, threads, smem, "runagg", "runagg_small1", nullptr, A, RA);
+    else if (small) rc = launch_kernel<gx_k_runagg<2, 2>>(ctx, optin, grid, threads, smem, "runagg", "runagg_small2", nullptr, A, RA);
+    else rc = launch_kernel<gx_k_runagg<RA_NV, FG_NC>>(ctx, optin, grid, threads, smem, "runagg", "runagg_wide", nullptr, A, RA);
+    long long c[4], direct = 0;
+    if (rc == GX_OK) rc = read_counters(ctx, c, &direct);
+    // an out-of-order outer side (flag 8) may also overrun the output: the general path answers either way
+    if (rc == GX_OK && !(c[1] & 8) && (c[1] & 6)) { GX_SET_ERR(ctx, "hash_agg: run-aggregate output overflowed (flags %lld)", c[1]); rc = GX_ERR_STATE; }
+    if (rc != GX_OK) { gx_tmp_free(ctx, g_tab); gx_tmp_free(ctx, d_out); return rc; }
+    if (!(c[1] & 8)) {
+        if (c[0] > 0) {
+            gx_launch_scope ls(ctx, "runagg_merge");
+            gx_k_compact_groups<<<(unsigned) ((g_cap + 255) / 256 < (long long) ctx->sm_count * 4 ? (g_cap + 255) / 256 : (long long) ctx->sm_count * 4), 256, 0, ctx->stream>>>(
+                g_tab, g_cap, A.P.nwords, d_out, ctx->d_scratch + 12);
+            GX_CUDA(ctx, cudaGetLastError());
+        }
+        gx_tmp_free(ctx, g_tab);
+        *out = new_result(ctx, plan, C.cp.L, d_out, direct + c[0], out_cap);
+        *done = true;
+        return GX_OK;
+    }
+    gx_tmp_free(ctx, g_tab); gx_tmp_free(ctx, d_out);      // keys descend somewhere: general path
+    A.g_tab = nullptr;
+    return GX_OK;
+}
 
+// the kernel of one attempt over a group table of S slots (gmax groups per lane of lp_warps lane-private warps of
+// lp_bytes; 0: none)
+static int launch_attempt(agg_call &C, long long S, int gmax, int lp_warps, size_t lp_bytes, bool use_fast, bool use_run, bool use_few)
+{
+    gx_ctx *ctx = C.ctx; const gx_agg_dev &A = C.cp.A;
+    const char *kname = A.chain_n > 1 ? "probe_agg_chain" : C.h ? "probe_agg" : "agg";
+    if (use_fast) return launch_fast(ctx, C.sw, A, C.FA, A.P.has_join != 0, A.need_w0 != 0, C.FA.vcol != nullptr, C.dense_bytes(S), kname, use_run);
+    if (use_few && C.countchar_ok)
+        return launch_kernel<gx_k_count_char>(ctx, -1, ctx->sm_count * 2, 512, 0, kname, "agg_count_char", nullptr, A, (const signed char *) A.P.gcols[0].col.data);
+    if (use_few) {
+        // <4, 768> unless GX_FG_VARIANT=0 asks for <8, 512>; the limit leaves room for the static shared memory
+        const int fg_threads = C.sw.fg_512 ? 512 : 768, fg_k = C.sw.fg_512 ? 8 : 4, lim = (int) ctx->smem_optin - 1024;
+        const size_t fg_smem = (size_t) (fg_threads / 32) * (1 + C.FG.nv) * (FG_G + 1) * 32 * 8;
+        const unsigned fg_grid = agg_grid(C.outer->nrows, (long long) fg_threads * fg_k, ctx->sm_count);
+        bool bytekey = C.plan->n_group_cols <= 2;
+        for (int c = 0; c < C.plan->n_group_cols; c++) bytekey = bytekey && A.P.gcols[c].type == GX_CHAR && A.P.gcols[c].word == 0;
+        auto fg = [&](auto b) {
+            if (C.sw.fg_512) return launch_kernel<gx_k_fewgroups<b, 8, 512>>(ctx, lim, fg_grid, 512, fg_smem, kname, "agg_fewgroups", nullptr, A, C.FG);
+            return launch_kernel<gx_k_fewgroups<b, 4, 768>>(ctx, lim, fg_grid, 768, fg_smem, kname, "agg_fewgroups", nullptr, A, C.FG);
+        };
+        return bytekey ? fg(std::true_type()) : fg(std::false_type());
+    }
+    if (gmax && C.lptile_ok) return launch_lptile(ctx, C.sw, A, lp_bytes, kname, lp_warps * 32);
+    if (gmax) return launch_agg<SINK_SMEM_LP>(ctx, A, lp_bytes, kname, lp_warps * 32);
+    if (C.strategy == 1) return launch_agg<SINK_SMEM>(ctx, A, C.dense_bytes(S), kname);
+    return launch_agg<SINK_GLOBAL>(ctx, A, 0, kname);
+}
+
+static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, gx_result **out,
+                        const chain_spec *ch = nullptr)
+{
+    agg_call C{};
+    int rc = agg_prepare(C, ctx, outer, h, plan, ch); if (rc) return rc;
+    bool done;
+    rc = try_runagg(C, out, &done); if (rc || done) return rc;
+    gx_agg_dev &A = C.cp.A;
+    const int nwords = A.P.nwords, RW = 3 + nwords;
     for (int attempt = 0; attempt < 8; attempt++) {
-        if (strategy == 2) { rc = need_wide(); if (rc) return rc; return run_radix(ctx, &cp, plan, outer->nrows, out); }
-        long long S = 16; while (S * 2 < est * 3 && S < smax) S *= 2;     // load factor <= 0.67
+        if (C.strategy == 2) { rc = C.need_wide(); if (rc) return rc; return run_radix(ctx, &C.cp, plan, outer->nrows, out); }
+        const long long est = C.est;
+        long long S = 16; while (S * 2 < est * 3 && S < C.smax) S *= 2;     // load factor <= 0.67
         // lane-private mode for a handful of groups: [warp][word][group][lane]
         int gmax = 0, lp_warps = 0; size_t lp_bytes = 0;
-        if (strategy == 1 && est <= 16) {
+        if (C.strategy == 1 && est <= 16) {
             // 8, 16 or 32 groups per CTA.  Sized to the estimate, not twice it: the accumulators are
             // words x groups x 8 B PER LANE, and a wrong estimate only costs the retry below — while
             // falling back to the CTA-shared table with a handful of groups serialises every atomic
             // (Q1 shape, 11 words: 212 ms instead of single-digit ms).
             gmax = 8; while (gmax < est) gmax *= 2;
             S = 4 * gmax;
-            size_t dir = (size_t) S * 8 * (1 + (tagkey ? 0 : A.P.nkw)) + ((S + 2) / 2 + 1) * 8;
+            size_t dir = (size_t) S * 8 * (1 + (C.tagkey ? 0 : A.P.nkw)) + ((S + 2) / 2 + 1) * 8;
             size_t per_warp = (size_t) nwords * gmax * 32 * 8;
-            lp_warps = (int) ((budget - dir) / per_warp); if (lp_warps > 32) lp_warps = 32;
-            if (lp_warps < 4) { gmax = 0; S = 16; while (S < est * 2 && S < smax) S *= 2; }   // too many words: use the dense table
+            lp_warps = (int) ((C.budget - dir) / per_warp); if (lp_warps > 32) lp_warps = 32;
+            if (lp_warps < 4) { gmax = 0; S = 16; while (S < est * 2 && S < C.smax) S *= 2; }   // too many words: use the dense table
             else lp_bytes = dir + per_warp * lp_warps;
         }
-        long long g_cap = gx_pow2_ceil((strategy == 1 ? S : est) * 4 + 1024);
+        long long g_cap = gx_pow2_ceil((C.strategy == 1 ? S : est) * 4 + 1024);
         unsigned long long *g_tab;
         GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &g_tab, (size_t) g_cap * RW * 8));
         GX_CUDA(ctx, cudaMemsetAsync(g_tab, 0, (size_t) g_cap * RW * 8, ctx->stream));
         GX_CUDA(ctx, cudaMemsetAsync(A.counters, 0, 4 * sizeof(long long), ctx->stream));
         A.g_tab = g_tab; A.g_mask = (unsigned long long) g_cap - 1;
-        A.s_slots = strategy == 1 ? (int) S : 0; A.s_log2 = ilog2(S); A.s_tagkey = tagkey; A.s_gmax = gmax;
-        const char *kname = A.chain_n > 1 ? "probe_agg_chain" : h ? "probe_agg" : "agg";
-        const bool use_fast = strategy == 1 && !gmax && fast_ok;
-        const bool use_run = use_fast && A.P.has_join && runjoin_env && dense_bytes(S) + run_bytes <= ctx->smem_optin - 1024;
-        if (!use_run) { rc = need_wide(); if (rc) { gx_tmp_free(ctx, g_tab); return rc; } }
-        const bool use_few = strategy == 1 && gmax && fewgroups_ok && est <= 2 * FG_G;
-        { const char *dbg = getenv("GX_DEBUG_AGG");
-          if (dbg && dbg[0] == '1')
-              fprintf(stderr, "gpuexec: hash_agg attempt %d strategy %d S %lld gmax %d fast_ok %d use_fast %d use_run %d cslots %d narrow %d slot mode %d seg %d tma %d rows %lld\n",
-                      attempt, strategy, S, gmax, (int) fast_ok, (int) use_fast, (int) use_run, A.cslots != nullptr, A.narrow != nullptr, A.sf.mode,
-                      (int) gx_runjoin_seg_enabled(), (int) gx_runjoin_tma_enabled(), (long long) outer->nrows); }
-        if (use_fast) rc = launch_fast(ctx, A, FA, A.P.has_join != 0, A.need_w0 != 0, FA.vcol != nullptr, dense_bytes(S), kname, use_run);
-        else if (use_few && countchar_ok) {
-            gx_launch_scope ls(ctx, kname);
-            gx_launch_scope which(ctx, "agg_count_char", 0);
-            gx_k_count_char<<<ctx->sm_count * 2, 512, 0, ctx->stream>>>(A, (const signed char *) A.P.gcols[0].col.data);
-            rc = cudaGetLastError() == cudaSuccess ? GX_OK : GX_ERR_CUDA;
-        } else if (use_few) {
-            const char *fv = getenv("GX_FG_VARIANT");
-            const bool v768 = !(fv && fv[0] == '0');                 // <4, 768> unless GX_FG_VARIANT=0 asks for <8, 512>
-            const int fg_threads = v768 ? 768 : 512, fg_k = v768 ? 4 : 8, fg_warps = fg_threads / 32;
-            const size_t fg_smem = (size_t) fg_warps * (1 + FG.nv) * (FG_G + 1) * 32 * 8;
-            bool bytekey = plan->n_group_cols <= 2;
-            for (int c = 0; c < plan->n_group_cols; c++) bytekey = bytekey && A.P.gcols[c].type == GX_CHAR && A.P.gcols[c].word == 0;
-            static bool fg_attr = false;
-            if (!fg_attr) {
-                const int lim = (int) ctx->smem_optin - 1024;        // static shared memory counts too
-                GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_fewgroups<true, 8, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-                GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_fewgroups<false, 8, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-                GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_fewgroups<true, 4, 768>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-                GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_fewgroups<false, 4, 768>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-                fg_attr = true;
-            }
-            long long nb = (outer->nrows + (long long) fg_warps * 32 * fg_k - 1) / ((long long) fg_warps * 32 * fg_k);
-            const unsigned fg_grid = (unsigned) (nb < ctx->sm_count ? nb : ctx->sm_count);
-            gx_launch_scope ls(ctx, kname);
-            gx_launch_scope which(ctx, "agg_fewgroups", 0);
-            if (v768) { if (bytekey) gx_k_fewgroups<true, 4, 768><<<fg_grid, 768, fg_smem, ctx->stream>>>(A, FG); else gx_k_fewgroups<false, 4, 768><<<fg_grid, 768, fg_smem, ctx->stream>>>(A, FG); }
-            else { if (bytekey) gx_k_fewgroups<true, 8, 512><<<fg_grid, 512, fg_smem, ctx->stream>>>(A, FG); else gx_k_fewgroups<false, 8, 512><<<fg_grid, 512, fg_smem, ctx->stream>>>(A, FG); }
-            rc = cudaGetLastError() == cudaSuccess ? GX_OK : GX_ERR_CUDA;
-        }
-        else if (strategy == 1 && gmax && lptile_ok) rc = launch_lptile(ctx, A, lp_bytes, kname, lp_warps * 32);
-        else if (strategy == 1 && gmax) rc = launch_agg<SINK_SMEM_LP>(ctx, A, lp_bytes, kname, lp_warps * 32);
-        else if (strategy == 1) rc = launch_agg<SINK_SMEM>(ctx, A, dense_bytes(S), kname);
-        else rc = launch_agg<SINK_GLOBAL>(ctx, A, 0, kname);
+        A.s_slots = C.strategy == 1 ? (int) S : 0; A.s_log2 = ilog2(S); A.s_tagkey = C.tagkey; A.s_gmax = gmax;
+        const bool use_fast = C.strategy == 1 && !gmax && C.fast_ok;
+        const bool use_run = use_fast && A.P.has_join && !C.sw.no_runjoin && C.dense_bytes(S) + 32 * sizeof(gx_runlist) <= ctx->smem_optin - 1024;
+        if (!use_run) { rc = C.need_wide(); if (rc) { gx_tmp_free(ctx, g_tab); return rc; } }
+        const bool use_few = C.strategy == 1 && gmax && C.fewgroups_ok && est <= 2 * FG_G;
+        if (C.sw.debug)
+            fprintf(stderr, "gpuexec: hash_agg attempt %d strategy %d S %lld gmax %d fast_ok %d use_fast %d use_run %d cslots %d narrow %d slot mode %d seg %d tma %d rows %lld\n",
+                    attempt, C.strategy, S, gmax, (int) C.fast_ok, (int) use_fast, (int) use_run, A.cslots != nullptr, A.narrow != nullptr, A.sf.mode,
+                    (int) C.sw.seg_on(), (int) C.sw.tma_on(), (long long) outer->nrows);
+        rc = launch_attempt(C, S, gmax, lp_warps, lp_bytes, use_fast, use_run, use_few);
         long long c[4];
         if (rc == GX_OK) rc = read_counters(ctx, c);
         if (rc != GX_OK) { gx_tmp_free(ctx, g_tab); return rc; }
         if (c[1] == 0) {
-            rc = table_to_result(ctx, &cp, plan, g_tab, g_cap, c[0], out);
+            rc = table_to_result(ctx, &C.cp, plan, g_tab, g_cap, c[0], out);
             gx_tmp_free(ctx, g_tab);
             return rc;
         }
@@ -3551,10 +3456,10 @@ static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, co
             fprintf(stderr, "gpuexec: a bounded mbarrier wait of gx_k_runjoin_seg / gx_k_runjoin_tma gave up; continuing with gx_k_runjoin\n");
             g_runjoin_seg_broken = true; continue;
         }
-        if (use_few) { fewgroups_ok = false; continue; }          // more than FG_G groups: same estimate, general kernels
+        if (use_few) { C.fewgroups_ok = false; continue; }        // more than FG_G groups: same estimate, general kernels
         // the planner's estimate was too low: grow, then fall over to radix
-        est = est < 8 ? 9 : est < 16 ? 17 : est * 8;
-        if (strategy == 1 && est * 3 / 2 > smax) strategy = (plan->strategy == 1) ? 3 : 2;
+        C.est = est < 8 ? 9 : est < 16 ? 17 : est * 8;
+        if (C.strategy == 1 && C.est * 3 / 2 > C.smax) C.strategy = (plan->strategy == 1) ? 3 : 2;
     }
     GX_SET_ERR(ctx, "hash_agg: group table kept overflowing");
     return GX_ERR_STATE;
@@ -3972,8 +3877,6 @@ int gx_aggregate_records(gx_ctx *ctx, gx_agg_dev A, unsigned long long *d_recs, 
     GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &d_over, (size_t) P * sizeof(int)));
     GX_CUDA(ctx, cudaMemsetAsync(d_over, 0, (size_t) P * sizeof(int), ctx->stream));
     GX_CUDA(ctx, cudaMemsetAsync(ctx->d_scratch + 12, 0, sizeof(long long), ctx->stream));
-    static bool attr = false;
-    if (!attr) { GX_CUDA(ctx, cudaFuncSetAttribute(gx_k_radix_agg, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ctx->smem_optin - 512)); attr = true; }
     {
         gx_launch_scope ls(ctx, "radix_partition", 3);
         gx_k_radix_hist<<<nblk, 512, P * sizeof(unsigned), ctx->stream>>>(d_recs, nrec, RW, bits, d_hist);
@@ -3981,12 +3884,9 @@ int gx_aggregate_records(gx_ctx *ctx, gx_agg_dev A, unsigned long long *d_recs, 
         gx_k_radix_scatter<<<nblk, 512, P * sizeof(unsigned), ctx->stream>>>(d_recs, nrec, RW, bits, d_hist, d_part);
     }
     A.s_slots = S2; A.s_log2 = ilog2(S2); A.rec_cap = nrec;
-    {
-        gx_launch_scope ls(ctx, "radix_agg");
-        unsigned grid = (unsigned) (P < ctx->sm_count ? P : ctx->sm_count);
-        gx_k_radix_agg<<<grid, 512, smem_bytes_for(S2, 2, nwords), ctx->stream>>>(A, d_part, d_hist, P, (int) nblk, d_groups, ctx->d_scratch + 12, d_over);
-    }
-    GX_CUDA(ctx, cudaGetLastError());
+    int rc = launch_kernel<gx_k_radix_agg>(ctx, (int) ctx->smem_optin - 512, agg_grid(P, 1, ctx->sm_count), 512, smem_bytes_for(S2, 2, nwords),
+                                           "radix_agg", nullptr, nullptr, A, d_part, d_hist, P, (int) nblk, d_groups, ctx->d_scratch + 12, d_over);
+    if (rc) return rc;
     // partitions that overflowed shared memory go through a global table
     int *h_over = (int *) malloc((size_t) P * sizeof(int));
     long long *h_hist0 = (long long *) malloc((size_t) P * sizeof(long long));
@@ -3998,7 +3898,6 @@ int gx_aggregate_records(gx_ctx *ctx, gx_agg_dev A, unsigned long long *d_recs, 
     long long over_recs = 0; int nover = 0;
     for (int p = 0; p < P; p++) if (h_over[p]) { nover++; over_recs += ((p + 1 < P) ? h_hist0[p + 1] : nrec) - h_hist0[p]; }
     free(h_over); free(h_hist0);
-    int rc = GX_OK;
     if (nover) {
         long long g_cap = gx_pow2_ceil(over_recs * 2 + 1024);
         unsigned long long *g_tab;
