@@ -398,7 +398,8 @@ int  gx_hash_probe(gx_ctx *ctx, const gx_table *outer, int key_col,
  * only), SEMI emits an outer row once on its first match, ANTI emits the outer rows without a match
  * (nodeHashjoin.c:628-634); SEMI/ANTI output carries no inner columns.  A NULL outer key never
  * matches.  RIGHT/FULL (HJ_FILL_INNER_TUPLES) are declined. */
-enum { GX_JOIN_INNER = 0, GX_JOIN_LEFT = 1, GX_JOIN_SEMI = 4, GX_JOIN_ANTI = 5 };
+enum { GX_JOIN_INNER = 0, GX_JOIN_LEFT = 1, GX_JOIN_SEMI = 4, GX_JOIN_ANTI = 5,
+       GX_JOIN_SEMI_RIGHT = 8, GX_JOIN_ANTI_RIGHT = 9 };   /* the last two: gx_hash_agg_right only */
 int  gx_hash_probe_ex(gx_ctx *ctx, const gx_table *outer, int key_col,
                       int n_preds, const gx_pred *preds, const gx_hash *h, int join_type,
                       int n_out_outer, const int32_t *out_outer_cols, gx_table **out);
@@ -439,6 +440,30 @@ typedef struct gx_join_step {
 } gx_join_step;
 int  gx_hash_agg_joins(gx_ctx *ctx, const gx_table *outer, int n_steps, const gx_join_step *steps,
                        const gx_agg_plan *plan, gx_result **out);
+
+/* Aggregate over a right semi or right anti hash join (JOIN_SEMI_RIGHT / JOIN_ANTI_RIGHT, nodes/nodes.h:897-900): the
+ * preserved relation is the BUILD side and the probe side only decides which of its rows survive (the bucket-delete
+ * arms of nodeHashjoin.c:580-607; HJ_FILL_INNER for ANTI_RIGHT, nodeHashjoin.c:880-882).
+ *   SEMI_RIGHT  a build row that passes the build quals and whose non-NULL key equals the key of at least one probe row
+ *               passing probe_preds is consumed once, however many probe rows match it; every build row of a matched
+ *               key is consumed.
+ *   ANTI_RIGHT  the build rows that pass the build quals and have no such partner, NULL keys included.
+ * An empty or fully filtered probe side gives SEMI_RIGHT nothing and ANTI_RIGHT every build row passing the build quals.
+ * Keys compare as for the other joins (INT4/DATE widened to int64, INT64_MIN an ordinary key).
+ *   h      gx_hash_build(build, key, build quals, n_payload = 0, ...): its payload is the build row number.
+ *   plan   an aggregate over build's columns (group columns side 0, arguments, preds), outer_key_col = -1 and
+ *          join_type = GX_JOIN_INNER; its preds are ANDed with the build quals.  Every aggregate, group key, NULL,
+ *          overflow and partial-state rule of gx_hash_agg applies; the result is an ordinary gx_result.
+ * The device marks the matched build rows (one bit per row; a unique table is read in the format its build wrote, a
+ * non-unique one walked in its 16-byte form, materialised as gx_hash_agg_joins does), compacts the consumed rows'
+ * plan columns in build row order, and aggregates them without a join.
+ * GX_ERR_ARG, the context staying usable: a join type other than GX_JOIN_SEMI_RIGHT / GX_JOIN_ANTI_RIGHT, an h with
+ * payload columns or not built from this build table at its current row count, a probe key column out of range or not
+ * INT4/INT8/DATE, plan->outer_key_col >= 0, plan->join_type != GX_JOIN_INNER, a plan column outside the build table,
+ * and whatever gx_hash_agg rejects for the plan.  gx_hash_agg, gx_hash_agg_joins and gx_exec_host reject these join
+ * types. */
+int  gx_hash_agg_right(gx_ctx *ctx, const gx_table *probe, int probe_key_col, int n_probe_preds, const gx_pred *probe_preds,
+                       const gx_table *build, const gx_hash *h, int join_type, const gx_agg_plan *plan, gx_result **out);
 
 /* Combine partial states across datanodes: redistribute groups on the group
  * key, then Finalize HashAggregate (xc_groupby.out:193-205; combine fns

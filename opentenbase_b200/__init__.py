@@ -30,6 +30,7 @@ GX_LT, GX_LE, GX_EQ, GX_GE, GX_GT, GX_NE = 1, 2, 3, 4, 5, 6
  GX_AGG_COVAR_SAMP_F8, GX_AGG_CORR_F8) = range(14, 26)
 GX_OP_COL, GX_OP_CONST, GX_OP_ADD, GX_OP_SUB, GX_OP_MUL, GX_OP_ARG2 = 1, 2, 3, 4, 5, 6
 GX_JOIN_INNER, GX_JOIN_LEFT, GX_JOIN_SEMI, GX_JOIN_ANTI = 0, 1, 4, 5
+GX_JOIN_SEMI_RIGHT, GX_JOIN_ANTI_RIGHT = 8, 9      # gx_hash_agg_right only: the build side is the preserved relation
 T_ORDERS, T_LINEITEM, T_CUSTOMER = 1, 2, 3
 # fixed schemas of include/gx_tpch_gen.h
 O_ORDERKEY, O_CUSTKEY, O_ORDERDATE, O_SHIPPRIORITY = 0, 1, 2, 3
@@ -178,6 +179,7 @@ def _declare(L):
         "gx_hash_probe_ex": (C.c_int, [vp, vp, C.c_int, C.c_int, C.POINTER(GxPred), vp, C.c_int, C.c_int, C.POINTER(i32), pp]),
         "gx_hash_agg": (C.c_int, [vp, vp, vp, C.POINTER(GxAggPlan), pp]),
         "gx_hash_agg_joins": (C.c_int, [vp, vp, C.c_int, C.POINTER(GxJoinStep), C.POINTER(GxAggPlan), pp]),
+        "gx_hash_agg_right": (C.c_int, [vp, vp, C.c_int, C.c_int, C.POINTER(GxPred), vp, vp, C.c_int, C.POINTER(GxAggPlan), pp]),
         "gx_result_combine": (C.c_int, [vp, vp]),
         "gx_result_ngroups": (i64, [vp]),
         "gx_result_fetch": (C.c_int, [vp, i64, vp, vp, vp]),
@@ -610,6 +612,17 @@ class Context:
             arr[i].join_type = st[2] if len(st) > 2 else GX_JOIN_INNER
         h = C.c_void_p()
         self._chk(lib().gx_hash_agg_joins(self.h, outer.h, len(steps), arr, C.byref(plan), C.byref(h)))
+        return Result(self, h, plan)
+
+    def hash_agg_right(self, probe: Table, probe_key_col, build: Table, ht: HashTable, join_type, plan: GxAggPlan,
+                       probe_preds=()) -> Result:
+        """gx_hash_agg_right: the plan aggregates build's rows that a right semi (GX_JOIN_SEMI_RIGHT) or right anti
+        (GX_JOIN_ANTI_RIGHT) join with the probe side consumes; ht = hash_build(build, key, preds=build quals) without
+        payload columns"""
+        pr = (GxPred * max(len(probe_preds), 1))(*[mk_pred(*p) for p in probe_preds])
+        h = C.c_void_p()
+        self._chk(lib().gx_hash_agg_right(self.h, probe.h, probe_key_col, len(probe_preds), pr, build.h, ht.h if ht else None,
+                                          join_type, C.byref(plan), C.byref(h)))
         return Result(self, h, plan)
 
     # ---- communicator / routing

@@ -3721,19 +3721,29 @@ __global__ void __launch_bounds__(256) gx_k_distinct_fold(const gx_distinct_args
     }
 }
 
+// stage 1's plan: the plan with col appended as a group column and without its count(DISTINCT) aggregates;
+// map[a] = plan aggregate a's stage-1 aggregate (-1: the DISTINCT word)
+static void distinct_stage1_plan(const gx_agg_plan *plan, int col, gx_agg_plan *p1, int *map)
+{
+    const int ng = plan->n_group_cols;
+    *p1 = *plan;
+    p1->n_group_cols = ng + 1;
+    p1->group_cols[ng].side = 0; p1->group_cols[ng].col = col;
+    int n1 = 0;
+    for (int a = 0; a < plan->n_aggs; a++) {
+        if (plan->aggs[a].fn == GX_AGG_COUNT_DISTINCT) { map[a] = -1; continue; }
+        map[a] = n1; p1->aggs[n1++] = plan->aggs[a];
+    }
+    p1->n_aggs = n1;
+}
+
 static int count_distinct_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, int col,
                               gx_result **out, const chain_spec *ch)
 {
     const int ng = plan->n_group_cols;
-    gx_agg_plan p1 = *plan;
-    p1.n_group_cols = ng + 1;
-    p1.group_cols[ng].side = 0; p1.group_cols[ng].col = col;
-    int map[GX_MAX_AGGS], n1 = 0;                      // plan aggregate -> stage-1 aggregate (-1: the DISTINCT word)
-    for (int a = 0; a < plan->n_aggs; a++) {
-        if (plan->aggs[a].fn == GX_AGG_COUNT_DISTINCT) { map[a] = -1; continue; }
-        map[a] = n1; p1.aggs[n1++] = plan->aggs[a];
-    }
-    p1.n_aggs = n1;
+    gx_agg_plan p1;
+    int map[GX_MAX_AGGS];
+    distinct_stage1_plan(plan, col, &p1, map);
     gx_result *s1 = nullptr;
     int rc = hash_agg_checked(ctx, outer, h, &p1, &s1, ch);
     if (rc != GX_OK) return rc;
@@ -3793,6 +3803,19 @@ static int hash_agg_entry(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, 
     int col;
     int rc = distinct_column(ctx, outer, plan, &col); if (rc) return rc;
     return col < 0 ? hash_agg_checked(ctx, outer, h, plan, out, ch) : count_distinct_run(ctx, outer, h, plan, col, out, ch);
+}
+
+int gx_check_agg_plan(gx_ctx *ctx, const gx_table *t, const gx_agg_plan *plan)
+{
+    int col;
+    int rc = distinct_column(ctx, t, plan, &col); if (rc) return rc;
+    gx_agg_plan p = *plan;
+    int map[GX_MAX_AGGS];
+    if (col >= 0) distinct_stage1_plan(plan, col, &p, map);
+    compiled_plan *cp = new compiled_plan;                 // host work only: the plan's checks and descriptors
+    rc = compile_plan(ctx, t, nullptr, &p, cp);
+    delete cp;
+    return rc;
 }
 
 extern "C" int gx_hash_agg(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, gx_result **out)

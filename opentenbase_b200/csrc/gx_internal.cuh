@@ -62,7 +62,9 @@ struct gx_table {
     void *cols[GX_MAX_COLS];
     uint8_t *nulls[GX_MAX_COLS];     // NULL when the column has no NULLs
     int64_t nrows, capacity;
+    uint64_t version;                // new, never reused value whenever the table is created or its rows or columns change
 };
+uint64_t gx_table_next_version();    // gx_table.cu
 
 struct gx_slot { long long key; unsigned long long payload; };   // 16 B
 // Compact slot (8 B).  With an order-preserving slot function the keys that can land in one
@@ -122,6 +124,9 @@ struct gx_hash {
     unsigned int amask;             // home slots are aligned to amask + 1 (2 for 16 B slots, 4 for compact ones)
     // rows whose key equals GX_EMPTY_KEY cannot live in the table: side list
     unsigned long long *special_payload; int special_cap; int special_count;
+    // what the build read, for gx_hash_agg_right: the table, its version then, and the build quals (applied again
+    // when the build rows are compacted)
+    const gx_table *src; uint64_t src_version; int n_preds; gx_pred preds[GX_MAX_PREDS];
 };
 
 int gx_hash_wide(gx_ctx *ctx, gx_hash *h);
@@ -213,8 +218,15 @@ static inline void gx_tmp_free(gx_ctx *ctx, void *p) { if (p) cudaFreeAsync(p, c
 
 int gx_table_alloc_like(gx_ctx *ctx, int ncols, const int32_t *types, const bool *has_nulls,
                         int64_t capacity, gx_table **out);
+// gx_scan_filter that also keeps only the rows whose bit in `mark` (one bit per input row) is set (keep_marked) or
+// clear; gx_table.cu
+int gx_filter_marked(gx_ctx *ctx, const gx_table *in, int n_preds, const gx_pred *preds, int n_out_cols,
+                     const int32_t *out_cols, const unsigned int *mark, bool keep_marked, gx_table **out);
 // GX_ERR_ARG unless the plan's join type is one gx_hash_agg runs (INNER, SEMI, ANTI)
 int gx_check_agg_join_type(gx_ctx *ctx, const gx_agg_plan *plan);
+// what gx_hash_agg(ctx, t, nullptr, plan) would reject before touching the device (GX_ERR_ARG), without running it; t's
+// column types and NULL arrays are read, not its rows.  gx_agg.cu
+int gx_check_agg_plan(gx_ctx *ctx, const gx_table *t, const gx_agg_plan *plan);
 
 // device-side plan descriptors -------------------------------------------
 struct gx_dcol { const void *data; const uint8_t *nulls; int type; int _pad; };

@@ -891,6 +891,8 @@ extern "C" int gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col, in
     int bytes = 0;
     gx_hash *h = (gx_hash *) calloc(1, sizeof(gx_hash));
     h->ctx = ctx; h->key_type = kt; h->n_payload = n_payload; h->unique = unique;
+    h->src = inner; h->src_version = inner->version; h->n_preds = n_preds;
+    if (n_preds > 0) memcpy(h->preds, preds, (size_t) n_preds * sizeof(gx_pred));      // n_preds checked by gx_fill_dpreds
     struct hash_guard { gx_hash *h; ~hash_guard() { if (h) gx_hash_free(h); } } guard{h};     // every early return frees the table
     for (int i = 0; i < n_payload; i++) {
         int c = payload_cols[i];
@@ -1533,4 +1535,200 @@ extern "C" int gx_hash_probe_ex(gx_ctx *ctx, const gx_table *outer, int key_col,
     t->nrows = ctx->h_scratch[0] < out_cap ? ctx->h_scratch[0] : out_cap;
     *out = t;
     return GX_OK;
+}
+
+// ------------------------------------------------- right semi / anti join under an aggregate
+// JOIN_SEMI_RIGHT / JOIN_ANTI_RIGHT (nodes.h:897-900): the preserved relation is the build side, and the probe side only
+// decides which build rows survive (the bucket-delete arms of nodeHashjoin.c:580-607, HJ_FILL_INNER for ANTI_RIGHT).
+// Three steps: a marking probe sets one bit per build row that has a partner, the build rows are compacted by their bit
+// (gx_k_filter_onepass, build row order kept), and the aggregate runs over the compacted rows without a join.
+struct gx_mark_args {
+    gx_dcol key;
+    int npreds, _pad;
+    gx_dpred preds[GX_MAX_PREDS];
+    long long nrows;
+    const gx_slot *slots; unsigned long long mask;
+    const gx_cslot *cslots; unsigned long long cspan;
+    const unsigned int *narrow;
+    const unsigned long long *special; int special_count; int _pad2; gx_slotfn sf;
+    unsigned int *bits;                 // one bit per build row (the build stored the row number as payload)
+};
+
+// set a build row's bit; a bit already set costs a load instead of an atomic
+__device__ __forceinline__ void gx_mark_row(unsigned int *bits, unsigned long long row)
+{
+    unsigned int *w = bits + (row >> 5);
+    const unsigned int b = 1u << (row & 31);
+    if (!(__ldcg(w) & b)) atomicOr(w, b);
+}
+
+// A warp takes tiles of PT_K x 32 probe rows, as gx_k_hash_probe_unique does: quals tile-wise, NULL keys skipped.  A lane
+// whose key equals the key of the lane below it marks nothing (the lane below marks the same rows), which keeps the
+// atomics down on a probe side clustered on the key (lineitem: ~4 rows per order).  WALK = false: a unique build, read in
+// the format the build wrote through gx_probe_first; WALK = true: every partner, walked in the 16-byte form.  Rows with
+// key INT64_MIN mark the side list.
+template <int F, bool WALK>
+__global__ void __launch_bounds__(256) gx_k_probe_mark(gx_mark_args a)
+{
+    const int lane = threadIdx.x & 31;
+    const long long nwarp = ((long long) gridDim.x * blockDim.x) >> 5, wid = ((long long) blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const long long tile = 32LL * PT_K;
+    for (long long base = wid * tile; base < a.nrows; base += nwarp * tile) {
+        long long r[PT_K], key[PT_K]; bool ok[PT_K];
+#pragma unroll
+        for (int j = 0; j < PT_K; j++) { r[j] = base + j * 32 + lane; ok[j] = r[j] < a.nrows; }
+        for (int p = 0; p < a.npreds; p++) pred_tile<PT_K>(a.preds[p], r, ok);
+#pragma unroll
+        for (int j = 0; j < PT_K; j++) {
+            ok[j] = ok[j] && !gx_is_null(a.key, r[j]);                     // a NULL key never matches (hashStrict)
+            key[j] = ok[j] ? gx_load_int(a.key, r[j]) : 0;
+            const long long kd = __shfl_up_sync(0xffffffffu, key[j], 1);
+            const bool od = __shfl_up_sync(0xffffffffu, ok[j], 1);
+            if (lane > 0 && od && kd == key[j]) ok[j] = false;
+            if (ok[j] && key[j] == GX_EMPTY_KEY) {
+                for (int i = 0; i < a.special_count; i++) gx_mark_row(a.bits, a.special[i]);
+                ok[j] = false;
+            }
+        }
+        if (!WALK) {
+            bool hit[PT_K]; unsigned long long pay[PT_K];
+            gx_probe_first<F, PT_K>(a, ok, key, hit, pay);
+#pragma unroll
+            for (int j = 0; j < PT_K; j++) if (hit[j]) gx_mark_row(a.bits, pay[j]);
+        } else {
+            unsigned long long s[PT_K]; long long k0[PT_K], k1[PT_K]; unsigned long long p0[PT_K], p1[PT_K];
+#pragma unroll
+            for (int j = 0; j < PT_K; j++) {                                // the home pairs' loads in flight together
+                s[j] = gx_slot_index(key[j], a.sf); k0[j] = k1[j] = GX_EMPTY_KEY; p0[j] = p1[j] = 0;
+                if (ok[j]) gx_ld_pair(a.slots + s[j], k0[j], p0[j], k1[j], p1[j]);
+            }
+#pragma unroll
+            for (int j = 0; j < PT_K; j++) {
+                if (!ok[j]) continue;
+                for (;;) {                                                  // linear probing: the run ends at an empty slot
+                    if (k0[j] == GX_EMPTY_KEY) break;
+                    if (k0[j] == key[j]) gx_mark_row(a.bits, p0[j]);
+                    if (k1[j] == GX_EMPTY_KEY) break;
+                    if (k1[j] == key[j]) gx_mark_row(a.bits, p1[j]);
+                    s[j] = gx_next_pair(s[j], a.mask);
+                    gx_ld_pair(a.slots + s[j], k0[j], p0[j], k1[j], p1[j]);
+                }
+            }
+        }
+    }
+}
+
+// the plan's build columns -> compacted table columns; GX_ERR_ARG for a column the build table does not have
+static int right_columns(gx_ctx *ctx, const gx_table *build, const gx_agg_plan *plan, bool plan_keeps_preds, int *map, int32_t *out_cols, int *n_out)
+{
+    for (int c = 0; c < GX_MAX_COLS; c++) map[c] = -1;
+    *n_out = 0;
+    auto use = [&](int col, const char *what, int i) -> int {
+        GX_CHECK_ARG(ctx, col >= 0 && col < build->ncols, "hash_agg_right: %s %d reads column %d of a %d-column build table", what, i, col, build->ncols);
+        if (map[col] < 0) { map[col] = *n_out; out_cols[(*n_out)++] = col; }
+        return GX_OK;
+    };
+    int rc;
+    GX_CHECK_ARG(ctx, plan->n_group_cols >= 0 && plan->n_group_cols <= GX_MAX_GROUP_COLS, "agg plan: n_group_cols %d", plan->n_group_cols);
+    GX_CHECK_ARG(ctx, plan->n_aggs >= 0 && plan->n_aggs <= GX_MAX_AGGS, "agg plan: n_aggs %d", plan->n_aggs);
+    GX_CHECK_ARG(ctx, plan->n_preds >= 0 && plan->n_preds <= GX_MAX_PREDS, "too many predicates (%d)", plan->n_preds);
+    for (int c = 0; c < plan->n_group_cols; c++) {
+        GX_CHECK_ARG(ctx, plan->group_cols[c].side == 0, "hash_agg_right: group column %d is on side %d (the build table is side 0)", c, plan->group_cols[c].side);
+        if ((rc = use(plan->group_cols[c].col, "group column", c))) return rc;
+    }
+    for (int a = 0; a < plan->n_aggs; a++) {
+        if (plan->aggs[a].fn == GX_AGG_COUNT_STAR) continue;              // takes no argument: its program is not read
+        const gx_expr &e = plan->aggs[a].arg;
+        GX_CHECK_ARG(ctx, e.nops >= 0 && e.nops <= GX_MAX_EXPR_OPS, "agg %d: %d ops", a, e.nops);
+        for (int k = 0; k < e.nops; k++) if (e.ops[k].op == GX_OP_COL && (rc = use(e.ops[k].col, "aggregate", a))) return rc;
+    }
+    if (plan_keeps_preds)
+        for (int p = 0; p < plan->n_preds; p++) if ((rc = use(plan->preds[p].col, "predicate", p))) return rc;
+    return GX_OK;
+}
+
+extern "C" int gx_hash_agg_right(gx_ctx *ctx, const gx_table *probe, int probe_key_col, int n_probe_preds, const gx_pred *probe_preds,
+                                 const gx_table *build, const gx_hash *h, int join_type, const gx_agg_plan *plan, gx_result **out)
+{
+    if (!ctx || !probe || !build || !plan || !out) return GX_ERR_ARG;
+    GX_CHECK_ARG(ctx, join_type == GX_JOIN_SEMI_RIGHT || join_type == GX_JOIN_ANTI_RIGHT,
+                 "hash_agg_right: join type %d (right semi %d, right anti %d)", join_type, GX_JOIN_SEMI_RIGHT, GX_JOIN_ANTI_RIGHT);
+    GX_CHECK_ARG(ctx, h != nullptr, "hash_agg_right: no join table");
+    GX_CHECK_ARG(ctx, h->n_payload == 0, "hash_agg_right: the join table carries %d payload columns (it must carry the build row number)", h->n_payload);
+    GX_CHECK_ARG(ctx, h->src == build && h->src_version == build->version,
+                 "hash_agg_right: the join table was not built from this build table as it is now");
+    GX_CHECK_ARG(ctx, probe_key_col >= 0 && probe_key_col < probe->ncols, "hash_agg_right: probe key column %d out of range", probe_key_col);
+    const int kt = probe->types[probe_key_col];
+    GX_CHECK_ARG(ctx, kt == GX_INT4 || kt == GX_INT8 || kt == GX_DATE, "hash_agg_right: probe key type %d (int4, int8 or date)", kt);
+    GX_CHECK_ARG(ctx, plan->outer_key_col < 0, "hash_agg_right: the plan's outer_key_col must be -1 (the probe key is an argument)");
+    GX_CHECK_ARG(ctx, plan->join_type == GX_JOIN_INNER, "hash_agg_right: the plan's join type must be inner (%d given)", plan->join_type);
+    gx_mark_args a; memset(&a, 0, sizeof(a));
+    int rc = gx_fill_dpreds(ctx, probe, n_probe_preds, probe_preds, a.preds); if (rc) return rc;
+    // the plan's quals join the build quals in the compaction when they fit one qual list, else the aggregate applies them
+    const bool plan_keeps_preds = h->n_preds + plan->n_preds > GX_MAX_PREDS;
+    int map[GX_MAX_COLS]; int32_t out_cols[GX_MAX_COLS]; int n_out = 0;
+    rc = right_columns(ctx, build, plan, plan_keeps_preds, map, out_cols, &n_out); if (rc) return rc;
+    if (n_out == 0) out_cols[n_out++] = 0;                                  // count(*) alone: the table needs a column
+    gx_pred cpreds[GX_MAX_PREDS]; int ncp = h->n_preds;                 // at most GX_MAX_PREDS: see plan_keeps_preds
+    memcpy(cpreds, h->preds, sizeof(h->preds));
+    if (!plan_keeps_preds) for (int p = 0; p < plan->n_preds; p++) cpreds[ncp++] = plan->preds[p];
+    gx_agg_plan p = *plan;                                                  // the plan over the compacted columns
+    for (int c = 0; c < p.n_group_cols; c++) p.group_cols[c].col = map[p.group_cols[c].col];
+    for (int i = 0; i < p.n_aggs; i++) {
+        if (p.aggs[i].fn == GX_AGG_COUNT_STAR) continue;
+        for (int k = 0; k < p.aggs[i].arg.nops; k++) if (p.aggs[i].arg.ops[k].op == GX_OP_COL) p.aggs[i].arg.ops[k].col = map[p.aggs[i].arg.ops[k].col];
+    }
+    if (plan_keeps_preds) for (int i = 0; i < p.n_preds; i++) p.preds[i].col = map[p.preds[i].col];
+    else p.n_preds = 0;
+    p.outer_key_col = -1; p.join_type = GX_JOIN_INNER;
+    {
+        // what the aggregate would reject is rejected before any device work: the compacted table's shape is known
+        gx_table shape; memset(&shape, 0, sizeof(shape));
+        shape.ctx = ctx; shape.ncols = n_out; shape.nrows = build->nrows; shape.capacity = build->nrows;
+        for (int c = 0; c < n_out; c++) {
+            shape.types[c] = build->types[out_cols[c]]; shape.cols[c] = build->cols[out_cols[c]]; shape.nulls[c] = build->nulls[out_cols[c]];
+        }
+        rc = gx_check_agg_plan(ctx, &shape, &p); if (rc) return rc;
+        gx_dpred dp[GX_MAX_PREDS];                                          // the compaction's quals: columns and operators
+        rc = gx_fill_dpreds(ctx, build, ncp, cpreds, dp); if (rc) return rc;
+    }
+
+    // 1. marking probe
+    // a row-number payload is never narrow (the narrow form carries one 4-byte payload column): wide or compact
+    const bool walk = !h->unique;
+    if (walk && probe->nrows > 0) { rc = gx_hash_wide(ctx, const_cast<gx_hash *>(h)); if (rc) return rc; }
+    const size_t nwords = (size_t) ((build->nrows + 31) / 32);
+    unsigned int *bits = nullptr;
+    cudaError_t e = gx_tmp_alloc(ctx, (void **) &bits, (nwords ? nwords : 1) * sizeof(unsigned int));
+    if (e == cudaSuccess) e = cudaMemsetAsync(bits, 0, (nwords ? nwords : 1) * sizeof(unsigned int), ctx->stream);
+    if (e == cudaSuccess && probe->nrows > 0) {
+        a.key.data = probe->cols[probe_key_col]; a.key.nulls = probe->nulls[probe_key_col]; a.key.type = kt;
+        a.npreds = n_probe_preds; a.nrows = probe->nrows;
+        a.slots = h->slots; a.mask = (unsigned long long) h->nslots - 1;
+        a.cslots = h->cslots; a.cspan = h->cspan;
+        a.special = h->special_payload; a.special_count = h->special_count;
+        a.sf = gx_hash_slotfn(h); a.bits = bits;
+        const long long nt = (probe->nrows + 32 * PT_K * 8 - 1) / (32 * PT_K * 8), maxb = (long long) ctx->sm_count * 8;
+        const unsigned grid = (unsigned) (nt < maxb ? nt : maxb);
+        gx_launch_scope ls(ctx, "probe_mark");
+        gx_launch_scope which(ctx, walk ? "probe_mark_walk" : h->cslots ? "probe_mark_compact" : "probe_mark_wide", 0);
+        if (walk) gx_k_probe_mark<GX_SLOTS_WIDE, true><<<grid, 256, 0, ctx->stream>>>(a);
+        else if (h->cslots) gx_k_probe_mark<GX_SLOTS_COMPACT, false><<<grid, 256, 0, ctx->stream>>>(a);
+        else gx_k_probe_mark<GX_SLOTS_WIDE, false><<<grid, 256, 0, ctx->stream>>>(a);
+        e = cudaGetLastError();
+    }
+    if (e != cudaSuccess) {
+        gx_tmp_free(ctx, bits);
+        GX_SET_ERR(ctx, "hash_agg_right: %s", cudaGetErrorString(e));
+        return e == cudaErrorMemoryAllocation ? GX_ERR_NOMEM : GX_ERR_CUDA;
+    }
+    // 2. the build rows the join consumes, in build row order
+    gx_table *kept = nullptr;
+    rc = gx_filter_marked(ctx, build, ncp, cpreds, n_out, out_cols, bits, join_type == GX_JOIN_SEMI_RIGHT, &kept);
+    gx_tmp_free(ctx, bits);
+    if (rc) return rc;
+    // 3. the aggregate, without a join
+    rc = gx_hash_agg(ctx, kept, nullptr, &p, out);
+    gx_table_free(kept);
+    return rc;
 }

@@ -4,12 +4,18 @@
 #include "../../include/gx_tpch_gen.h"
 
 // --------------------------------------------------------------- lifecycle
+uint64_t gx_table_next_version()
+{
+    static unsigned long long next = 0;
+    return (uint64_t) __atomic_add_fetch(&next, 1ULL, __ATOMIC_RELAXED);
+}
+
 int gx_table_alloc_like(gx_ctx *ctx, int ncols, const int32_t *types, const bool *has_nulls,
                         int64_t capacity, gx_table **out)
 {
     GX_CHECK_ARG(ctx, ncols > 0 && ncols <= GX_MAX_COLS, "table: ncols %d out of range", ncols);
     gx_table *t = (gx_table *) calloc(1, sizeof(gx_table));
-    t->ctx = ctx; t->ncols = ncols; t->capacity = capacity < 1 ? 1 : capacity;
+    t->ctx = ctx; t->ncols = ncols; t->capacity = capacity < 1 ? 1 : capacity; t->version = gx_table_next_version();
     for (int c = 0; c < ncols; c++) {
         int sz = gx_type_size(types[c]);
         if (!sz) { free(t); GX_SET_ERR(ctx, "table: column %d has unknown type %d", c, types[c]); return GX_ERR_ARG; }
@@ -43,7 +49,7 @@ extern "C" void gx_table_free(gx_table *t)
 }
 extern "C" int64_t gx_table_nrows(const gx_table *t) { return t ? t->nrows : -1; }
 extern "C" int gx_table_ncols(const gx_table *t) { return t ? t->ncols : -1; }
-extern "C" int gx_table_truncate(gx_table *t) { if (!t) return GX_ERR_ARG; t->nrows = 0; return GX_OK; }
+extern "C" int gx_table_truncate(gx_table *t) { if (!t) return GX_ERR_ARG; t->nrows = 0; t->version = gx_table_next_version(); return GX_OK; }
 // End of a load: wait for the enqueued appends and report a NULL that arrived in a column staged as NOT NULL
 extern "C" int gx_table_load_finish(gx_table *t)
 {
@@ -61,6 +67,7 @@ extern "C" int gx_table_drop_column(gx_table *t, int col)
     gx_tmp_free(t->ctx, t->cols[col]); gx_tmp_free(t->ctx, t->nulls[col]);
     for (int c = col; c + 1 < t->ncols; c++) { t->cols[c] = t->cols[c + 1]; t->nulls[c] = t->nulls[c + 1]; t->types[c] = t->types[c + 1]; }
     t->ncols--;
+    t->version = gx_table_next_version();
     t->cols[t->ncols] = nullptr; t->nulls[t->ncols] = nullptr; t->types[t->ncols] = 0;
     return GX_OK;
 }
@@ -123,6 +130,7 @@ extern "C" int gx_table_append_columns(gx_table *t, const void *const *host_cols
         }
     }
     t->nrows += nrows;
+    t->version = gx_table_next_version();
     return GX_OK;
 }
 
@@ -324,6 +332,7 @@ static int generate_impl(gx_table *t, int table_id, int sf, int64_t o0, int64_t 
     gx_tmp_free(ctx, d_sums);
     if (e != cudaSuccess) { GX_SET_ERR(ctx, "generate: %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
     t->nrows += total;
+    t->version = gx_table_next_version();
     return GX_OK;
 }
 
@@ -371,9 +380,11 @@ __device__ __forceinline__ bool filter_pass(const gx_filter_args &a, long long r
     return ok;
 }
 
-// FT_K rows per thread and tile (8: tiles of 2048 rows; 16: tiles of 4096 rows, half the barriers and look-backs per row)
-template <int FT_K>
-__global__ void __launch_bounds__(FT_THREADS, 4) gx_k_filter_onepass(gx_filter_args a, unsigned long long *tile_state, unsigned int *ticket, long long ntiles, long long *total_out)
+// FT_K rows per thread and tile (8: tiles of 2048 rows; 16: tiles of 4096 rows, half the barriers and look-backs per row).
+// MARK 0: the quals decide; 1: a row must also have its bit set in `mark` (one bit per input row); 2: its bit clear
+template <int FT_K, int MARK>
+__device__ __forceinline__ void filter_onepass(const gx_filter_args &a, const unsigned int *mark, unsigned long long *tile_state, unsigned int *ticket,
+                                               long long ntiles, long long *total_out)
 {
     constexpr int FT_ROWS = FT_THREADS * FT_K;
     constexpr int NCNT = FT_K * (FT_THREADS / 32);          // (k, warp) counts per tile: 64 or 128
@@ -397,6 +408,12 @@ __global__ void __launch_bounds__(FT_THREADS, 4) gx_k_filter_onepass(gx_filter_a
             for (int k = 0; k < FT_K; k++) { rr[k] = base + k * FT_THREADS + threadIdx.x; keep[k] = rr[k] < a.nrows; }
 #pragma unroll
             for (int p = 0; p < GX_MAX_PREDS; p++) if (p < a.npreds) pred_tile<FT_K>(a.preds[p], rr, keep);
+            if (MARK != 0) {
+                // a warp's 32 rows share one bitmap word (tiles start at multiples of FT_ROWS): one broadcast load
+#pragma unroll
+                for (int k = 0; k < FT_K; k++)
+                    if (keep[k]) keep[k] = ((__ldg(mark + (rr[k] >> 5)) >> (rr[k] & 31)) & 1u) == (MARK == 1 ? 1u : 0u);
+            }
         }
 #pragma unroll
         for (int k = 0; k < FT_K; k++) {
@@ -455,6 +472,18 @@ __global__ void __launch_bounds__(FT_THREADS, 4) gx_k_filter_onepass(gx_filter_a
         __syncthreads();                                        // wc / woff / s_* are reused by the next tile
     }
 }
+template <int FT_K>
+__global__ void __launch_bounds__(FT_THREADS, 4) gx_k_filter_onepass(gx_filter_args a, unsigned long long *tile_state, unsigned int *ticket, long long ntiles, long long *total_out)
+{
+    filter_onepass<FT_K, 0>(a, nullptr, tile_state, ticket, ntiles, total_out);
+}
+// the same compaction restricted to the marked (MARK 1) or unmarked (MARK 2) rows: the build side of gx_hash_agg_right
+template <int FT_K, int MARK>
+__global__ void __launch_bounds__(FT_THREADS, 4) gx_k_filter_onepass(gx_filter_args a, unsigned long long *tile_state, unsigned int *ticket, long long ntiles, long long *total_out,
+                                                                  const unsigned int *mark)
+{
+    filter_onepass<FT_K, MARK>(a, mark, tile_state, ticket, ntiles, total_out);
+}
 
 static gx_dcol make_dcol(const gx_table *t, int c)
 {
@@ -472,10 +501,10 @@ int gx_fill_dpreds(gx_ctx *ctx, const gx_table *t, int n_preds, const gx_pred *p
     return GX_OK;
 }
 
-extern "C" int gx_scan_filter(gx_ctx *ctx, const gx_table *in, int n_preds, const gx_pred *preds,
-                              int n_out_cols, const int32_t *out_cols, gx_table **out)
+// mark_mode 0: quals only; 1 / 2: also the rows whose bit in `mark` is set / clear (gx_filter_marked)
+static int scan_filter_run(gx_ctx *ctx, const gx_table *in, int n_preds, const gx_pred *preds,
+                           int n_out_cols, const int32_t *out_cols, const unsigned int *mark, int mark_mode, gx_table **out)
 {
-    if (!ctx || !in || !out || !out_cols) return GX_ERR_ARG;
     GX_CHECK_ARG(ctx, n_out_cols > 0 && n_out_cols <= GX_MAX_COLS, "scan_filter: bad output column count");
     gx_filter_args a; memset(&a, 0, sizeof(a));
     a.npreds = n_preds; a.ncols = n_out_cols; a.nrows = in->nrows;
@@ -493,7 +522,7 @@ extern "C" int gx_scan_filter(gx_ctx *ctx, const gx_table *in, int n_preds, cons
     if (in->nrows > 0) {
         for (int c = 0; c < n_out_cols; c++) { a.out[c] = t->cols[c]; a.out_nulls[c] = t->nulls[c]; }
         const char *k16 = getenv("GX_FILTER_K16");
-        const bool big = !(k16 && k16[0] == '0');                 // 4096-row tiles unless GX_FILTER_K16=0
+        const bool big = mark_mode != 0 || !(k16 && k16[0] == '0');    // 4096-row tiles unless GX_FILTER_K16=0 (marked rows: always)
         const long long tile_rows = (long long) FT_THREADS * (big ? 16 : 8);
         const long long ntiles = (in->nrows + tile_rows - 1) / tile_rows;
         unsigned long long *d_state = nullptr;
@@ -501,10 +530,13 @@ extern "C" int gx_scan_filter(gx_ctx *ctx, const gx_table *in, int n_preds, cons
         if (e == cudaSuccess) e = cudaMemsetAsync(d_state, 0, (size_t) (ntiles + 1) * sizeof(unsigned long long), ctx->stream);
         if (e == cudaSuccess) {
             gx_launch_scope ls(ctx, "filter");
+            gx_launch_scope which(ctx, mark_mode ? "filter_marked" : nullptr, 0);
             long long maxb = (long long) ctx->sm_count * 8;
             const unsigned fgrid = (unsigned) (ntiles < maxb ? ntiles : maxb);
             unsigned int *tk = (unsigned int *) (d_state + ntiles);
-            if (big) gx_k_filter_onepass<16><<<fgrid, FT_THREADS, 0, ctx->stream>>>(a, d_state, tk, ntiles, ctx->d_scratch);
+            if (mark_mode == 1) gx_k_filter_onepass<16, 1><<<fgrid, FT_THREADS, 0, ctx->stream>>>(a, d_state, tk, ntiles, ctx->d_scratch, mark);
+            else if (mark_mode == 2) gx_k_filter_onepass<16, 2><<<fgrid, FT_THREADS, 0, ctx->stream>>>(a, d_state, tk, ntiles, ctx->d_scratch, mark);
+            else if (big) gx_k_filter_onepass<16><<<fgrid, FT_THREADS, 0, ctx->stream>>>(a, d_state, tk, ntiles, ctx->d_scratch);
             else gx_k_filter_onepass<8><<<fgrid, FT_THREADS, 0, ctx->stream>>>(a, d_state, tk, ntiles, ctx->d_scratch);
             e = cudaGetLastError();
         }
@@ -517,6 +549,17 @@ extern "C" int gx_scan_filter(gx_ctx *ctx, const gx_table *in, int n_preds, cons
     t->nrows = total;
     *out = t;
     return GX_OK;
+}
+extern "C" int gx_scan_filter(gx_ctx *ctx, const gx_table *in, int n_preds, const gx_pred *preds,
+                              int n_out_cols, const int32_t *out_cols, gx_table **out)
+{
+    if (!ctx || !in || !out || !out_cols) return GX_ERR_ARG;
+    return scan_filter_run(ctx, in, n_preds, preds, n_out_cols, out_cols, nullptr, 0, out);
+}
+int gx_filter_marked(gx_ctx *ctx, const gx_table *in, int n_preds, const gx_pred *preds, int n_out_cols,
+                     const int32_t *out_cols, const unsigned int *mark, bool keep_marked, gx_table **out)
+{
+    return scan_filter_run(ctx, in, n_preds, preds, n_out_cols, out_cols, mark, keep_marked ? 1 : 2, out);
 }
 
 // ------------------------------------------------- K0 heap-page deform
@@ -704,7 +747,7 @@ extern "C" int gx_table_append_heap_pages(gx_table *t, const void *pages, int64_
             gx_k_deform<<<(unsigned) ((nthreads + 255) / 256), 256, 0, ctx->stream>>>(a, d_offs);
             e = cudaGetLastError();
         }
-        if (e == cudaSuccess) { t->nrows += total; e = gx_stage_mark(ctx, pages); }
+        if (e == cudaSuccess) { t->nrows += total; t->version = gx_table_next_version(); e = gx_stage_mark(ctx, pages); }
     } else if (e == cudaSuccess) {
         a.pages = d_pages; a.vis = d_vis; a.vis_counts = d_cnt;
         {
@@ -728,7 +771,7 @@ extern "C" int gx_table_append_heap_pages(gx_table *t, const void *pages, int64_
                     gx_k_deform<<<(unsigned) ((nthreads + 255) / 256), 256, 0, ctx->stream>>>(a, d_offs);
                 }
                 e = cudaStreamSynchronize(ctx->stream);
-                if (e == cudaSuccess) t->nrows += total;
+                if (e == cudaSuccess) { t->nrows += total; t->version = gx_table_next_version(); }
             }
         }
     }

@@ -71,4 +71,15 @@ gpuexec_path_cost(const gpuexec_cost_params *p, double pages, double staged_byte
 	*total_cost = run + p->cpu_tuple_cost * groups;
 }
 
+/*
+ * staged_bytes of a right semi / right anti join (gx_hash_agg_right): the hashed relation's referenced columns, read by
+ * the build, by the compaction of the consumed rows and by the aggregate over them (three passes); its join table
+ * (16-byte slots at load factor <= 2/3: 32 B per row) and match bitmap; and the probe side's key and qual columns once.
+ */
+static inline double
+gpuexec_right_join_bytes(double build_rows, double build_row_bytes, double probe_rows, double probe_row_bytes)
+{
+	return build_rows * (3.0 * build_row_bytes + 32.0 + 0.125) + probe_rows * probe_row_bytes;
+}
+
 #endif							/* GPUEXEC_COST_H */

@@ -133,6 +133,13 @@ typedef struct GpuJoinStep
 /* the descriptor word after the version for a join chain: 0 is no join, 1 + GX_JOIN_* a single join */
 #define GPUEXEC_DESC_CHAIN 100
 
+/* a right semi / right anti join: the outer slot holds the hashed (preserved) relation, join[0] the probing one */
+static inline bool
+is_right_join(int jt)
+{
+	return jt == GX_JOIN_SEMI_RIGHT || jt == GX_JOIN_ANTI_RIGHT;
+}
+
 typedef struct GpuExecState
 {
 	CustomScanState css;
@@ -681,14 +688,28 @@ gpuexec_run(GpuExecState *st, EState *estate)
 
 	INSTR_TIME_SET_CURRENT(t0);
 	/* the tables in chain order; every one is in st before the next call, so an ERROR frees them all */
-	for (int i = 0; i < st->n_joins; i++)
+	for (int i = 0; i < st->n_joins && !is_right_join(st->plan.join_type); i++)
 	{
 		GpuJoinStep *j = &st->join[i];
 
 		GX_CHECK(gx_hash_build(backend_ctx, j->tab, j->key_col, j->n_preds, j->preds, j->n_payload, j->payload_cols, j->unique, &j->hash));
 		CHECK_FOR_INTERRUPTS();
 	}
-	if (st->n_joins >= 2)
+	if (is_right_join(st->plan.join_type))
+	{
+		/* the hashed relation is the outer table (its row numbers ride in the slots); join[0] probes it */
+		GpuJoinStep *j = &st->join[0];
+		gx_agg_plan cp = st->plan;
+
+		GX_CHECK(gx_hash_build(backend_ctx, st->outer_tab, cp.outer_key_col, cp.n_preds, cp.preds, 0, NULL, j->unique, &j->hash));
+		CHECK_FOR_INTERRUPTS();
+		cp.outer_key_col = -1;
+		cp.n_preds = 0;			/* applied by the build, and again when the consumed rows are compacted */
+		cp.join_type = GX_JOIN_INNER;
+		GX_CHECK(gx_hash_agg_right(backend_ctx, j->tab, j->key_col, j->n_preds, j->preds, st->outer_tab, j->hash,
+								   st->plan.join_type, &cp, &st->result));
+	}
+	else if (st->n_joins >= 2)
 	{
 		gx_join_step steps[GX_MAX_JOINS];
 		gx_agg_plan cp = st->plan;
@@ -912,7 +933,9 @@ gpuexec_explain(CustomScanState *node, List *ancestors, ExplainState *es)
 
 	ExplainPropertyText("GPU Strategy", st->n_joins ? "hash build + fused probe/aggregate" : "scan + hash aggregate", es);
 	if (st->n_joins)
-		ExplainPropertyText("GPU Join Type", st->plan.join_type == GX_JOIN_SEMI ? "Semi" : st->plan.join_type == GX_JOIN_ANTI ? "Anti" : "Inner", es);
+		ExplainPropertyText("GPU Join Type", st->plan.join_type == GX_JOIN_SEMI ? "Semi" : st->plan.join_type == GX_JOIN_ANTI ? "Anti"
+							: st->plan.join_type == GX_JOIN_SEMI_RIGHT ? "Right Semi" : st->plan.join_type == GX_JOIN_ANTI_RIGHT ? "Right Anti"
+							: "Inner", es);
 	if (st->n_joins > 1)
 		ExplainPropertyInteger("GPU Joins", NULL, st->n_joins, es);
 	for (i = 0; i < st->plan.n_aggs; i++)
@@ -1483,8 +1506,11 @@ join_level(PlannerInfo *root, HashPath *hp, Var **ov, Var **iv)
 }
 
 /* Agg over HashJoin(HashJoin(... SeqScan(F), SeqScan(D1)) ..., SeqScan(Dn)), 1 <= n <= GX_MAX_JOINS: step s builds Ds.
- * One join may be INNER, SEMI or ANTI (EXISTS / NOT EXISTS); a chain (gx_hash_agg_joins) must be INNER with a unique
- * build side on every level.  LEFT, RIGHT, FULL and the JOIN_UNIQUE_* forms stay on the CPU.  Step 1's probe key is a
+ * One join may be INNER, SEMI or ANTI (EXISTS / NOT EXISTS), or SEMI_RIGHT / ANTI_RIGHT; a chain (gx_hash_agg_joins) must
+ * be INNER with a unique build side on every level.  LEFT, RIGHT, FULL and the JOIN_UNIQUE_* forms stay on the CPU.
+ * A right semi / right anti join preserves its hashed (inner) relation: that relation takes the outer slot of the
+ * descriptor (its key, quals, GROUP BY and argument columns), and the probing relation the join step, with its key and
+ * quals only (gx_hash_agg_right).  Step 1's probe key is a
  * column of F; a later step's is a column of F or of an earlier D, carried in that step's payload (which has no NULL
  * flag: the column must be NOT NULL). */
 static bool
@@ -1522,10 +1548,27 @@ match_joins(PlannerInfo *root, HashPath *top, GpuExecState *out, double *est_byt
 		int			c,
 					t = 0;
 
-		if (n == 1 ? (jt != JOIN_INNER && jt != JOIN_SEMI && jt != JOIN_ANTI) : (jt != JOIN_INNER || !hp->jpath.inner_unique))
+		if (n == 1 ? (jt != JOIN_INNER && jt != JOIN_SEMI && jt != JOIN_ANTI && jt != JOIN_SEMI_RIGHT && jt != JOIN_ANTI_RIGHT)
+			: (jt != JOIN_INNER || !hp->jpath.inner_unique))
 			return false;
 		if (!join_level(root, hp, &ov, &iv))
 			return false;
+		if (jt == JOIN_SEMI_RIGHT || jt == JOIN_ANTI_RIGHT)
+		{
+			/* the probe relation p (F so far) becomes the join step; the hashed relation the outer slot */
+			plan->join_type = jt == JOIN_SEMI_RIGHT ? GX_JOIN_SEMI_RIGHT : GX_JOIN_ANTI_RIGHT;
+			j->unique = hp->jpath.inner_unique;
+			j->tuples = p->parent->tuples;
+			j->rel.rti = out->outer.rti;
+			out->outer.rti = iv->varno;
+			*est_bytes = irel->tuples;		/* the rows the aggregate's columns are staged for */
+			*est_pages += irel->pages;
+			plan->outer_key_col = rel_column(&out->outer, iv->varno, iv->varattno, iv->vartype, iv->vartypmod);
+			j->key_col = rel_column(&j->rel, ov->varno, ov->varattno, ov->vartype, ov->vartypmod);
+			return plan->outer_key_col >= 0 && j->key_col >= 0 &&
+				match_quals(irel->baserestrictinfo, &out->outer, plan->preds, &plan->n_preds) &&
+				match_quals(p->parent->baserestrictinfo, &j->rel, j->preds, &j->n_preds);
+		}
 		plan->join_type = jt == JOIN_SEMI ? GX_JOIN_SEMI : jt == JOIN_ANTI ? GX_JOIN_ANTI : GX_JOIN_INNER;
 		j->unique = hp->jpath.inner_unique;
 		j->tuples = irel->tuples;
@@ -1841,6 +1884,15 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 
 		for (i = 0; i < out->outer.ncols; i++)
 			bytes += outer_rows * staged_type_bytes(out->outer.types[i]);
+		if (is_right_join(plan->join_type))
+		{
+			double		probe_row = 0;
+
+			for (i = 0; i < out->join[0].rel.ncols; i++)
+				probe_row += staged_type_bytes(out->join[0].rel.types[i]);
+			bytes = gpuexec_right_join_bytes(outer_rows, bytes / Max(outer_rows, 1), out->join[0].tuples, probe_row);
+		}
+		else
 		for (i = 0; i < out->n_joins; i++)
 		{
 			const GpuJoinStep *j = &out->join[i];

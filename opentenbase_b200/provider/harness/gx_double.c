@@ -176,6 +176,21 @@ int gx_hash_agg_joins(gx_ctx *ctx, const gx_table *outer, int n_steps, const gx_
 	fprintf(stderr, "\n");
 	return gx_hash_agg(ctx, outer, steps[0].h, plan, out);
 }
+/* the probe side and the table, then the canned result of gx_hash_agg */
+int gx_hash_agg_right(gx_ctx *ctx, const gx_table *probe, int probe_key_col, int n_probe_preds, const gx_pred *probe_preds,
+					  const gx_table *build, const gx_hash *h, int join_type, const gx_agg_plan *plan, gx_result **out)
+{
+	int			i;
+
+	if (!probe->finished) { snprintf(last_error, sizeof(last_error), "double: hash_agg_right before load_finish"); return GX_ERR_STATE; }
+	if (!h || h->n_payload != 0 || plan->outer_key_col >= 0 || plan->join_type != GX_JOIN_INNER)
+	{ snprintf(last_error, sizeof(last_error), "double: hash_agg_right with a payload or a join in the plan"); return GX_ERR_ARG; }
+	fprintf(stderr, "double: hash_agg_right type %d probe rows %lld key %d table key %d preds", join_type, (long long) probe->rows,
+			probe_key_col, h->key_col);
+	for (i = 0; i < n_probe_preds; i++) fprintf(stderr, " (%d %d %lld)", probe_preds[i].col, probe_preds[i].op, (long long) probe_preds[i].ival);
+	fprintf(stderr, "\n");
+	return gx_hash_agg(ctx, build, NULL, plan, out);
+}
 int64_t gx_result_ngroups(const gx_result *r) { return r->ngroups; }
 int gx_result_fetch(gx_result *r, int64_t max_groups, int64_t *key_out, double *agg_out, uint8_t *null_out)
 {

@@ -535,9 +535,19 @@ static int plan_main(const char *path)
 			ip->pathtype = remote ? T_RemoteSubplan : T_SeqScan; ip->parent = plan_rels[r2].rel; ip->rows = ip->parent->tuples; ip->total_cost = ip->parent->pages + 0.01 * ip->rows;
 			ri->clause = plan_op(lv->vartype == INT8OID ? F_INT8EQ : lv->vartype == INT4OID ? F_INT4EQ : F_TEXTEQ, swap ? (Node *) rv : (Node *) lv, swap ? (Node *) lv : (Node *) rv);
 			hp->jpath.path.pathtype = T_HashJoin; hp->jpath.inner_unique = u != 0;
-			hp->jpath.jointype = strstr(line, "left") ? JOIN_LEFT : strstr(line, "semi") ? JOIN_SEMI : strstr(line, "anti") ? JOIN_ANTI :
+			/* the right forms first: their words contain "semi", "anti" and "right" */
+			hp->jpath.jointype = strstr(line, "semi_right") ? JOIN_SEMI_RIGHT : strstr(line, "anti_right") ? JOIN_ANTI_RIGHT :
+				strstr(line, "left") ? JOIN_LEFT : strstr(line, "semi") ? JOIN_SEMI : strstr(line, "anti") ? JOIN_ANTI :
 				strstr(line, "right") ? JOIN_RIGHT : strstr(line, "full") ? JOIN_FULL : JOIN_INNER;
 			hp->jpath.outerjoinpath = op; hp->jpath.innerjoinpath = ip; hp->jpath.joinrestrictinfo = list_make1(ri); hp->path_hashclauses = list_make1(ri);
+			if (strstr(line, "extra_clause"))
+			{
+				/* a second join clause next to the hash clause (a join filter the fused paths do not evaluate) */
+				RestrictInfo *ri2 = makeNode(RestrictInfo);
+
+				ri2->clause = ri->clause;
+				hp->jpath.joinrestrictinfo = lappend(hp->jpath.joinrestrictinfo, ri2);
+			}
 			input_rel = makeNode(RelOptInfo); input_rel->reloptkind = RELOPT_JOINREL; input_rel->rows = op->rows;
 			hp->jpath.path.parent = input_rel; hp->jpath.path.rows = op->rows; hp->jpath.path.total_cost = op->total_cost + ip->total_cost + 0.02 * op->rows;
 			input_rel->cheapest_total_path = &hp->jpath.path;

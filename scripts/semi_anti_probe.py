@@ -10,11 +10,16 @@ Shapes (DATE_Q3 = 1995-03-15):
          (orders: an unordered, non-unique build side, about 10 rows per key)
   semi   lineitem SEMI orders[o_orderdate < DATE_Q3], GROUP BY l_shipdate count(*), sum(l_extendedprice), against the INNER
          plan with the same outer-only GROUP BY; both on the unique build
+  q4_right_semi / q4_right_anti   the right form of q4 (gx_hash_agg_right): orders hashed (unique, key-ordered),
+         lineitem[l_shipdate > DATE_Q3] probing it, GROUP BY o_orderdate count(*)
+  q22_right_anti                  the right form of q22: customer hashed (unique), orders probing it, GROUP BY c_mktsegment
 Per shape: the median step time over --steps steps (table build + probe/aggregate + fetch), the per-kernel profile of
 one more pass over the same steps, and the bytes the probe must read (outer columns + the join table once) over its
 kernel time against the H100 SXM's 3.35 TB/s.  Built-in checks: on the unique build the SEMI counts equal the INNER
 counts exactly, and per group count(SEMI) + count(ANTI) equals the count with no join exactly (sums within 1e-9
-relative).  Prints the card's name and power limit and one JSON line; --out also writes it to DIR/semi_anti_probe.json."""
+relative); each right form's counts equal its left form's, group for group.  For a right form the kernel time is the
+marking probe's (probe_mark), its bytes the probe side's key and qual columns plus the join table and the bitmap once.
+Prints the card's name and power limit and one JSON line; --out also writes it to DIR/semi_anti_probe.json."""
 import argparse
 import json
 import os
@@ -29,7 +34,7 @@ import opentenbase_b200 as g                                     # noqa: E402
 
 DATE_Q3 = -1752
 HBM_TBPS = 3.35
-KERNELS = ("probe_agg", "agg", "probe_agg_exist_wide", "probe_agg_exist_compact", "probe_agg_exist_narrow", "build",
+KERNELS = ("probe_mark", "probe_mark_wide", "probe_mark_compact", "probe_mark_walk", "filter", "probe_agg", "agg", "probe_agg_exist_wide", "probe_agg_exist_compact", "probe_agg_exist_narrow", "build",
            "build_expand", "agg_smem", "agg_smem_lp", "agg_global", "agg_records", "agg_compact", "agg_inf_scan")
 SLOT_BYTES = {"probe_agg_exist_wide": 16, "probe_agg_exist_compact": 8, "probe_agg_exist_narrow": 4}
 
@@ -81,6 +86,49 @@ def measure(ctx, name, inner, ikey, ipreds, unique, outer, plan, outer_bytes_per
     return s, out
 
 
+def measure_right(ctx, name, build, bkey, probe, pkey, ppreds, jt, plan, probe_bytes_per_row, steps, warmup):
+    """measure() for gx_hash_agg_right: the build (no payload: the row number) is timed with every step"""
+    def step():
+        ht = ctx.hash_build(build, bkey, [], unique=True)
+        r = ctx.hash_agg_right(probe, pkey, build, ht, jt, plan, probe_preds=ppreds)
+        out = r.fetch()
+        slots = ht.nslots
+        r.free()
+        ht.free()
+        return out, slots
+    for _ in range(warmup):
+        step()
+    times = []
+    for _ in range(steps):
+        ctx.timer_start()
+        out, slots = step()
+        times.append(ctx.timer_stop())
+    ctx.profile(True)
+    for _ in range(steps):
+        step()
+    prof = {k: ctx.profile_get(k) for k in KERNELS}
+    ctx.profile(False)
+    prof = {k: {"ms_per_step": round(ms / steps, 4), "launches_per_step": n / steps} for k, (ms, n) in prof.items() if n}
+    kms = prof["probe_mark"]["ms_per_step"]
+    fmt = [k for k in ("probe_mark_compact", "probe_mark_wide", "probe_mark_walk") if k in prof]
+    nbytes = probe.nrows * probe_bytes_per_row + slots * (8 if fmt == ["probe_mark_compact"] else 16) + build.nrows // 8
+    s = {"shape": name, "median_step_ms": round(float(np.median(times)), 4), "min_step_ms": round(float(np.min(times)), 4),
+         "steps": steps, "kernel": "probe_mark", "kernel_ms": kms, "format": fmt[0] if fmt else None, "outer_rows": probe.nrows,
+         "bytes": nbytes, "gb_per_s": round(nbytes / (kms * 1e-3) / 1e9, 1), "frac_of_3.35TBps": round(nbytes / (kms * 1e-3) / (HBM_TBPS * 1e12), 3),
+         "profile": prof}
+    print(json.dumps(s), flush=True)
+    return s, out
+
+
+def same_counts(right, left):
+    """per group: the right form's count equals the left form's exactly"""
+    kr, kl = by_key(right[0], right[1]), by_key(left[0], left[1])
+    assert set(kr) == set(kl), "group keys differ"
+    for k in kl:
+        assert int(kr[k][0:1].view(np.int64)[0]) == int(kl[k][0:1].view(np.int64)[0]), k
+    return len(kl)
+
+
 def counts_add_up(semi, anti, none, sum_col=None):
     """per group: count(SEMI) + count(ANTI) == count(no join) exactly; sums within 1e-9 relative"""
     ks, ka, kn = by_key(semi[0], semi[1]), by_key(anti[0], anti[1]), by_key(none[0], none[1])
@@ -128,6 +176,14 @@ def main():
     s, q4n = run("q4_nojoin", None, 0, (), False, orders, g.make_plan(group_cols=[(0, 2)], aggs=cnt, est_groups=2406), 4)
     res["shapes"].append(s)
     res["q4_groups_checked"] = counts_add_up(q4s, q4a, q4n)
+    # the right forms of Q4: lineitem[l_shipdate > DATE_Q3] probes orders (l_orderkey 8 B + l_shipdate 4 B per probe row)
+    rrun = lambda *a: measure_right(ctx, *a, steps=args.steps, warmup=args.warmup)
+    rplan = g.make_plan(group_cols=[(0, 2)], aggs=cnt, est_groups=2406)
+    s, q4rs = rrun("q4_right_semi", orders, 0, lineitem, 0, lq, g.GX_JOIN_SEMI_RIGHT, rplan, 12)
+    res["shapes"].append(s)
+    s, q4ra = rrun("q4_right_anti", orders, 0, lineitem, 0, lq, g.GX_JOIN_ANTI_RIGHT, rplan, 12)
+    res["shapes"].append(s)
+    res["q4_right_equals_left_groups"] = same_counts(q4rs, q4s) + same_counts(q4ra, q4a)
     # Q22: customer ANTI orders on c_custkey = o_custkey (c_custkey 4 B, c_mktsegment 1 B)
     s, q22a = run("q22_anti", orders, 1, (), False, customer, plan(0, 1, cnt, 5, g.GX_JOIN_ANTI), 5)
     res["shapes"].append(s)
@@ -136,6 +192,11 @@ def main():
     s, q22n = run("q22_nojoin", None, 0, (), False, customer, g.make_plan(group_cols=[(0, 1)], aggs=cnt, est_groups=5), 1)
     res["shapes"].append(s)
     res["q22_groups_checked"] = counts_add_up(q22s, q22a, q22n)
+    # the right form of Q22: orders probes customer (o_custkey 4 B per probe row)
+    s, q22ra = rrun("q22_right_anti", customer, 0, orders, 1, (), g.GX_JOIN_ANTI_RIGHT,
+                    g.make_plan(group_cols=[(0, 1)], aggs=cnt, est_groups=5), 4)
+    res["shapes"].append(s)
+    res["q22_right_equals_left_groups"] = same_counts(q22ra, q22a)
     # lineitem SEMI orders[o_orderdate < DATE_Q3] against INNER, GROUP BY l_shipdate (8 + 4 + 8 B per outer row)
     oq = [(2, g.GX_LT, DATE_Q3)]
     aggs = cnt + [(g.GX_AGG_SUM_F8, [(g.GX_OP_COL, 1, 0)])]
