@@ -23,10 +23,21 @@ struct gx_build_args {
     gx_slot *slots; unsigned long long mask;
     unsigned long long *special; int special_cap;
     gx_slotfn sf;                 // gx_slot_index
-    long long *counters;          // [0] entries inserted, [1] special count
+    long long *counters;          // ctx->d_scratch: the SW_* words
     // direct build only: rows claimed per sub-table, how many one sub-table may hold, and the largest
     // claim count seen past that limit (0 = none)
     unsigned int *sub_claims; unsigned int sub_limit; unsigned int *sub_over;
+};
+// Words of ctx->d_scratch / h_scratch the build uses (word 2 is gx_hash_probe_ex's output cursor).  The sample's key range
+// shares word 5 with the chain steps, which are counted only after it is read.  OVF_*: bits of the key-ordered fill's
+// overflow word; OVF_FULL also flags the bucketing's overflow.
+enum {
+    SW_INSERTED = 0, SW_SPECIAL = 1,    // entries the direct build inserted; side-list rows
+    SW_PLACED = 3, SW_STEPS = 5,        // entries the fills placed; their chain steps
+    SW_KRANGE = 4, SW_PRANGE = 16,      // the sample's key, payload min and max
+    SW_UNSORTED = 6, SW_OVERFLOW = 7,   // key-ordered build: rows out of key order; OVF_* bits (both int)
+    SW_ENDS = 20,                       // the key column's first and last key
+    OVF_FULL = 1, OVF_STUCK = 2, OVF_PAYLOAD = 4   // a sub-table is full; a staged wait gave up; a payload outside the narrow window
 };
 
 __device__ __forceinline__ unsigned long long pack_payload(const gx_build_args &a, long long r)
@@ -58,7 +69,7 @@ __global__ void __launch_bounds__(256) gx_k_hash_build(gx_build_args a)
         long long key = gx_load_int(a.key, r);
         unsigned long long payload = pack_payload(a, r);
         if (key == GX_EMPTY_KEY) {
-            int idx = (int) atomicAdd((unsigned long long *) &a.counters[1], 1ULL);
+            int idx = (int) atomicAdd((unsigned long long *) &a.counters[SW_SPECIAL], 1ULL);
             if (idx < a.special_cap) a.special[idx] = payload;
             continue;
         }
@@ -80,7 +91,7 @@ __global__ void __launch_bounds__(256) gx_k_hash_build(gx_build_args a)
     // one atomic per warp
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) inserted += __shfl_down_sync(0xffffffffu, inserted, o);
-    if ((threadIdx.x & 31) == 0 && inserted) atomicAdd((unsigned long long *) &a.counters[0], (unsigned long long) inserted);
+    if ((threadIdx.x & 31) == 0 && inserted) atomicAdd((unsigned long long *) &a.counters[SW_INSERTED], (unsigned long long) inserted);
 }
 
 __global__ void gx_k_fill_slots(gx_slot *slots, long long n)
@@ -143,7 +154,7 @@ __global__ void __launch_bounds__(256) gx_k_bbuild_scatter(gx_bbuild_args a)
 #pragma unroll
         for (int u = 0; u < BSCAT; u++) {
             if (ok[u] && key[u] == GX_EMPTY_KEY) {
-                int idx = (int) atomicAdd((unsigned long long *) &a.b.counters[1], 1ULL);
+                int idx = (int) atomicAdd((unsigned long long *) &a.b.counters[SW_SPECIAL], 1ULL);
                 if (idx < a.b.special_cap) a.b.special[idx] = payload[u];
                 ok[u] = false;
             }
@@ -153,7 +164,7 @@ __global__ void __launch_bounds__(256) gx_k_bbuild_scatter(gx_bbuild_args a)
 #pragma unroll
         for (int u = 0; u < BSCAT; u++) {
             if (!ok[u]) continue;
-            if (pos[u] >= GX_SUB - 1) { *a.overflow = 1; continue; }      // a sub-table keeps one slot free
+            if (pos[u] >= GX_SUB - 1) { *a.overflow = OVF_FULL; continue; }      // a sub-table keeps one slot free
             longlong2 v; v.x = key[u]; v.y = (long long) payload[u];
             ((longlong2 *) a.pairs)[sub[u] * GX_SUB + pos[u]] = v;
         }
@@ -247,7 +258,7 @@ __global__ void __launch_bounds__(BP_THREADS, 2) gx_k_bpart1(gx_bpart_args a)
             key[u] = ok[u] ? gx_load_int(a.b.key, r) : 0;
             payload[u] = ok[u] ? pack_payload(a.b, r) : 0;
             if (ok[u] && key[u] == GX_EMPTY_KEY) {
-                int idx = (int) atomicAdd((unsigned long long *) &a.b.counters[1], 1ULL);
+                int idx = (int) atomicAdd((unsigned long long *) &a.b.counters[SW_SPECIAL], 1ULL);
                 if (idx < a.b.special_cap) a.b.special[idx] = payload[u];
                 ok[u] = false;
             }
@@ -260,7 +271,7 @@ __global__ void __launch_bounds__(BP_THREADS, 2) gx_k_bpart1(gx_bpart_args a)
         for (unsigned int j = threadIdx.x; j < total; j += blockDim.x) {
             unsigned int d = m.bid[j];
             long long pos = (long long) m.gbase[d] + (j - m.base[d]);
-            if (pos >= a.cap1) { *a.overflow = 1; continue; }
+            if (pos >= a.cap1) { *a.overflow = OVF_FULL; continue; }
             ((longlong2 *) a.l1)[(long long) d * a.cap1 + pos] = m.stage[j];
         }
         __syncthreads();
@@ -297,7 +308,7 @@ __global__ void __launch_bounds__(BP_THREADS, 2) gx_k_bpart2(gx_bpart_args a)
         for (unsigned int j = threadIdx.x; j < total; j += blockDim.x) {
             unsigned int d = m.bid[j];
             unsigned int pos = m.gbase[d] + (j - m.base[d]);
-            if (pos >= GX_SUB - 1) { *a.overflow = 1; continue; }       // a sub-table keeps one slot free
+            if (pos >= GX_SUB - 1) { *a.overflow = OVF_FULL; continue; }       // a sub-table keeps one slot free
             ((longlong2 *) a.pairs)[(((long long) b1 << a.bits_lo) | d) * GX_SUB + pos] = m.stage[j];
         }
         __syncthreads();
@@ -475,8 +486,8 @@ __device__ __forceinline__ void fill_report(const gx_build_args &b, unsigned int
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) { steps += __shfl_down_sync(0xffffffffu, steps, o); placed += __shfl_down_sync(0xffffffffu, placed, o); }
     if ((threadIdx.x & 31) == 0) {
-        if (steps) atomicAdd((unsigned long long *) &b.counters[5], (unsigned long long) steps);      // chain statistics decide whether
-        if (placed) atomicAdd((unsigned long long *) &b.counters[3], (unsigned long long) placed);    // the slot function is kept
+        if (steps) atomicAdd((unsigned long long *) &b.counters[SW_STEPS], (unsigned long long) steps);      // chain statistics decide whether
+        if (placed) atomicAdd((unsigned long long *) &b.counters[SW_PLACED], (unsigned long long) placed);    // the slot function is kept
     }
 }
 
@@ -590,7 +601,7 @@ __global__ void __launch_bounds__(FILL_THREADS, F != GX_SLOTS_WIDE ? 5 : 4) gx_k
         const long long nsubn = sub + gridDim.x;
         if (nsubn < a.nsub) { nlo = a.start[nsubn]; nhi = a.start[nsubn + 1]; }
         unsigned int n = (unsigned int) (hi - lo);
-        if (hi - lo >= GX_SUB) { n = 0; if (threadIdx.x == 0) atomicOr(a.overflow, 1); }     // a sub-table keeps one slot free
+        if (hi - lo >= GX_SUB) { n = 0; if (threadIdx.x == 0) atomicOr(a.overflow, OVF_FULL); }     // a sub-table keeps one slot free
         if (VERIFY && hi < lo) { n = 0; bad = 1; }
         if (!VERIFY)
             gx_subtable_build<F>(sm, n, a.b.sf,
@@ -612,7 +623,7 @@ __global__ void __launch_bounds__(FILL_THREADS, F != GX_SLOTS_WIDE ? 5 : 4) gx_k
         lo = nlo; hi = nhi;
     }
     if (VERIFY && bad) *a.unsorted = 1;
-    if (pay_miss) atomicOr(a.overflow, 4);
+    if (pay_miss) atomicOr(a.overflow, OVF_PAYLOAD);
     fill_report(a.b, steps, placed);
 }
 
@@ -679,7 +690,7 @@ __global__ void __launch_bounds__(FILL_THREADS, F != GX_SLOTS_WIDE ? 3 : 2) gx_k
         if (__syncthreads_or(!gx_mbar_wait(&st.bar, (unsigned int) ((s - s0) >> 1) & 1u))) { stuck = true; break; }
         const long long lo = st.lo, hi = st.hi;
         unsigned int n = (unsigned int) (hi - lo);
-        if (hi - lo >= GX_SUB) { n = 0; if (threadIdx.x == 0) atomicOr(a.overflow, 1); }       // a sub-table keeps one slot free
+        if (hi - lo >= GX_SUB) { n = 0; if (threadIdx.x == 0) atomicOr(a.overflow, OVF_FULL); }       // a sub-table keeps one slot free
         if (hi < lo) { n = 0; bad = 1; }
         const long long *sk = st.key + (lo - ((lo > 0 ? lo - 1 : 0) & ~1LL));                 // row lo; sk[-1] is row lo - 1
         const unsigned int *sp = st.pay + (lo & 3);
@@ -696,9 +707,9 @@ __global__ void __launch_bounds__(FILL_THREADS, F != GX_SLOTS_WIDE ? 3 : 2) gx_k
         // gx_subtable_build ends with a barrier: nobody reads this stage any more
         if (threadIdx.x == 0 && s + 2 < s1) issue(s + 2, st);
     }
-    if (stuck && threadIdx.x == 0) atomicOr(a.overflow, 2);
+    if (stuck && threadIdx.x == 0) atomicOr(a.overflow, OVF_STUCK);
     if (VERIFY && bad) *a.unsorted = 1;
-    if (pay_miss) atomicOr(a.overflow, 4);
+    if (pay_miss) atomicOr(a.overflow, OVF_PAYLOAD);
     fill_report(a.b, steps, placed);
 }
 // ---------------------------------------------------------------------------
@@ -787,7 +798,7 @@ __global__ void gx_k_sorted_special(gx_build_args a, const long long *start, con
     for (long long r = threadIdx.x; r < n; r += blockDim.x) {
         if (gx_is_null(a.key, r) || gx_load_int(a.key, r) != GX_EMPTY_KEY) continue;
         if (!build_row_ok(a, r)) continue;
-        int idx = (int) atomicAdd((unsigned long long *) &a.counters[1], 1ULL);
+        int idx = (int) atomicAdd((unsigned long long *) &a.counters[SW_SPECIAL], 1ULL);
         if (idx < a.special_cap) a.special[idx] = pack_payload(a, r);
     }
 }
@@ -832,14 +843,27 @@ __global__ void gx_k_key_range(gx_dcol key, gx_dcol pay, long long nrows, long l
 // average chain exceeds 4 is redone with the mixing hash.
 #define GX_INTERP_MAX_SPREAD 256.0
 
+// the build's environment switches (README), read once per build
+struct build_switches {
+    unsigned int win;                 // GX_SLOT_WIN (31)
+    int slot_mode;                    // GX_SLOT_MODE: 0 mixing hash without a sample, 1 interpolation at any key spread (-1)
+    bool wide, direct, nosorted, onepass, nosearch, nocompact;   // GX_SLOT_WIDE, GX_BUILD_{DIRECT,NOSORTED,ONEPASS},
+};                                                               // GX_NO_BOUNDS_SEARCH, GX_NO_COMPACT = 1
+static bool switch_on(const char *name) { const char *e = getenv(name); return e && e[0] == '1'; }
+static build_switches read_build_switches()
+{
+    const char *win = getenv("GX_SLOT_WIN"), *mode = getenv("GX_SLOT_MODE");
+    return { win ? (unsigned int) atoi(win) : 31u, mode ? atoi(mode) : -1, switch_on("GX_SLOT_WIDE"), switch_on("GX_BUILD_DIRECT"),
+             switch_on("GX_BUILD_NOSORTED"), switch_on("GX_BUILD_ONEPASS"), switch_on("GX_NO_BOUNDS_SEARCH"), switch_on("GX_NO_COMPACT") };
+}
+
 // interpolation slot function over [kmin, kmin + range): slots [0, nslots - GX_SUB), monotone in the key.
-// Narrow ranges (< 2^32, the usual case: at most 16 keys of range per row) use 32-bit arithmetic.
-static void gx_set_interpolation(gx_hash *h, long long kmin, double range_d)
+// Narrow ranges (< 2^32, the usual case: at most 16 keys of range per row) use 32-bit arithmetic unless `wide`.
+static void gx_set_interpolation(gx_hash *h, long long kmin, double range_d, bool wide)
 {
     const long double ratio = (long double) (h->nslots - GX_SUB) / (long double) range_d;
     h->kmin = kmin;
-    const char *wide = getenv("GX_SLOT_WIDE");
-    if (range_d < 4294967295.0 && !(wide && wide[0] == '1')) {
+    if (range_d < 4294967295.0 && !wide) {
         int sh = 0;
         while (sh < 62 && ratio * (long double) (1ULL << (sh + 1)) < 4294967295.0L) sh++;
         h->mode = 2; h->shift = (unsigned int) sh;
@@ -876,373 +900,348 @@ template <int F, bool VERIFY> static void sorted_fill(gx_ctx *ctx, const gx_bbui
     gx_k_sorted_fill<F, VERIFY><<<ctx->sm_count * (F != GX_SLOTS_WIDE ? 10 : 8), FILL_THREADS, bytes, ctx->stream>>>(ba);
 }
 
-extern "C" int gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col, int n_preds, const gx_pred *preds,
-                             int n_payload, const int32_t *payload_cols, int unique, gx_hash **out)
+// gx_hash_slotfn's inverse (the mask follows nslots)
+static void set_slotfn(gx_hash *h, const gx_slotfn &f)
+{ h->mode = f.mode; h->win = f.win; h->kmin = f.kmin; h->scale = f.scale; h->shift = f.shift; h->amask = f.amask; h->tbits = f.tbits; h->pbase = f.pbase; }
+template <class T> struct tmp_buf {                 // a temporary device buffer, freed at scope exit
+    gx_ctx *ctx; T *p = nullptr;
+    explicit tmp_buf(gx_ctx *c) : ctx(c) {}
+    ~tmp_buf() { gx_tmp_free(ctx, p); }
+    cudaError_t alloc(size_t n) { cudaError_t e = gx_tmp_alloc(ctx, (void **) &p, n * sizeof(T)); if (e != cudaSuccess) p = nullptr; return e; }
+};
+static cudaError_t clear_scratch(gx_ctx *ctx, int w0, int w1) { return cudaMemsetAsync(ctx->d_scratch + w0, 0, (w1 - w0 + 1) * sizeof(long long), ctx->stream); }
+static double fill_avg_chain(const long long *w) { return w[SW_PLACED] > 0 ? (double) w[SW_STEPS] / (double) w[SW_PLACED] : 0.0; }
+// One join-table build.  h owns the slot function: a.sf = gx_hash_slotfn(h) before every launch.
+struct build_job {
+    gx_ctx *ctx; const gx_table *inner; int key_col; build_switches sw;
+    gx_build_args a; int payload_bytes;
+    gx_hash *h;                       // freed unless handed out
+    build_job(gx_ctx *c, const gx_table *t, int k) : ctx(c), inner(t), key_col(k), sw(read_build_switches()), payload_bytes(0), h(nullptr) { memset(&a, 0, sizeof(a)); }
+    ~build_job() { if (h) gx_hash_free(h); }
+};
+
+// argument checks, build arguments, and the table's slots and side list
+static int build_setup(build_job &j, int n_preds, const gx_pred *preds, int n_payload, const int32_t *payload_cols, int unique)
 {
-    if (!ctx || !inner || !out) return GX_ERR_ARG;
+    gx_ctx *ctx = j.ctx; const gx_table *inner = j.inner; const int key_col = j.key_col; gx_build_args &a = j.a;
     GX_CHECK_ARG(ctx, key_col >= 0 && key_col < inner->ncols, "hash_build: key column %d out of range", key_col);
     int kt = inner->types[key_col];
     GX_CHECK_ARG(ctx, kt == GX_INT4 || kt == GX_INT8 || kt == GX_DATE, "hash_build: key type %d not hashable here (int4/int8/date only)", kt);
     GX_CHECK_ARG(ctx, n_payload >= 0 && n_payload <= GX_MAX_PAYLOAD, "hash_build: n_payload %d", n_payload);
-    gx_build_args a; memset(&a, 0, sizeof(a));
     a.key.data = inner->cols[key_col]; a.key.nulls = inner->nulls[key_col]; a.key.type = kt;
     a.npreds = n_preds; a.n_payload = n_payload; a.nrows = inner->nrows;
     int rc = gx_fill_dpreds(ctx, inner, n_preds, preds, a.preds); if (rc) return rc;
-    int bytes = 0;
-    gx_hash *h = (gx_hash *) calloc(1, sizeof(gx_hash));
-    h->ctx = ctx; h->key_type = kt; h->n_payload = n_payload; h->unique = unique;
-    h->src = inner; h->src_version = inner->version; h->n_preds = n_preds;
+    gx_hash *h = j.h = (gx_hash *) calloc(1, sizeof(gx_hash));
+    h->ctx = ctx; h->key_type = kt; h->n_payload = n_payload; h->unique = unique; h->src = inner; h->src_version = inner->version; h->n_preds = n_preds;
     if (n_preds > 0) memcpy(h->preds, preds, (size_t) n_preds * sizeof(gx_pred));      // n_preds checked by gx_fill_dpreds
-    struct hash_guard { gx_hash *h; ~hash_guard() { if (h) gx_hash_free(h); } } guard{h};     // every early return frees the table
     for (int i = 0; i < n_payload; i++) {
         int c = payload_cols[i];
         if (c < 0 || c >= inner->ncols) { GX_SET_ERR(ctx, "hash_build: payload column %d out of range", c); return GX_ERR_ARG; }
         if (inner->nulls[c]) { GX_SET_ERR(ctx, "hash_build: nullable payload column %d not supported in-slot", c); return GX_ERR_ARG; }
         a.payload[i].data = inner->cols[c]; a.payload[i].nulls = nullptr; a.payload[i].type = inner->types[c];
         h->payload_types[i] = inner->types[c];
-        bytes += gx_type_size(inner->types[c]);
+        j.payload_bytes += gx_type_size(inner->types[c]);
     }
-    if (bytes > 8) { GX_SET_ERR(ctx, "hash_build: payload columns total %d bytes > 8", bytes); return GX_ERR_ARG; }
-
-    int64_t want = inner->nrows + inner->nrows / 2 + 16;       // load factor <= 0.67
-    h->nslots = gx_pow2_ceil(want);
-    h->special_cap = 1 << 16;
+    if (j.payload_bytes > 8) { GX_SET_ERR(ctx, "hash_build: payload columns total %d bytes > 8", j.payload_bytes); return GX_ERR_ARG; }
+    h->nslots = gx_pow2_ceil(inner->nrows + inner->nrows / 2 + 16); h->special_cap = 1 << 16;      // load factor <= 0.67
     cudaError_t e = gx_tmp_alloc(ctx, (void **) &h->slots, (size_t) h->nslots * sizeof(gx_slot));
     if (e == cudaSuccess) e = gx_tmp_alloc(ctx, (void **) &h->special_payload, (size_t) h->special_cap * sizeof(unsigned long long));
-    if (e != cudaSuccess) {
-        GX_SET_ERR(ctx, "hash_build: cudaMalloc of %lld slots failed: %s", (long long) h->nslots, cudaGetErrorString(e));
-        return GX_ERR_NOMEM;
-    }
-    // choose the slot function from a strided key sample (64 K keys): interpolation when the
-    // keys span at most GX_INTERP_MAX_SPREAD x their count
-    h->mode = 0; h->kmin = 0; h->scale = 0; h->shift = 0; h->amask = 1u;
-    bool have_ends = false, counts_read = false;
-    // one int4/date payload column: its sampled range decides whether the narrow slot form can hold it
-    const bool pay4 = n_payload == 1 && (a.payload[0].type == GX_INT4 || a.payload[0].type == GX_DATE);
-    bool have_prange = false; long long pmin = 0, pmax = 0;
-    { const char *w = getenv("GX_SLOT_WIN"); h->win = w ? (unsigned int) atoi(w) : 31u; }
-    {
-        const char *fm = getenv("GX_SLOT_MODE");
-        int want = fm ? atoi(fm) : -1;
-        if (inner->nrows >= 4096 && h->nslots >= 64 * GX_SUB && want != 0) {
-            const long long nsample = 65536;
-            long long stride = inner->nrows / nsample; if (stride < 1) stride = 1;
-            long long nthreads = (inner->nrows + stride - 1) / stride;
-            long long init[2] = { 0x7fffffffffffffffLL, -0x7fffffffffffffffLL - 1 };
-            GX_CUDA(ctx, cudaMemcpyAsync(ctx->d_scratch + 4, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
-            GX_CUDA(ctx, cudaMemcpyAsync(ctx->d_scratch + 16, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
-            gx_dcol pay; memset(&pay, 0, sizeof(pay));
-            if (pay4) pay = a.payload[0];
-            { gx_launch_scope ls(ctx, "build_sample"); gx_k_key_range<<<(unsigned) ((nthreads + 255) / 256), 256, 0, ctx->stream>>>(a.key, pay, inner->nrows, stride, ctx->d_scratch + 4, ctx->d_scratch + 16); }
-            GX_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + 4, ctx->d_scratch + 4, 2 * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream));
-            GX_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + 16, ctx->d_scratch + 16, 2 * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream));
-            // the column's first and last key ride along: the key-ordered build path below needs them
-            {
-                const int ksz0 = gx_type_size(kt);
-                ctx->h_scratch[20] = ctx->h_scratch[21] = 0;
-                GX_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + 20, (const char *) inner->cols[key_col], ksz0, cudaMemcpyDeviceToHost, ctx->stream));
-                GX_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + 21, (const char *) inner->cols[key_col] + (size_t) (inner->nrows - 1) * ksz0, ksz0, cudaMemcpyDeviceToHost, ctx->stream));
-                have_ends = true;
-            }
-            GX_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-            long long lo = ctx->h_scratch[4], hi = ctx->h_scratch[5];
-            pmin = ctx->h_scratch[16]; pmax = ctx->h_scratch[17]; have_prange = pay4 && pmin <= pmax;
-            if (hi > lo) {
-                double range = (double) hi - (double) lo + 1.0;
-                if (range <= GX_INTERP_MAX_SPREAD * (double) inner->nrows || want == 1) {
-                    // widen the sampled range a little: keys outside it still map (they just wrap)
-                    double pad = range / 1024.0 + 64.0;
-                    double lo_d = (double) lo - pad, range_d = range + 2 * pad;
-                    if (lo_d > -9.0e18 && lo_d + range_d < 9.0e18) {
-                        gx_set_interpolation(h, (long long) lo_d, range_d);
-                    }
-                }
-            }
-        }
-    }
-    a.sf.mode = h->mode; a.sf.win = h->win; a.sf.shift = h->shift; a.sf.amask = h->amask; a.sf.kmin = h->kmin; a.sf.scale = h->scale; a.sf.mask = (unsigned long long) h->nslots - 1;
+    if (e != cudaSuccess) { GX_SET_ERR(ctx, "hash_build: cudaMalloc of %lld slots failed: %s", (long long) h->nslots, cudaGetErrorString(e)); return GX_ERR_NOMEM; }
+    h->win = j.sw.win; h->amask = 1u;                           // the mixing hash until the sample says otherwise
     a.slots = h->slots; a.mask = (unsigned long long) h->nslots - 1;
-    a.special = h->special_payload; a.special_cap = h->special_cap;
-    a.counters = ctx->d_scratch;
-    GX_CUDA(ctx, cudaMemsetAsync(ctx->d_scratch, 0, 2 * sizeof(long long), ctx->stream));
-    // big tables: bucket by sub-table, build each sub-table in shared memory
-    const char *force = getenv("GX_BUILD_DIRECT");
-    bool bucketed = h->nslots >= 64 * GX_SUB && !(force && force[0] == '1');
-    long long nscattered = -1;
-    for (int pass = 0; pass < 2 && inner->nrows > 0 && bucketed && nscattered < 0; pass++) {
-        // second pass only when the interpolation slot function produced long chains / overflow
-        GX_CUDA(ctx, cudaMemsetAsync(ctx->d_scratch, 0, 2 * sizeof(long long), ctx->stream));
-        a.sf.mode = h->mode; a.sf.win = h->win; a.sf.shift = h->shift; a.sf.amask = h->amask; a.sf.kmin = h->kmin; a.sf.scale = h->scale;
-        gx_bbuild_args ba; memset(&ba, 0, sizeof(ba));
-        ba.nsub = h->nslots / GX_SUB;
-        // ---- key-ordered build side + order-preserving slots: no bucketing needed
-        const char *nosort = getenv("GX_BUILD_NOSORTED");
-        if (h->mode != 0 && !(nosort && nosort[0] == '1')) {
-            int *d_flag = (int *) (ctx->d_scratch + 6);
-            long long ends[2];
-            int ksz = gx_type_size(kt);
-            cudaMemsetAsync(d_flag, 0, 2 * sizeof(long long), ctx->stream);          // [6] unsorted flag, [7] overflow
-            if (!have_ends) {
-                ctx->h_scratch[20] = ctx->h_scratch[21] = 0;
-                cudaMemcpyAsync(ctx->h_scratch + 20, (const char *) inner->cols[key_col], ksz, cudaMemcpyDeviceToHost, ctx->stream);
-                cudaMemcpyAsync(ctx->h_scratch + 21, (const char *) inner->cols[key_col] + (size_t) (inner->nrows - 1) * ksz, ksz, cudaMemcpyDeviceToHost, ctx->stream);
-                GX_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-                have_ends = true;
-            }
-            ends[0] = ctx->h_scratch[20]; ends[1] = ctx->h_scratch[21];
-            long long kmin = ksz == 4 ? (long long) (int) ends[0] : ends[0], kmax = ksz == 4 ? (long long) (int) ends[1] : ends[1];
-            if (kmin == GX_EMPTY_KEY) kmin = kmin + 1;                                  // the reserved key lives in the side list
-            double range_d = (double) kmax - (double) kmin + 1.0;
-            long long *d_start = nullptr;
-            if (range_d >= 1.0 && range_d < 9.0e18 && range_d <= GX_INTERP_MAX_SPREAD * (double) inner->nrows &&
-                gx_tmp_alloc(ctx, (void **) &d_start, (size_t) (ba.nsub + 1) * sizeof(long long)) == cudaSuccess) {
-                // exact bounds (if the column really is ordered): every key maps below nslots - GX_SUB, monotonically
-                const long long save_kmin = h->kmin; const unsigned long long save_scale = h->scale;
-                const int save_mode = h->mode; const unsigned int save_shift = h->shift;
-                gx_set_interpolation(h, kmin, range_d);
-                a.sf.mode = h->mode; a.sf.kmin = h->kmin; a.sf.scale = h->scale; a.sf.shift = h->shift; a.sf.amask = h->amask;
-                ba.b = a; ba.overflow = (int *) (ctx->d_scratch + 7); ba.start = d_start; ba.unsorted = d_flag;
-                cudaMemsetAsync(ctx->d_scratch + 3, 0, sizeof(long long), ctx->stream);
-                cudaMemsetAsync(ctx->d_scratch + 5, 0, sizeof(long long), ctx->stream);
-                int pk = 0;
-                if (kt == GX_INT8 && a.key.nulls == nullptr && a.npreds == 0) {
-                    if (a.n_payload == 0) pk = 2;
-                    else if (a.n_payload == 1 && (a.payload[0].type == GX_INT4 || a.payload[0].type == GX_DATE)) pk = 1;
-                }
-                // int8 key without NULLs whose first key is an ordinary key: bounds by search, order and
-                // placement verified by the fill (see sorted_lower_bound)
-                const char *nosearch = getenv("GX_NO_BOUNDS_SEARCH");
-                const bool searched = kt == GX_INT8 && a.key.nulls == nullptr && ends[0] != GX_EMPTY_KEY && ((uintptr_t) a.key.data & 15) == 0 &&
-                                      !(nosearch && nosearch[0] == '1');
-                // compact 8-byte slots when the exact key span and the payload fit 32 bits each
-                const char *nocompact = getenv("GX_NO_COMPACT");
-                const bool small_payload = a.n_payload == 0 ? inner->nrows < 0xffffffffLL : bytes <= 4;
-                // (a sub-table's keys must be told apart by 31 bits: its key span is range / #sub-tables)
-                const double keys_per_slot = range_d / (double) (h->nslots - GX_SUB);
-                bool compact = (pk != 0 || searched) && small_payload && h->mode != 0 && keys_per_slot * GX_SUB < 268435456.0 &&
-                               !(nocompact && nocompact[0] == '1');
-                // narrow 4-byte slots (pk 1) when the tag the key span needs leaves room for the sampled payload range, which
-                // is centred in the window; a payload the sample missed is caught by the fill (bit 4 of the overflow word)
-                bool narrow = false;
-                if (compact && pk == 1 && have_prange) {
-                    const unsigned int tbits = gx_nslot_tbits(keys_per_slot);
-                    const long long pwin = tbits < 32 ? 1LL << (32 - tbits) : 0;         // payload values a slot holds
-                    if (pmax - pmin < pwin) {
-                        long long pb = pmin - (pwin - 1 - (pmax - pmin)) / 2;
-                        if (pb < (long long) INT32_MIN) pb = INT32_MIN;                     // the window stays inside int4
-                        if (pb > (long long) INT32_MAX - (pwin - 1)) pb = (long long) INT32_MAX - (pwin - 1);
-                        narrow = true; h->tbits = tbits; h->pbase = (int) pb;
-                    }
-                }
-                h->keys_per_slot = keys_per_slot;
-                if (narrow && gx_tmp_alloc(ctx, (void **) &h->narrow, (size_t) h->nslots * sizeof(unsigned int)) != cudaSuccess) { h->narrow = nullptr; narrow = false; }
-                if (!narrow) { h->tbits = 0; h->pbase = 0; }
-                if (compact && !narrow && gx_tmp_alloc(ctx, (void **) &h->cslots, (size_t) h->nslots * sizeof(gx_cslot)) != cudaSuccess) { h->cslots = nullptr; compact = false; }
-                h->amask = compact ? 3u : 1u; h->cspan = compact ? (unsigned long long) (kmax - kmin) + 1ULL : 0ULL;
-                a.sf.amask = h->amask; a.sf.tbits = h->tbits; a.sf.pbase = h->pbase; ba.b = a; ba.cslots = h->cslots; ba.narrow = h->narrow;
-                auto drop_compact = [&]() {
-                    gx_tmp_free(ctx, h->cslots); gx_tmp_free(ctx, h->narrow); h->cslots = nullptr; h->narrow = nullptr;
-                    h->amask = 1u; h->cspan = 0; h->tbits = 0; h->pbase = 0; a.sf.tbits = 0; a.sf.pbase = 0;
-                };
-                // the staged fill copies 16-byte aligned blocks of the key and payload columns
-                if (pk != 0 && (((uintptr_t) a.key.data & 15) != 0 || (pk == 1 && ((uintptr_t) a.payload[0].data & 15) != 0))) pk = 0;
-                auto fill = [&](int use_pk) {
-                    if (narrow) { if (searched) sorted_fill<GX_SLOTS_NARROW, true>(ctx, ba, use_pk); else sorted_fill<GX_SLOTS_NARROW, false>(ctx, ba, use_pk); }
-                    else if (compact) { if (searched) sorted_fill<GX_SLOTS_COMPACT, true>(ctx, ba, use_pk); else sorted_fill<GX_SLOTS_COMPACT, false>(ctx, ba, use_pk); }
-                    else if (searched) sorted_fill<GX_SLOTS_WIDE, true>(ctx, ba, use_pk);
-                    else sorted_fill<GX_SLOTS_WIDE, false>(ctx, ba, use_pk);
-                };
-                if (searched) {
-                    { gx_launch_scope ls(ctx, "build_bounds"); gx_k_sorted_bounds_search<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>((const long long *) a.key.data, inner->nrows, a.sf, ba.nsub, h->nslots, d_start); }
-                    gx_launch_scope ls(ctx, "build");
-                    gx_launch_scope path(ctx, "build_sorted_search", 0);           // second profile names: which build path ran
-                    gx_launch_scope form(ctx, compact ? "build_compact" : nullptr, 0);
-                    gx_launch_scope nform(ctx, narrow ? "build_narrow" : nullptr, 0);
-                    fill(pk);
-                } else {
-                    {
-                        gx_launch_scope ls(ctx, "build_bounds");
-                        if (kt == GX_INT8 && a.key.nulls == nullptr && ((uintptr_t) a.key.data & 15) == 0)
-                            gx_k_sorted_bounds_i8<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>((const long long *) a.key.data, inner->nrows, a.sf, ba.nsub, d_start, d_flag);
-                        else
-                            gx_k_sorted_bounds<<<ctx->sm_count * 16, 256, 0, ctx->stream>>>(a, ba.nsub, d_start, d_flag);
-                    }
-                    {
-                        gx_launch_scope ls(ctx, "build", 2);
-                        gx_launch_scope path(ctx, "build_sorted_pass", 0);
-                        gx_launch_scope form(ctx, compact ? "build_compact" : nullptr, 0);
-                        gx_launch_scope nform(ctx, narrow ? "build_narrow" : nullptr, 0);
-                        gx_k_sorted_special<<<1, 256, 0, ctx->stream>>>(a, d_start, d_flag);
-                        fill(pk);
-                    }
-                }
-                cudaError_t e2 = cudaGetLastError();
-                if (e2 == cudaSuccess) e2 = cudaMemcpyAsync(ctx->h_scratch, ctx->d_scratch, 8 * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream);
-                if (e2 == cudaSuccess) e2 = cudaStreamSynchronize(ctx->stream);
-                // the fill once more, in the form `compact` / `narrow` now name; `why` is its second profile name
-                auto refill = [&](int use_pk, const char *why) {
-                    cudaMemsetAsync(ctx->d_scratch + 3, 0, sizeof(long long), ctx->stream);
-                    cudaMemsetAsync(ctx->d_scratch + 5, 0, 3 * sizeof(long long), ctx->stream);      // [5] steps, [6] unsorted, [7] overflow
-                    {
-                        gx_launch_scope ls(ctx, "build");
-                        gx_launch_scope path(ctx, searched ? "build_sorted_search" : "build_sorted_pass", 0);
-                        gx_launch_scope form(ctx, compact ? "build_compact" : nullptr, 0);
-                        gx_launch_scope nform(ctx, why, 0);
-                        fill(use_pk);
-                    }
-                    e2 = cudaGetLastError();
-                    if (e2 == cudaSuccess) e2 = cudaMemcpyAsync(ctx->h_scratch, ctx->d_scratch, 8 * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream);
-                    if (e2 == cudaSuccess) e2 = cudaStreamSynchronize(ctx->stream);
-                };
-                // a bounded wait of the staged fill gave up: the same build with the generic row loader
-                auto stuck = [&]() { return e2 == cudaSuccess && pk != 0 && ((int) ctx->h_scratch[7] & 2); };
-                const char *stuck_msg = "gpuexec: a bounded mbarrier wait of gx_k_sorted_fill_staged gave up; rebuilding with gx_k_sorted_fill\n";
-                if (stuck()) { fprintf(stderr, "%s", stuck_msg); refill(0, narrow ? "build_narrow" : nullptr); }
-                if (e2 == cudaSuccess && narrow && ((int) ctx->h_scratch[7] & 4) && (int) ctx->h_scratch[6] == 0) {
-                    // a payload outside the narrow window (a value the sample missed): the same build in the 8-byte form
-                    gx_tmp_free(ctx, h->narrow); h->narrow = nullptr; narrow = false;
-                    h->tbits = 0; h->pbase = 0; a.sf.tbits = 0; a.sf.pbase = 0;
-                    if (gx_tmp_alloc(ctx, (void **) &h->cslots, (size_t) h->nslots * sizeof(gx_cslot)) != cudaSuccess) {
-                        h->cslots = nullptr; gx_tmp_free(ctx, d_start);
-                        GX_SET_ERR(ctx, "hash_build: cudaMalloc of %lld compact slots failed", (long long) h->nslots);
-                        return GX_ERR_NOMEM;
-                    }
-                    ba.b = a; ba.cslots = h->cslots; ba.narrow = nullptr;
-                    refill(pk, "build_narrow_refill");
-                    if (stuck()) { fprintf(stderr, "%s", stuck_msg); refill(0, "build_narrow_refill"); }
-                }
-                gx_tmp_free(ctx, d_start);
-                if (e2 != cudaSuccess) { GX_SET_ERR(ctx, "hash_build: %s", cudaGetErrorString(e2)); return GX_ERR_CUDA; }
-                if ((int) ctx->h_scratch[6] == 0) {
-                    h->avg_chain = ctx->h_scratch[3] > 0 ? (double) ctx->h_scratch[5] / (double) ctx->h_scratch[3] : 0.0;
-                    if (((int) ctx->h_scratch[7] & ~4) == 0 && h->avg_chain <= 4.0) {      // bit 4 was answered by the refill above
-                        nscattered = ctx->h_scratch[3]; h->sorted_build = 1; counts_read = true;
-                        if (compact) { gx_tmp_free(ctx, h->slots); h->slots = nullptr; }      // the 16-byte form is made on demand (gx_hash_wide)
-                        break;
-                    }
-                    if (compact) drop_compact();
-                    h->mode = 0; continue;                                               // clustered keys: rebuild with the mixing hash
-                }
-                if (compact) drop_compact();
-                // not in key order: back to the sampled slot function and the bucketing passes
-                h->kmin = save_kmin; h->scale = save_scale; h->mode = save_mode; h->shift = save_shift;
-                a.sf.mode = h->mode; a.sf.kmin = h->kmin; a.sf.scale = h->scale; a.sf.shift = h->shift; a.sf.amask = h->amask;
-                GX_CUDA(ctx, cudaMemsetAsync(ctx->d_scratch, 0, 2 * sizeof(long long), ctx->stream));
-            }
+    a.special = h->special_payload; a.special_cap = h->special_cap; a.counters = ctx->d_scratch;
+    return GX_OK;
+}
+// the sample's key and payload ranges, the key column's first and last key, and the slot function chosen
+struct key_sample { long long lo, hi, pmin, pmax, first, last; bool have_prange, have_ends; gx_slotfn sf; };
+// the key column's first and last key (this synchronises the stream)
+static int fetch_key_ends(const build_job &j, key_sample &s)
+{
+    gx_ctx *ctx = j.ctx; const int ksz = gx_type_size(j.a.key.type); const char *col = (const char *) j.a.key.data;
+    long long *w = ctx->h_scratch + SW_ENDS; w[0] = w[1] = 0;
+    GX_CUDA(ctx, cudaMemcpyAsync(w, col, ksz, cudaMemcpyDeviceToHost, ctx->stream));
+    GX_CUDA(ctx, cudaMemcpyAsync(w + 1, col + (size_t) (j.inner->nrows - 1) * ksz, ksz, cudaMemcpyDeviceToHost, ctx->stream));
+    GX_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    s.first = ksz == 4 ? (long long) (int) w[0] : w[0]; s.last = ksz == 4 ? (long long) (int) w[1] : w[1]; s.have_ends = true;
+    return GX_OK;
+}
+// choose the slot function from a strided key sample (64 K keys): interpolation when the
+// keys span at most GX_INTERP_MAX_SPREAD x their count
+static int sample_keys(build_job &j, key_sample &s)
+{
+    gx_ctx *ctx = j.ctx; const long long nrows = j.inner->nrows; s = key_sample();
+    if (nrows >= 4096 && j.h->nslots >= 64 * GX_SUB && j.sw.slot_mode != 0) {
+        long long stride = nrows / 65536; if (stride < 1) stride = 1;
+        const long long nthreads = (nrows + stride - 1) / stride, init[2] = { 0x7fffffffffffffffLL, -0x7fffffffffffffffLL - 1 };
+        long long *krange = ctx->d_scratch + SW_KRANGE, *prange = ctx->d_scratch + SW_PRANGE;
+        GX_CUDA(ctx, cudaMemcpyAsync(krange, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
+        GX_CUDA(ctx, cudaMemcpyAsync(prange, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
+        // one int4/date payload column: its sampled range decides whether the narrow slot form can hold it
+        const bool pay4 = j.a.n_payload == 1 && (j.a.payload[0].type == GX_INT4 || j.a.payload[0].type == GX_DATE);
+        gx_dcol pay; memset(&pay, 0, sizeof(pay)); if (pay4) pay = j.a.payload[0];
+        { gx_launch_scope ls(ctx, "build_sample"); gx_k_key_range<<<(unsigned) ((nthreads + 255) / 256), 256, 0, ctx->stream>>>(j.a.key, pay, nrows, stride, krange, prange); }
+        GX_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + SW_KRANGE, krange, 2 * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream));
+        GX_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + SW_PRANGE, prange, 2 * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream));
+        int rc = fetch_key_ends(j, s); if (rc) return rc;          // the sample's one synchronise
+        const long long *w = ctx->h_scratch;
+        s.lo = w[SW_KRANGE]; s.hi = w[SW_KRANGE + 1]; s.pmin = w[SW_PRANGE]; s.pmax = w[SW_PRANGE + 1]; s.have_prange = pay4 && s.pmin <= s.pmax;
+        // widen the sampled range a little: keys outside it still map (they just wrap)
+        const double range = (double) s.hi - (double) s.lo + 1.0, pad = range / 1024.0 + 64.0, lo_d = (double) s.lo - pad, range_d = range + 2 * pad;
+        if (s.hi > s.lo && (range <= GX_INTERP_MAX_SPREAD * (double) nrows || j.sw.slot_mode == 1) && lo_d > -9.0e18 && lo_d + range_d < 9.0e18)
+            gx_set_interpolation(j.h, (long long) lo_d, range_d, j.sw.wide);
+    }
+    s.sf = gx_hash_slotfn(j.h);
+    return GX_OK;
+}
+// the key-ordered build's form: pk, the staged fill's loader (1: one 4-byte payload column, 2: row number, 0: generic);
+// searched: bounds by search; compact: 8-byte slots; narrow: 4-byte slots instead of compact ones
+struct sorted_form { int pk; bool searched, compact, narrow; };
+// One key-ordered fill (the bounds pass's first with gx_k_sorted_special), then the scratch words read back.
+// The second profile names tell the path, the form and `why`: the narrow form, or the refill that replaced it.
+static int sorted_fill_pass(build_job &j, const gx_bbuild_args &ba, const sorted_form &f, int pk, const char *why, bool refill)
+{
+    gx_ctx *ctx = j.ctx; const bool special = !refill && !f.searched;
+    if (refill) GX_CUDA(ctx, clear_scratch(ctx, SW_PLACED, SW_OVERFLOW));
+    {
+        gx_launch_scope ls(ctx, "build", special ? 2 : 1);
+        gx_launch_scope path(ctx, f.searched ? "build_sorted_search" : "build_sorted_pass", 0);
+        gx_launch_scope form(ctx, f.compact ? "build_compact" : nullptr, 0);
+        gx_launch_scope nform(ctx, why, 0);
+        if (special) gx_k_sorted_special<<<1, 256, 0, ctx->stream>>>(ba.b, ba.start, ba.unsorted);
+        if (f.narrow) { if (f.searched) sorted_fill<GX_SLOTS_NARROW, true>(ctx, ba, pk); else sorted_fill<GX_SLOTS_NARROW, false>(ctx, ba, pk); }
+        else if (f.compact) { if (f.searched) sorted_fill<GX_SLOTS_COMPACT, true>(ctx, ba, pk); else sorted_fill<GX_SLOTS_COMPACT, false>(ctx, ba, pk); }
+        else if (f.searched) sorted_fill<GX_SLOTS_WIDE, true>(ctx, ba, pk);
+        else sorted_fill<GX_SLOTS_WIDE, false>(ctx, ba, pk);
+    }
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->h_scratch, ctx->d_scratch, (SW_OVERFLOW + 1) * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) { GX_SET_ERR(ctx, "hash_build: %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
+    return GX_OK;
+}
+// a bounded wait of the staged fill gave up: the same build with the generic row loader
+static int staged_fallback(build_job &j, const gx_bbuild_args &ba, const sorted_form &f, const char *why)
+{
+    if (f.pk == 0 || !((int) j.ctx->h_scratch[SW_OVERFLOW] & OVF_STUCK)) return GX_OK;
+    fprintf(stderr, "gpuexec: a bounded mbarrier wait of gx_k_sorted_fill_staged gave up; rebuilding with gx_k_sorted_fill\n");
+    return sorted_fill_pass(j, ba, f, 0, why, true);
+}
+// a payload outside the narrow window (a value the sample missed): the same build in the 8-byte form
+static int narrow_refill(build_job &j, gx_bbuild_args &ba, sorted_form &f)
+{
+    gx_hash *h = j.h; gx_tmp_free(j.ctx, h->narrow); h->narrow = nullptr; f.narrow = false; h->tbits = 0; h->pbase = 0;
+    if (gx_tmp_alloc(j.ctx, (void **) &h->cslots, (size_t) h->nslots * sizeof(gx_cslot)) != cudaSuccess)
+        { h->cslots = nullptr; GX_SET_ERR(j.ctx, "hash_build: cudaMalloc of %lld compact slots failed", (long long) h->nslots); return GX_ERR_NOMEM; }
+    j.a.sf = gx_hash_slotfn(h); ba.b = j.a; ba.cslots = h->cslots; ba.narrow = nullptr;
+    int rc = sorted_fill_pass(j, ba, f, f.pk, "build_narrow_refill", true);
+    return rc ? rc : staged_fallback(j, ba, f, "build_narrow_refill");
+}
+// Key-ordered build side: no bucketing, a sub-table's rows are one row range.  Not tried (UNORDERED, h unchanged) when the
+// key span is too wide; unless BUILT, h is left in 16-byte slots.
+enum sorted_outcome { SORTED_BUILT, SORTED_CLUSTERED, SORTED_UNORDERED };
+static int sorted_build(build_job &j, key_sample &ks, sorted_outcome &out, long long &nplaced)
+{
+    gx_ctx *ctx = j.ctx; gx_hash *h = j.h; const gx_build_args &a = j.a; const long long *w = ctx->h_scratch; out = SORTED_UNORDERED;
+    GX_CUDA(ctx, clear_scratch(ctx, SW_UNSORTED, SW_OVERFLOW));
+    if (!ks.have_ends) { int rc = fetch_key_ends(j, ks); if (rc) return rc; }
+    const long long kmin = ks.first == GX_EMPTY_KEY ? ks.first + 1 : ks.first, kmax = ks.last;      // the reserved key lives in the side list
+    const double range_d = (double) kmax - (double) kmin + 1.0;
+    const long long nsub = h->nslots / GX_SUB;
+    tmp_buf<long long> start(ctx);
+    if (!(range_d >= 1.0 && range_d < 9.0e18 && range_d <= GX_INTERP_MAX_SPREAD * (double) a.nrows && start.alloc(nsub + 1) == cudaSuccess)) return GX_OK;
+    // exact bounds (if the column really is ordered): every key maps below nslots - GX_SUB, monotonically
+    gx_set_interpolation(h, kmin, range_d, j.sw.wide);
+    GX_CUDA(ctx, clear_scratch(ctx, SW_INSERTED, SW_SPECIAL));
+    GX_CUDA(ctx, clear_scratch(ctx, SW_PLACED, SW_STEPS));
+    const bool i8 = a.key.type == GX_INT8 && a.key.nulls == nullptr, pay4 = a.n_payload == 1 && (a.payload[0].type == GX_INT4 || a.payload[0].type == GX_DATE);
+    sorted_form f = { i8 && a.npreds == 0 ? (a.n_payload == 0 ? 2 : pay4 ? 1 : 0) : 0, false, false, false };
+    // int8 key without NULLs whose first key is an ordinary key: bounds by search, order and
+    // placement verified by the fill (see sorted_lower_bound)
+    f.searched = i8 && ks.first != GX_EMPTY_KEY && ((uintptr_t) a.key.data & 15) == 0 && !j.sw.nosearch;
+    // compact 8-byte slots when the exact key span and the payload fit 32 bits each (a sub-table's keys must be told
+    // apart by 31 bits: its key span is range / #sub-tables)
+    const bool small_payload = a.n_payload == 0 ? a.nrows < 0xffffffffLL : j.payload_bytes <= 4;
+    const double keys_per_slot = range_d / (double) (h->nslots - GX_SUB);
+    f.compact = (f.pk != 0 || f.searched) && small_payload && h->mode != 0 && keys_per_slot * GX_SUB < 268435456.0 && !j.sw.nocompact;
+    // narrow 4-byte slots (pk 1) when the tag the key span needs leaves room for the sampled payload range, which
+    // is centred in the window; a payload the sample missed is caught by the fill (OVF_PAYLOAD)
+    if (f.compact && f.pk == 1 && ks.have_prange) {
+        const unsigned int tbits = gx_nslot_tbits(keys_per_slot);
+        const long long pwin = tbits < 32 ? 1LL << (32 - tbits) : 0;         // payload values a slot holds
+        if (ks.pmax - ks.pmin < pwin) {
+            long long pb = ks.pmin - (pwin - 1 - (ks.pmax - ks.pmin)) / 2;
+            if (pb < (long long) INT32_MIN) pb = INT32_MIN;                     // the window stays inside int4
+            if (pb > (long long) INT32_MAX - (pwin - 1)) pb = (long long) INT32_MAX - (pwin - 1);
+            f.narrow = true; h->tbits = tbits; h->pbase = (int) pb;
         }
-        ba.b = a;
-        cudaError_t e = gx_tmp_alloc(ctx, (void **) &ba.cursor, (size_t) ba.nsub * sizeof(unsigned int) + sizeof(int));
-        if (e == cudaSuccess) e = gx_tmp_alloc(ctx, (void **) &ba.pairs, (size_t) h->nslots * sizeof(gx_slot));
-        if (e != cudaSuccess) {
-            gx_tmp_free(ctx, ba.cursor);
-            GX_SET_ERR(ctx, "hash_build: cudaMalloc of the bucketing buffers failed: %s", cudaGetErrorString(e));
-            return GX_ERR_NOMEM;
+    }
+    h->keys_per_slot = keys_per_slot;
+    if (f.narrow && gx_tmp_alloc(ctx, (void **) &h->narrow, (size_t) h->nslots * sizeof(unsigned int)) != cudaSuccess) { h->narrow = nullptr; f.narrow = false; }
+    if (!f.narrow) { h->tbits = 0; h->pbase = 0; }
+    if (f.compact && !f.narrow && gx_tmp_alloc(ctx, (void **) &h->cslots, (size_t) h->nslots * sizeof(gx_cslot)) != cudaSuccess) { h->cslots = nullptr; f.compact = false; }
+    h->amask = f.compact ? 3u : 1u; h->cspan = f.compact ? (unsigned long long) (kmax - kmin) + 1ULL : 0ULL;
+    // the staged fill copies 16-byte aligned blocks of the key and payload columns
+    if (f.pk != 0 && (((uintptr_t) a.key.data & 15) != 0 || (f.pk == 1 && ((uintptr_t) a.payload[0].data & 15) != 0))) f.pk = 0;
+    j.a.sf = gx_hash_slotfn(h);
+    gx_bbuild_args ba; memset(&ba, 0, sizeof(ba));
+    ba.b = a; ba.nsub = nsub; ba.start = start.p; ba.cslots = h->cslots; ba.narrow = h->narrow;
+    ba.unsorted = (int *) (ctx->d_scratch + SW_UNSORTED); ba.overflow = (int *) (ctx->d_scratch + SW_OVERFLOW);
+    {
+        gx_launch_scope ls(ctx, "build_bounds");
+        const long long *keys = (const long long *) a.key.data;
+        if (f.searched) gx_k_sorted_bounds_search<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(keys, a.nrows, a.sf, nsub, h->nslots, ba.start);
+        else if (a.key.type == GX_INT8 && a.key.nulls == nullptr && ((uintptr_t) keys & 15) == 0) gx_k_sorted_bounds_i8<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(keys, a.nrows, a.sf, nsub, ba.start, ba.unsorted);
+        else gx_k_sorted_bounds<<<ctx->sm_count * 16, 256, 0, ctx->stream>>>(a, nsub, ba.start, ba.unsorted);
+    }
+    const char *why = f.narrow ? "build_narrow" : nullptr;
+    int rc = sorted_fill_pass(j, ba, f, f.pk, why, false);
+    if (!rc) rc = staged_fallback(j, ba, f, why);
+    if (!rc && f.narrow && ((int) w[SW_OVERFLOW] & OVF_PAYLOAD) && (int) w[SW_UNSORTED] == 0) rc = narrow_refill(j, ba, f);
+    if (rc) return rc;
+    if ((int) w[SW_UNSORTED] == 0) {
+        h->avg_chain = fill_avg_chain(w);
+        if (((int) w[SW_OVERFLOW] & ~OVF_PAYLOAD) == 0 && h->avg_chain <= 4.0) {     // OVF_PAYLOAD was answered by narrow_refill
+            nplaced = w[SW_PLACED]; h->sorted_build = 1; out = SORTED_BUILT;
+            if (f.compact) { gx_tmp_free(ctx, h->slots); h->slots = nullptr; }      // the 16-byte form is made on demand (gx_hash_wide)
+            return GX_OK;
         }
-        ba.overflow = (int *) (ba.cursor + ba.nsub);
-        cudaMemsetAsync(ba.cursor, 0, (size_t) ba.nsub * sizeof(unsigned int) + sizeof(int), ctx->stream);
-        cudaMemsetAsync(ctx->d_scratch + 3, 0, sizeof(long long), ctx->stream);
-        cudaMemsetAsync(ctx->d_scratch + 5, 0, sizeof(long long), ctx->stream);
-        long long ntiles = (inner->nrows + 256 * BSCAT - 1) / (256 * BSCAT), maxb = (long long) ctx->sm_count * 8;
-        unsigned grid = (unsigned) (ntiles < maxb ? ntiles : maxb);
-        int log2nsub = 0; while (((long long) 1 << log2nsub) < ba.nsub) log2nsub++;
-        const char *onepass = getenv("GX_BUILD_ONEPASS");
-        bool two_level = log2nsub >= 12 && log2nsub <= 18 && !(onepass && onepass[0] == '1');
-        if (two_level) {
-            gx_bpart_args pa; memset(&pa, 0, sizeof(pa));
-            pa.b = a; pa.nsub = ba.nsub; pa.bits_hi = (log2nsub + 1) / 2; pa.bits_lo = log2nsub - pa.bits_hi;
-            pa.pairs = ba.pairs; pa.cursor = ba.cursor; pa.overflow = ba.overflow;
-            const long long B1 = (long long) 1 << pa.bits_hi;
-            pa.cap1 = (inner->nrows / B1) + (inner->nrows / B1) / 4 + 2 * BP_TILE;
-            pa.tiles_per_l1 = (pa.cap1 + BP_TILE - 1) / BP_TILE;
-            e = gx_tmp_alloc(ctx, (void **) &pa.l1, (size_t) B1 * pa.cap1 * sizeof(gx_slot));
-            if (e == cudaSuccess) e = gx_tmp_alloc(ctx, (void **) &pa.cur1, (size_t) B1 * sizeof(unsigned int));
-            if (e == cudaSuccess) {
-                cudaMemsetAsync(pa.cur1, 0, (size_t) B1 * sizeof(unsigned int), ctx->stream);
-                static bool attr = false;
-                if (!attr) {
-                    cudaFuncSetAttribute(gx_k_bpart1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) bp_smem_bytes(512));
-                    cudaFuncSetAttribute(gx_k_bpart2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) bp_smem_bytes(512));
-                    attr = true;
-                }
-                gx_launch_scope ls(ctx, "build_scatter", 2);
-                gx_launch_scope which(ctx, "build_bucket2", 0);
-                gx_k_bpart1<<<ctx->sm_count * 2, BP_THREADS, bp_smem_bytes(1 << pa.bits_hi), ctx->stream>>>(pa);
-                gx_k_bpart2<<<ctx->sm_count * 2, BP_THREADS, bp_smem_bytes(1 << pa.bits_lo), ctx->stream>>>(pa);
-            }
-            gx_tmp_free(ctx, pa.l1); gx_tmp_free(ctx, pa.cur1);
-            if (e != cudaSuccess) two_level = false;            // no room for the level-1 buffer: one-pass scatter
-        }
-        if (!two_level) {
-            gx_launch_scope ls(ctx, "build_scatter");
-            gx_launch_scope which(ctx, "build_bucket1", 0);
-            gx_k_bbuild_scatter<<<grid, 256, 0, ctx->stream>>>(ba);
-        }
-        {
+        out = SORTED_CLUSTERED;
+    }
+    gx_tmp_free(ctx, h->cslots); gx_tmp_free(ctx, h->narrow); h->cslots = nullptr; h->narrow = nullptr; h->amask = 1u; h->cspan = 0; h->tbits = 0; h->pbase = 0;
+    return GX_OK;
+}
+
+// Bucketed build (two-level scatter for 2^12 .. 2^18 sub-tables).  REHASH: interpolation overflowed a sub-table or made long
+// chains (keys less uniform than sampled); OVERFLOW: the mixing hash did.
+enum bucket_outcome { BUCKET_BUILT, BUCKET_REHASH, BUCKET_OVERFLOW };
+static int bucketed_build(build_job &j, bucket_outcome &out, long long &nplaced)
+{
+    gx_ctx *ctx = j.ctx; gx_hash *h = j.h; const long long nrows = j.inner->nrows;
+    GX_CUDA(ctx, clear_scratch(ctx, SW_INSERTED, SW_SPECIAL));
+    j.a.sf = gx_hash_slotfn(h);
+    gx_bbuild_args ba; memset(&ba, 0, sizeof(ba)); ba.b = j.a; ba.nsub = h->nslots / GX_SUB;
+    tmp_buf<unsigned int> cursor(ctx); tmp_buf<gx_slot> pairs(ctx);
+    cudaError_t e = cursor.alloc(ba.nsub + 1);                      // the last word is the overflow flag
+    if (e == cudaSuccess) e = pairs.alloc(h->nslots);
+    if (e != cudaSuccess) { GX_SET_ERR(ctx, "hash_build: cudaMalloc of the bucketing buffers failed: %s", cudaGetErrorString(e)); return GX_ERR_NOMEM; }
+    ba.cursor = cursor.p; ba.pairs = pairs.p; ba.overflow = (int *) (ba.cursor + ba.nsub);
+    GX_CUDA(ctx, cudaMemsetAsync(ba.cursor, 0, (size_t) ba.nsub * sizeof(unsigned int) + sizeof(int), ctx->stream));
+    GX_CUDA(ctx, clear_scratch(ctx, SW_PLACED, SW_STEPS));
+    long long ntiles = (nrows + 256 * BSCAT - 1) / (256 * BSCAT), maxb = (long long) ctx->sm_count * 8;
+    unsigned grid = (unsigned) (ntiles < maxb ? ntiles : maxb);
+    int log2nsub = 0; while (((long long) 1 << log2nsub) < ba.nsub) log2nsub++;
+    bool two_level = log2nsub >= 12 && log2nsub <= 18 && !j.sw.onepass;
+    if (two_level) {
+        gx_bpart_args pa; memset(&pa, 0, sizeof(pa));
+        pa.b = ba.b; pa.nsub = ba.nsub; pa.bits_hi = (log2nsub + 1) / 2; pa.bits_lo = log2nsub - pa.bits_hi;
+        pa.pairs = ba.pairs; pa.cursor = ba.cursor; pa.overflow = ba.overflow;
+        const long long B1 = (long long) 1 << pa.bits_hi;
+        pa.cap1 = (nrows / B1) + (nrows / B1) / 4 + 2 * BP_TILE; pa.tiles_per_l1 = (pa.cap1 + BP_TILE - 1) / BP_TILE;
+        tmp_buf<gx_slot> l1(ctx); tmp_buf<unsigned int> cur1(ctx);
+        e = l1.alloc((size_t) B1 * pa.cap1); if (e == cudaSuccess) e = cur1.alloc((size_t) B1);
+        if (e == cudaSuccess) {
+            pa.l1 = l1.p; pa.cur1 = cur1.p;
+            GX_CUDA(ctx, cudaMemsetAsync(pa.cur1, 0, (size_t) B1 * sizeof(unsigned int), ctx->stream));
             static bool attr = false;
-            if (!attr) { cudaFuncSetAttribute(gx_k_bbuild_fill, cudaFuncAttributeMaxDynamicSharedMemorySize, FILL_SMEM_BYTES); attr = true; }
-            gx_launch_scope ls(ctx, "build", 2);
-            gx_k_bbuild_fill<<<ctx->sm_count * 8, FILL_THREADS, FILL_SMEM_BYTES, ctx->stream>>>(ba);
-            gx_k_bbuild_total<<<ctx->sm_count, 256, 0, ctx->stream>>>(ba.cursor, ba.nsub, ctx->d_scratch + 3);
-        }
-        int h_over = 0;
+            if (!attr) { cudaFuncSetAttribute(gx_k_bpart1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) bp_smem_bytes(512));
+                         cudaFuncSetAttribute(gx_k_bpart2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) bp_smem_bytes(512)); attr = true; }
+            gx_launch_scope ls(ctx, "build_scatter", 2);
+            gx_launch_scope which(ctx, "build_bucket2", 0);
+            gx_k_bpart1<<<ctx->sm_count * 2, BP_THREADS, bp_smem_bytes(1 << pa.bits_hi), ctx->stream>>>(pa);
+            gx_k_bpart2<<<ctx->sm_count * 2, BP_THREADS, bp_smem_bytes(1 << pa.bits_lo), ctx->stream>>>(pa);
+        } else two_level = false;                                   // no room for the level-1 buffer: one-pass scatter
+    }
+    if (!two_level) {
+        gx_launch_scope ls(ctx, "build_scatter");
+        gx_launch_scope which(ctx, "build_bucket1", 0);
+        gx_k_bbuild_scatter<<<grid, 256, 0, ctx->stream>>>(ba);
+    }
+    {
+        static bool attr = false;
+        if (!attr) { cudaFuncSetAttribute(gx_k_bbuild_fill, cudaFuncAttributeMaxDynamicSharedMemorySize, FILL_SMEM_BYTES); attr = true; }
+        gx_launch_scope ls(ctx, "build", 2);
+        gx_k_bbuild_fill<<<ctx->sm_count * 8, FILL_THREADS, FILL_SMEM_BYTES, ctx->stream>>>(ba);
+        gx_k_bbuild_total<<<ctx->sm_count, 256, 0, ctx->stream>>>(ba.cursor, ba.nsub, ctx->d_scratch + SW_PLACED);
+    }
+    int h_over = 0; e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->h_scratch + SW_PLACED, ctx->d_scratch + SW_PLACED, (SW_STEPS - SW_PLACED + 1) * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&h_over, ba.overflow, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) { GX_SET_ERR(ctx, "hash_build: %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
+    h->avg_chain = fill_avg_chain(ctx->h_scratch);
+    if (h->mode != 0 && (h_over || h->avg_chain > 4.0)) out = BUCKET_REHASH;
+    else if (h_over) out = BUCKET_OVERFLOW;
+    else { out = BUCKET_BUILT; nplaced = ctx->h_scratch[SW_PLACED]; }
+    return GX_OK;
+}
+
+// Direct build: CAS insertion into the cleared table
+static int direct_build(build_job &j)
+{
+    gx_ctx *ctx = j.ctx; gx_hash *h = j.h; gx_build_args &a = j.a;
+    GX_CUDA(ctx, clear_scratch(ctx, SW_INSERTED, SW_SPECIAL));
+    { gx_launch_scope ls(ctx, "build_clear"); gx_k_fill_slots<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(h->slots, h->nslots); }
+    // probe walks wrap inside a sub-table (or the whole table when it is smaller): each keeps a free slot
+    const long long wrap = h->nslots < GX_SUB ? h->nslots : GX_SUB, nsub = h->nslots / wrap;
+    tmp_buf<unsigned int> claims(ctx); GX_CUDA(ctx, claims.alloc(nsub + 1));
+    GX_CUDA(ctx, cudaMemsetAsync(claims.p, 0, (size_t) (nsub + 1) * sizeof(unsigned int), ctx->stream));
+    a.sf = gx_hash_slotfn(h); a.sub_claims = claims.p; a.sub_limit = (unsigned int) (wrap - 1); a.sub_over = claims.p + nsub;
+    unsigned int h_sub_over = 0; cudaError_t e;
+    {
+        gx_launch_scope ls(ctx, "build");
+        gx_launch_scope which(ctx, "build_direct", 0);
+        const long long nb = (a.nrows + 255) / 256, maxb = (long long) ctx->sm_count * 8;
+        gx_k_hash_build<<<(unsigned) (nb < maxb ? nb : maxb), 256, 0, ctx->stream>>>(a);
         e = cudaGetLastError();
-        if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->h_scratch + 3, ctx->d_scratch + 3, 3 * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(&h_over, ba.overflow, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-        gx_tmp_free(ctx, ba.cursor); gx_tmp_free(ctx, ba.pairs);
-        if (e != cudaSuccess) { GX_SET_ERR(ctx, "hash_build: %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
-        h->avg_chain = ctx->h_scratch[3] > 0 ? (double) ctx->h_scratch[5] / (double) ctx->h_scratch[3] : 0.0;
-        if (h->mode != 0 && (h_over || h->avg_chain > 4.0)) { h->mode = 0; continue; }   // keys were not as uniform as the sample said
-        if (h_over) bucketed = false;                 // a sub-table overflowed (heavy key skew): build it the direct way
-        else nscattered = ctx->h_scratch[3];
     }
-    a.sf.mode = h->mode; a.sf.win = h->win; a.sf.shift = h->shift; a.sf.amask = h->amask; a.sf.kmin = h->kmin; a.sf.scale = h->scale;
-    if (inner->nrows > 0 && !bucketed) {
-        GX_CUDA(ctx, cudaMemsetAsync(ctx->d_scratch, 0, 2 * sizeof(long long), ctx->stream));
-        { gx_launch_scope ls(ctx, "build_clear"); gx_k_fill_slots<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(h->slots, h->nslots); }
-        // probe walks wrap inside a sub-table (or the whole table when it is smaller): each keeps a free slot
-        const long long wrap = h->nslots < GX_SUB ? h->nslots : GX_SUB, nsub = h->nslots / wrap;
-        unsigned int *claims = nullptr;
-        GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &claims, (size_t) (nsub + 1) * sizeof(unsigned int)));
-        GX_CUDA(ctx, cudaMemsetAsync(claims, 0, (size_t) (nsub + 1) * sizeof(unsigned int), ctx->stream));
-        a.sub_claims = claims; a.sub_limit = (unsigned int) (wrap - 1); a.sub_over = claims + nsub;
-        unsigned int h_sub_over = 0;
-        cudaError_t e;
-        {
-            gx_launch_scope ls(ctx, "build");
-            gx_launch_scope which(ctx, "build_direct", 0);
-            long long nb = (inner->nrows + 255) / 256;
-            long long maxb = (long long) ctx->sm_count * 8;
-            gx_k_hash_build<<<(unsigned) (nb < maxb ? nb : maxb), 256, 0, ctx->stream>>>(a);
-            e = cudaGetLastError();
-        }
-        if (e == cudaSuccess) e = cudaMemcpyAsync(&h_sub_over, a.sub_over, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-        gx_tmp_free(ctx, claims);
-        if (e != cudaSuccess) { GX_SET_ERR(ctx, "hash_build: %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
-        if (h_sub_over) {
-            GX_SET_ERR(ctx, "hash_build: %u build rows hash into one %lld-slot sub-table of the join table, which holds at most %lld "
-                       "(a build key repeated that often, or keys that collide under the table's hash)",
-                       h_sub_over, wrap, wrap - 1);
-            return GX_ERR_ARG;
-        }
-    } else if (inner->nrows == 0) {
-        gx_launch_scope ls(ctx, "build_clear"); gx_k_fill_slots<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(h->slots, h->nslots);
-    }
-    GX_CUDA(ctx, cudaGetLastError());
-    if (!counts_read) {
-        GX_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch, ctx->d_scratch, 2 * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream));
-        GX_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    }
-    if (nscattered >= 0) ctx->h_scratch[0] = nscattered;
-    h->nentries = ctx->h_scratch[0] + ctx->h_scratch[1];
-    h->special_count = (int) ctx->h_scratch[1];
-    if (h->special_count > h->special_cap) {
-        GX_SET_ERR(ctx, "hash_build: %d rows carry key INT64_MIN (side list holds %d)", h->special_count, h->special_cap);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&h_sub_over, a.sub_over, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) { GX_SET_ERR(ctx, "hash_build: %s", cudaGetErrorString(e)); return GX_ERR_CUDA; }
+    if (h_sub_over) {
+        GX_SET_ERR(ctx, "hash_build: %u build rows hash into one %lld-slot sub-table of the join table, which holds at most %lld "
+                   "(a build key repeated that often, or keys that collide under the table's hash)", h_sub_over, wrap, wrap - 1);
         return GX_ERR_ARG;
     }
-    guard.h = nullptr;
-    *out = h;
+    return GX_OK;
+}
+
+extern "C" int gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col, int n_preds, const gx_pred *preds,
+                             int n_payload, const int32_t *payload_cols, int unique, gx_hash **out)
+{
+    if (!ctx || !inner || !out) return GX_ERR_ARG;
+    build_job j(ctx, inner, key_col);
+    int rc = build_setup(j, n_preds, preds, n_payload, payload_cols, unique); if (rc) return rc;
+    gx_hash *h = j.h; long long *w = ctx->h_scratch;
+    key_sample ks; rc = sample_keys(j, ks); if (rc) return rc;
+    GX_CUDA(ctx, clear_scratch(ctx, SW_INSERTED, SW_SPECIAL));
+    long long nplaced = -1;                                         // entries a fill placed (key-ordered or bucketed build)
+    if (inner->nrows == 0) { gx_launch_scope ls(ctx, "build_clear"); gx_k_fill_slots<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(h->slots, h->nslots); }
+    else {
+        bool direct = h->nslots < 64 * GX_SUB || j.sw.direct;      // big tables: bucket by sub-table, build each in shared memory
+        sorted_outcome so = SORTED_UNORDERED;
+        if (!direct && h->mode != 0 && !j.sw.nosorted) {
+            rc = sorted_build(j, ks, so, nplaced); if (rc) return rc;
+            if (so == SORTED_CLUSTERED) h->mode = 0;               // clustered keys: the mixing hash
+            else if (so == SORTED_UNORDERED) set_slotfn(h, ks.sf);  // not in key order: back to the sampled slot function
+        }
+        if (!direct && so != SORTED_BUILT) {
+            bucket_outcome bo; rc = bucketed_build(j, bo, nplaced); if (rc) return rc;
+            if (bo == BUCKET_REHASH) { h->mode = 0; rc = bucketed_build(j, bo, nplaced); if (rc) return rc; }
+            direct = bo == BUCKET_OVERFLOW;
+        }
+        if (direct) { rc = direct_build(j); if (rc) return rc; }
+    }
+    // the entry count and the side list (the key-ordered build read them with its fill's counters)
+    GX_CUDA(ctx, cudaGetLastError());
+    if (!h->sorted_build) {
+        GX_CUDA(ctx, cudaMemcpyAsync(w, ctx->d_scratch, 2 * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream));
+        GX_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    }
+    if (nplaced >= 0) w[SW_INSERTED] = nplaced;
+    h->nentries = w[SW_INSERTED] + w[SW_SPECIAL];
+    h->special_count = (int) w[SW_SPECIAL];
+    GX_CHECK_ARG(ctx, h->special_count <= h->special_cap, "hash_build: %d rows carry key INT64_MIN (side list holds %d)", h->special_count, h->special_cap);
+    *out = h; j.h = nullptr;
     return GX_OK;
 }
 
