@@ -28,9 +28,7 @@
  * and are EXECUTED by provider/harness (a stub-linked fake backend: fake EState,
  * heapgetpage() fed from heap-page images, real libgpuexec.so; see
  * tests/test_provider_harness.py).  The planner hook recognises the plan shapes
- * of BASELINE configs 1-3 and Q1 (single-relation or two-relation inner equi-join
- * on one int4/int8 key, "Var op Const" quals, Var group keys, count(*) / count /
- * sum / avg / min / max over float8 Var/Const arithmetic) and offers
+ * listed above gpuexec_match_plan, with the aggregates of gpuexec_aggs, and offers
  *   - the whole aggregation pushed down when the GROUP BY covers the input's
  *     distribution key (grouping_distribution_match, planner.c:8588-8668), or
  *   - PARTIAL states (AGGSPLIT_INITIAL_SERIAL) under the reference's own
@@ -264,6 +262,84 @@ gpuexec_type_of(Oid typid)
 		default:
 			return 0;
 	}
+}
+
+/* ------------------------------------------------------------ aggregates */
+/* the argument an aggregate takes */
+typedef enum
+{
+	AGG_ARG_NONE,				/* count(*) */
+	AGG_ARG_COLUMN,				/* one column (or float8 constant), a program of one op */
+	AGG_ARG_F8,					/* one float8 expression */
+	AGG_ARG_F8_PAIR				/* (Y, X): Y's program, GX_OP_ARG2, X's program */
+} GpuAggArg;
+
+/* the transition value a partial (AGGSPLIT_INITIAL_SERIAL) aggregate emits: what the reference's combine function
+ * expects (pg_aggregate.h:178-316) */
+typedef enum
+{
+	PARTIAL_VALUE,				/* the final value: float8 for sum/min/max(float8), int8 for sum(int4) */
+	PARTIAL_COUNT,				/* int8 N (int8pl) */
+	PARTIAL_AVG,				/* float8[3] {N, Sx, 0}: only var/stddev read Sxx; float8_combine (float.c:2725) keeps it finite */
+	PARTIAL_VAR,				/* float8_accum's float8[3] {N, Sx, Sxx}, Sxx from gx_result_fetch_sxx */
+	PARTIAL_REGR				/* float8[6] {N, Sx, Sxx, Sy, Syy, Sxy} (float8_regr_combine, float.c:3244), gx_result_fetch_regr */
+} GpuAggPartial;
+
+typedef struct GpuAggDef
+{
+	Oid			aggfnoid;		/* pg_aggregate.aggfnoid */
+	int			fn;				/* GX_AGG_* */
+	GpuAggArg	arg;
+	GpuAggPartial partial;
+} GpuAggDef;
+
+/* Every aggregate the planner hook pushes down; an Aggref of any other aggfnoid declines the plan.  count(DISTINCT x) is
+ * count(any)'s row under stricter rules (GX_AGG_COUNT_DISTINCT, match_aggregates). */
+static const GpuAggDef gpuexec_aggs[] = {
+	{2803, GX_AGG_COUNT_STAR, AGG_ARG_NONE, PARTIAL_COUNT},			/* count(*) */
+	{2147, GX_AGG_COUNT, AGG_ARG_COLUMN, PARTIAL_COUNT},			/* count(any) */
+	{2108, GX_AGG_SUM_I4, AGG_ARG_COLUMN, PARTIAL_VALUE},			/* sum(int4) */
+	{2111, GX_AGG_SUM_F8, AGG_ARG_F8, PARTIAL_VALUE},				/* sum(float8) */
+	{2105, GX_AGG_AVG_F8, AGG_ARG_F8, PARTIAL_AVG},					/* avg(float8) */
+	{2136, GX_AGG_MIN_F8, AGG_ARG_F8, PARTIAL_VALUE},				/* min(float8) */
+	{2120, GX_AGG_MAX_F8, AGG_ARG_F8, PARTIAL_VALUE},				/* max(float8) */
+	{2722, GX_AGG_VAR_POP_F8, AGG_ARG_F8, PARTIAL_VAR},				/* var_pop(float8) */
+	{2645, GX_AGG_VAR_SAMP_F8, AGG_ARG_F8, PARTIAL_VAR},			/* var_samp(float8) */
+	{2152, GX_AGG_VAR_SAMP_F8, AGG_ARG_F8, PARTIAL_VAR},			/* variance(float8) */
+	{2728, GX_AGG_STDDEV_POP_F8, AGG_ARG_F8, PARTIAL_VAR},			/* stddev_pop(float8) */
+	{2716, GX_AGG_STDDEV_SAMP_F8, AGG_ARG_F8, PARTIAL_VAR},			/* stddev_samp(float8) */
+	{2158, GX_AGG_STDDEV_SAMP_F8, AGG_ARG_F8, PARTIAL_VAR},			/* stddev(float8) */
+	{2818, GX_AGG_REGR_COUNT, AGG_ARG_F8_PAIR, PARTIAL_COUNT},		/* regr_count(float8, float8) */
+	{2819, GX_AGG_REGR_SXX_F8, AGG_ARG_F8_PAIR, PARTIAL_REGR},		/* regr_sxx */
+	{2820, GX_AGG_REGR_SYY_F8, AGG_ARG_F8_PAIR, PARTIAL_REGR},		/* regr_syy */
+	{2821, GX_AGG_REGR_SXY_F8, AGG_ARG_F8_PAIR, PARTIAL_REGR},		/* regr_sxy */
+	{2822, GX_AGG_REGR_AVGX_F8, AGG_ARG_F8_PAIR, PARTIAL_REGR},		/* regr_avgx */
+	{2823, GX_AGG_REGR_AVGY_F8, AGG_ARG_F8_PAIR, PARTIAL_REGR},		/* regr_avgy */
+	{2824, GX_AGG_REGR_R2_F8, AGG_ARG_F8_PAIR, PARTIAL_REGR},		/* regr_r2 */
+	{2825, GX_AGG_REGR_SLOPE_F8, AGG_ARG_F8_PAIR, PARTIAL_REGR},	/* regr_slope */
+	{2826, GX_AGG_REGR_INTERCEPT_F8, AGG_ARG_F8_PAIR, PARTIAL_REGR},	/* regr_intercept */
+	{2827, GX_AGG_COVAR_POP_F8, AGG_ARG_F8_PAIR, PARTIAL_REGR},		/* covar_pop */
+	{2828, GX_AGG_COVAR_SAMP_F8, AGG_ARG_F8_PAIR, PARTIAL_REGR},	/* covar_samp */
+	{2829, GX_AGG_CORR_F8, AGG_ARG_F8_PAIR, PARTIAL_REGR},			/* corr */
+};
+
+static const GpuAggDef *
+agg_by_oid(Oid aggfnoid)
+{
+	for (int i = 0; i < (int) lengthof(gpuexec_aggs); i++)
+		if (gpuexec_aggs[i].aggfnoid == aggfnoid)
+			return &gpuexec_aggs[i];
+	return NULL;
+}
+
+/* the row of a descriptor's aggregate, which carries no OID (an alias has its function's row); NULL for count(DISTINCT) */
+static const GpuAggDef *
+agg_by_fn(int fn)
+{
+	for (int i = 0; i < (int) lengthof(gpuexec_aggs); i++)
+		if (gpuexec_aggs[i].fn == fn)
+			return &gpuexec_aggs[i];
+	return NULL;
 }
 
 /* ------------------------------------------------ K0: heap page loader
@@ -664,11 +740,6 @@ gpuexec_begin(CustomScanState *node, EState *estate, int eflags)
 	live_handles = h;
 }
 
-static bool is_variance_fn(int fn);
-static bool plan_has_variance(const gx_agg_plan *plan);
-static bool is_regr_fn(int fn);
-static bool plan_has_regr(const gx_agg_plan *plan);
-
 static void
 gpuexec_run(GpuExecState *st, EState *estate)
 {
@@ -738,14 +809,24 @@ gpuexec_run(GpuExecState *st, EState *estate)
 	st->nulls = (uint8 *) palloc(Max(n * (ng + na), 1));
 	if (st->partial)
 	{
+		bool		sxx = false,
+					regr = false;
+
+		for (int a = 0; a < na; a++)
+		{
+			const GpuAggDef *def = agg_by_fn(st->plan.aggs[a].fn);
+
+			sxx |= def && def->partial == PARTIAL_VAR;
+			regr |= def && def->arg == AGG_ARG_F8_PAIR;
+		}
 		st->cnts = (int64 *) palloc(sizeof(int64) * Max(n * na, 1));
 		GX_CHECK(gx_result_fetch_states(st->result, n, st->keys, st->aggs, st->cnts, st->nulls));
-		if (plan_has_variance(&st->plan))
+		if (sxx)
 		{
 			st->sxx = (double *) palloc(sizeof(double) * Max(n * na, 1));
 			GX_CHECK(gx_result_fetch_sxx(st->result, n, st->sxx));
 		}
-		if (plan_has_regr(&st->plan))
+		if (regr)
 		{
 			st->regr = (double *) palloc(sizeof(double) * 6 * Max(n * na, 1));
 			GX_CHECK(gx_result_fetch_regr(st->result, n, st->regr));
@@ -768,10 +849,7 @@ gpuexec_run(GpuExecState *st, EState *estate)
  * aggregates in descriptor order) — whatever order the query's own target list has; the
  * plan's targetlist is projected over it (ExecAssignScanProjectionInfoWithVarno,
  * nodeCustom.c:100-101) below.  In partial mode an aggregate column carries the transition
- * value the reference's combine function expects (pg_aggregate.h:178-252): int8 for
- * count/sum(int4), float8 for sum/min/max(float8), float8[3] {N, Sx, Sxx} for avg(float8) and the
- * variances and standard deviations of float8, float8[6] {N, Sx, Sxx, Sy, Syy, Sxy} for the regression aggregates
- * (float8_regr_combine, float.c:3244) and int8 for regr_count (int8pl). */
+ * value its row of gpuexec_aggs names. */
 static TupleTableSlot *
 gpuexec_exec(CustomScanState *node)
 {
@@ -842,22 +920,21 @@ gpuexec_exec(CustomScanState *node)
 		{
 			int			a = i - ng;
 			double		d = st->aggs[g * na + a];
-			int			fn = st->plan.aggs[a].fn;
+			const GpuAggDef *def = agg_by_fn(st->plan.aggs[a].fn);
+			GpuAggPartial form = st->partial && def ? def->partial : PARTIAL_VALUE;
 
-			if (st->partial && (fn == GX_AGG_AVG_F8 || is_variance_fn(fn)))
+			if (form == PARTIAL_AVG || form == PARTIAL_VAR)
 			{
-				/* float8_accum's transition value {N, Sx, Sxx}; avg's Sxx is not carried (only
-				 * var/stddev read it; float8_combine, float.c:2725, keeps it finite) */
 				MemoryContext old = MemoryContextSwitchTo(econtext->ecxt_per_tuple_memory);
 				Datum		elems[3];
 
 				elems[0] = Float8GetDatum((double) st->cnts[g * na + a]);
 				elems[1] = Float8GetDatum(d);
-				elems[2] = Float8GetDatum(fn == GX_AGG_AVG_F8 ? 0.0 : st->sxx[g * na + a]);
+				elems[2] = Float8GetDatum(form == PARTIAL_AVG ? 0.0 : st->sxx[g * na + a]);
 				slot->tts_values[i] = PointerGetDatum(construct_array(elems, 3, FLOAT8OID, sizeof(float8), FLOAT8PASSBYVAL, 'd'));
 				MemoryContextSwitchTo(old);
 			}
-			else if (st->partial && is_regr_fn(fn) && fn != GX_AGG_REGR_COUNT)
+			else if (form == PARTIAL_REGR)
 			{
 				MemoryContext old = MemoryContextSwitchTo(econtext->ecxt_per_tuple_memory);
 				Datum		elems[6];
@@ -868,7 +945,7 @@ gpuexec_exec(CustomScanState *node)
 				slot->tts_values[i] = PointerGetDatum(construct_array(elems, 6, FLOAT8OID, sizeof(float8), FLOAT8PASSBYVAL, 'd'));
 				MemoryContextSwitchTo(old);
 			}
-			else if (st->partial && (fn == GX_AGG_COUNT_STAR || fn == GX_AGG_COUNT || fn == GX_AGG_REGR_COUNT))
+			else if (form == PARTIAL_COUNT)
 				slot->tts_values[i] = Int64GetDatum(st->cnts[g * na + a]);
 			else if (typid == INT8OID)
 			{
@@ -1008,26 +1085,22 @@ gpuexec_plan_path(PlannerInfo *root, RelOptInfo *rel, CustomPath *best_path,
  *            Agg over a left-deep chain of 2..GX_MAX_JOINS such INNER joins with unique build sides (star joins:
  *            TPC-H Q3), GROUP BY columns from any relation, aggregate arguments from the outer one (match_joins)
  * with "Var op Const" quals on the scans, Var group keys, no HAVING / grouping sets /
- * DISTINCT / ORDER BY aggregates / FILTER, and aggregates count(*), count(x),
- * sum/avg/min/max(float8 expr), sum(int4); every target-list entry must be a group Var or a
+ * ORDER BY aggregates / FILTER, and the aggregates of gpuexec_aggs; every target-list entry must be a group Var or a
  * bare Aggref.  Anything else returns false and the CPU paths stay untouched — the same
  * "eligibility test" idea as jit_compile_hashjoin (jit/jit.c:253-303). */
-#define AGG_COUNT_STAR 2803
-#define AGG_COUNT_ANY  2147
-#define AGG_SUM_F8     2111
-#define AGG_AVG_F8     2105
-#define AGG_MAX_F8     2120
-#define AGG_MIN_F8     2136
-#define AGG_SUM_I4     2108
-#define AGG_VAR_POP_F8     2722
-#define AGG_VAR_SAMP_F8    2645
-#define AGG_VARIANCE_F8    2152
-#define AGG_STDDEV_POP_F8  2728
-#define AGG_STDDEV_SAMP_F8 2716
-#define AGG_STDDEV_F8      2158
-/* the SQL:2003 binary aggregates over (float8, float8), pg_aggregate.h:305-316: aggfnoid - AGG_REGR_COUNT + GX_AGG_REGR_COUNT */
-#define AGG_REGR_COUNT     2818
-#define AGG_CORR           2829
+
+/* what the matcher learns besides the descriptor: the planner hook reads the Aggrefs and the estimates */
+typedef struct GpuPlanMatch
+{
+	List	   *agg_refs;		/* the Aggrefs, in descriptor order */
+	int32		key_types[GX_MAX_GROUP_COLS + 1];	/* staged types of the group columns, then of the DISTINCT column */
+	Var		   *distinct_arg;	/* the column of the query's count(DISTINCT) aggregates */
+	double		outer_rows;		/* rows of the relation in the descriptor's outer slot */
+	double		pages;			/* heap pages of every relation the plan scans */
+	double		groups;
+	double		pairs;			/* count(DISTINCT): the (group, value) pairs of its first stage; 0 without one */
+	double		bytes;			/* HBM the plan needs */
+} GpuPlanMatch;
 
 /* column number of (rti, attno) in the descriptor, appended on first use */
 static int
@@ -1051,40 +1124,6 @@ rel_column(GpuRelInfo *r, Index rti, AttrNumber attno, Oid typid, int32 typmod)
 }
 
 /* float8 expression -> postfix program over outer columns */
-static bool
-is_variance_fn(int fn)
-{
-	return fn == GX_AGG_VAR_POP_F8 || fn == GX_AGG_VAR_SAMP_F8 || fn == GX_AGG_STDDEV_POP_F8 || fn == GX_AGG_STDDEV_SAMP_F8;
-}
-
-static bool
-plan_has_variance(const gx_agg_plan *plan)
-{
-	int			a;
-
-	for (a = 0; a < plan->n_aggs; a++)
-		if (is_variance_fn(plan->aggs[a].fn))
-			return true;
-	return false;
-}
-
-static bool
-is_regr_fn(int fn)
-{
-	return fn >= GX_AGG_REGR_COUNT && fn <= GX_AGG_CORR_F8;
-}
-
-static bool
-plan_has_regr(const gx_agg_plan *plan)
-{
-	int			a;
-
-	for (a = 0; a < plan->n_aggs; a++)
-		if (is_regr_fn(plan->aggs[a].fn))
-			return true;
-	return false;
-}
-
 static bool
 match_f8_expr(Node *n, GpuRelInfo *outer, gx_expr *e)
 {
@@ -1324,7 +1363,7 @@ column_is_not_null(PlannerInfo *root, Index rti, AttrNumber attno)
 }
 
 /*
- * The library's state words per group (csrc/gx_agg.cu, compile_plan), restated so that a variance plan the library
+ * The library's state words per group (csrc/gx_agg.cu, compile_plan), restated so that a plan the library
  * would refuse with "too many state words" is declined here, at plan time.  Word 0 counts the group's rows; a count
  * of a nullable column takes one word, a sum(int4) two when its column is nullable; sum, avg, min and max of float8
  * take a value word and, over a nullable argument, a count word; sum, avg and the variances of one argument share
@@ -1350,7 +1389,8 @@ same_f8_expr(const gx_expr *x, const gx_expr *y)
 static bool
 state_words_fit(PlannerInfo *root, const GpuRelInfo *outer, const gx_agg_plan *plan)
 {
-	bool		var_words[GX_MAX_AGGS] = {false};
+	bool		sum_words[GX_MAX_AGGS] = {false},
+				var_words[GX_MAX_AGGS] = {false};
 	bool		distinct = false,
 				regr_full = false;
 	int			nw = 1,
@@ -1362,9 +1402,11 @@ state_words_fit(PlannerInfo *root, const GpuRelInfo *outer, const gx_agg_plan *p
 	/* the two-argument aggregates share one state, over one (Y, X) pair: a second pair is declined */
 	for (a = 0; a < plan->n_aggs; a++)
 	{
-		if (!is_regr_fn(plan->aggs[a].fn))
+		const GpuAggDef *def = agg_by_fn(plan->aggs[a].fn);
+
+		if (def == NULL || def->arg != AGG_ARG_F8_PAIR)
 			continue;
-		if (plan->aggs[a].fn != GX_AGG_REGR_COUNT)
+		if (def->partial == PARTIAL_REGR)
 			regr_full = true;
 		if (regr_owner < 0)
 			regr_owner = a;
@@ -1375,41 +1417,33 @@ state_words_fit(PlannerInfo *root, const GpuRelInfo *outer, const gx_agg_plan *p
 	for (a = 0; a < plan->n_aggs; a++)
 	{
 		const gx_agg *g = &plan->aggs[a];
-		bool		var = is_variance_fn(g->fn),
-					nullable = false;
+		const GpuAggDef *def = agg_by_fn(g->fn);
+		bool		nullable = false;
 		int			twin = -1;
 
-		if (g->fn != GX_AGG_COUNT_DISTINCT && !is_regr_fn(g->fn) && nw + (var ? 5 : 2) > GPUEXEC_MAX_STATE_WORDS)
-			return false;
+		if (def == NULL)		/* count(DISTINCT) */
+		{
+			distinct = true;
+			continue;
+		}
 		for (k = 0; k < g->arg.nops; k++)
 			if (g->arg.ops[k].op == GX_OP_COL && !column_is_not_null(root, outer->rti, outer->attnums[g->arg.ops[k].col] + 1))
 				nullable = true;
+		if (def->arg == AGG_ARG_F8_PAIR)
+		{
+			/* the first of them owns the pair count (when a side is nullable) and, unless all are regr_count,
+			 * {Sx, Sy, Cx, S1x, S2x, Cy, S1y, S2y, Sxy'}; never shared with sum / avg */
+			if (a == regr_owner)
+				nw += (nullable ? 1 : 0) + (regr_full ? 9 : 0);
+			if (nw > GPUEXEC_MAX_STATE_WORDS)
+				return false;
+			continue;
+		}
+		if (nw + (def->partial == PARTIAL_VAR ? 5 : 2) > GPUEXEC_MAX_STATE_WORDS)
+			return false;
 		switch (g->fn)
 		{
 			case GX_AGG_COUNT_STAR:
-				break;
-			case GX_AGG_COUNT_DISTINCT:
-				distinct = true;
-				break;
-			case GX_AGG_REGR_COUNT:
-			case GX_AGG_REGR_SXX_F8:
-			case GX_AGG_REGR_SYY_F8:
-			case GX_AGG_REGR_SXY_F8:
-			case GX_AGG_REGR_AVGX_F8:
-			case GX_AGG_REGR_AVGY_F8:
-			case GX_AGG_REGR_R2_F8:
-			case GX_AGG_REGR_SLOPE_F8:
-			case GX_AGG_REGR_INTERCEPT_F8:
-			case GX_AGG_COVAR_POP_F8:
-			case GX_AGG_COVAR_SAMP_F8:
-			case GX_AGG_CORR_F8:
-				/* the first of them owns the pair count (when a side is nullable) and, unless all are regr_count,
-				 * {Sx, Sy, Cx, S1x, S2x, Cy, S1y, S2y, Sxy'}; never shared with sum / avg */
-				if (a != regr_owner)
-					break;
-				nw += (nullable ? 1 : 0) + (regr_full ? 9 : 0);
-				if (nw > GPUEXEC_MAX_STATE_WORDS)
-					return false;
 				break;
 			case GX_AGG_COUNT:
 				nw += nullable ? 1 : 0;
@@ -1420,16 +1454,16 @@ state_words_fit(PlannerInfo *root, const GpuRelInfo *outer, const gx_agg_plan *p
 				nw += nullable ? 2 : 1;
 				break;
 			default:			/* sum, avg and the variances of float8 */
+				sum_words[a] = true;
 				for (b = 0; b < a && twin < 0; b++)
-					if ((plan->aggs[b].fn == GX_AGG_SUM_F8 || plan->aggs[b].fn == GX_AGG_AVG_F8 || is_variance_fn(plan->aggs[b].fn)) &&
-						same_f8_expr(&plan->aggs[b].arg, &g->arg))
+					if (sum_words[b] && same_f8_expr(&plan->aggs[b].arg, &g->arg))
 						twin = b;
 				if (twin < 0)
 				{
 					twin = a;
 					nw += nullable ? 2 : 1;
 				}
-				if (var && !var_words[twin])
+				if (def->partial == PARTIAL_VAR && !var_words[twin])
 				{
 					var_words[twin] = true;
 					nw += 3;
@@ -1514,7 +1548,7 @@ join_level(PlannerInfo *root, HashPath *hp, Var **ov, Var **iv)
  * column of F; a later step's is a column of F or of an earlier D, carried in that step's payload (which has no NULL
  * flag: the column must be NOT NULL). */
 static bool
-match_joins(PlannerInfo *root, HashPath *top, GpuExecState *out, double *est_bytes, double *est_pages)
+match_joins(PlannerInfo *root, HashPath *top, GpuExecState *out, GpuPlanMatch *m)
 {
 	HashPath   *lv[GX_MAX_JOINS];
 	Path	   *p = &top->jpath.path;
@@ -1535,8 +1569,8 @@ match_joins(PlannerInfo *root, HashPath *top, GpuExecState *out, double *est_byt
 	if (relation_is_protected(root, out->outer.rti))
 		return false;
 	out->n_joins = n;
-	*est_bytes = p->parent->tuples;
-	*est_pages = p->parent->pages;
+	m->outer_rows = p->parent->tuples;
+	m->pages = p->parent->pages;
 	for (s = 1; s <= n; s++)
 	{
 		HashPath   *hp = lv[n - s];
@@ -1561,8 +1595,8 @@ match_joins(PlannerInfo *root, HashPath *top, GpuExecState *out, double *est_byt
 			j->tuples = p->parent->tuples;
 			j->rel.rti = out->outer.rti;
 			out->outer.rti = iv->varno;
-			*est_bytes = irel->tuples;		/* the rows the aggregate's columns are staged for */
-			*est_pages += irel->pages;
+			m->outer_rows = irel->tuples;
+			m->pages += irel->pages;
 			plan->outer_key_col = rel_column(&out->outer, iv->varno, iv->varattno, iv->vartype, iv->vartypmod);
 			j->key_col = rel_column(&j->rel, ov->varno, ov->varattno, ov->vartype, ov->vartypmod);
 			return plan->outer_key_col >= 0 && j->key_col >= 0 &&
@@ -1604,53 +1638,45 @@ match_joins(PlannerInfo *root, HashPath *top, GpuExecState *out, double *est_byt
 		}
 		if (!match_quals(irel->baserestrictinfo, &j->rel, j->preds, &j->n_preds))
 			return false;
-		*est_pages += irel->pages;
+		m->pages += irel->pages;
 	}
 	return true;
 }
 
+/* the outer relation: a base-relation scan, or a join (match_joins) */
 static bool
-gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_rel, GpuExecState *out,
-				   List **agg_refs, double *est_rows, double *est_groups, double *est_bytes, double *est_pages,
-				   double *est_pairs)
+match_input(PlannerInfo *root, RelOptInfo *input_rel, GpuExecState *out, GpuPlanMatch *m)
 {
-	Var		   *distinct_arg = NULL;	/* the column of the query's count(DISTINCT) aggregates, */
-	int			distinct_c = -1;		/* and its outer column number */
-	Query	   *parse = root->parse;
 	Path	   *in = input_rel->cheapest_total_path;
-	gx_agg_plan *plan = &out->plan;
-	ListCell   *lc;
-	int			i;
-
-	if (parse->groupingSets || parse->havingQual || parse->hasWindowFuncs || parse->hasTargetSRFs || in == NULL)
-		return false;
-	plan->outer_key_col = -1;
 
 	if (in->pathtype == T_SeqScan && input_rel->reloptkind == RELOPT_BASEREL)
 	{
 		out->outer.rti = input_rel->relid;
 		if (relation_is_protected(root, input_rel->relid) ||
-			!match_quals(input_rel->baserestrictinfo, &out->outer, plan->preds, &plan->n_preds))
+			!match_quals(input_rel->baserestrictinfo, &out->outer, out->plan.preds, &out->plan.n_preds))
 			return false;
-		*est_bytes = input_rel->tuples;
-		*est_pages = input_rel->pages;
+		m->outer_rows = input_rel->tuples;
+		m->pages = input_rel->pages;
+		return true;
 	}
-	else if (IsA(in, HashPath))
-	{
-		if (!match_joins(root, (HashPath *) in, out, est_bytes, est_pages))
-			return false;
-	}
-	else
-		return false;
+	return IsA(in, HashPath) && match_joins(root, (HashPath *) in, out, m);
+}
 
-	/* GROUP BY: plain Vars of the outer side, or of a build side under INNER joins, riding in that join's payload */
+/* GROUP BY: plain Vars of the outer side, or of a build side under INNER joins, riding in that join's payload */
+static bool
+match_group_by(PlannerInfo *root, GpuExecState *out, GpuPlanMatch *m)
+{
+	Query	   *parse = root->parse;
+	gx_agg_plan *plan = &out->plan;
+	ListCell   *lc;
+
 	foreach(lc, parse->groupClause)
 	{
 		SortGroupClause *sgc = (SortGroupClause *) lfirst(lc);
 		TargetEntry *tle = get_sortgroupclause_tle(sgc, parse->targetList);
 		Var		   *v = (Var *) tle->expr;
 		int			c,
-					s;
+					s = 0;
 
 		if (!IsA(v, Var) || plan->n_group_cols >= GX_MAX_GROUP_COLS)
 			return false;
@@ -1659,8 +1685,7 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 			c = rel_column(&out->outer, v->varno, v->varattno, v->vartype, v->vartypmod);
 			if (c < 0)
 				return false;
-			plan->group_cols[plan->n_group_cols].side = 0;
-			plan->group_cols[plan->n_group_cols].col = c;
+			m->key_types[plan->n_group_cols] = out->outer.types[c];
 		}
 		else if (plan->join_type == GX_JOIN_INNER && (s = join_step_of(out, v->varno)) > 0)
 		{
@@ -1670,54 +1695,69 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 			c = rel_column(&j->rel, v->varno, v->varattno, v->vartype, v->vartypmod);
 			if (c < 0 || !column_is_not_null(root, v->varno, v->varattno))
 				return false;		/* gx_hash_build carries payload columns inside the slot: no room for a NULL flag */
+			m->key_types[plan->n_group_cols] = j->rel.types[c];
 			c = payload_slot(j->payload_cols, &j->n_payload, c);
 			if (c < 0)
 				return false;
-			plan->group_cols[plan->n_group_cols].side = s;
-			plan->group_cols[plan->n_group_cols].col = c;
 		}
 		else
 			return false;
-		plan->n_group_cols++;
+		plan->group_cols[plan->n_group_cols].side = s;
+		plan->group_cols[plan->n_group_cols++].col = c;
 	}
+	return true;
+}
 
-	/* Limits the library would only report at execution time (GX_ERR_ARG -> ERROR): decline here instead, the CPU plan stays.
-	 * A join's payload is one 8-byte word (gx_hash_build, csrc/gx_join.cu); the group key is two 8-byte words filled first-fit
-	 * in GROUP BY order (compile_plan, csrc/gx_agg.cu). */
+/* the library's group key is two 8-byte words, filled first-fit in key order (compile_plan, csrc/gx_agg.cu): do columns
+ * of these staged types fit? */
+static bool
+group_key_fits(const int32 *types, int n)
+{
+	int			used[2] = {0, 0};
+
+	for (int i = 0; i < n; i++)
 	{
-		int			used[2] = {0, 0};
+		int			b = staged_type_bytes(types[i]),
+					w = used[0] + b <= 8 ? 0 : 1;
 
-		for (i = 0; i < out->n_joins; i++)
-		{
-			const GpuJoinStep *j = &out->join[i];
-			int			k,
-						payload_bytes = 0;
-
-			for (k = 0; k < j->n_payload; k++)
-				payload_bytes += staged_type_bytes(j->rel.types[j->payload_cols[k]]);
-			if (payload_bytes > 8)
-				return false;
-		}
-		for (i = 0; i < plan->n_group_cols; i++)
-		{
-			const gx_colref *gc = &plan->group_cols[i];
-			int32		t = gc->side == 0 ? out->outer.types[gc->col]
-				: out->join[gc->side - 1].rel.types[out->join[gc->side - 1].payload_cols[gc->col]];
-			int			b = staged_type_bytes(t),
-						w = used[0] + b <= 8 ? 0 : 1;
-
-			if (used[w] + b > 8)
-				return false;
-			used[w] += b;
-		}
+		if (used[w] + b > 8)
+			return false;
+		used[w] += b;
 	}
+	return true;
+}
 
-	/* every target-list entry is either one of the GROUP BY expressions or a bare Aggref; the
-	 * Aggrefs, in target-list order, are the descriptor's aggregates and the tail of the scan tuple */
+/* Limits the library would only report at execution time (GX_ERR_ARG -> ERROR): decline here instead, the CPU plan stays.
+ * A join's payload is one 8-byte word (gx_hash_build, csrc/gx_join.cu), and the GROUP BY key must fit the group key. */
+static bool
+within_library_limits(const GpuExecState *out, const GpuPlanMatch *m)
+{
+	for (int i = 0; i < out->n_joins; i++)
+	{
+		const GpuJoinStep *j = &out->join[i];
+		int			payload_bytes = 0;
+
+		for (int k = 0; k < j->n_payload; k++)
+			payload_bytes += staged_type_bytes(j->rel.types[j->payload_cols[k]]);
+		if (payload_bytes > 8)
+			return false;
+	}
+	return group_key_fits(m->key_types, out->plan.n_group_cols);
+}
+
+/* every target-list entry is either one of the GROUP BY expressions or a bare Aggref of gpuexec_aggs; the Aggrefs, in
+ * target-list order, are the descriptor's aggregates and the tail of the scan tuple */
+static bool
+match_aggregates(Query *parse, GpuExecState *out, GpuPlanMatch *m)
+{
+	gx_agg_plan *plan = &out->plan;
+	ListCell   *lc;
+
 	foreach(lc, parse->targetList)
 	{
 		TargetEntry *tle = (TargetEntry *) lfirst(lc);
 		Aggref	   *a = (Aggref *) tle->expr;
+		const GpuAggDef *def;
 		gx_agg	   *g;
 
 		if (IsA(a, Var))
@@ -1732,9 +1772,11 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 				return false;	/* functionally dependent column: not carried */
 			continue;
 		}
-		if (!IsA(a, Aggref) || a->aggorder || a->aggfilter || a->aggdirectargs || plan->n_aggs >= GX_MAX_AGGS)
+		if (!IsA(a, Aggref) || a->aggorder || a->aggfilter || a->aggdirectargs || plan->n_aggs >= GX_MAX_AGGS ||
+			(def = agg_by_oid(a->aggfnoid)) == NULL)
 			return false;
 		g = &plan->aggs[plan->n_aggs];
+		g->fn = def->fn;
 		if (a->aggdistinct)
 		{
 			/* count(DISTINCT col) over a plain int4 / int8 / date column of the outer relation (GX_AGG_COUNT_DISTINCT):
@@ -1744,7 +1786,7 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 			Var		   *v;
 			int			c;
 
-			if (a->aggfnoid != AGG_COUNT_ANY || list_length(a->args) != 1 || list_length(a->aggdistinct) != 1)
+			if (def->fn != GX_AGG_COUNT || list_length(a->args) != 1 || list_length(a->aggdistinct) != 1)
 				return false;
 			arg = (TargetEntry *) linitial(a->args);
 			sgc = (SortGroupClause *) linitial(a->aggdistinct);
@@ -1753,146 +1795,89 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 				(v->vartype != INT4OID && v->vartype != INT8OID && v->vartype != DATEOID))
 				return false;
 			c = rel_column(&out->outer, v->varno, v->varattno, v->vartype, v->vartypmod);
-			if (c < 0 || (distinct_arg != NULL && !equal(distinct_arg, v)))
+			if (c < 0 || (m->distinct_arg != NULL && !equal(m->distinct_arg, v)))
 				return false;
-			distinct_arg = v;
-			distinct_c = c;
+			m->distinct_arg = v;
+			m->key_types[plan->n_group_cols] = out->outer.types[c];	/* count(DISTINCT)'s first stage groups by it too */
 			g->fn = GX_AGG_COUNT_DISTINCT;
 			g->arg.nops = 1;
 			g->arg.ops[0].op = GX_OP_COL;
 			g->arg.ops[0].col = c;
-			*agg_refs = lappend(*agg_refs, a);
-			plan->n_aggs++;
-			continue;
-		}
-		switch (a->aggfnoid)
-		{
-			case AGG_COUNT_STAR:
-				g->fn = GX_AGG_COUNT_STAR;
-				break;
-			case AGG_SUM_F8:
-				g->fn = GX_AGG_SUM_F8;
-				break;
-			case AGG_AVG_F8:
-				g->fn = GX_AGG_AVG_F8;
-				break;
-			case AGG_MIN_F8:
-				g->fn = GX_AGG_MIN_F8;
-				break;
-			case AGG_MAX_F8:
-				g->fn = GX_AGG_MAX_F8;
-				break;
-			case AGG_SUM_I4:
-				g->fn = GX_AGG_SUM_I4;
-				break;
-			case AGG_COUNT_ANY:
-				g->fn = GX_AGG_COUNT;
-				break;
-			case AGG_VAR_POP_F8:
-				g->fn = GX_AGG_VAR_POP_F8;
-				break;
-			case AGG_VAR_SAMP_F8:
-			case AGG_VARIANCE_F8:
-				g->fn = GX_AGG_VAR_SAMP_F8;
-				break;
-			case AGG_STDDEV_POP_F8:
-				g->fn = GX_AGG_STDDEV_POP_F8;
-				break;
-			case AGG_STDDEV_SAMP_F8:
-			case AGG_STDDEV_F8:
-				g->fn = GX_AGG_STDDEV_SAMP_F8;
-				break;
-			default:
-				if (a->aggfnoid < AGG_REGR_COUNT || a->aggfnoid > AGG_CORR)
-					return false;
-				break;
-		}
-		if (a->aggfnoid >= AGG_REGR_COUNT && a->aggfnoid <= AGG_CORR)
-		{
-			/* regr_* / covar_* / corr (Y, X): Y's program, GX_OP_ARG2, X's program, within GX_MAX_EXPR_OPS */
-			g->fn = GX_AGG_REGR_COUNT + (int) (a->aggfnoid - AGG_REGR_COUNT);
-			if (list_length(a->args) != 2 ||
-				!match_f8_expr((Node *) ((TargetEntry *) linitial(a->args))->expr, &out->outer, &g->arg) ||
-				g->arg.nops >= GX_MAX_EXPR_OPS)
-				return false;
-			g->arg.ops[g->arg.nops++].op = GX_OP_ARG2;
-			if (!match_f8_expr((Node *) ((TargetEntry *) lsecond(a->args))->expr, &out->outer, &g->arg))
-				return false;
-		}
-		else if (g->fn != GX_AGG_COUNT_STAR)
-		{
-			TargetEntry *arg;
-
-			if (list_length(a->args) != 1)
-				return false;
-			arg = (TargetEntry *) linitial(a->args);
-			if (!match_f8_expr((Node *) arg->expr, &out->outer, &g->arg))
-				return false;
-			if ((g->fn == GX_AGG_SUM_I4 || g->fn == GX_AGG_COUNT) && g->arg.nops != 1)
-				return false;
-		}
-		*agg_refs = lappend(*agg_refs, a);
-		plan->n_aggs++;
-	}
-	if (plan->n_aggs == 0 && plan->n_group_cols == 0)
-		return false;
-	if ((plan_has_variance(plan) || plan_has_regr(plan)) && !state_words_fit(root, &out->outer, plan))
-		return false;
-	*est_rows = in->rows;
-	*est_groups = output_rel->rows > 0 ? output_rel->rows : 1;
-	plan->est_groups = (int64) *est_groups;
-	if (distinct_arg)
-	{
-		/* the library groups by the key plus the DISTINCT column first: that key must fit too (first fit, the column
-		 * packed last), and est_groups is read as the number of distinct (group, value) pairs */
-		List	   *exprs = NIL;
-		int			used[2] = {0, 0},
-					b;
-		double		pairs;
-
-		if (plan->n_group_cols >= GX_MAX_GROUP_COLS)
-			return false;
-		for (i = 0; i <= plan->n_group_cols; i++)
-		{
-			const gx_colref *gc = i < plan->n_group_cols ? &plan->group_cols[i] : NULL;
-			int32		t = gc == NULL ? out->outer.types[distinct_c]
-				: gc->side == 0 ? out->outer.types[gc->col]
-				: out->join[gc->side - 1].rel.types[out->join[gc->side - 1].payload_cols[gc->col]];
-			int			w;
-
-			b = staged_type_bytes(t);
-			w = used[0] + b <= 8 ? 0 : 1;
-			if (used[w] + b > 8)
-				return false;
-			used[w] += b;
-		}
-		foreach(lc, parse->groupClause)
-			exprs = lappend(exprs, get_sortgroupclause_tle((SortGroupClause *) lfirst(lc), parse->targetList)->expr);
-		exprs = lappend(exprs, distinct_arg);
-		pairs = estimate_num_groups(root, exprs, in->rows, NULL);
-		if (pairs > in->rows)
-			pairs = in->rows;
-		if (pairs < 1)
-			pairs = 1;
-		plan->est_groups = (int64) pairs;
-		*est_pairs = pairs;
-	}
-	/* HBM the plan needs: the referenced columns of every row, plus 16 B x 2 per build row */
-	{
-		double		bytes = 0;
-		double		outer_rows = *est_bytes;
-
-		for (i = 0; i < out->outer.ncols; i++)
-			bytes += outer_rows * staged_type_bytes(out->outer.types[i]);
-		if (is_right_join(plan->join_type))
-		{
-			double		probe_row = 0;
-
-			for (i = 0; i < out->join[0].rel.ncols; i++)
-				probe_row += staged_type_bytes(out->join[0].rel.types[i]);
-			bytes = gpuexec_right_join_bytes(outer_rows, bytes / Max(outer_rows, 1), out->join[0].tuples, probe_row);
 		}
 		else
+			switch (def->arg)
+			{
+				case AGG_ARG_NONE:
+					break;
+				case AGG_ARG_COLUMN:
+				case AGG_ARG_F8:
+					if (list_length(a->args) != 1 ||
+						!match_f8_expr((Node *) ((TargetEntry *) linitial(a->args))->expr, &out->outer, &g->arg))
+						return false;
+					if (def->arg == AGG_ARG_COLUMN && g->arg.nops != 1)
+						return false;
+					break;
+				case AGG_ARG_F8_PAIR:
+					/* Y's program, GX_OP_ARG2, X's program, within GX_MAX_EXPR_OPS */
+					if (list_length(a->args) != 2 ||
+						!match_f8_expr((Node *) ((TargetEntry *) linitial(a->args))->expr, &out->outer, &g->arg) ||
+						g->arg.nops >= GX_MAX_EXPR_OPS)
+						return false;
+					g->arg.ops[g->arg.nops++].op = GX_OP_ARG2;
+					if (!match_f8_expr((Node *) ((TargetEntry *) lsecond(a->args))->expr, &out->outer, &g->arg))
+						return false;
+					break;
+			}
+		m->agg_refs = lappend(m->agg_refs, a);
+		plan->n_aggs++;
+	}
+	return plan->n_aggs > 0 || plan->n_group_cols > 0;
+}
+
+/* count(DISTINCT): the library groups by the key plus the DISTINCT column first, so that key must fit too (first fit, the
+ * column packed last), and est_groups is read as the number of distinct (group, value) pairs */
+static bool
+size_distinct_pairs(PlannerInfo *root, double input_rows, GpuExecState *out, GpuPlanMatch *m)
+{
+	Query	   *parse = root->parse;
+	gx_agg_plan *plan = &out->plan;
+	List	   *exprs = NIL;
+	ListCell   *lc;
+	double		pairs;
+
+	if (plan->n_group_cols >= GX_MAX_GROUP_COLS || !group_key_fits(m->key_types, plan->n_group_cols + 1))
+		return false;
+	foreach(lc, parse->groupClause)
+		exprs = lappend(exprs, get_sortgroupclause_tle((SortGroupClause *) lfirst(lc), parse->targetList)->expr);
+	exprs = lappend(exprs, m->distinct_arg);
+	pairs = estimate_num_groups(root, exprs, input_rows, NULL);
+	if (pairs > input_rows)
+		pairs = input_rows;
+	if (pairs < 1)
+		pairs = 1;
+	plan->est_groups = (int64) pairs;
+	m->pairs = pairs;
+	return true;
+}
+
+/* HBM the plan needs: the referenced columns of every row, plus 16 B x 2 per build row */
+static double
+hbm_bytes(const GpuExecState *out, const GpuPlanMatch *m)
+{
+	double		bytes = 0;
+	int			i;
+
+	for (i = 0; i < out->outer.ncols; i++)
+		bytes += m->outer_rows * staged_type_bytes(out->outer.types[i]);
+	if (is_right_join(out->plan.join_type))
+	{
+		double		probe_row = 0;
+
+		for (i = 0; i < out->join[0].rel.ncols; i++)
+			probe_row += staged_type_bytes(out->join[0].rel.types[i]);
+		bytes = gpuexec_right_join_bytes(m->outer_rows, bytes / Max(m->outer_rows, 1), out->join[0].tuples, probe_row);
+	}
+	else
 		for (i = 0; i < out->n_joins; i++)
 		{
 			const GpuJoinStep *j = &out->join[i];
@@ -1902,12 +1887,31 @@ gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_
 				bytes += j->tuples * staged_type_bytes(j->rel.types[k]);
 			bytes += j->tuples * 32;
 		}
-		/* count(DISTINCT): one record of (3 + state words) 8-byte words per pair, held about three times over while the
-		 * fold reads the stage-1 records and partitions its copy of them (csrc/gx_agg.cu, count_distinct_run) */
-		if (distinct_arg)
-			bytes += *est_pairs * 8.0 * (3 + 1 + 2 * plan->n_aggs) * 3;
-		*est_bytes = bytes * 1.25;
-	}
+	/* count(DISTINCT): one record of (3 + state words) 8-byte words per pair, held about three times over while the
+	 * fold reads the stage-1 records and partitions its copy of them (csrc/gx_agg.cu, count_distinct_run) */
+	if (m->distinct_arg)
+		bytes += m->pairs * 8.0 * (3 + 1 + 2 * out->plan.n_aggs) * 3;
+	return bytes * 1.25;
+}
+
+/* The steps run in this order: rel_column() numbers the descriptor's columns in the order they are first met. */
+static bool
+gpuexec_match_plan(PlannerInfo *root, RelOptInfo *input_rel, RelOptInfo *output_rel, GpuExecState *out, GpuPlanMatch *m)
+{
+	Query	   *parse = root->parse;
+	Path	   *in = input_rel->cheapest_total_path;
+
+	if (parse->groupingSets || parse->havingQual || parse->hasWindowFuncs || parse->hasTargetSRFs || in == NULL)
+		return false;
+	out->plan.outer_key_col = -1;
+	if (!match_input(root, input_rel, out, m) || !match_group_by(root, out, m) || !within_library_limits(out, m) ||
+		!match_aggregates(parse, out, m) || !state_words_fit(root, &out->outer, &out->plan))
+		return false;
+	m->groups = output_rel->rows > 0 ? output_rel->rows : 1;
+	out->plan.est_groups = (int64) m->groups;
+	if (m->distinct_arg && !size_distinct_pairs(root, in->rows, out, m))
+		return false;
+	m->bytes = hbm_bytes(out, m);
 	return true;
 }
 
@@ -1915,14 +1919,9 @@ static void
 gpuexec_upper_paths_hook(PlannerInfo *root, UpperRelationKind stage, RelOptInfo *input_rel, RelOptInfo *output_rel)
 {
 	GpuExecState desc;
+	GpuPlanMatch m = {0};
 	Query	   *parse = root->parse;
-	List	   *agg_refs = NIL;
 	List	   *scan_exprs = NIL;
-	double		rows,
-				groups,
-				bytes = 0,
-				pages = 0,
-				pairs = 0;
 	ListCell   *lc;
 
 	if (prev_upper_paths_hook)
@@ -1930,11 +1929,11 @@ gpuexec_upper_paths_hook(PlannerInfo *root, UpperRelationKind stage, RelOptInfo 
 	if (!gpuexec_enabled || stage != UPPERREL_GROUP_AGG)
 		return;
 	memset(&desc, 0, sizeof(desc));
-	if (!gpuexec_match_plan(root, input_rel, output_rel, &desc, &agg_refs, &rows, &groups, &bytes, &pages, &pairs))
+	if (!gpuexec_match_plan(root, input_rel, output_rel, &desc, &m))
 		return;					/* decline: the CPU paths stay as they are */
 	/* capacity (the analogue of ExecChooseHashTableSize deciding on batches, nodeHash.c:864): there is
 	 * no spill path on the device, so a plan that would not fit is left to the CPU executor */
-	if (bytes > (double) gpuexec_hbm_limit_mb * 1024.0 * 1024.0)
+	if (m.bytes > (double) gpuexec_hbm_limit_mb * 1024.0 * 1024.0)
 		return;
 	{
 		CustomPath *cpath = makeNode(CustomPath);
@@ -1944,7 +1943,7 @@ gpuexec_upper_paths_hook(PlannerInfo *root, UpperRelationKind stage, RelOptInfo 
 
 		desc.partial = !pushdown;
 		/* a count(DISTINCT) result has no partial state, and distinct counts do not add across datanodes */
-		if (desc.partial && pairs > 0)
+		if (desc.partial && m.pairs > 0)
 			return;
 		/* the scan tuple: GROUP BY expressions, then the aggregates (partial Aggrefs in two-phase mode) */
 		scan_target = create_empty_pathtarget();
@@ -1956,7 +1955,7 @@ gpuexec_upper_paths_hook(PlannerInfo *root, UpperRelationKind stage, RelOptInfo 
 			scan_exprs = lappend(scan_exprs, tle->expr);
 			add_column_to_pathtarget(scan_target, tle->expr, sgc->tleSortGroupRef);
 		}
-		foreach(lc, agg_refs)
+		foreach(lc, m.agg_refs)
 		{
 			Aggref	   *a = (Aggref *) lfirst(lc);
 
@@ -1976,7 +1975,7 @@ gpuexec_upper_paths_hook(PlannerInfo *root, UpperRelationKind stage, RelOptInfo 
 		cpath->path.param_info = NULL;
 		cpath->path.parallel_aware = false;
 		cpath->path.parallel_safe = false;	/* the GPU replaces intra-node parallelism */
-		cpath->path.rows = groups;
+		cpath->path.rows = m.groups;
 		/* the aggregate runs where the data lives */
 		cpath->path.distribution = cheapest_in->distribution;
 		/* priced like the reference's own paths — per datanode, in units of a sequential page fetch — so that add_path()
@@ -1997,7 +1996,7 @@ gpuexec_upper_paths_hook(PlannerInfo *root, UpperRelationKind stage, RelOptInfo 
 			cp.startup_us = gpuexec_startup_us;
 			if (num_nodes < 1)
 				num_nodes = 1;
-			gpuexec_path_cost(&cp, pages / num_nodes, bytes / num_nodes, groups, &startup, &total);
+			gpuexec_path_cost(&cp, m.pages / num_nodes, m.bytes / num_nodes, m.groups, &startup, &total);
 			cpath->path.startup_cost = startup;
 			cpath->path.total_cost = total;
 		}
@@ -2025,7 +2024,7 @@ gpuexec_upper_paths_hook(PlannerInfo *root, UpperRelationKind stage, RelOptInfo 
 			add_path(output_rel, (Path *)
 					 create_agg_path(root, output_rel, remote, output_rel->reltarget,
 									 parse->groupClause ? AGG_HASHED : AGG_PLAIN, AGGSPLIT_FINAL_DESERIAL,
-									 parse->groupClause, NIL, &final_costs, groups));
+									 parse->groupClause, NIL, &final_costs, m.groups));
 		}
 	}
 }

@@ -253,6 +253,7 @@ def test_an_inner_column_grouped_twice_takes_one_payload_slot(att, typ):
     ("GROUP BY text", ["rel 1 tuples 10 pages 1 cols text float8", "scan 1", "group 1.1", "target agg sum_f8 v1.2", "dist none"], False),
     ("bpchar(1) = 'R'", [LINEITEM, "scan 1", "qual 1 7 bpchareq bpchar1 R", "group 1.8", "target agg count_star", "dist none"], True),
     ("bpchar(1) = 'RX'", [LINEITEM, "scan 1", "qual 1 7 bpchareq bpchar1 RX", "group 1.8", "target agg count_star", "dist none"], False),
+    ("sum(int4)", [ORDERS, "scan 2", "group 2.3", "target agg sum_i4 v2.2", "dist none"], True),
 ], ids=lambda x: x if isinstance(x, str) else None)
 def test_capacity_edges_decline_cleanly(name, lines, accepted):
     """The descriptor's fixed capacities (GX_MAX_AGGS 8, GX_MAX_GROUP_COLS 4, GX_MAX_PREDS 4, GX_MAX_EXPR_OPS 12) and type limits:
