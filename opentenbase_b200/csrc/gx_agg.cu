@@ -1893,6 +1893,55 @@ __device__ __forceinline__ void packed_flush(unsigned long long *tab, double *ts
     if (HAS_SUM) atomicAdd(&tsum[s], sum);
 }
 
+// The fold of gx_k_runjoin_tma and gx_k_mergejoin: a warp's tile of four rows per lane (act: the lane has rows, keys in
+// order) to one (key, rows, sum) entry per run of equal keys in Q, in row order; returns the number of runs.  Runs that
+// start in a lane are stored by it, the rows that continue the previous lane's run are added to that run afterwards.
+template <bool HAS_SUM>
+__device__ __forceinline__ int runjoin_fold(gx_runlist &Q, const long long (&k)[4], const double (&v)[4], bool act, int lane)
+{
+    // ---- run heads and their numbering inside the warp
+    const long long prevk = __shfl_up_sync(0xffffffffu, k[3], 1);
+    bool hd[4];
+    hd[0] = lane == 0 || k[0] != prevk; hd[1] = k[1] != k[0]; hd[2] = k[2] != k[1]; hd[3] = k[3] != k[2];
+    const int nh = act ? (int) hd[0] + (int) hd[1] + (int) hd[2] + (int) hd[3] : 0;
+    int inc = nh;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { int t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
+    const int base = inc - nh;
+    const int NR = __shfl_sync(0xffffffffu, inc, 31);
+    // ---- fold
+    unsigned int c0 = 0; double s0 = -0.0;
+    if (act) {
+        int rid = base - 1; unsigned int c = 0; double sacc = -0.0;
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            if (hd[i]) {
+                if (rid >= base) { Q.cnt[rid] = c; if (HAS_SUM) Q.sum[rid] = sacc; } else { c0 = c; s0 = sacc; }
+                rid++; Q.key[rid] = k[i]; c = 0; sacc = -0.0;
+            }
+            c++; if (HAS_SUM) sacc = __dadd_rn(sacc, v[i]);
+        }
+        if (rid >= base) { Q.cnt[rid] = c; if (HAS_SUM) Q.sum[rid] = sacc; } else { c0 = c; s0 = sacc; }
+    }
+    __syncwarp();
+    if (c0) { atomicAdd(&Q.cnt[base - 1], c0); if (HAS_SUM) atomicAdd(&Q.sum[base - 1], s0); }
+    __syncwarp();
+    return NR;
+}
+// a CTA's packed group table (packed_flush) into the global one
+template <bool HAS_SUM>
+__device__ __forceinline__ void packed_merge(const unsigned long long *tab, const double *tsum, int S, const gx_agg_dev &A, int sum_word)
+{
+    for (int i = threadIdx.x; i < S; i += blockDim.x) {
+        const unsigned long long t = tab[i];
+        if (t == 0) continue;
+        unsigned long long *rec = global_upsert(A, t & 0xFFFFFFFFULL, 0ULL, 0u);
+        if (!rec) { atomicOr((unsigned long long *) &A.counters[1], 2ULL); continue; }
+        merge_word(&rec[3], WK_ADD_I64, (t >> 32) & 0x7FFFFFFFULL);
+        if (HAS_SUM) merge_word(&rec[3 + sum_word], WK_ADD_F64, (unsigned long long) __double_as_longlong(tsum[i]));
+    }
+}
+
 template <bool HAS_SUM, int FMT>
 __global__ void __launch_bounds__(512, 2) gx_k_runjoin2(const __grid_constant__ gx_agg_dev A, const gx_fast_args F)
 {
@@ -1973,14 +2022,7 @@ __global__ void __launch_bounds__(512, 2) gx_k_runjoin2(const __grid_constant__ 
         }
     }
     __syncthreads();
-    for (int i = threadIdx.x; i < S; i += blockDim.x) {             // the CTA's table into the global one
-        const unsigned long long t = tab[i];
-        if (t == 0) continue;
-        unsigned long long *rec = global_upsert(A, t & 0xFFFFFFFFULL, 0ULL, 0u);
-        if (!rec) { atomicOr((unsigned long long *) &A.counters[1], 2ULL); continue; }
-        merge_word(&rec[3], WK_ADD_I64, (t >> 32) & 0x7FFFFFFFULL);
-        if (HAS_SUM) merge_word(&rec[3 + F.sum_word], WK_ADD_F64, (unsigned long long) __double_as_longlong(tsum[i]));
-    }
+    packed_merge<HAS_SUM>(tab, tsum, S, A, F.sum_word);
 }
 
 // ---------------------------------------------------------------------------
@@ -2119,34 +2161,7 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin_tma(const __grid_constan
             if (cc) { atomicAdd(&Q.cnt[base - 1], cc); if (HAS_SUM) atomicAdd(&Q.sum[base - 1], sc); }
             __syncwarp();
         } else {
-            // ---- run heads and their numbering inside the warp
-            const long long prevk = __shfl_up_sync(0xffffffffu, k[3], 1);
-            bool hd[4];
-            hd[0] = lane == 0 || k[0] != prevk; hd[1] = k[1] != k[0]; hd[2] = k[2] != k[1]; hd[3] = k[3] != k[2];
-            const int nh = act ? (int) hd[0] + (int) hd[1] + (int) hd[2] + (int) hd[3] : 0;
-            int inc = nh;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) { int t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
-            const int base = inc - nh;
-            NR = __shfl_sync(0xffffffffu, inc, 31);
-            // ---- fold: runs that start in this lane are stored, the rows that continue the previous
-            // lane's run are added to that run afterwards
-            unsigned int c0 = 0; double s0 = -0.0;
-            if (act) {
-                int rid = base - 1; unsigned int c = 0; double sacc = -0.0;
-#pragma unroll
-                for (int i = 0; i < 4; i++) {
-                    if (hd[i]) {
-                        if (rid >= base) { Q.cnt[rid] = c; if (HAS_SUM) Q.sum[rid] = sacc; } else { c0 = c; s0 = sacc; }
-                        rid++; Q.key[rid] = k[i]; c = 0; sacc = -0.0;
-                    }
-                    c++; if (HAS_SUM) sacc = __dadd_rn(sacc, v[i]);
-                }
-                if (rid >= base) { Q.cnt[rid] = c; if (HAS_SUM) Q.sum[rid] = sacc; } else { c0 = c; s0 = sacc; }
-            }
-            __syncwarp();
-            if (c0) { atomicAdd(&Q.cnt[base - 1], c0); if (HAS_SUM) atomicAdd(&Q.sum[base - 1], s0); }
-            __syncwarp();
+            NR = runjoin_fold<HAS_SUM>(Q, k, v, act, lane);
         }
         // ---- one run per lane
         if (CARRY) {
@@ -2169,14 +2184,162 @@ __global__ void __launch_bounds__(1024, 1) gx_k_runjoin_tma(const __grid_constan
         }
     }
     __syncthreads();
-    for (int i = threadIdx.x; i < S; i += blockDim.x) {             // the CTA's table into the global one
-        const unsigned long long t = tab[i];
-        if (t == 0) continue;
-        unsigned long long *rec = global_upsert(A, t & 0xFFFFFFFFULL, 0ULL, 0u);
-        if (!rec) { atomicOr((unsigned long long *) &A.counters[1], 2ULL); continue; }
-        merge_word(&rec[3], WK_ADD_I64, (t >> 32) & 0x7FFFFFFFULL);
-        if (HAS_SUM) merge_word(&rec[3 + F.sum_word], WK_ADD_F64, (unsigned long long) __double_as_longlong(tsum[i]));
+    packed_merge<HAS_SUM>(tab, tsum, S, A, F.sum_word);
+}
+
+// ---------------------------------------------------------------------------
+// gx_k_mergejoin: gx_k_runjoin_tma's plan over a deferred key-ordered build (gx_hash::deferred).  Instead of a table lookup
+// each run is matched against the build rows themselves, which ascend as the outer rows do: the build side is read once,
+// and no join table is written or read.
+//  * Warp w owns the outer rows [r0_w, r0_w + rows_per_warp), tiles of 128 rows through the copy engine onto the warp's own
+//    mbarrier as in gx_k_runjoin_tma, and the build rows [b_w, b_w+1) with b_w = lower_bound(key(r0_w)) (warp 0: 0, warps
+//    past the outer rows: nbuild), plus row b_w+1 itself, which a run split across the warps' boundary may need.
+//  * The build rows pass through a register window of 32 rows, one per lane, the next 32 already requested.  A run finds
+//    its row by a 5-step search over the lanes; the window moves on when every key in it lies below every waiting run's.
+//  * Every adjacent pair of outer rows is checked to ascend, and every adjacent pair of build rows in [b_w - 1, b_w+1) to
+//    ascend strictly (an equal pair breaks the build's unique promise).  The ranges tile both inputs, so when no flag is
+//    raised every adjacent pair of both has been compared, whatever the searches returned.  MJ_ORDER, like flag 16 (a
+//    bounded wait gave up), sends the host to the filled table.
+//  * A warp whose build range holds more than max_build rows (outer keys that cover only part of the build's key range, or
+//    skip a long stretch of it) would walk that stretch alone, 32 rows per DRAM round trip: it raises MJ_SPAN before
+//    walking, and the host fills the table instead.
+#define MJ_ORDER 32ULL
+#define MJ_SPAN  64ULL
+struct gx_merge_args { const long long *bkey; const int *bpay; long long nbuild, rows_per_warp, max_build; };
+
+template <bool HAS_SUM>
+__global__ void __launch_bounds__(1024, 1) gx_k_mergejoin(const __grid_constant__ gx_agg_dev A, const gx_fast_args F, const gx_merge_args M)
+{
+    extern __shared__ __align__(128) unsigned long long smem_mj[];
+    const int S = A.s_slots;
+    unsigned long long *const tab = smem_mj; double *const tsum = (double *) (smem_mj + S);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    gx_runlist &Q = ((gx_runlist *) (smem_mj + (size_t) S * 2))[warp];
+    gx_rowstage &R = ((gx_rowstage *) (smem_mj + (size_t) S * 2 + 32 * (sizeof(gx_runlist) / 8)))[warp];
+    unsigned long long *const bar = smem_mj + (size_t) S * 2 + 32 * (sizeof(gx_runlist) / 8) + 32 * (sizeof(gx_rowstage) / 8) + warp;
+    for (int i = threadIdx.x; i < S; i += blockDim.x) { tab[i] = 0ULL; tsum[i] = -0.0; }
+    if (lane == 0) {
+        gx_mbar_init(bar, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     }
+    __syncthreads();
+    const long long gw = (long long) blockIdx.x * (blockDim.x >> 5) + warp;
+    const long long r0 = A.row0 + gw * M.rows_per_warp;
+    long long r1 = r0 + M.rows_per_warp < A.row1 ? r0 + M.rows_per_warp : A.row1;
+    const long long *const bkey = M.bkey; const int *const bpay = M.bpay; const int nb = (int) M.nbuild;     // < 2^31 rows (try_merge)
+    unsigned int flags = 0;                                     // warp-uniform
+    if (r0 < A.row1) {
+        // ---- the warp's build rows; the search starts from the key's place under uniform keys
+        const long long kf = __ldg(bkey), kl = __ldg(bkey + nb - 1);
+        auto lower_bound = [&](long long key) -> int {
+            const double f = kl > kf ? ((double) key - (double) kf) / ((double) kl - (double) kf) : 0.0;
+            const long long g = f <= 0.0 ? 0 : f >= 1.0 ? nb : (long long) (f * (double) nb);
+            return (int) gx_warp_lower_bound(nb, g, lane, [&](long long r) { return __ldg(bkey + r) >= key; });
+        };
+        const int b0 = gw == 0 ? 0 : lower_bound(__ldg(F.okey + r0));
+        int b1 = r1 < A.row1 ? lower_bound(__ldg(F.okey + r1)) : nb;
+        if (b1 < b0) { flags |= MJ_ORDER; b1 = b0; }
+        if (b1 - b0 > M.max_build) { flags |= MJ_SPAN; b1 = b0; r1 = r0; }            // nothing to do: the table answers
+        const int be = b1 < nb ? b1 + 1 : nb;                   // where the window ends
+        int wb = b0; long long wk = 0, nk = 0; int wp = 0, np = 0;     // the window [wb, wb + 32): key and payload of row wb + lane; the next one
+        auto load = [&](int base, long long &k, int &p) { const int r = base + lane; if (r < be) { k = __ldg(bkey + r); p = __ldg(bpay + r); } };
+        // the window's rows ascend strictly, the first one above `before` (the key of row wb - 1, if there is one)
+        auto check = [&](long long before, bool has_before) {
+            const long long up = __shfl_up_sync(0xffffffffu, wk, 1);
+            const bool bad = wb + lane < be && (lane > 0 ? up >= wk : has_before && before >= wk);
+            if (__any_sync(0xffffffffu, bad)) flags |= MJ_ORDER;
+        };
+        auto advance = [&]() {                                  // to the next window (callers know there is one: wb + 32 < be)
+            const long long before = __shfl_sync(0xffffffffu, wk, 31);
+            wb += 32; wk = nk; wp = np;
+            load(wb + 32, nk, np);
+            check(before, true);
+        };
+        load(wb, wk, wp); load(wb + 32, nk, np);
+        check(b0 > 0 ? __ldg(bkey + b0 - 1) : 0, b0 > 0);
+        // ---- runs Q[0, NR) (keys ascending) against the window, 32 at a time
+        auto resolve = [&](int NR) {
+            for (int base = 0; base < NR; base += 32) {
+                const int j = base + lane;
+                bool pend = j < NR;
+                const long long rk = pend ? Q.key[j] : 0;
+                for (;;) {
+                    const int left = be - wb;
+                    const int wn = left < 32 ? (left > 0 ? left : 0) : 32;          // rows in the window
+                    const long long wlast = __shfl_sync(0xffffffffu, wk, wn > 0 ? wn - 1 : 0);
+                    int pos = 0;                                    // window keys below rk
+#pragma unroll
+                    for (int st = 16; st >= 1; st >>= 1) {
+                        const long long x = __shfl_sync(0xffffffffu, wk, pos + st - 1);
+                        if (pos + st <= wn && x < rk) pos += st;
+                    }
+                    const long long xk = __shfl_sync(0xffffffffu, wk, pos & 31);
+                    const int xp = __shfl_sync(0xffffffffu, wp, pos & 31);
+                    const bool can = pend && (left <= 32 || rk <= wlast);     // the window holds rk's place
+                    if (can && pos < wn && xk == rk) packed_flush<HAS_SUM>(tab, tsum, S, A, xp, Q.cnt[j], HAS_SUM ? Q.sum[j] : -0.0);
+                    pend = pend && !can;
+                    if (!__any_sync(0xffffffffu, pend)) break;
+                    advance();
+                }
+            }
+        };
+        // ---- the outer rows
+        const long long *const okey = F.okey; const double *const vcol = F.vcol;
+        auto request = [&](long long t) {
+            const long long n = r1 - t < 128 ? r1 - t : 128;
+            const unsigned int bytes = (unsigned int) (n >> 2) << 5;
+            if (bytes == 0 || lane != 0) return;
+            gx_mbar_arrive_expect_tx(bar, HAS_SUM ? 2u * bytes : bytes);
+            gx_bulk_g2s(R.key, okey + t, bytes, bar);
+            if (HAS_SUM) gx_bulk_g2s(R.val, vcol + t, bytes, bar);
+        };
+        long long t = r0, prevk = r0 > A.row0 ? __ldg(okey + r0 - 1) : (long long) INT64_MIN;     // the key before the tile
+        bool stuck = false;
+        unsigned int parity = 0;
+        request(t);
+        while (r1 - t >= 4) {                                   // warp-uniform; the (< 4) rows at the end of the input follow
+            const int nvec = (int) ((r1 - t < 128 ? r1 - t : 128) >> 2);
+            const bool act = lane < nvec;
+            long long k[4]; double v[4];
+            if (!gx_mbar_wait(bar, parity)) { stuck = true; break; }
+            parity ^= 1u;
+            if (act) {
+                const longlong2 ka = *(const longlong2 *) &R.key[lane * 4], kb = *(const longlong2 *) &R.key[lane * 4 + 2];
+                k[0] = ka.x; k[1] = ka.y; k[2] = kb.x; k[3] = kb.y;
+                if (HAS_SUM) {
+                    const double2 a = *(const double2 *) &R.val[lane * 4], b = *(const double2 *) &R.val[lane * 4 + 2];
+                    v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y;
+                }
+            }
+            // the stage is free again (the proxy fence: see gx_k_runjoin_tma)
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            __syncwarp();
+            t += (long long) nvec << 2;
+            request(t);
+            const long long up = __shfl_up_sync(0xffffffffu, k[3], 1);
+            const bool bad = act && (k[0] < (lane > 0 ? up : prevk) || k[1] < k[0] || k[2] < k[1] || k[3] < k[2]);
+            if (__any_sync(0xffffffffu, bad)) flags |= MJ_ORDER;
+            prevk = __shfl_sync(0xffffffffu, k[3], nvec - 1);
+            resolve(runjoin_fold<HAS_SUM>(Q, k, v, act, lane));
+            __syncwarp();
+        }
+        if (!stuck && t < r1) {                                 // the (< 4) rows at the end of the input: a run each
+            const bool act = t + lane < r1;
+            const long long key = act ? __ldg(okey + t + lane) : 0;
+            const long long up = __shfl_up_sync(0xffffffffu, key, 1);
+            if (__any_sync(0xffffffffu, act && key < (lane > 0 ? up : prevk))) flags |= MJ_ORDER;
+            if (act) { Q.key[lane] = key; Q.cnt[lane] = 1u; if (HAS_SUM) Q.sum[lane] = __ldg(vcol + t + lane); }
+            __syncwarp();
+            resolve((int) (r1 - t));
+        }
+        // ---- the rest of the window's rows, for the order check
+        if (!stuck) { while (wb + 32 < be) advance(); }
+        else flags |= 16;
+    }
+    if (lane == 0 && flags) atomicOr((unsigned long long *) &A.counters[1], flags);
+    __syncthreads();
+    packed_merge<HAS_SUM>(tab, tsum, S, A, F.sum_word);
 }
 
 // ---------------------------------------------------------------------------
@@ -3399,12 +3562,81 @@ static int launch_attempt(agg_call &C, long long S, int gmax, int lp_warps, size
     return launch_agg<SINK_GLOBAL>(ctx, A, 0, kname);
 }
 
+// A deferred key-ordered build (gx_hash::deferred) under gx_k_runjoin_tma's plan shape: gx_k_mergejoin over the build rows,
+// when a sample of the outer keys ascends and the outer side has at least as many rows (a warp walks the build rows up to
+// its successor's first key, so a build far larger than the outer side would leave few warps walking long stretches).
+// *done stays false when the shape does not fit, when the group table would outgrow gx_k_runjoin_tma's, and when the
+// kernel saw keys out of order or a bounded wait gave up: the caller then fills the table and takes the general path.
+static int try_merge(agg_call &C, gx_result **out, bool *done)
+{
+    gx_ctx *ctx = C.ctx; gx_agg_dev &A = C.cp.A; const gx_hash *h = C.h;
+    *done = false;
+    if (!h->deferred || h->nbuild < 0 || h->nbuild >= INT32_MAX - 64 || !C.fast_ok || !A.P.has_join || C.outer->nrows < h->nbuild || (A.row0 & 1) != 0 ||
+        ((uintptr_t) C.FA.okey & 15) != 0 || ((uintptr_t) C.FA.vcol & 15) != 0)
+        return GX_OK;
+    // the group table the first attempt would take (the lane-private and global-table plans have no run-folding kernel)
+    auto slots = [&](long long est) { long long S = 16; while (S * 2 < est * 3 && S < C.smax) S *= 2; return S; };
+    auto smem_of = [&](long long S) { return (size_t) S * 16 + 32 * sizeof(gx_runlist) + 32 * sizeof(gx_rowstage) + 32 * 8; };
+    if (C.strategy != 1 || C.est <= 16 || slots(C.est) > 4096 || smem_of(slots(C.est)) + 1024 > ctx->smem_optin) return GX_OK;
+    int order = 0;
+    int rc = gx_sample_order(ctx, C.FA.okey + A.row0, A.row1 - A.row0, &order); if (rc) return rc;
+    if (order & 1) return GX_OK;
+    const long long nrows = A.row1 - A.row0;
+    long long warps = (long long) ctx->sm_count * 32;          // one CTA of 32 warps per SM; 31-bit row counters per CTA
+    while (((nrows + warps - 1) / warps + 127) / 128 * 128 * 32 >= (1LL << 31)) warps *= 2;
+    gx_merge_args M; M.bkey = h->bkey; M.bpay = h->bpay; M.nbuild = h->nbuild;
+    M.rows_per_warp = ((nrows + warps - 1) / warps + 127) / 128 * 128;
+    const unsigned grid = (unsigned) (((nrows + M.rows_per_warp - 1) / M.rows_per_warp + 31) / 32);
+    // a warp's share of the build rows when the outer keys spread over the build's key range, with room for uneven keys
+    M.max_build = 16 * ((h->nbuild + (long long) grid * 32 - 1) / ((long long) grid * 32)) + 4096;
+    const int RW = 3 + A.P.nwords;
+    for (int attempt = 0; attempt < 8; attempt++) {
+        const long long est = C.est;
+        if (C.strategy != 1 || est <= 16) return GX_OK;
+        const long long S = slots(est);
+        const size_t smem = smem_of(S);
+        if (S > 4096 || smem + 1024 > ctx->smem_optin) return GX_OK;
+        const long long g_cap = gx_pow2_ceil(S * 4 + 1024);
+        unsigned long long *g_tab;
+        GX_CUDA(ctx, gx_tmp_alloc(ctx, (void **) &g_tab, (size_t) g_cap * RW * 8));
+        GX_CUDA(ctx, cudaMemsetAsync(g_tab, 0, (size_t) g_cap * RW * 8, ctx->stream));
+        GX_CUDA(ctx, cudaMemsetAsync(A.counters, 0, 4 * sizeof(long long), ctx->stream));
+        A.g_tab = g_tab; A.g_mask = (unsigned long long) g_cap - 1;
+        A.s_slots = (int) S; A.s_log2 = ilog2(S); A.s_tagkey = C.tagkey; A.s_gmax = 0;
+        const int optin = (int) ctx->smem_optin;
+        rc = C.FA.vcol ? launch_kernel<gx_k_mergejoin<true>>(ctx, optin, grid, 1024, smem, "probe_agg", "probe_agg_merge", nullptr, A, C.FA, M)
+                       : launch_kernel<gx_k_mergejoin<false>>(ctx, optin, grid, 1024, smem, "probe_agg", "probe_agg_merge", nullptr, A, C.FA, M);
+        long long c[4];
+        if (rc == GX_OK) rc = read_counters(ctx, c);
+        if (rc != GX_OK) { gx_tmp_free(ctx, g_tab); return rc; }
+        if (c[1] == 0) {
+            rc = table_to_result(ctx, &C.cp, C.plan, g_tab, g_cap, c[0], out);
+            gx_tmp_free(ctx, g_tab);
+            *done = rc == GX_OK;
+            return rc;
+        }
+        gx_tmp_free(ctx, g_tab);
+        A.g_tab = nullptr;
+        if (c[1] & (MJ_ORDER | MJ_SPAN | 16)) return GX_OK;
+        // a group table overflowed: the planner's estimate was too low, grown as the attempt loop grows it
+        C.est = est < 8 ? 9 : est < 16 ? 17 : est * 8;
+        if (C.est * 3 / 2 > C.smax) return GX_OK;
+    }
+    return GX_OK;
+}
+
 static int hash_agg_run(gx_ctx *ctx, const gx_table *outer, const gx_hash *h, const gx_agg_plan *plan, gx_result **out,
                         const chain_spec *ch = nullptr)
 {
     agg_call C{};
     int rc = agg_prepare(C, ctx, outer, h, plan, ch); if (rc) return rc;
     bool done;
+    if (h && h->deferred) {
+        rc = try_merge(C, out, &done); if (rc || done) return rc;
+        rc = hash_materialize(const_cast<gx_hash *>(h)); if (rc) return rc;
+        C = agg_call{};                                           // the plan over the filled table
+        rc = agg_prepare(C, ctx, outer, h, plan, ch); if (rc) return rc;
+    }
     rc = try_runagg(C, out, &done); if (rc || done) return rc;
     gx_agg_dev &A = C.cp.A;
     const int nwords = A.P.nwords, RW = 3 + nwords;
@@ -3834,6 +4066,8 @@ extern "C" int gx_hash_agg_joins(gx_ctx *ctx, const gx_table *outer, int n_steps
     GX_CHECK_ARG(ctx, n_steps >= 1 && n_steps <= GX_MAX_JOINS && steps != nullptr, "join chain: %d steps (1..%d)", n_steps, GX_MAX_JOINS);
     GX_CHECK_ARG(ctx, plan->outer_key_col < 0, "join chain: the plan's outer_key_col must be -1 (the steps carry the keys)");
     GX_CHECK_ARG(ctx, plan->join_type == GX_JOIN_INNER, "join chain: plan join type %d (inner only)", plan->join_type);
+    for (int s = 0; s < n_steps; s++)
+        if (steps[s].h) { int rc = hash_materialize(const_cast<gx_hash *>(steps[s].h)); if (rc) return rc; }
     for (int s = 0; s < n_steps; s++) {
         const gx_join_step &st = steps[s];
         GX_CHECK_ARG(ctx, st.join_type == GX_JOIN_INNER, "join chain: step %d has join type %d (inner only)", s + 1, st.join_type);

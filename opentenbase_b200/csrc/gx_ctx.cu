@@ -41,6 +41,7 @@ extern "C" int gx_init(int device, gx_ctx **out)
     ctx->cc_major = prop.major; ctx->cc_minor = prop.minor;
     ctx->hbm_bytes = prop.totalGlobalMem;
     ctx->smem_optin = prop.sharedMemPerBlockOptin;
+    { int l2 = 0; cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, device); ctx->l2_bytes = (size_t) l2; }
     // L2 fetch granularity: a random 32-byte sector miss may otherwise drag in 64 bytes
     {
         const char *g = getenv("GX_L2_FETCH");

@@ -29,6 +29,7 @@ struct gx_ctx {
     int sm_count, cc_major, cc_minor;
     size_t hbm_bytes;
     size_t smem_optin;           // max dynamic smem per block
+    size_t l2_bytes;             // cudaDevAttrL2CacheSize
     cudaStream_t stream;         // all kernels
     cudaStream_t copy_streams[GX_NCOPY];   // H2D staging: chunks go round-robin over these (gx_exec.cu)
     cudaEvent_t copy_ev[2][GX_NCOPY];      // [0] inner table landed, [1] outer table landed (per copy stream)
@@ -63,8 +64,13 @@ struct gx_table {
     uint8_t *nulls[GX_MAX_COLS];     // NULL when the column has no NULLs
     int64_t nrows, capacity;
     uint64_t version;                // new, never reused value whenever the table is created or its rows or columns change
+    struct gx_hash *deferred;        // join tables built on this table whose fill is deferred (gx_hash::next_deferred)
 };
 uint64_t gx_table_next_version();    // gx_table.cu
+// Fill the join tables built on t whose fill was deferred, before t's rows, columns or storage change: each then answers
+// for the table as it was at build time.  freeing: t goes away whatever happens (a table whose fill failed then reports
+// that failure on every use).  gx_join.cu
+int gx_table_settle(gx_table *t, bool freeing = false);
 
 struct gx_slot { long long key; unsigned long long payload; };   // 16 B
 // Compact slot (8 B).  With an order-preserving slot function the keys that can land in one
@@ -127,9 +133,21 @@ struct gx_hash {
     // what the build read, for gx_hash_agg_right: the table, its version then, and the build quals (applied again
     // when the build rows are compacted)
     const gx_table *src; uint64_t src_version; int n_preds; gx_pred preds[GX_MAX_PREDS];
+    // Deferred key-ordered build (gx_join.cu, hash_materialize): the build rows themselves, not yet a table.  Set only for a
+    // unique int8 key without NULLs over strictly ascending sampled keys, one int4/date payload column and no build quals,
+    // whose narrowest table would not fit L2.  The merge probe (gx_agg.cu) reads bkey / bpay; every other reader fills the
+    // table first.
+    struct gx_deferred *deferred;   // nullptr: the table is filled
+    const long long *bkey; const int *bpay; long long nbuild;
+    gx_hash *next_deferred;         // src->deferred list
 };
 
 int gx_hash_wide(gx_ctx *ctx, gx_hash *h);
+// fill a deferred table exactly as gx_hash_build would have (no-op for a filled one); gx_join.cu
+int hash_materialize(gx_hash *h);
+// strided sample of an int8 key column without NULLs: *order bit 0 = two sampled keys descend, bit 1 = two are equal
+// (one launch and one synchronise); gx_join.cu
+int gx_sample_order(gx_ctx *ctx, const long long *keys, long long nrows, int *order);
 // the slot function (and slot format parameters) a table was built with
 static inline gx_slotfn gx_hash_slotfn(const gx_hash *h)
 {
@@ -603,6 +621,63 @@ __device__ __forceinline__ void gx_probe_first(const TAB &a, const bool (&ok)[K]
             }
         }
     }
+}
+
+// One warp's search for the first row of [0, nrows) at which pred holds, pred false before it and true from it on (nrows:
+// none): the 32 rows around the guess g decide it in one round when the guess is within 16 rows; otherwise a bracket is
+// grown (x16 per round) and narrowed 32-ary.  Over rows that are not so ordered the result is some row in [0, nrows].
+template <class PRED>
+__device__ __forceinline__ long long gx_warp_lower_bound(long long nrows, long long g, int lane, PRED pred_in)
+{
+    auto pred = [&](long long r) -> bool {                      // true from the bound onwards
+        if (r >= nrows) return true;
+        if (r < 0) return false;
+        return pred_in(r);
+    };
+    if (g > nrows) g = nrows;
+    // one round when the guess is within 16 rows
+    {
+        const long long pos = g - 16;
+        const unsigned int b = __ballot_sync(0xffffffffu, pred(pos + lane));
+        if (b != 0u && b != 0xffffffffu) return pos + (__ffs((int) b) - 1);
+    }
+    // grow a bracket [lo, hi]: pred(lo - 1) false (or lo == 0), pred(hi) true (or hi == nrows)
+    long long lo = 0, hi = nrows;
+    for (long long e = 256; ; e *= 16) {
+        const long long cl = g - e > 0 ? g - e : 0, ch = g + e < nrows ? g + e : nrows;
+        const bool p = lane == 0 ? pred(cl - 1) : (lane == 1 ? pred(ch) : false);
+        const unsigned int b = __ballot_sync(0xffffffffu, p);
+        const bool lo_ok = cl == 0 || !(b & 1u), hi_ok = ch == nrows || (b & 2u);
+        if (lo_ok) lo = cl;
+        if (hi_ok) hi = ch;
+        if ((lo_ok && hi_ok) || (cl == 0 && ch == nrows)) break;
+    }
+    // 32-ary narrowing
+    for (int round = 0; round < 16 && hi - lo > 32; round++) {
+        const long long step = (hi - lo + 31) / 32;
+        const long long r = lo + (long long) lane * step;
+        const unsigned int b = __ballot_sync(0xffffffffu, r >= hi ? true : pred(r));
+        if (b == 0u) { lo = lo + 31 * step + 1; continue; }
+        const int f = __ffs((int) b) - 1;
+        hi = lo + (long long) f * step < hi ? lo + (long long) f * step : hi;
+        if (f > 0) lo = lo + (long long) (f - 1) * step + 1;
+    }
+    {
+        const long long r = lo + lane;
+        const unsigned int b = __ballot_sync(0xffffffffu, r >= hi ? true : pred(r));
+        return b ? lo + (__ffs((int) b) - 1) : hi;
+    }
+}
+// lower_bound(s) of the key-ordered build = first row whose key maps to sub-table >= s (gx_k_sorted_bounds_search).  The guess:
+// the global density, or — better — the previous bound plus one sub-table's worth of rows (a datanode's 1/N pseudo-random
+// subset of the keys wanders off the global density by hundreds of rows, but only by a dozen per sub-table)
+__device__ __forceinline__ long long sorted_lower_bound(const long long *__restrict__ keys, long long nrows, const gx_slotfn &sf,
+                                                        long long s, long long nsub, double rows_per_sub, int lane, long long seed = -1)
+{
+    if (s <= 0) return 0;
+    if (s >= nsub) return nrows;
+    const long long g = seed >= 0 ? seed + (long long) rows_per_sub : (long long) ((double) s * rows_per_sub);
+    return gx_warp_lower_bound(nrows, g, lane, [&](long long r) { return (long long) (gx_slot_index(__ldg(keys + r), sf) >> GX_SUB_LOG2) >= s; });
 }
 
 // the key of a compact or narrow entry in slot i from its tag bits v = (key - kmin) mod 2^mbits: the offset congruent to v

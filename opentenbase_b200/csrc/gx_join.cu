@@ -37,6 +37,7 @@ enum {
     SW_KRANGE = 4, SW_PRANGE = 16,      // the sample's key, payload min and max
     SW_UNSORTED = 6, SW_OVERFLOW = 7,   // key-ordered build: rows out of key order; OVF_* bits (both int)
     SW_ENDS = 20,                       // the key column's first and last key
+    SW_ORDER = 18,                      // the sample's order bits (gx_k_key_range, int)
     OVF_FULL = 1, OVF_STUCK = 2, OVF_PAYLOAD = 4   // a sub-table is full; a staged wait gave up; a payload outside the narrow window
 };
 
@@ -724,54 +725,7 @@ __global__ void __launch_bounds__(FILL_THREADS, F != GX_SLOTS_WIDE ? 3 : 2) gx_k
 //    start[0] = 0 and start[nsub] = nrows are fixed and the ranges [start[s], start[s+1]) tile
 //    [0, nrows), so if no CTA raises the flag every adjacent pair of rows has been compared and
 //    every row sits in the right sub-table — whatever the search returned.  A raised flag sends
-//    the host down the bucketing path.
-__device__ __forceinline__ long long sorted_lower_bound(const long long *__restrict__ keys, long long nrows, const gx_slotfn &sf,
-                                                        long long s, long long nsub, double rows_per_sub, int lane, long long seed = -1)
-{
-    if (s <= 0) return 0;
-    if (s >= nsub) return nrows;
-    auto pred = [&](long long r) -> bool {                      // true from the bound onwards
-        if (r >= nrows) return true;
-        if (r < 0) return false;
-        return (long long) (gx_slot_index(__ldg(keys + r), sf) >> GX_SUB_LOG2) >= s;
-    };
-    // guess: the global density, or — better — the previous bound plus one sub-table's worth of rows (a datanode's 1/N
-    // pseudo-random subset of the keys wanders off the global density by hundreds of rows, but only by a dozen per sub-table)
-    long long g = seed >= 0 ? seed + (long long) rows_per_sub : (long long) ((double) s * rows_per_sub);
-    if (g > nrows) g = nrows;
-    // one round when the guess is within 16 rows
-    {
-        const long long pos = g - 16;
-        const unsigned int b = __ballot_sync(0xffffffffu, pred(pos + lane));
-        if (b != 0u && b != 0xffffffffu) return pos + (__ffs((int) b) - 1);
-    }
-    // grow a bracket [lo, hi]: pred(lo - 1) false (or lo == 0), pred(hi) true (or hi == nrows)
-    long long lo = 0, hi = nrows;
-    for (long long e = 256; ; e *= 16) {
-        const long long cl = g - e > 0 ? g - e : 0, ch = g + e < nrows ? g + e : nrows;
-        const bool p = lane == 0 ? pred(cl - 1) : (lane == 1 ? pred(ch) : false);
-        const unsigned int b = __ballot_sync(0xffffffffu, p);
-        const bool lo_ok = cl == 0 || !(b & 1u), hi_ok = ch == nrows || (b & 2u);
-        if (lo_ok) lo = cl;
-        if (hi_ok) hi = ch;
-        if ((lo_ok && hi_ok) || (cl == 0 && ch == nrows)) break;
-    }
-    // 32-ary narrowing
-    for (int round = 0; round < 16 && hi - lo > 32; round++) {
-        const long long step = (hi - lo + 31) / 32;
-        const long long r = lo + (long long) lane * step;
-        const unsigned int b = __ballot_sync(0xffffffffu, r >= hi ? true : pred(r));
-        if (b == 0u) { lo = lo + 31 * step + 1; continue; }
-        const int f = __ffs((int) b) - 1;
-        hi = lo + (long long) f * step < hi ? lo + (long long) f * step : hi;
-        if (f > 0) lo = lo + (long long) (f - 1) * step + 1;
-    }
-    {
-        const long long r = lo + lane;
-        const unsigned int b = __ballot_sync(0xffffffffu, r >= hi ? true : pred(r));
-        return b ? lo + (__ffs((int) b) - 1) : hi;
-    }
-}
+//    the host down the bucketing path.  The search itself: sorted_lower_bound (gx_internal.cuh).
 
 // start[s] for every sub-table by search: one warp per bound, ~one 256-byte read each
 __global__ void __launch_bounds__(256) gx_k_sorted_bounds_search(const long long *__restrict__ keys, long long nrows, gx_slotfn sf,
@@ -815,14 +769,19 @@ __global__ void gx_k_bbuild_total(const unsigned int *cursor, long long n, long 
 __global__ void gx_k_scan_i64(long long *v, long long n, long long *total);   // gx_agg.cu
 
 // key-density estimate for the slot function: min / max over a strided sample; the same for the payload column
-// (pay.data non-null: the narrow slot form's payload window) of the sampled rows with a key
-__global__ void gx_k_key_range(gx_dcol key, gx_dcol pay, long long nrows, long long stride, long long *minmax, long long *pminmax)
+// (pay.data non-null: the narrow slot form's payload window) of the sampled rows with a key.  *order (when not null): bit 0
+// = a sampled key is below the one a stride before it, bit 1 = equal to it (a NULL counts as neither)
+__global__ void gx_k_key_range(gx_dcol key, gx_dcol pay, long long nrows, long long stride, long long *minmax, long long *pminmax, int *order)
 {
     long long i = ((long long) blockIdx.x * blockDim.x + threadIdx.x) * stride;
     long long lo = 0x7fffffffffffffffLL, hi = -0x7fffffffffffffffLL - 1, plo = lo, phi = hi;
     if (i < nrows && !gx_is_null(key, i)) {
         lo = hi = gx_load_int(key, i);
         if (pay.data) plo = phi = gx_load_int(pay, i);
+        if (order && i + stride < nrows && !gx_is_null(key, i + stride)) {
+            const long long next = gx_load_int(key, i + stride);
+            if (next <= lo) atomicOr(order, next < lo ? 1 : 2);
+        }
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
@@ -831,7 +790,7 @@ __global__ void gx_k_key_range(gx_dcol key, gx_dcol pay, long long nrows, long l
         a = __shfl_down_sync(0xffffffffu, plo, o); b = __shfl_down_sync(0xffffffffu, phi, o);
         plo = a < plo ? a : plo; phi = b > phi ? b : phi;
     }
-    if ((threadIdx.x & 31) == 0) {
+    if ((threadIdx.x & 31) == 0 && minmax) {
         atomicMin(&minmax[0], lo); atomicMax(&minmax[1], hi);
         if (pay.data) { atomicMin(&pminmax[0], plo); atomicMax(&pminmax[1], phi); }
     }
@@ -944,16 +903,22 @@ static int build_setup(build_job &j, int n_preds, const gx_pred *preds, int n_pa
     }
     if (j.payload_bytes > 8) { GX_SET_ERR(ctx, "hash_build: payload columns total %d bytes > 8", j.payload_bytes); return GX_ERR_ARG; }
     h->nslots = gx_pow2_ceil(inner->nrows + inner->nrows / 2 + 16); h->special_cap = 1 << 16;      // load factor <= 0.67
+    h->win = j.sw.win; h->amask = 1u;                           // the mixing hash until the sample says otherwise
+    a.mask = (unsigned long long) h->nslots - 1; a.special_cap = h->special_cap; a.counters = ctx->d_scratch;
+    return GX_OK;
+}
+// the table's slots and side list
+static int alloc_table(build_job &j)
+{
+    gx_ctx *ctx = j.ctx; gx_hash *h = j.h;
     cudaError_t e = gx_tmp_alloc(ctx, (void **) &h->slots, (size_t) h->nslots * sizeof(gx_slot));
     if (e == cudaSuccess) e = gx_tmp_alloc(ctx, (void **) &h->special_payload, (size_t) h->special_cap * sizeof(unsigned long long));
     if (e != cudaSuccess) { GX_SET_ERR(ctx, "hash_build: cudaMalloc of %lld slots failed: %s", (long long) h->nslots, cudaGetErrorString(e)); return GX_ERR_NOMEM; }
-    h->win = j.sw.win; h->amask = 1u;                           // the mixing hash until the sample says otherwise
-    a.slots = h->slots; a.mask = (unsigned long long) h->nslots - 1;
-    a.special = h->special_payload; a.special_cap = h->special_cap; a.counters = ctx->d_scratch;
+    j.a.slots = h->slots; j.a.special = h->special_payload;
     return GX_OK;
 }
 // the sample's key and payload ranges, the key column's first and last key, and the slot function chosen
-struct key_sample { long long lo, hi, pmin, pmax, first, last; bool have_prange, have_ends; gx_slotfn sf; };
+struct key_sample { long long lo, hi, pmin, pmax, first, last; bool have_prange, have_ends, sampled; int order; gx_slotfn sf; };
 // the key column's first and last key (this synchronises the stream)
 static int fetch_key_ends(const build_job &j, key_sample &s)
 {
@@ -976,15 +941,19 @@ static int sample_keys(build_job &j, key_sample &s)
         long long *krange = ctx->d_scratch + SW_KRANGE, *prange = ctx->d_scratch + SW_PRANGE;
         GX_CUDA(ctx, cudaMemcpyAsync(krange, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
         GX_CUDA(ctx, cudaMemcpyAsync(prange, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
+        int *order = (int *) (ctx->d_scratch + SW_ORDER);
+        GX_CUDA(ctx, cudaMemsetAsync(order, 0, sizeof(long long), ctx->stream));
         // one int4/date payload column: its sampled range decides whether the narrow slot form can hold it
         const bool pay4 = j.a.n_payload == 1 && (j.a.payload[0].type == GX_INT4 || j.a.payload[0].type == GX_DATE);
         gx_dcol pay; memset(&pay, 0, sizeof(pay)); if (pay4) pay = j.a.payload[0];
-        { gx_launch_scope ls(ctx, "build_sample"); gx_k_key_range<<<(unsigned) ((nthreads + 255) / 256), 256, 0, ctx->stream>>>(j.a.key, pay, nrows, stride, krange, prange); }
+        { gx_launch_scope ls(ctx, "build_sample"); gx_k_key_range<<<(unsigned) ((nthreads + 255) / 256), 256, 0, ctx->stream>>>(j.a.key, pay, nrows, stride, krange, prange, order); }
         GX_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + SW_KRANGE, krange, 2 * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream));
         GX_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + SW_PRANGE, prange, 2 * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream));
+        GX_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + SW_ORDER, order, sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream));
         int rc = fetch_key_ends(j, s); if (rc) return rc;          // the sample's one synchronise
         const long long *w = ctx->h_scratch;
         s.lo = w[SW_KRANGE]; s.hi = w[SW_KRANGE + 1]; s.pmin = w[SW_PRANGE]; s.pmax = w[SW_PRANGE + 1]; s.have_prange = pay4 && s.pmin <= s.pmax;
+        s.sampled = true; s.order = *(const int *) (w + SW_ORDER);
         // widen the sampled range a little: keys outside it still map (they just wrap)
         const double range = (double) s.hi - (double) s.lo + 1.0, pad = range / 1024.0 + 64.0, lo_d = (double) s.lo - pad, range_d = range + 2 * pad;
         if (s.hi > s.lo && (range <= GX_INTERP_MAX_SPREAD * (double) nrows || j.sw.slot_mode == 1) && lo_d > -9.0e18 && lo_d + range_d < 9.0e18)
@@ -1205,14 +1174,11 @@ static int direct_build(build_job &j)
     return GX_OK;
 }
 
-extern "C" int gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col, int n_preds, const gx_pred *preds,
-                             int n_payload, const int32_t *payload_cols, int unique, gx_hash **out)
+// The table from the sample on: slots, fill, entry count and side list
+static int build_fill(build_job &j, key_sample &ks)
 {
-    if (!ctx || !inner || !out) return GX_ERR_ARG;
-    build_job j(ctx, inner, key_col);
-    int rc = build_setup(j, n_preds, preds, n_payload, payload_cols, unique); if (rc) return rc;
-    gx_hash *h = j.h; long long *w = ctx->h_scratch;
-    key_sample ks; rc = sample_keys(j, ks); if (rc) return rc;
+    gx_ctx *ctx = j.ctx; const gx_table *inner = j.inner; gx_hash *h = j.h; long long *w = ctx->h_scratch;
+    int rc = alloc_table(j); if (rc) return rc;
     GX_CUDA(ctx, clear_scratch(ctx, SW_INSERTED, SW_SPECIAL));
     long long nplaced = -1;                                         // entries a fill placed (key-ordered or bucketed build)
     if (inner->nrows == 0) { gx_launch_scope ls(ctx, "build_clear"); gx_k_fill_slots<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(h->slots, h->nslots); }
@@ -1241,7 +1207,101 @@ extern "C" int gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col, in
     h->nentries = w[SW_INSERTED] + w[SW_SPECIAL];
     h->special_count = (int) w[SW_SPECIAL];
     GX_CHECK_ARG(ctx, h->special_count <= h->special_cap, "hash_build: %d rows carry key INT64_MIN (side list holds %d)", h->special_count, h->special_cap);
+    return GX_OK;
+}
+
+// What a deferred build keeps for its fill: the build as gx_hash_build set it up and sampled it
+struct gx_deferred { gx_build_args a; int payload_bytes; build_switches sw; key_sample ks; };
+
+// Defer the fill?  A key-ordered merge (gx_agg.cu, gx_k_mergejoin) can then read the build rows themselves instead of a table
+// written once and read once.  Only the staged narrow build's shape (unique int8 key without NULLs, one int4/date payload, no
+// quals, 16-byte aligned columns) over strictly ascending sampled keys, and only when even its narrowest table (4-byte
+// slots) is larger than L2: a smaller table stays in L2 between the fill and the probe, and every other reader fills it
+// anyway.
+static bool defer_fill(const build_job &j, const key_sample &ks)
+{
+    const gx_build_args &a = j.a; const gx_hash *h = j.h;
+    return ks.sampled && ks.order == 0 && h->unique && a.key.type == GX_INT8 && a.key.nulls == nullptr && a.npreds == 0 &&
+           a.n_payload == 1 && (a.payload[0].type == GX_INT4 || a.payload[0].type == GX_DATE) &&
+           ((uintptr_t) a.key.data & 15) == 0 && ((uintptr_t) a.payload[0].data & 15) == 0 &&
+           (size_t) h->nslots * sizeof(unsigned int) > j.ctx->l2_bytes && !j.sw.direct && !j.sw.nosorted;
+}
+
+extern "C" int gx_hash_build(gx_ctx *ctx, const gx_table *inner, int key_col, int n_preds, const gx_pred *preds,
+                             int n_payload, const int32_t *payload_cols, int unique, gx_hash **out)
+{
+    if (!ctx || !inner || !out) return GX_ERR_ARG;
+    build_job j(ctx, inner, key_col);
+    int rc = build_setup(j, n_preds, preds, n_payload, payload_cols, unique); if (rc) return rc;
+    key_sample ks; rc = sample_keys(j, ks); if (rc) return rc;
+    gx_hash *h = j.h;
+    if (defer_fill(j, ks)) {
+        h->deferred = new gx_deferred{ j.a, j.payload_bytes, j.sw, ks };
+        h->bkey = (const long long *) j.a.key.data; h->bpay = (const int *) j.a.payload[0].data; h->nbuild = inner->nrows;
+        gx_table *src = const_cast<gx_table *>(inner);
+        h->next_deferred = src->deferred; src->deferred = h;
+    } else {
+        rc = build_fill(j, ks); if (rc) return rc;
+    }
     *out = h; j.h = nullptr;
+    return GX_OK;
+}
+
+static void unlink_deferred(gx_hash *h)
+{
+    gx_table *src = const_cast<gx_table *>(h->src);
+    if (!src) return;                               // its table is gone (gx_table_settle): nothing links to it
+    for (gx_hash **p = &src->deferred; *p; p = &(*p)->next_deferred)
+        if (*p == h) { *p = h->next_deferred; break; }
+    h->next_deferred = nullptr;
+}
+// the buffers and statistics of a fill, back to what the sample left
+static void drop_fill(gx_hash *h)
+{
+    gx_tmp_free(h->ctx, h->slots); gx_tmp_free(h->ctx, h->cslots); gx_tmp_free(h->ctx, h->narrow); gx_tmp_free(h->ctx, h->special_payload);
+    h->slots = nullptr; h->cslots = nullptr; h->narrow = nullptr; h->special_payload = nullptr;
+    h->nentries = 0; h->special_count = 0; h->avg_chain = 0.0; h->sorted_build = 0; h->cspan = 0; h->keys_per_slot = 0.0;
+}
+int hash_materialize(gx_hash *h)
+{
+    if (!h->deferred) return GX_OK;
+    if (h->nbuild < 0) { GX_SET_ERR(h->ctx, "join table: its build table was freed before the deferred fill could run"); return GX_ERR_STATE; }
+    gx_deferred *d = h->deferred;
+    build_job j(h->ctx, h->src, 0);
+    j.a = d->a; j.payload_bytes = d->payload_bytes; j.sw = d->sw; j.h = h;
+    set_slotfn(h, d->ks.sf);
+    key_sample ks = d->ks;
+    const int rc = build_fill(j, ks);
+    j.h = nullptr;                                  // the caller's handle: never freed here
+    if (rc) { drop_fill(h); set_slotfn(h, d->ks.sf); return rc; }     // still deferred: a later call tries again
+    unlink_deferred(h);
+    delete d; h->deferred = nullptr;
+    return GX_OK;
+}
+int gx_table_settle(gx_table *t, bool freeing)
+{
+    while (t->deferred) {
+        gx_hash *h = t->deferred;
+        const int rc = hash_materialize(h);
+        if (rc && !freeing) return rc;
+        if (rc) { unlink_deferred(h); h->nbuild = -1; h->src = nullptr; }      // its rows are gone: every later use reports the failure
+    }
+    return GX_OK;
+}
+// a strided sample of 64 K keys, as the build's
+int gx_sample_order(gx_ctx *ctx, const long long *keys, long long nrows, int *order)
+{
+    long long stride = nrows / 65536; if (stride < 1) stride = 1;
+    const long long nthreads = (nrows + stride - 1) / stride;
+    int *d_order = (int *) (ctx->d_scratch + SW_ORDER);
+    gx_dcol key; memset(&key, 0, sizeof(key)); key.data = keys; key.type = GX_INT8;
+    gx_dcol pay; memset(&pay, 0, sizeof(pay));
+    GX_CUDA(ctx, cudaMemsetAsync(d_order, 0, sizeof(long long), ctx->stream));
+    { gx_launch_scope ls(ctx, "agg_sample"); gx_k_key_range<<<(unsigned) ((nthreads + 255) / 256), 256, 0, ctx->stream>>>(key, pay, nrows, stride, nullptr, nullptr, d_order); }
+    GX_CUDA(ctx, cudaGetLastError());
+    GX_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + SW_ORDER, d_order, sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream));
+    GX_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    *order = *(const int *) (ctx->h_scratch + SW_ORDER);
     return GX_OK;
 }
 
@@ -1270,6 +1330,7 @@ __global__ void gx_k_expand_slots(const void *c, gx_slot *w, long long nslots, g
 }
 int gx_hash_wide(gx_ctx *ctx, gx_hash *h)
 {
+    int rc = hash_materialize(h); if (rc) return rc;
     if (h->slots || (!h->cslots && !h->narrow)) return GX_OK;
     cudaError_t e = gx_tmp_alloc(ctx, (void **) &h->slots, (size_t) h->nslots * sizeof(gx_slot));
     if (e != cudaSuccess) { h->slots = nullptr; GX_SET_ERR(ctx, "hash table: cudaMalloc of %lld slots failed: %s", (long long) h->nslots, cudaGetErrorString(e)); return GX_ERR_NOMEM; }
@@ -1280,11 +1341,13 @@ int gx_hash_wide(gx_ctx *ctx, gx_hash *h)
     return GX_OK;
 }
 
-extern "C" int64_t gx_hash_nentries(const gx_hash *h) { return h ? h->nentries : -1; }
-extern "C" int64_t gx_hash_nslots(const gx_hash *h) { return h ? h->nslots : -1; }
+// the statistics describe the filled table: a deferred one is filled first (a failure: -1 / the error, gx_last_error says why)
+extern "C" int64_t gx_hash_nentries(const gx_hash *h) { return h && hash_materialize(const_cast<gx_hash *>(h)) == GX_OK ? h->nentries : -1; }
+extern "C" int64_t gx_hash_nslots(const gx_hash *h) { return h && hash_materialize(const_cast<gx_hash *>(h)) == GX_OK ? h->nslots : -1; }
 extern "C" int gx_hash_info(const gx_hash *h, int *slot_mode, double *avg_chain)
 {
     if (!h) return GX_ERR_ARG;
+    int rc = hash_materialize(const_cast<gx_hash *>(h)); if (rc) return rc;
     if (slot_mode) *slot_mode = h->sorted_build ? 2 : (h->mode != 0 ? 1 : 0);
     if (avg_chain) *avg_chain = h->avg_chain;
     return GX_OK;
@@ -1292,6 +1355,7 @@ extern "C" int gx_hash_info(const gx_hash *h, int *slot_mode, double *avg_chain)
 extern "C" void gx_hash_free(gx_hash *h)
 {
     if (!h) return;
+    if (h->deferred) { unlink_deferred(h); delete h->deferred; }
     gx_tmp_free(h->ctx, h->slots);
     gx_tmp_free(h->ctx, h->cslots);
     gx_tmp_free(h->ctx, h->narrow);
@@ -1469,6 +1533,7 @@ extern "C" int gx_hash_probe_ex(gx_ctx *ctx, const gx_table *outer, int key_col,
                                 const gx_hash *h, int join_type, int n_out_outer, const int32_t *out_outer_cols, gx_table **out)
 {
     if (!ctx || !outer || !h || !out) return GX_ERR_ARG;
+    int rc = hash_materialize(const_cast<gx_hash *>(h)); if (rc) return rc;
     GX_CHECK_ARG(ctx, key_col >= 0 && key_col < outer->ncols, "hash_probe: key column %d out of range", key_col);
     int kt = outer->types[key_col];
     GX_CHECK_ARG(ctx, kt == GX_INT4 || kt == GX_INT8 || kt == GX_DATE, "hash_probe: key type %d not supported", kt);
@@ -1488,7 +1553,7 @@ extern "C" int gx_hash_probe_ex(gx_ctx *ctx, const gx_table *outer, int key_col,
     a.cslots = h->cslots; a.narrow = h->narrow; a.cspan = h->cspan;
     a.special = h->special_payload; a.special_count = h->special_count;
     a.sf = gx_hash_slotfn(h);
-    int rc = gx_fill_dpreds(ctx, outer, n_preds, preds, a.preds); if (rc) return rc;
+    rc = gx_fill_dpreds(ctx, outer, n_preds, preds, a.preds); if (rc) return rc;
     int32_t types[GX_MAX_COLS]; bool hn[GX_MAX_COLS];
     for (int c = 0; c < n_out_outer; c++) {
         int oc = out_outer_cols[c];
@@ -1653,6 +1718,7 @@ extern "C" int gx_hash_agg_right(gx_ctx *ctx, const gx_table *probe, int probe_k
     GX_CHECK_ARG(ctx, join_type == GX_JOIN_SEMI_RIGHT || join_type == GX_JOIN_ANTI_RIGHT,
                  "hash_agg_right: join type %d (right semi %d, right anti %d)", join_type, GX_JOIN_SEMI_RIGHT, GX_JOIN_ANTI_RIGHT);
     GX_CHECK_ARG(ctx, h != nullptr, "hash_agg_right: no join table");
+    int rc = hash_materialize(const_cast<gx_hash *>(h)); if (rc) return rc;
     GX_CHECK_ARG(ctx, h->n_payload == 0, "hash_agg_right: the join table carries %d payload columns (it must carry the build row number)", h->n_payload);
     GX_CHECK_ARG(ctx, h->src == build && h->src_version == build->version,
                  "hash_agg_right: the join table was not built from this build table as it is now");
@@ -1662,7 +1728,7 @@ extern "C" int gx_hash_agg_right(gx_ctx *ctx, const gx_table *probe, int probe_k
     GX_CHECK_ARG(ctx, plan->outer_key_col < 0, "hash_agg_right: the plan's outer_key_col must be -1 (the probe key is an argument)");
     GX_CHECK_ARG(ctx, plan->join_type == GX_JOIN_INNER, "hash_agg_right: the plan's join type must be inner (%d given)", plan->join_type);
     gx_mark_args a; memset(&a, 0, sizeof(a));
-    int rc = gx_fill_dpreds(ctx, probe, n_probe_preds, probe_preds, a.preds); if (rc) return rc;
+    rc = gx_fill_dpreds(ctx, probe, n_probe_preds, probe_preds, a.preds); if (rc) return rc;
     // the plan's quals join the build quals in the compaction when they fit one qual list, else the aggregate applies them
     const bool plan_keeps_preds = h->n_preds + plan->n_preds > GX_MAX_PREDS;
     int map[GX_MAX_COLS]; int32_t out_cols[GX_MAX_COLS]; int n_out = 0;

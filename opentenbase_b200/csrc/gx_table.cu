@@ -44,12 +44,18 @@ extern "C" int gx_table_create(gx_ctx *ctx, int ncols, const int32_t *types, int
 extern "C" void gx_table_free(gx_table *t)
 {
     if (!t) return;
+    gx_table_settle(t, true);
     for (int c = 0; c < t->ncols; c++) { if (t->cols[c]) gx_tmp_free(t->ctx, t->cols[c]); if (t->nulls[c]) gx_tmp_free(t->ctx, t->nulls[c]); }
     free(t);
 }
 extern "C" int64_t gx_table_nrows(const gx_table *t) { return t ? t->nrows : -1; }
 extern "C" int gx_table_ncols(const gx_table *t) { return t ? t->ncols : -1; }
-extern "C" int gx_table_truncate(gx_table *t) { if (!t) return GX_ERR_ARG; t->nrows = 0; t->version = gx_table_next_version(); return GX_OK; }
+extern "C" int gx_table_truncate(gx_table *t)
+{
+    if (!t) return GX_ERR_ARG;
+    int rc = gx_table_settle(t); if (rc) return rc;
+    t->nrows = 0; t->version = gx_table_next_version(); return GX_OK;
+}
 // End of a load: wait for the enqueued appends and report a NULL that arrived in a column staged as NOT NULL
 extern "C" int gx_table_load_finish(gx_table *t)
 {
@@ -64,6 +70,7 @@ extern "C" int gx_table_load_finish(gx_table *t)
 extern "C" int gx_table_drop_column(gx_table *t, int col)
 {
     if (!t || col < 0 || col >= t->ncols || t->ncols < 2) return GX_ERR_ARG;
+    int rc = gx_table_settle(t); if (rc) return rc;
     gx_tmp_free(t->ctx, t->cols[col]); gx_tmp_free(t->ctx, t->nulls[col]);
     for (int c = col; c + 1 < t->ncols; c++) { t->cols[c] = t->cols[c + 1]; t->nulls[c] = t->nulls[c + 1]; t->types[c] = t->types[c + 1]; }
     t->ncols--;
@@ -74,6 +81,7 @@ extern "C" int gx_table_drop_column(gx_table *t, int col)
 extern "C" int gx_table_column_devptr(gx_table *t, int col, void **dptr)
 {
     if (!t || col < 0 || col >= t->ncols || !dptr) return GX_ERR_ARG;
+    int rc = gx_table_settle(t); if (rc) return rc;      // the caller may write the column
     *dptr = t->cols[col];
     return GX_OK;
 }
@@ -83,6 +91,7 @@ extern "C" int gx_table_reserve(gx_table *t, int64_t capacity_rows)
 {
     if (!t || capacity_rows < 0) return GX_ERR_ARG;
     if (capacity_rows <= t->capacity) return GX_OK;
+    int rc = gx_table_settle(t); if (rc) return rc;
     gx_ctx *ctx = t->ctx;
     for (int c = 0; c < t->ncols; c++) {
         const int sz = gx_type_size(t->types[c]);
@@ -114,6 +123,7 @@ extern "C" int gx_table_append_columns(gx_table *t, const void *const *host_cols
                                        const uint8_t *const *host_nulls, int64_t nrows)
 {
     if (!t || !host_cols || nrows < 0) return GX_ERR_ARG;
+    int rc = gx_table_settle(t); if (rc) return rc;
     gx_ctx *ctx = t->ctx;
     GX_CHECK_ARG(ctx, t->nrows + nrows <= t->capacity, "append_columns: %lld + %lld rows exceed capacity %lld",
                  (long long) t->nrows, (long long) nrows, (long long) t->capacity);
@@ -339,6 +349,7 @@ static int generate_impl(gx_table *t, int table_id, int sf, int64_t o0, int64_t 
 extern "C" int gx_table_generate(gx_table *t, int table_id, int sf, int64_t order0, int64_t order1, int node, int nnodes)
 {
     if (!t) return GX_ERR_ARG;
+    int rc = gx_table_settle(t); if (rc) return rc;
     return generate_impl(t, table_id, sf, order0, order1, node, nnodes, nullptr);
 }
 // colmap[c] = schema column number feeding table column c (bench: only the referenced columns)
@@ -346,6 +357,7 @@ extern "C" int gx_table_generate_cols(gx_table *t, int table_id, int sf, int64_t
                                       int node, int nnodes, const int32_t *colmap)
 {
     if (!t || !colmap) return GX_ERR_ARG;
+    int rc = gx_table_settle(t); if (rc) return rc;
     return generate_impl(t, table_id, sf, order0, order1, node, nnodes, colmap);
 }
 
@@ -685,6 +697,7 @@ extern "C" int gx_table_append_heap_pages(gx_table *t, const void *pages, int64_
                                           const uint16_t *vis_offsets, const int32_t *vis_counts, int32_t vis_stride)
 {
     if (!t || !pages || !desc || npages < 0) return GX_ERR_ARG;
+    int rc = gx_table_settle(t); if (rc) return rc;
     gx_ctx *ctx = t->ctx;
     GX_CHECK_ARG(ctx, desc->natts > 0 && desc->natts <= 64, "heap desc: natts %d out of range", desc->natts);
     GX_CHECK_ARG(ctx, desc->ncols == t->ncols, "heap desc: ncols %d != table ncols %d", desc->ncols, t->ncols);
@@ -736,7 +749,7 @@ extern "C" int gx_table_append_heap_pages(gx_table *t, const void *pages, int64_
         if (e == cudaSuccess) e = cudaMemcpyAsync(d_vis, vis_offsets, (size_t) npages * vis_stride * sizeof(uint16_t), cudaMemcpyHostToDevice, ctx->stream);
         if (e == cudaSuccess) e = cudaMemcpyAsync(d_cnt, vis_counts, (size_t) npages * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream);
     }
-    int rc = GX_OK;
+    rc = GX_OK;
     if (e == cudaSuccess && host_counts) {
         a.pages = d_pages; a.vis = d_vis; a.vis_counts = d_cnt;
         // h_offs is pageable: the copy is staged by the driver before the call returns
